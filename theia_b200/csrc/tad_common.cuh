@@ -117,7 +117,6 @@ constexpr int kGroupCap = 4096;       // rows a bucket may hold to take the shar
 constexpr int kGroupCapMid = 2048;    // second capacity class
 constexpr int kGroupCapSmall = 1024;  // first capacity class (highest occupancy)
 constexpr int kGroupTarget = 768;     // mean rows per bucket pick_logb aims for
-constexpr int kGroupThreads = 256;
 constexpr int kGroupHT = 2 * kGroupCap;
 
 
