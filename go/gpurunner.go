@@ -78,6 +78,16 @@ func newGPUJobRunner(device int) (*gpuJobRunner, error) {
 	return &gpuJobRunner{ctx: ctx}, nil
 }
 
+// SetMemoryBudget caps the device memory the runner's context holds (0 = what is free when a job starts, less a
+// headroom).  A job larger than the budget runs in hash-range passes instead of failing; it takes effect for jobs that
+// start after the call.  The controller sets it once after newGPUJobRunner when the GPU is shared.
+func (r *gpuJobRunner) SetMemoryBudget(bytes uint64) error {
+	if rc := C.tad_set_memory_budget(r.ctx, C.uint64_t(bytes)); rc != C.TAD_OK {
+		return fmt.Errorf("tad_set_memory_budget: %s", C.GoString(C.tad_strerror(rc)))
+	}
+	return nil
+}
+
 func algoCode(a string) C.int32_t {
 	switch a {
 	case "ARIMA":

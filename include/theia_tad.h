@@ -201,6 +201,19 @@ int tad_result(tad_job *job, tad_rows *rows);
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
 
+/* Device memory this context's workspace may hold (bytes).  0 (default) = what is free on the device when a job starts,
+ * plus what the context already holds, less a headroom of 512 MiB.  A job that does not fit runs in hash-range passes:
+ * the connections are split by the low bits of their key hash into 2, 4, ... 64 disjoint sets, each run through the
+ * whole pipeline; the result rows are the same rows a one-pass run gives.  Host-resident input is read over PCIe once
+ * per pass.  A job fails with TAD_ERR_NOMEM only when a 1/64 hash range of it does not fit.  Caller-owned columns and
+ * pinned host memory are not counted.  If the budget drops below what the context holds, the workspace is freed before
+ * the next job.  Applies to jobs that start after the call; single GPU only (TAD_ERR_UNSUPPORTED when world_size > 1);
+ * TAD_ERR_INVALID_ARG below the floor of 64 MiB. */
+int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
+/* For a COMPLETED job: the passes it ran in and the largest device workspace the context held while it ran
+ * (TAD_ERR_STATE otherwise). */
+int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes);
+
 const char *tad_strerror(int err);
 int tad_abi_version(void);
 

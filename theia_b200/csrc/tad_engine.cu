@@ -145,6 +145,8 @@ struct tad_job {
     PinnedBlock result_block;
     tad_rows rows{};
     double t_submit = 0;
+    uint32_t passes = 0;             // hash-range passes the job ran in (tad_job_memory)
+    uint64_t peak_workspace = 0;     // largest device workspace the context held while the job ran
 };
 
 struct tad_ctx {
@@ -189,6 +191,13 @@ struct tad_ctx {
     bool peers_mapped = false;
     size_t x_agreed = 0;                            // exported size all ranks agreed on at the last (re)mapping
     DevBuf xcnt, xtotal;                            // per-source counts / totals of the owned bucket range
+    // memory budget and hash-range passes (DESIGN.md section 9)
+    std::atomic<uint64_t> budget{0};                // tad_set_memory_budget; 0 = free device memory at job start + held - headroom
+    size_t held = 0;                                // device bytes the workspace holds (ensure)
+    size_t peak = 0;                                // largest `held` since the running job started
+    size_t limit = 0;                               // while a job runs under a budget: ensure() never grows `held` past it
+    DevBuf stage, pcnt;                             // pass mode: double-buffered host chunk staging; pass counters + cursor
+    cudaEvent_t stage_ev[2]{};                      // staging half free again (the split kernel of its last chunk is done)
 };
 
 namespace {
@@ -220,21 +229,64 @@ struct JobFail {
                  cudaGetErrorString(_e), __FILE__, __LINE__);                                            \
     } while (0)
 
-void ensure(DevBuf &b, size_t bytes)
+size_t alloc_bytes(size_t bytes) { return (bytes + bytes / 16 + 256 + 255) & ~size_t(255); }   // what ensure() asks for
+size_t exact_bytes(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+// Grow-only workspace buffer.  Under a budget (ctx->limit != 0) the 1/16 slack is dropped where it would not fit, and
+// growth past the budget is a planning error: the planner sized every buffer it can know in advance.
+void ensure(tad_ctx *ctx, DevBuf &b, size_t bytes)
 {
     if (bytes <= b.cap) return;
+    const size_t rest = ctx->held - b.cap;
     if (b.p) CU(cudaFree(b.p));
     b.p = nullptr;
     b.cap = 0;
-    size_t want = bytes + bytes / 16 + 256;
-    want = (want + 255) & ~size_t(255);
+    ctx->held = rest;
+    size_t want = alloc_bytes(bytes);
+    if (ctx->limit && rest + want > ctx->limit) want = exact_bytes(bytes);
+    if (ctx->limit && rest + want > ctx->limit)
+        fail(TAD_ERR_INTERNAL, "workspace would grow to %zu bytes, past the memory budget of %zu bytes", rest + want, ctx->limit);
     cudaError_t e = cudaMalloc(&b.p, want);
     if (e != cudaSuccess) {
         cudaGetLastError();
-        want = (bytes + 255) & ~size_t(255);
+        want = exact_bytes(bytes);
         CU(cudaMalloc(&b.p, want));
     }
     b.cap = want;
+    ctx->held = rest + want;
+    ctx->peak = std::max(ctx->peak, ctx->held);
+}
+
+// Whether ensure(b, bytes) stays inside the budget (always, without one).
+bool fits(const tad_ctx *ctx, const DevBuf &b, size_t bytes)
+{
+    return !ctx->limit || bytes <= b.cap || ctx->held - b.cap + exact_bytes(bytes) <= ctx->limit;
+}
+
+// A pass whose oversized-bucket spill scratch or result buffer (sizes known only while it runs) would not fit the budget:
+// the job driver splits it by the next hash bit.
+struct PassSplit {};
+
+// Every workspace buffer of a single-GPU job except the exported multi-GPU buffer and its mappings.
+std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
+{
+    std::vector<DevBuf *> v = {&ctx->hist, &ctx->offsets, &ctx->cursor, &ctx->big_list, &ctx->big_base, &ctx->cls_list,
+                               &ctx->csr_p, &ctx->stats, &ctx->part, &ctx->csr_v, &ctx->csr_t, &ctx->nsb, &ctx->npb,
+                               &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx, &ctx->dbi, &ctx->exch,
+                               &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total, &ctx->entries,
+                               &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
+                               &ctx->stage, &ctx->pcnt};
+    for (int i = 0; i < 10; i++) v.push_back(&ctx->d_col[i]);
+    return v;
+}
+
+void free_workspace(tad_ctx *ctx)
+{
+    for (DevBuf *b : workspace_bufs(ctx)) {
+        if (b->p) CU(cudaFree(b->p));
+        ctx->held -= b->cap;
+        *b = DevBuf{};
+    }
 }
 
 PinnedBlock take_pinned(tad_ctx *ctx, size_t bytes)
@@ -269,7 +321,7 @@ void set_progress(tad_job *job, int state, int completed)
 {
     std::lock_guard<std::mutex> lk(job->mu);
     job->st.state = state;
-    job->st.completed_stages = completed;
+    job->st.completed_stages = std::max(job->st.completed_stages, completed);    // passes rerun the stages
 }
 
 int pick_logb(const tad_ctx *ctx, uint64_t rows)
@@ -346,10 +398,99 @@ OutCols out_cols(void *base, const OutLayout &L)
     return o;
 }
 
-void run_job(tad_ctx *ctx, tad_job *job)
+// first guess of the result capacity; detect reruns with the exact count when more rows are flagged
+uint64_t out_cap_guess(uint64_t points, bool emit_all)
+{
+    uint64_t out_cap = emit_all ? points : (points / 8 + (1u << 16));
+    if (out_cap > points) out_cap = points;
+    return out_cap ? out_cap : 1;
+}
+
+// Device bytes of every workspace buffer one single-GPU pipeline run sizes from its shape: the one description of the
+// layout.  run_pipeline() sizes its buffers from it (with the counts it knows at each stage) and the planner sums it with
+// upper bounds (rows for owned rows, series and points).  Not in it: the spill scratch (known after grouping), a detect
+// rerun's larger result buffer, and buffers of a few KB (kFixedBytes).
+struct PipeShape {
+    uint64_t rows = 0;               // input rows
+    const tad_columns *host = nullptr;   // host input: the columns copied to d_col[]
+    int algo = TAD_ALGO_EWMA;
+    uint32_t B = 1, Bl = 1;          // buckets; buckets this GPU owns
+    bool optimistic = false;         // fixed-capacity bucket slots instead of the exact partition
+    uint64_t owned = 0, series = 0, out_cap = 1;
+};
+struct PipeSizes {
+    size_t col[10], part, slots, ovf, entries, hist, offsets, cursor, big_list, big_base, cls_list, nsb, npb, csr_v, csr_t,
+        csr_p, sbase, outb, dbx, dbi, ar_y, ar_pred, ar_lam;
+};
+constexpr size_t kOutWidth[11] = {8, 8, 8, 4, 4, 4, 4, 2, 2, 1, 1};   // bytes per result row of each out_layout column
+constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad_set_memory_budget accepts
+constexpr uint64_t kBudgetHeadroom = 512ull << 20; // default budget: device memory left free for the CUDA context and others
+constexpr size_t kFixedBytes = 1u << 20;        // stats, scan flags, ns_ignore list, small staging
+constexpr uint64_t kSlotBudget = 40ull << 30;   // optimistic slot buffer at most half of an 80 GB H100
+
+PipeSizes pipe_sizes(const PipeShape &s)
+{
+    PipeSizes z{};
+    for (int i = 0; i < 10; i++) z.col[i] = s.host && col_ptr(*s.host, i) ? col_bytes(i, s.rows) : 0;
+    const size_t B = s.B, cap_rows = s.owned ? s.owned : 1;
+    z.part = (s.rows ? s.rows : 1) * sizeof(Row32);
+    z.slots = s.optimistic ? B * kGroupCap * sizeof(Row32) : 0;
+    z.ovf = s.optimistic ? std::max<uint64_t>(1u << 20, s.rows / 32) * sizeof(Row32) : 0;
+    z.entries = s.optimistic ? cap_rows * sizeof(SeriesEntry) : 0;
+    z.hist = z.cursor = z.big_list = B * 4;
+    z.nsb = z.npb = (size_t)s.Bl * 4;
+    z.offsets = z.big_base = (B + 1) * 4;
+    z.cls_list = B * 4 * 3;
+    z.csr_v = cap_rows * 8 + 64;       // + one sector: the direct detector reads whole 32-byte sectors
+    z.csr_t = cap_rows * 4;
+    z.csr_p = z.dbx = s.algo == TAD_ALGO_DBSCAN ? cap_rows * 4 : 0;
+    z.dbi = s.algo == TAD_ALGO_DBSCAN ? cap_rows : 0;
+    z.sbase = sbase_words(s.B, cap_rows) * 4;
+    z.outb = out_layout(s.out_cap).total;
+    z.ar_y = z.ar_pred = s.algo == TAD_ALGO_ARIMA ? cap_rows * 8 : 0;
+    z.ar_lam = s.algo == TAD_ALGO_ARIMA ? ((size_t)s.series + 1) * 8 : 0;
+    return z;
+}
+
+// (buffer, bytes) of every buffer in PipeSizes
+std::vector<std::pair<DevBuf *, size_t>> pipe_bufs(tad_ctx *ctx, const PipeSizes &z)
+{
+    std::vector<std::pair<DevBuf *, size_t>> v = {
+        {&ctx->part, std::max(z.part, z.slots)}, {&ctx->ovf, z.ovf}, {&ctx->entries, z.entries}, {&ctx->hist, z.hist},
+        {&ctx->offsets, z.offsets}, {&ctx->cursor, z.cursor}, {&ctx->big_list, z.big_list}, {&ctx->big_base, z.big_base},
+        {&ctx->cls_list, z.cls_list}, {&ctx->nsb, z.nsb}, {&ctx->npb, z.npb}, {&ctx->csr_v, z.csr_v}, {&ctx->csr_t, z.csr_t},
+        {&ctx->csr_p, z.csr_p}, {&ctx->sbase, z.sbase}, {&ctx->outb, z.outb}, {&ctx->dbx, z.dbx}, {&ctx->dbi, z.dbi},
+        {&ctx->ar_y, z.ar_y}, {&ctx->ar_pred, z.ar_pred}, {&ctx->ar_lam, z.ar_lam}};
+    for (int i = 0; i < 10; i++) v.push_back({&ctx->d_col[i], z.col[i]});
+    return v;
+}
+
+// Workspace the context holds once every listed buffer has grown to its size: `held` plus the growth, each buffer sized
+// as ensure() sizes it.  With `held` = 0 and empty buffers (fresh = true): the need of a job on an empty workspace.
+size_t workspace_after(tad_ctx *ctx, const std::vector<std::pair<DevBuf *, size_t>> &bufs, bool fresh)
+{
+    size_t total = (fresh ? 0 : ctx->held) + kFixedBytes;
+    for (const auto &b : bufs) {
+        const size_t cap = fresh ? 0 : b.first->cap;
+        if (b.second > cap) total += alloc_bytes(b.second) - cap;
+    }
+    return total;
+}
+
+// Result of one pipeline run: a one-pass job or one hash-range pass.
+struct PassOut {
+    uint64_t kept = 0, owned = 0, points = 0, series = 0, out_rows = 0, spill_rows = 0, launches = 0;
+    double phase_ms[TAD_NPHASES] = {0};
+    double device_ms = 0;
+    PinnedBlock block;               // result rows, out_layout(out_rows) in pinned host memory
+};
+
+// The pipeline (ingest, partition, exchange, group, detect, egress) over `hc`.  `filters`: apply the job's time window
+// and ns_ignore list (passes were filtered by the split kernel already).  `force_exact`: the exact partition even where
+// the optimistic slot buffer would be used (the planner found it does not fit the budget).
+void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filters, bool force_exact, PassOut &out)
 {
     const tad_job_spec &sp = job->spec;
-    const tad_columns &hc = job->cols;
     const uint64_t R = hc.rows;
     cudaStream_t st = ctx->stream;
     uint64_t launches = 0;
@@ -367,11 +508,11 @@ void run_job(tad_ctx *ctx, tad_job *job)
 
     CU(cudaSetDevice(ctx->cfg.device));
     set_progress(job, TAD_STATE_RUNNING, 0);
-    ensure(ctx->stats, 64 * sizeof(uint32_t));
+    ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
     uint32_t *d_stats = static_cast<uint32_t *>(ctx->stats.p);
     CU(cudaMemsetAsync(d_stats, 0, 64 * sizeof(uint32_t), st));
     if (!ctx->scan_sync.p) {
-        ensure(ctx->scan_sync, scan_sync_bytes());
+        ensure(ctx, ctx->scan_sync, scan_sync_bytes());
         CU(cudaMemsetAsync(ctx->scan_sync.p, 0, scan_sync_bytes(), st));
     }
 
@@ -381,6 +522,11 @@ void run_job(tad_ctx *ctx, tad_job *job)
     ColPtrs c{};
     const void *dcol[10];
     const bool host_input = hc.mem != TAD_MEM_DEVICE && R > 0;
+    PipeShape shape;
+    shape.rows = R;
+    shape.host = host_input ? &hc : nullptr;
+    shape.algo = sp.algo;
+    PipeSizes z = pipe_sizes(shape);
     for (int i = 0; i < 10; i++) {
         void *src = col_ptr(hc, i);
         dcol[i] = nullptr;
@@ -388,7 +534,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
         if (hc.mem == TAD_MEM_DEVICE) {
             dcol[i] = src;
         } else {
-            ensure(ctx->d_col[i], col_bytes(i, R));
+            ensure(ctx, ctx->d_col[i], z.col[i]);
             dcol[i] = ctx->d_col[i].p;
         }
     }
@@ -427,10 +573,10 @@ void run_job(tad_ctx *ctx, tad_job *job)
     c.src_ns = (const uint32_t *)dcol[8]; c.dst_ns = (const uint32_t *)dcol[9];
 
     RowFilter f{};
-    f.start_time = sp.start_time;
-    f.end_time = sp.end_time;
-    if (!job->ns_ignore.empty() && (c.src_ns || c.dst_ns)) {
-        ensure(ctx->ns_ignore, job->ns_ignore.size() * 4);
+    f.start_time = filters ? sp.start_time : 0;
+    f.end_time = filters ? sp.end_time : 0;
+    if (filters && !job->ns_ignore.empty() && (c.src_ns || c.dst_ns)) {
+        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
         CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
         f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
         f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
@@ -439,7 +585,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
     // ---- partition -------------------------------------------------------------------------
     const int world = ctx->cfg.world_size, me = ctx->cfg.rank;
     uint64_t R_total = R;
-    ensure(ctx->small, 4096);
+    ensure(ctx, ctx->small, 4096);
     unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
     if (world > 1 && sp.global_rows) {
         R_total = sp.global_rows;      // the host counted the table: no start-of-job collective, no host sync
@@ -461,17 +607,24 @@ void run_job(tad_ctx *ctx, tad_job *job)
     const uint32_t B = 1u << logB;                 // global buckets
     const uint32_t Bl = B >> logW;                 // buckets owned by one rank
     const uint32_t b_lo = Bl * (uint32_t)me;
-    ensure(ctx->hist, (size_t)B * 4);
-    ensure(ctx->offsets, ((size_t)B + 1) * 4);
-    ensure(ctx->cursor, (size_t)B * 4);
-    ensure(ctx->big_list, (size_t)B * 4);
-    ensure(ctx->big_base, ((size_t)B + 1) * 4);
-    ensure(ctx->cls_list, (size_t)B * 4 * 3);
-    ensure(ctx->nsb, (size_t)Bl * 4);
-    ensure(ctx->npb, (size_t)Bl * 4);
+    // slot buffer at most half of an 80 GB H100: the inputs, series entries and per-series arrays need the rest
+    constexpr uint32_t kSlot = kGroupCap;      // = the largest shared-memory class: overflow is as rare as a spill was
+    const uint64_t slot_rows = (uint64_t)B * kSlot;
+    shape.B = B;
+    shape.Bl = Bl;
+    shape.optimistic = world == 1 && ctx->optimistic && R > 0 && slot_rows * sizeof(Row32) <= kSlotBudget && !force_exact;
+    z = pipe_sizes(shape);
+    ensure(ctx, ctx->hist, z.hist);
+    ensure(ctx, ctx->offsets, z.offsets);
+    ensure(ctx, ctx->cursor, z.cursor);
+    ensure(ctx, ctx->big_list, z.big_list);
+    ensure(ctx, ctx->big_base, z.big_base);
+    ensure(ctx, ctx->cls_list, z.cls_list);
+    ensure(ctx, ctx->nsb, z.nsb);
+    ensure(ctx, ctx->npb, z.npb);
     // part[] (exact partition: 32 B per local row) is not needed when the multi-GPU optimistic path runs out of the exported
     // slot buffer; the exact multi-GPU branch allocates it on demand
-    if (world == 1) ensure(ctx->part, (R ? R : 1) * sizeof(Row32));
+    if (world == 1) ensure(ctx, ctx->part, z.part);
     uint32_t *hist = (uint32_t *)ctx->hist.p, *offsets = (uint32_t *)ctx->offsets.p, *cursor = (uint32_t *)ctx->cursor.p;
     uint32_t *big_base = (uint32_t *)ctx->big_base.p;
     uint32_t *cls_list = (uint32_t *)ctx->cls_list.p;
@@ -504,13 +657,10 @@ void run_job(tad_ctx *ctx, tad_job *job)
     // row that finds its slot full goes to the overflow list, and such buckets take the spill path.  With host input
     // the scatter of H2D chunk i runs while chunk i+1 is on the bus.  Falls back to the exact two-pass partition
     // when the overflow list fills up (heavily skewed tables).
-    constexpr uint32_t kSlot = kGroupCap;      // = the largest shared-memory class: overflow is as rare as a spill was
-    const uint64_t slot_rows = (uint64_t)B * kSlot;
-    // slot buffer at most half of an 80 GB H100: the inputs, series entries and per-series arrays need the rest
-    if (world == 1 && ctx->optimistic && R > 0 && slot_rows * sizeof(Row32) <= (40ull << 30)) {
-        const uint64_t ovf_cap = std::max<uint64_t>(1u << 20, R / 32);
-        ensure(ctx->part, slot_rows * sizeof(Row32));
-        ensure(ctx->ovf, ovf_cap * sizeof(Row32));
+    if (shape.optimistic) {
+        const uint64_t ovf_cap = z.ovf / sizeof(Row32);
+        ensure(ctx, ctx->part, z.slots);
+        ensure(ctx, ctx->ovf, z.ovf);
         part = (Row32 *)ctx->part.p;
         Row32 *ovf = (Row32 *)ctx->ovf.p;
         CU(cudaMemsetAsync(cursor, 0, (size_t)B * 4, st));
@@ -544,7 +694,8 @@ void run_job(tad_ctx *ctx, tad_job *job)
             seg.base[0] = part;
             seg.off[0] = offsets;
             seg.stride = kSlot;
-            ensure(ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
+            shape.owned = owned;
+            ensure(ctx, ctx->entries, pipe_sizes(shape).entries);
             entries = static_cast<SeriesEntry *>(ctx->entries.p);
         } else {
             CU(cudaMemsetAsync(d_stats, 0, 64 * sizeof(uint32_t), st));      // discard; redo exactly
@@ -571,7 +722,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
         ctx->peers_mapped = false;
         memset(ctx->h_small, 0, 16 * 8);
         gather16();
-        ensure(ctx->xbuf, need);
+        ensure(ctx, ctx->xbuf, need);
         cudaIpcMemHandle_t mine;
         CU(cudaIpcGetMemHandle(&mine, ctx->xbuf.p));
         memset(ctx->h_small, 0, 16 * 8);
@@ -610,8 +761,8 @@ void run_job(tad_ctx *ctx, tad_job *job)
         ensure_exported(x_need);
         uint32_t *xcursor = static_cast<uint32_t *>(ctx->xbuf.p);
         Row32 *xpart = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->xbuf.p) + x_cnt_bytes);
-        ensure(ctx->xcnt, (size_t)Bl * 4 * world);
-        ensure(ctx->xtotal, (size_t)Bl * 4);
+        ensure(ctx, ctx->xcnt, (size_t)Bl * 4 * world);
+        ensure(ctx, ctx->xtotal, (size_t)Bl * 4);
         uint32_t *xcnt = (uint32_t *)ctx->xcnt.p, *xtotal = (uint32_t *)ctx->xtotal.p;
         CU(cudaMemsetAsync(xcursor, 0, (size_t)B * 4, st));
         mark(-1);
@@ -657,7 +808,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
                 seg.base[r] = reinterpret_cast<const Row32 *>(xb + x_cnt_bytes);
                 seg.off[r] = xcnt + (size_t)r * Bl;
             }
-            ensure(ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
+            ensure(ctx, ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
             entries = static_cast<SeriesEntry *>(ctx->entries.p);
         } else {
             CU(cudaMemsetAsync(d_stats, 0, 64 * sizeof(uint32_t), st));      // discard; redo exactly (every rank does)
@@ -718,15 +869,15 @@ void run_job(tad_ctx *ctx, tad_job *job)
             ensure_exported(x_cnt_bytes + max_rows * sizeof(Row32));
             part = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->xbuf.p) + x_cnt_bytes);
         } else {
-            ensure(ctx->part, (R ? R : 1) * sizeof(Row32));
+            ensure(ctx, ctx->part, (R ? R : 1) * sizeof(Row32));
             part = (Row32 *)ctx->part.p;
         }
-        ensure(ctx->hist, (size_t)B * 4 * K);
-        ensure(ctx->offsets, ((size_t)B + 1) * 4 * K);
-        ensure(ctx->cursor, (size_t)B * 4 * K);
-        ensure(ctx->hist_all, (size_t)B * 4 * NS);
-        ensure(ctx->seg_off, ((size_t)Bl + 1) * 4 * NS);
-        ensure(ctx->seg_total, (size_t)Bl * 4);
+        ensure(ctx, ctx->hist, (size_t)B * 4 * K);
+        ensure(ctx, ctx->offsets, ((size_t)B + 1) * 4 * K);
+        ensure(ctx, ctx->cursor, (size_t)B * 4 * K);
+        ensure(ctx, ctx->hist_all, (size_t)B * 4 * NS);
+        ensure(ctx, ctx->seg_off, ((size_t)Bl + 1) * 4 * NS);
+        ensure(ctx, ctx->seg_total, (size_t)Bl * 4);
         hist = (uint32_t *)ctx->hist.p; offsets = (uint32_t *)ctx->offsets.p; cursor = (uint32_t *)ctx->cursor.p;
         uint32_t *hist_all = (uint32_t *)ctx->hist_all.p, *seg_off = (uint32_t *)ctx->seg_off.p;
         uint32_t *seg_total = (uint32_t *)ctx->seg_total.p;
@@ -780,7 +931,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
             }
             sync_at_end = true;
         } else {
-        ensure(ctx->exch, recv_total ? recv_total : 32);
+        ensure(ctx, ctx->exch, recv_total ? recv_total : 32);
         for (int cx = 0; cx < K; cx++) {
             const uint64_t lo = xlo(cx), hi = xlo(cx + 1);
             if (hi > lo) { CU(launch_scatter(st, offset_cols(lo), hi - lo, f, logB, cursor + (size_t)cx * B, part + lo)); launches++; }
@@ -812,7 +963,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
         mark(TAD_PHASE_EXCHANGE);           // = the part of the exchange NOT hidden behind the scatter
         CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        ensure(ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
+        ensure(ctx, ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
         entries = static_cast<SeriesEntry *>(ctx->entries.p);
     }
     check_cancel();
@@ -821,14 +972,15 @@ void run_job(tad_ctx *ctx, tad_job *job)
     set_progress(job, TAD_STATE_RUNNING, 3);    // ingest, partition, exchange
 
     // ---- group ------------------------------------------------------------------------------
-    const uint64_t cap_rows = owned ? owned : 1;
-    ensure(ctx->csr_v, cap_rows * 8 + 64);       // + one sector: the direct detector reads whole 32-byte sectors
-    ensure(ctx->csr_t, cap_rows * 4);
+    shape.owned = owned;
+    z = pipe_sizes(shape);
+    ensure(ctx, ctx->csr_v, z.csr_v);
+    ensure(ctx, ctx->csr_t, z.csr_t);
     uint64_t *csr_v = (uint64_t *)ctx->csr_v.p;
     uint32_t *csr_t = (uint32_t *)ctx->csr_t.p;
     uint32_t *csr_p = nullptr;
     if (sp.algo == TAD_ALGO_DBSCAN) {
-        ensure(ctx->csr_p, cap_rows * 4);
+        ensure(ctx, ctx->csr_p, z.csr_p);
         csr_p = (uint32_t *)ctx->csr_p.p;
     }
     mark(-1);
@@ -838,7 +990,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
         if (ctx->sort_classes) {
             // class lists in ascending bucket order: concurrently running CTAs then touch neighbouring slots / csr stretches
             const size_t need = sort_lists_scratch_bytes(Bl);
-            ensure(ctx->sortb, need);
+            ensure(ctx, ctx->sortb, need);
             int bits = 1;
             while ((1u << bits) < Bl && bits < 32) bits++;
             for (int k = 0; k < 3; k++)
@@ -850,14 +1002,15 @@ void run_job(tad_ctx *ctx, tad_job *job)
     mark(TAD_PHASE_GROUP);
     if (n_big) {
         const size_t need = spill_scratch_bytes(big_rows);
-        ensure(ctx->spill, need);
+        if (!fits(ctx, ctx->spill, need)) throw PassSplit{};
+        ensure(ctx, ctx->spill, need);
         int l = 0;
         CU(run_spill(st, seg, entries, offsets, big_list, big_base, n_big, big_rows, ctx->spill.p, ctx->spill.cap, csr_v, csr_t,
                      nsb, npb, sp.reducer, &l, ovf_rows, n_ovf));
         launches += l;
         mark(TAD_PHASE_SPILL);
     }
-    ensure(ctx->sbase, sbase_words(Bl, cap_rows) * 4);      // series base per bucket + bucket hint per 32 series
+    ensure(ctx, ctx->sbase, z.sbase);      // series base per bucket + bucket hint per 32 series
     uint32_t *sbase = (uint32_t *)ctx->sbase.p;
     CU(launch_series_scan(st, nsb, npb, sbase, Bl, d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
     CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
@@ -869,15 +1022,17 @@ void run_job(tad_ctx *ctx, tad_job *job)
 
     // ---- detect -----------------------------------------------------------------------------
     const bool emit_all = (sp.flags & TAD_FLAG_EMIT_ALL) != 0;
-    uint64_t out_cap = emit_all ? points : (points / 8 + (1u << 16));
-    if (out_cap > points) out_cap = points;
-    if (out_cap == 0) out_cap = 1;
+    uint64_t out_cap = out_cap_guess(points, emit_all);
     uint64_t out_rows = 0;
     OutLayout L{};
     OutCols oc{};
+    shape.series = S;
     for (int attempt = 0; attempt < 3; attempt++) {
+        shape.out_cap = out_cap;
+        z = pipe_sizes(shape);
         L = out_layout(out_cap);
-        ensure(ctx->outb, L.total);
+        if (!fits(ctx, ctx->outb, z.outb)) throw PassSplit{};
+        ensure(ctx, ctx->outb, z.outb);
         oc = out_cols(ctx->outb.p, L);
         CU(cudaMemsetAsync(d_stats + ST_OUTCOUNT, 0, 4, st));
         mark(-1);
@@ -885,15 +1040,15 @@ void run_job(tad_ctx *ctx, tad_job *job)
             CU(launch_detect_ewma(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, oc, (uint32_t)out_cap, d_stats, emit_all));
             launches += S ? 1 : 0;
         } else if (sp.algo == TAD_ALGO_DBSCAN) {
-            ensure(ctx->dbx, cap_rows * 4);         // prefix count of core points, per point slot
-            ensure(ctx->dbi, cap_rows);             // noise flag, per point slot
+            ensure(ctx, ctx->dbx, z.dbx);         // prefix count of core points, per point slot
+            ensure(ctx, ctx->dbi, z.dbi);         // noise flag, per point slot
             CU(launch_detect_dbscan(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, csr_p, (uint32_t *)ctx->dbx.p,
                                     (uint8_t *)ctx->dbi.p, oc, (uint32_t)out_cap, d_stats, emit_all));
             launches += S ? 1 : 0;
         } else if (sp.algo == TAD_ALGO_ARIMA) {
-            ensure(ctx->ar_y, cap_rows * 8);
-            ensure(ctx->ar_pred, cap_rows * 8);
-            ensure(ctx->ar_lam, ((size_t)S + 1) * 8);
+            ensure(ctx, ctx->ar_y, z.ar_y);
+            ensure(ctx, ctx->ar_pred, z.ar_pred);
+            ensure(ctx, ctx->ar_lam, z.ar_lam);
             CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (double *)ctx->ar_y.p,
                                    (double *)ctx->ar_pred.p, (double *)ctx->ar_lam.p, attempt == 0, oc, (uint32_t)out_cap,
                                    d_stats, emit_all));
@@ -922,20 +1077,12 @@ void run_job(tad_ctx *ctx, tad_job *job)
     // ---- egress: result rows -> pinned host memory -------------------------------------------
     mark(-1);
     {
-        static const size_t w[11] = {8, 8, 8, 4, 4, 4, 4, 2, 2, 1, 1};
         OutLayout HL = out_layout(out_rows ? out_rows : 1);
-        job->result_block = take_pinned(ctx, HL.total);
-        char *hb = static_cast<char *>(job->result_block.p);
+        out.block = take_pinned(ctx, HL.total);
+        char *hb = static_cast<char *>(out.block.p);
         const char *db = static_cast<const char *>(ctx->outb.p);
         for (int i = 0; i < 11 && out_rows; i++)
-            CU(cudaMemcpyAsync(hb + HL.off[i], db + L.off[i], w[i] * out_rows, cudaMemcpyDeviceToHost, st));
-        OutCols ho = out_cols(hb, HL);
-        job->rows.rows = out_rows;
-        job->rows.src_ip = ho.src_ip; job->rows.dst_ip = ho.dst_ip;
-        job->rows.src_port = ho.src_port; job->rows.dst_port = ho.dst_port;
-        job->rows.proto = ho.proto; job->rows.flow_start = ho.flow_start; job->rows.flow_end = ho.flow_end;
-        job->rows.stddev = ho.stddev; job->rows.algo_calc = ho.algo_calc; job->rows.throughput = ho.throughput;
-        job->rows.anomaly = ho.anomaly;
+            CU(cudaMemcpyAsync(hb + HL.off[i], db + L.off[i], kOutWidth[i] * out_rows, cudaMemcpyDeviceToHost, st));
     }
     mark(TAD_PHASE_D2H);
     CU(cudaStreamSynchronize(st));
@@ -957,22 +1104,330 @@ void run_job(tad_ctx *ctx, tad_job *job)
         if (ev_phase[i] == TAD_PHASE_DETECT || (ev_phase[i] == TAD_PHASE_SYNC && last_k >= 0)) last_k = i;
     }
     if (first_k >= 0 && last_k > first_k) CU(cudaEventElapsedTime(&total, ctx->ev[first_k], ctx->ev[last_k]));
+    out.kept = kept;
+    out.owned = owned;
+    out.points = points;
+    out.series = S;
+    out.out_rows = out_rows;
+    out.spill_rows = big_rows;
+    out.launches = launches;
+    out.device_ms = total;
+    for (int i = 0; i < TAD_NPHASES; i++) out.phase_ms[i] = phase_ms[i];
+}
+void publish_rows(tad_job *job, PinnedBlock block, uint64_t rows)
+{
+    job->result_block = block;
+    OutCols ho = out_cols(block.p, out_layout(rows ? rows : 1));
+    job->rows.rows = rows;
+    job->rows.src_ip = ho.src_ip; job->rows.dst_ip = ho.dst_ip;
+    job->rows.src_port = ho.src_port; job->rows.dst_port = ho.dst_port;
+    job->rows.proto = ho.proto; job->rows.flow_start = ho.flow_start; job->rows.flow_end = ho.flow_end;
+    job->rows.stddev = ho.stddev; job->rows.algo_calc = ho.algo_calc; job->rows.throughput = ho.throughput;
+    job->rows.anomaly = ho.anomaly;
+}
+
+// Workspace of one pass of `rows` rows: the pipeline over device columns, the pass's key/value columns (d_col[0..7],
+// `col_rows` rows each), the host chunk staging and the pass counters.  fresh: on an empty workspace.
+size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_rows, bool optimistic, size_t stage_bytes,
+                 bool fresh)
+{
+    PipeShape s;
+    s.rows = rows;
+    s.algo = job->spec.algo;
+    s.B = s.Bl = 1u << pick_logb(ctx, rows);
+    s.optimistic = optimistic && ctx->optimistic && rows > 0 && (uint64_t)s.B * kGroupCap * sizeof(Row32) <= kSlotBudget;
+    s.owned = s.series = rows;
+    s.out_cap = out_cap_guess(rows, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
+    PipeSizes z = pipe_sizes(s);
+    for (int i = 0; i < 8; i++) z.col[i] = col_ptr(job->cols, i) ? col_bytes(i, col_rows) : 0;
+    auto bufs = pipe_bufs(ctx, z);
+    bufs.push_back({&ctx->stage, stage_bytes});
+    bufs.push_back({&ctx->pcnt, (kMaxPasses + 1) * 4});
+    return workspace_after(ctx, bufs, fresh);
+}
+
+void add_pass(PassOut &acc, const PassOut &o)
+{
+    acc.kept += o.kept;
+    acc.owned += o.owned;
+    acc.points += o.points;
+    acc.series += o.series;
+    acc.out_rows += o.out_rows;
+    acc.spill_rows += o.spill_rows;
+    acc.launches += o.launches;
+    acc.device_ms += o.device_ms;
+    for (int i = 0; i < TAD_NPHASES; i++) acc.phase_ms[i] += o.phase_ms[i];
+}
+
+// A single-GPU job larger than `budget`, in hash-range passes (DESIGN.md section 9).  Pass (v, M) holds the rows whose
+// key hash has (h & (M - 1)) == v.  The first sweep counts the rows of every residue mod 64, which sizes every pass of
+// every M exactly; a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).
+// Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
+uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
+{
+    cudaStream_t st = ctx->stream;
+    const tad_columns &hc = job->cols;
+    const uint64_t R = hc.rows;
+    const bool host_input = hc.mem != TAD_MEM_DEVICE;
+    const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
+    auto staged = [&](int i) { return col_ptr(hc, i) && (i < 8 || ns); };
+    // host input: double-buffered chunk staging, at most 1/16 of the budget
+    size_t row_bytes = 0;
+    for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
+    uint64_t chunk = 0;
+    size_t half_bytes = 0;
+    if (host_input) {
+        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes))) & ~uint64_t(2047);
+        for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
+    }
+    const size_t stage_bytes = 2 * half_bytes;
+    // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits the budget
+    uint64_t lo = 0, hi = R;
+    while (lo < hi) {
+        const uint64_t mid = lo + (hi - lo + 1) / 2;
+        if (pass_need(ctx, job, mid, mid, false, stage_bytes, true) <= budget) lo = mid; else hi = mid - 1;
+    }
+    const uint64_t cap = lo;
+    if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
+    free_workspace(ctx);
+    for (int i = 0; i < 8; i++)
+        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, cap));
+    if (stage_bytes) ensure(ctx, ctx->stage, stage_bytes);
+    ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 4);
+    ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
+    PassCols pcols{};
+    pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
+    pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
+    pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
+    pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
+    RowFilter f{};
+    f.start_time = job->spec.start_time;
+    f.end_time = job->spec.end_time;
+    if (ns) {
+        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
+        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
+        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
+        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
+    }
+    auto set_col = [](ColPtrs &c, int i, const void *p) {
+        switch (i) {
+        case 0: c.src_ip = (const uint32_t *)p; break;
+        case 1: c.dst_ip = (const uint32_t *)p; break;
+        case 2: c.src_port = (const uint16_t *)p; break;
+        case 3: c.dst_port = (const uint16_t *)p; break;
+        case 4: c.proto = (const uint8_t *)p; break;
+        case 5: c.flow_start = (const uint32_t *)p; break;
+        case 6: c.flow_end = (const uint32_t *)p; break;
+        case 7: c.value = (const uint64_t *)p; break;
+        case 8: c.src_ns = (const uint32_t *)p; break;
+        default: c.dst_ns = (const uint32_t *)p; break;
+        }
+    };
+    uint32_t *d_cnt = static_cast<uint32_t *>(ctx->pcnt.p);          // [0, 64): rows per residue, [64]: pass cursor
+    const uint32_t *h_cnt = reinterpret_cast<const uint32_t *>(ctx->h_small);
+    // one sweep over the table: the rows of pass (v, M) -> the pass columns; returns the rows of the pass
+    auto sweep = [&](uint32_t v, uint32_t M) -> uint64_t {
+        CU(cudaMemsetAsync(d_cnt, 0, (kMaxPasses + 1) * 4, st));
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (!host_input) {
+            ColPtrs c{};
+            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(hc, i));
+            CU(launch_pass_split(st, c, R, f, M - 1, v, pcols, (uint32_t)cap, d_cnt + kMaxPasses, d_cnt));
+            acc.launches++;
+        } else {
+            CU(cudaEventRecord(ctx->start_ev, st));
+            CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
+            for (uint64_t k = 0; k * chunk < R; k++) {
+                const uint64_t lo_r = k * chunk, n = std::min<uint64_t>(chunk, R - lo_r);
+                const int h = (int)(k & 1);
+                if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
+                ColPtrs c{};
+                char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+                for (int i = 0; i < 10; i++) {
+                    if (!staged(i)) continue;
+                    const size_t w = col_bytes(i, 1);
+                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(hc, i)) + lo_r * w, n * w, cudaMemcpyHostToDevice,
+                                       ctx->copy_stream));
+                    set_col(c, i, dst);
+                    dst += exact_bytes(col_bytes(i, chunk));
+                }
+                CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
+                CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)cap, d_cnt + kMaxPasses, d_cnt));
+                acc.launches++;
+                CU(cudaEventRecord(ctx->stage_ev[h], st));
+            }
+        }
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaMemcpyAsync(ctx->h_small, d_cnt, (kMaxPasses + 1) * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        acc.phase_ms[host_input ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;      // the split runs behind the copies
+        acc.device_ms += ms;
+        return h_cnt[kMaxPasses];
+    };
+    uint32_t P = 1;
+    while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
+    const uint64_t got0 = sweep(0, P);
+    uint64_t counts[kMaxPasses];
+    for (int j = 0; j < kMaxPasses; j++) counts[j] = h_cnt[j];
+    auto pass_rows = [&](uint32_t v, uint32_t M) {
+        uint64_t n = 0;
+        for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M) n += counts[j];
+        return n;
+    };
+    auto largest = [&](uint32_t M) {
+        uint64_t m = 0;
+        for (uint32_t v = 0; v < M; v++) m = std::max(m, pass_rows(v, M));
+        return m;
+    };
+    const uint32_t P0 = P;
+    while (P < (uint32_t)kMaxPasses && largest(P) > cap) P *= 2;
+    auto too_big = [&](uint64_t rows) {
+        fail(TAD_ERR_NOMEM, "one 1/%d hash range of the table (%llu rows) needs %zu bytes of device workspace; the memory "
+             "budget is %llu bytes", kMaxPasses, (unsigned long long)rows,
+             pass_need(ctx, job, rows, rows, false, stage_bytes, true), (unsigned long long)budget);
+    };
+    if (largest(P) > cap) too_big(largest(kMaxPasses));
+    bool loaded = P == P0 && got0 <= cap;         // pass (0, P) is in the pass columns already
+    std::deque<std::pair<uint32_t, uint32_t>> todo;
+    for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
+    std::vector<PassOut> outs;
+    uint32_t passes = 0;
+    try {
+        while (!todo.empty()) {
+            if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+            const uint32_t v = todo.front().first, M = todo.front().second;
+            todo.pop_front();
+            const uint64_t rows = pass_rows(v, M);
+            if (!loaded && rows) sweep(v, M);
+            loaded = false;
+            if (rows) {
+                tad_columns pc{};
+                pc.rows = pc.capacity = rows;
+                pc.mem = TAD_MEM_DEVICE;
+                pc.src_ip = col_ptr(hc, 0) ? pcols.src_ip : nullptr; pc.dst_ip = col_ptr(hc, 1) ? pcols.dst_ip : nullptr;
+                pc.src_port = col_ptr(hc, 2) ? pcols.src_port : nullptr; pc.dst_port = col_ptr(hc, 3) ? pcols.dst_port : nullptr;
+                pc.proto = col_ptr(hc, 4) ? pcols.proto : nullptr; pc.flow_start = col_ptr(hc, 5) ? pcols.flow_start : nullptr;
+                pc.flow_end = pcols.flow_end; pc.value = pcols.value;
+                // optimistic partition where its slot buffer fits next to what the context holds; else the exact one, on
+                // a workspace cleared of earlier passes' buffers if need be (the planner sized `cap` for that)
+                const bool opt = pass_need(ctx, job, rows, cap, true, stage_bytes, false) <= budget;
+                if (!opt && pass_need(ctx, job, rows, cap, false, stage_bytes, false) > budget) {
+                    for (DevBuf *b : workspace_bufs(ctx)) {
+                        // kept: the pass columns, staging, counters and the ns_ignore list the sweeps read
+                        if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore ||
+                            (b >= ctx->d_col && b < ctx->d_col + 8))
+                            continue;
+                        if (b->p) CU(cudaFree(b->p));
+                        ctx->held -= b->cap;
+                        *b = DevBuf{};
+                    }
+                }
+                PassOut o;
+                try {
+                    run_pipeline(ctx, job, pc, false, !opt, o);
+                } catch (const PassSplit &) {
+                    CU(cudaStreamSynchronize(st));
+                    if (M >= (uint32_t)kMaxPasses) too_big(rows);
+                    todo.push_front({v + M, 2 * M});
+                    todo.push_front({v, 2 * M});
+                    continue;
+                }
+                add_pass(acc, o);
+                outs.push_back(o);
+            }
+            passes++;
+        }
+        // one contiguous result block, pass after pass
+        const OutLayout HL = out_layout(acc.out_rows ? acc.out_rows : 1);
+        acc.block = take_pinned(ctx, HL.total);
+        uint64_t at = 0;
+        for (PassOut &o : outs) {
+            const OutLayout PL = out_layout(o.out_rows ? o.out_rows : 1);
+            for (int i = 0; i < 11; i++)
+                memcpy(static_cast<char *>(acc.block.p) + HL.off[i] + at * kOutWidth[i],
+                       static_cast<const char *>(o.block.p) + PL.off[i], kOutWidth[i] * o.out_rows);
+            at += o.out_rows;
+            give_pinned(ctx, o.block);
+            o.block = PinnedBlock{};
+        }
+    } catch (...) {
+        for (PassOut &o : outs) give_pinned(ctx, o.block);
+        throw;
+    }
+    return passes;
+}
+
+void run_job(tad_ctx *ctx, tad_job *job)
+{
+    CU(cudaSetDevice(ctx->cfg.device));
+    const tad_columns &hc = job->cols;
+    const uint64_t R = hc.rows;
+    ctx->limit = 0;
+    // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
+    uint64_t budget = 0;
+    bool force_exact = false, split = false;
+    if (ctx->cfg.world_size == 1 && R > 0) {
+        const uint64_t set = ctx->budget.load();
+        budget = set;
+        if (!set) {
+            size_t free_b = 0, total_b = 0;
+            CU(cudaMemGetInfo(&free_b, &total_b));
+            budget = free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
+        }
+        PipeShape s;
+        s.rows = R;
+        s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
+        s.algo = job->spec.algo;
+        s.B = s.Bl = 1u << pick_logb(ctx, R);
+        s.optimistic = ctx->optimistic && (uint64_t)s.B * kGroupCap * sizeof(Row32) <= kSlotBudget;
+        s.owned = s.series = R;
+        s.out_cap = out_cap_guess(R, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
+        if (workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), true) > budget) {
+            s.optimistic = false;
+            force_exact = true;
+            split = workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), true) > budget;
+        }
+        if (set || force_exact) {
+            ctx->limit = budget;
+            if (split || workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), false) > budget) free_workspace(ctx);
+        }
+    }
+    ctx->peak = ctx->held;
+    PassOut acc;
+    uint32_t passes = 1;
+    if (!split) {
+        try {
+            run_pipeline(ctx, job, hc, true, force_exact, acc);
+        } catch (const PassSplit &) {          // thrown only under a budget
+            CU(cudaStreamSynchronize(ctx->stream));
+            acc = PassOut{};
+            split = true;
+        }
+    }
+    if (split) passes = run_passes(ctx, job, budget, acc);
+    publish_rows(job, acc.block, acc.out_rows);
+    ctx->limit = 0;
     {
         std::lock_guard<std::mutex> lk(job->mu);
         tad_status &s = job->st;
         s.rows_in = R;
-        s.rows_kept = kept;
-        s.rows_owned = owned;
-        s.points = points;
-        s.series = S;
-        s.result_rows = out_rows;
-        s.spill_rows = big_rows;
-        s.gpu_launches = launches;
-        s.device_ms = total;
-        for (int i = 0; i < TAD_NPHASES; i++) s.phase_ms[i] = phase_ms[i];
+        s.rows_kept = acc.kept;
+        s.rows_owned = acc.owned;
+        s.points = acc.points;
+        s.series = acc.series;
+        s.result_rows = acc.out_rows;
+        s.spill_rows = acc.spill_rows;
+        s.gpu_launches = acc.launches;
+        s.device_ms = acc.device_ms;
+        for (int i = 0; i < TAD_NPHASES; i++) s.phase_ms[i] = acc.phase_ms[i];
         s.total_ms = now_ms() - job->t_submit;
         s.completed_stages = kTotalStages;
         s.state = TAD_STATE_COMPLETED;
+        job->passes = passes;
+        job->peak_workspace = ctx->peak;
         job->cv.notify_all();     // last touch of `job` by the worker (tad_release may free it now)
     }
 }
@@ -1096,6 +1551,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     ok = ok && cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
     for (int i = 0; ok && i < kMaxChunks; i++) ok = cudaEventCreateWithFlags(&ctx->chunk_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->start_ev, cudaEventDisableTiming) == cudaSuccess;
+    for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && i <= kMaxXChunks; i++) ok = cudaEventCreateWithFlags(&ctx->x_ev[i], cudaEventDisableTiming) == cudaSuccess;
     if (const char *e = getenv("TAD_OPTIMISTIC")) ctx->optimistic = atoi(e);
     // defaults = the fastest measured configuration per world size (DESIGN.md section 6): peer pull everywhere, the exact fallback
@@ -1148,14 +1604,9 @@ void tad_shutdown(tad_ctx *ctx)
         ctx->peers_mapped = false;
     }
     nccl_comm_destroy(&ctx->nccl);
-    DevBuf *bufs[] = {&ctx->xbuf, &ctx->xcnt, &ctx->xtotal, &ctx->sortb, &ctx->hist, &ctx->offsets, &ctx->cursor, &ctx->big_list, &ctx->big_base, &ctx->cls_list, &ctx->csr_p, &ctx->stats, &ctx->part, &ctx->csr_v,
-                      &ctx->csr_t, &ctx->nsb, &ctx->npb, &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx,
-                      &ctx->dbi, &ctx->exch, &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total,
-                      &ctx->entries, &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf};
-    for (DevBuf *b : bufs)
+    if (ctx->xbuf.p) cudaFree(ctx->xbuf.p);
+    for (DevBuf *b : workspace_bufs(ctx))
         if (b->p) cudaFree(b->p);
-    for (int i = 0; i < 10; i++)
-        if (ctx->d_col[i].p) cudaFree(ctx->d_col[i].p);
     for (auto &b : ctx->pinned_pool) cudaFreeHost(b.p);
     if (ctx->h_stats) cudaFreeHost(ctx->h_stats);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
@@ -1164,6 +1615,8 @@ void tad_shutdown(tad_ctx *ctx)
     for (int i = 0; i < kMaxChunks; i++)
         if (ctx->chunk_ev[i]) cudaEventDestroy(ctx->chunk_ev[i]);
     if (ctx->start_ev) cudaEventDestroy(ctx->start_ev);
+    for (int i = 0; i < 2; i++)
+        if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
     for (int i = 0; i <= kMaxXChunks; i++)
         if (ctx->x_ev[i]) cudaEventDestroy(ctx->x_ev[i]);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
@@ -1297,6 +1750,25 @@ int tad_cancel(tad_job *job)
 {
     if (!job) return TAD_ERR_INVALID_ARG;
     job->cancel.store(1);
+    return TAD_OK;
+}
+
+int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes)
+{
+    if (!ctx) return TAD_ERR_INVALID_ARG;
+    if (ctx->cfg.world_size > 1) return TAD_ERR_UNSUPPORTED;
+    if (bytes && bytes < kBudgetFloor) return TAD_ERR_INVALID_ARG;
+    ctx->budget.store(bytes);
+    return TAD_OK;
+}
+
+int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes)
+{
+    if (!job) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->st.state != TAD_STATE_COMPLETED) return TAD_ERR_STATE;
+    if (passes) *passes = job->passes;
+    if (peak_workspace_bytes) *peak_workspace_bytes = job->peak_workspace;
     return TAD_OK;
 }
 

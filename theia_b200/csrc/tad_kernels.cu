@@ -144,6 +144,50 @@ __device__ __forceinline__ void load_row_scalar(const ColPtrs &c, const RowFilte
     r.keep = row_keep(f, c, i, fs, fe);
 }
 
+// Rows [base, base + 8) of 16-byte aligned columns, every column read with 128-bit (64-bit for the u8 column) streaming
+// loads; keep = the stage-A filters.  flow_end is read when `need_end`, value when VALUE.  The same loads as the
+// vector branch of partition_kernel below, which keeps its own inline copy: routing it through this helper changes its
+// instruction schedule.
+template <bool VALUE>
+__device__ __forceinline__ void load_rows8(const ColPtrs &c, const RowFilter &f, uint64_t base, bool need_end, RowRegs (&r)[8])
+{
+    uint4 z = make_uint4(0, 0, 0, 0);
+    uint4 sip0 = z, sip1 = z, dip0 = z, dip1 = z, fs0 = z, fs1 = z, fe0 = z, fe1 = z, sp = z, dp = z;
+    uint4 v0 = z, v1 = z, v2 = z, v3 = z;
+    uint2 pr = make_uint2(0, 0);
+    if (c.src_ip) { sip0 = ldg_stream128(c.src_ip + base); sip1 = ldg_stream128(c.src_ip + base + 4); }
+    if (c.dst_ip) { dip0 = ldg_stream128(c.dst_ip + base); dip1 = ldg_stream128(c.dst_ip + base + 4); }
+    if (c.flow_start) { fs0 = ldg_stream128(c.flow_start + base); fs1 = ldg_stream128(c.flow_start + base + 4); }
+    if (need_end) { fe0 = ldg_stream128(c.flow_end + base); fe1 = ldg_stream128(c.flow_end + base + 4); }
+    if (c.src_port) sp = ldg_stream128(c.src_port + base);
+    if (c.dst_port) dp = ldg_stream128(c.dst_port + base);
+    if (c.proto) pr = ldg_stream64(c.proto + base);
+    if (VALUE) {
+        v0 = ldg_stream128(c.value + base); v1 = ldg_stream128(c.value + base + 2);
+        v2 = ldg_stream128(c.value + base + 4); v3 = ldg_stream128(c.value + base + 6);
+    }
+    const uint32_t sipv[8] = {sip0.x, sip0.y, sip0.z, sip0.w, sip1.x, sip1.y, sip1.z, sip1.w};
+    const uint32_t dipv[8] = {dip0.x, dip0.y, dip0.z, dip0.w, dip1.x, dip1.y, dip1.z, dip1.w};
+    const uint32_t fsv[8] = {fs0.x, fs0.y, fs0.z, fs0.w, fs1.x, fs1.y, fs1.z, fs1.w};
+    const uint32_t fev[8] = {fe0.x, fe0.y, fe0.z, fe0.w, fe1.x, fe1.y, fe1.z, fe1.w};
+    const uint32_t spw[4] = {sp.x, sp.y, sp.z, sp.w};
+    const uint32_t dpw[4] = {dp.x, dp.y, dp.z, dp.w};
+    const uint32_t vlo[8] = {v0.x, v0.z, v1.x, v1.z, v2.x, v2.z, v3.x, v3.z};
+    const uint32_t vhi[8] = {v0.y, v0.w, v1.y, v1.w, v2.y, v2.w, v3.y, v3.w};
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const uint32_t sport = (spw[i >> 1] >> (16 * (i & 1))) & 0xffffu;
+        const uint32_t dport = (dpw[i >> 1] >> (16 * (i & 1))) & 0xffffu;
+        const uint32_t pw = i < 4 ? pr.x : pr.y;
+        r[i].a = pack64(dipv[i], sipv[i]);
+        r[i].b = pack64((sport << 16) | dport, fsv[i]);
+        r[i].proto = (pw >> (8 * (i & 3))) & 0xffu;
+        r[i].t = fev[i];
+        r[i].value = pack64(vlo[i], vhi[i]);
+        r[i].keep = row_keep(f, c, base + i, fsv[i], fev[i]);
+    }
+}
+
 // 8 rows per thread, every column read with 128-bit (64-bit for the u8 column) streaming loads.
 template <bool SCATTER, bool VEC>
 __global__ void __launch_bounds__(256) partition_kernel(ColPtrs c, uint64_t R, RowFilter f, int bshift,
@@ -218,6 +262,87 @@ __global__ void __launch_bounds__(256) partition_kernel(ColPtrs c, uint64_t R, R
             }
         }
     }
+}
+
+// ----------------------------------------------------------------------------------------
+// Hash-range passes (DESIGN.md section 9): a job larger than the memory budget runs once per pass over the rows whose
+// key hash has (h & pass_mask) == pass_val.  The pass bits are the LOW hash bits: the top bits pick the bucket (and,
+// across GPUs, the owner rank) and the 24 below them are the group kernel's hash tag, so neither is biased.
+// One tile = 256 threads x 8 rows.  Rows that pass the stage-A filters and belong to the pass are compacted per tile
+// (block scan, one global atomic) into the pass's eight key/value columns; the order of rows inside a pass does not
+// matter (the group kernel time-sorts every series and the max / sum reduce is integer).  Every filtered row is also
+// counted under its low kMaxPasses hash bits, so the first sweep gives the exact size of every pass of any P <= 64.
+// Rows past `cap` are counted but not written: the host then replans and sweeps again.
+// ----------------------------------------------------------------------------------------
+template <bool VEC>
+__global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t pass_mask, uint32_t pass_val,
+                                                         PassCols o, uint32_t cap, uint32_t *__restrict__ cursor,
+                                                         uint32_t *__restrict__ counts)
+{
+    __shared__ uint32_t s_cnt[kMaxPasses];
+    __shared__ uint32_t s_warp[8];
+    __shared__ uint32_t s_base;
+    for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x) s_cnt[i] = 0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t ntiles = (R + 2047) / 2048;
+    __syncthreads();
+    for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const uint64_t base = tile * 2048 + (uint64_t)threadIdx.x * 8;
+        RowRegs r[8];
+        if (VEC && base + 8 <= R) {
+            load_rows8<true>(c, f, base, true, r);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                if (base + i < R) load_row_scalar(c, f, base + i, true, r[i]);
+                else r[i].keep = false;
+            }
+        }
+        uint32_t mine = 0;
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            if (!r[i].keep) continue;
+            const uint32_t h = (uint32_t)key_hash(r[i].a, r[i].b, r[i].proto);
+            atomicAdd(&s_cnt[h & (kMaxPasses - 1)], 1u);
+            if ((h & pass_mask) == pass_val) mine |= 1u << i;
+        }
+        // exclusive block scan of the per-thread counts
+        const uint32_t n = __popc(mine);
+        uint32_t incl = n;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t t = 0;
+            for (int w = 0; w < 8; w++) { const uint32_t x = s_warp[w]; s_warp[w] = t; t += x; }
+            s_base = t ? atomicAdd(cursor, t) : 0u;
+        }
+        __syncthreads();
+        uint32_t pos = s_base + s_warp[warp] + incl - n;
+        // a warp's kept rows land in one contiguous stretch of every column
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            if (!(mine & (1u << i))) continue;
+            if (pos < cap) {
+                if (o.src_ip) o.src_ip[pos] = (uint32_t)(r[i].a >> 32);     // a = src_ip << 32 | dst_ip
+                if (o.dst_ip) o.dst_ip[pos] = (uint32_t)r[i].a;
+                if (o.src_port) o.src_port[pos] = (uint16_t)(r[i].b >> 16);
+                if (o.dst_port) o.dst_port[pos] = (uint16_t)r[i].b;
+                if (o.proto) o.proto[pos] = (uint8_t)r[i].proto;
+                if (o.flow_start) o.flow_start[pos] = (uint32_t)(r[i].b >> 32);
+                o.flow_end[pos] = r[i].t;
+                o.value[pos] = r[i].value;
+            }
+            pos++;
+        }
+        __syncthreads();           // s_warp / s_base are rewritten by the next tile
+    }
+    for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x)
+        if (s_cnt[i]) atomicAdd(&counts[i], s_cnt[i]);
 }
 
 // ----------------------------------------------------------------------------------------
@@ -1196,6 +1321,20 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
         partition_kernel<true, true><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
     else
         partition_kernel<true, false><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
+                              uint32_t pass_val, const PassCols &out, uint32_t cap, uint32_t *cursor, uint32_t *counts)
+{
+    if (R == 0) return cudaSuccess;
+    const uint64_t tiles = (R + 2047) / 2048;
+    const uint64_t lim = (uint64_t)num_sms() * 8;
+    const uint32_t grid = (uint32_t)(tiles < lim ? tiles : lim);
+    if (cols_aligned16(c))
+        pass_split_kernel<true><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
+    else
+        pass_split_kernel<false><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
     return cudaGetLastError();
 }
 

@@ -11,6 +11,18 @@ cudaError_t launch_hist(cudaStream_t st, const ColPtrs &c, uint64_t R, const Row
 cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, int logB, uint32_t *cursor,
                            Row32 *part, uint32_t slot_cap = 0, Row32 *ovf = nullptr, uint32_t ovf_cap = 0,
                            uint32_t *ovf_count = nullptr);
+// Hash-range passes: the rows of `c` that pass the stage-A filters and whose key hash has (h & pass_mask) == pass_val
+// are appended at out[*cursor ...) (rows past `cap` are dropped, *cursor still counts them); counts[kMaxPasses] gains
+// the filtered rows of every low-hash-bit residue.  Null key columns of `out` are skipped (they read as 0 anyway).
+constexpr int kMaxPasses = 64;
+struct PassCols {
+    uint32_t *src_ip, *dst_ip, *flow_start, *flow_end;
+    uint16_t *src_port, *dst_port;
+    uint8_t *proto;
+    uint64_t *value;
+};
+cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
+                              uint32_t pass_val, const PassCols &out, uint32_t cap, uint32_t *cursor, uint32_t *counts);
 cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *offsets, uint32_t *cursor, uint32_t B,
                                uint32_t cap, uint32_t *big_list, uint32_t *big_base, uint32_t *cls_list /* 3 x B or null */,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);

@@ -136,6 +136,14 @@ class Job:
             out[name] = a.copy() if copy else a
         return out
 
+    def memory(self) -> dict:
+        """Of a COMPLETED job: the hash-range passes it ran in and the largest device workspace the context held."""
+        passes, peak = C.c_uint32(), C.c_uint64()
+        rc = self.eng.lib.tad_job_memory(self.h, C.byref(passes), C.byref(peak))
+        if rc != 0:
+            raise TadError(rc, "tad_job_memory")
+        return {"passes": passes.value, "peak_workspace_bytes": peak.value}
+
     def cancel(self):
         self.eng.lib.tad_cancel(self.h)
 
@@ -146,7 +154,8 @@ class Job:
 
 
 class TadEngine:
-    def __init__(self, device: int = 0, world_size: int = 1, rank: int = 0, nccl_unique_id: bytes | None = None):
+    def __init__(self, device: int = 0, world_size: int = 1, rank: int = 0, nccl_unique_id: bytes | None = None,
+                 memory_budget: int | None = None):
         self.lib = L.load()
         cfg = L.TadConfig()
         cfg.device, cfg.world_size, cfg.rank = device, world_size, rank
@@ -160,6 +169,14 @@ class TadEngine:
         if rc != 0:
             raise TadError(rc, "tad_init(device=%d)" % device)
         self.ctx = ctx
+        if memory_budget is not None:
+            self.set_memory_budget(memory_budget)
+
+    def set_memory_budget(self, nbytes: int):
+        """Device bytes the context's workspace may hold (0 = free memory at job start); larger jobs run in passes."""
+        rc = self.lib.tad_set_memory_budget(self.ctx, int(nbytes))
+        if rc != 0:
+            raise TadError(rc, "tad_set_memory_budget(%d)" % nbytes)
 
     @staticmethod
     def get_unique_id() -> bytes:
@@ -199,15 +216,21 @@ class TadEngine:
             raise TadError(rc, msg)
         return job
 
-    def run(self, table: dict, on_job=None, **kw):
+    def run(self, table: dict, on_job=None, memory_budget: int | None = None, **kw):
         """Convenience: numpy table in, (result dict, status dict) out.  ``on_job(job)`` is called right after tad_submit
-        (the caller may poll it from another thread) and ``on_job(None)`` before the handle is released."""
+        (the caller may poll it from another thread) and ``on_job(None)`` before the handle is released.
+        ``memory_budget``: set the context's budget (tad_set_memory_budget) before the job; the status then carries
+        ``memory`` = Job.memory()."""
+        if memory_budget is not None:
+            self.set_memory_budget(memory_budget)
         cols = self.columns_from_numpy(table)
         job = self.submit(cols, **kw)
         if on_job is not None:
             on_job(job)
         try:
             st = job.wait()
+            if memory_budget is not None:
+                st["memory"] = job.memory()
             return job.result(), st
         finally:
             if on_job is not None:

@@ -58,6 +58,13 @@ def owner_rank(table: dict, world: int, total_rows: int | None = None) -> np.nda
     return (bucket >> np.uint64(logb - logw)).astype(np.int64)
 
 
+def pass_of(table: dict, passes: int) -> np.ndarray:
+    """Hash-range pass of each row when a single-GPU job runs in ``passes`` passes (a power of two up to 64): the LOW
+    key-hash bits (tad_kernels.cu: pass_split_kernel), disjoint from the bucket / owner-rank bits at the top."""
+    assert passes >= 1 and passes & (passes - 1) == 0 and passes <= 64
+    return (key_hash(table) & np.uint64(passes - 1)).astype(np.int64)
+
+
 def shard_rows(table: dict, rank: int, world: int) -> dict:
     """Range-shard by row index (how north_star hands rows to the GPUs)."""
     n = len(table["flow_end"])

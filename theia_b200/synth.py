@@ -190,6 +190,27 @@ def make_flows_torch_sharded(series_per_gpu: int, points_per_series: int, seed: 
     }
 
 
+def fill_columns_blocks(cols, n_series: int, points_per_series: int, seed: int, device, block_series: int = 1_000_000,
+                        noisy: bool = False):
+    """Fill library-owned pinned host ``Columns`` (engine.Columns, capacity >= n_series * points) block by block of
+    ``block_series`` connections: each block is generated on ``device`` by ``make_flows_torch`` (seed derived from
+    ``seed`` and the block index) and copied to the host, so a 1e9-row host table needs one block in HBM at a time,
+    not the several-times-the-table temporaries of one ``make_flows_torch`` call.  Rows are shuffled within a block."""
+    R = n_series * points_per_series
+    assert cols.c.capacity >= R
+    at = 0
+    for b, s0 in enumerate(range(0, n_series, block_series)):
+        sb = min(block_series, n_series - s0)
+        t = make_flows_torch(sb, points_per_series, seed=seed * 100003 + b, device=device, noisy=noisy)
+        n = sb * points_per_series
+        for name, dt in COLUMN_DTYPES.items():
+            cols.view(name)[at:at + n] = t[name].cpu().numpy().view(dt)
+        at += n
+        del t
+    cols.c.rows = R
+    return cols
+
+
 def torch_cols_to_numpy(cols_t: dict, mask=None) -> dict:
     """Device columns (bit patterns in torch's signed dtypes) -> the numpy table the oracle takes; ``mask`` selects rows."""
     out = {}
