@@ -3,8 +3,9 @@
 //   hist     (K1)  columns -> key pack -> 64-bit hash -> bucket histogram      reads 17-21 B/row
 //                  (exact path only: multi-GPU, or fallback of the optimistic partition)
 //   bscan    (K1b) exclusive scan of the bucket counts, capacity-class lists, oversized-bucket list
-//   scatter  (K2)  columns -> 32 B packed rows, hash-partitioned; on one GPU optimistically
-//                  into fixed-capacity bucket slots with an overflow list      reads 29, writes 32 B/row
+//   scatter  (K2)  columns -> 32 B packed rows, hash-partitioned, each row one full-sector store from a lane pair;
+//                  on one GPU optimistically into fixed-capacity bucket slots with an overflow list
+//                                                                              reads 29, writes 32 B/row
 //   group    (K3)  one CTA per bucket: TMA bulk load into shared memory, hash-group by
 //                  key, O(n) bucket-sort of each series by flowEndSeconds, reduce duplicates,
 //                  write per-series arrays + series entries                   reads 32, writes 12 B/row
@@ -39,16 +40,14 @@ __device__ __forceinline__ uint2 ldg_stream64(const void *p)
     asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
     return r;
 }
-// one 32-byte row = one full DRAM sector, written by one thread as two adjacent 128-bit stores (sm_90 has no 256-bit
-// store).  Each of the two store instructions of a warp sends 32 half-sector writes to L2: on an H100 a random 32-byte
-// scatter written this way runs at about a third of the rate of full-sector requests (lane pairs or 32-byte TMA bulk
-// stores, profiles/microbench/scatter_tma.cu), so the scatter is request bound here (NEXT.md).
-__device__ __forceinline__ void stg256(void *p, uint4 lo, uint4 hi)
+// One half of a 32-byte row (one full DRAM sector; sm_90 has no 256-bit store).  The scatter writes a row from a lane
+// pair, both halves in the same warp store instruction, so that every row reaches L2 as one full-sector request: on an
+// H100 random 32-byte rows written that way take about a third of the time of two 128-bit stores from one thread, which
+// send 32 half-sector writes per instruction (profiles/microbench/scatter_tma.cu).
+__device__ __forceinline__ void stg128(void *p, uint4 v)
 {
-    asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%2,%3,%4};\n\t"
-                 "st.global.L1::no_allocate.v4.b32 [%0+16], {%5,%6,%7,%8};"
-                 :: "l"(p), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w)
-                 : "memory");
+    asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%2,%3,%4};"
+                 :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 __device__ __forceinline__ uint32_t smem_u32(const void *p)
 {
@@ -93,41 +92,21 @@ struct OptScatter {
     uint32_t *ovf_count;
 };
 
-__device__ __forceinline__ void place_row(const RowRegs &r, uint32_t bucket, uint32_t pos, Row32 *part, const OptScatter &o)
+// Where a kept row with arrival index `pos` in `bucket` goes; null = counted but not written (the overflow list is full,
+// or absent: several GPUs pass none, and their overflow count alone sends every rank to the exact partition).
+__device__ __forceinline__ Row32 *row_dest(uint32_t bucket, uint32_t pos, Row32 *part, const OptScatter &o)
 {
-    const uint4 lo = make_uint4((uint32_t)r.a, (uint32_t)(r.a >> 32), (uint32_t)r.b, (uint32_t)(r.b >> 32));
-    const uint4 hi = make_uint4((uint32_t)r.value, (uint32_t)(r.value >> 32), r.t, r.proto);
-    if (o.cap == 0) {
-        stg256(part + pos, lo, hi);
-    } else if (pos < o.cap) {
-        stg256(part + (size_t)bucket * o.cap + pos, lo, hi);
-    } else {
-        const uint32_t k = atomicAdd(o.ovf_count, 1u);
-        if (k < o.ovf_cap) stg256(o.ovf + k, lo, hi);
-    }
+    if (o.cap == 0) return part + pos;
+    if (pos < o.cap) return part + (size_t)bucket * o.cap + pos;
+    const uint32_t k = atomicAdd(o.ovf_count, 1u);
+    return k < o.ovf_cap ? o.ovf + k : nullptr;
 }
-
 
 // The scatter already has the 64-bit key hash in registers: the 24 bits right below the bucket bits travel with
 // the row in the spare bytes of its protocol word, so the group kernel picks its hash slot without hashing again.
 __device__ __forceinline__ uint32_t hash_tag(uint64_t h, int bshift)
 {
     return (uint32_t)((h << (64 - min(bshift, 64))) >> 40);
-}
-
-template <bool SCATTER>
-__device__ __forceinline__ void emit_row(const RowRegs &r, int bshift, uint32_t *counters, Row32 *part, const OptScatter &o)
-{
-    if (!r.keep) return;
-    const uint64_t h = key_hash(r.a, r.b, r.proto);
-    const uint32_t bucket = bshift >= 64 ? 0u : (uint32_t)(h >> bshift);
-    if (SCATTER) {
-        RowRegs rt = r;
-        rt.proto |= hash_tag(h, bshift) << 8;
-        place_row(rt, bucket, atomicAdd(&counters[bucket], 1u), part, o);
-    } else {
-        atomicAdd(&counters[bucket], 1u);
-    }
 }
 
 __device__ __forceinline__ void load_row_scalar(const ColPtrs &c, const RowFilter &f, uint64_t i, bool need_tv, RowRegs &r)
@@ -145,9 +124,7 @@ __device__ __forceinline__ void load_row_scalar(const ColPtrs &c, const RowFilte
 }
 
 // Rows [base, base + 8) of 16-byte aligned columns, every column read with 128-bit (64-bit for the u8 column) streaming
-// loads; keep = the stage-A filters.  flow_end is read when `need_end`, value when VALUE.  The same loads as the
-// vector branch of partition_kernel below, which keeps its own inline copy: routing it through this helper changes its
-// instruction schedule.
+// loads; keep = the stage-A filters.  flow_end is read when `need_end`, value when VALUE.
 template <bool VALUE>
 __device__ __forceinline__ void load_rows8(const ColPtrs &c, const RowFilter &f, uint64_t base, bool need_end, RowRegs (&r)[8])
 {
@@ -188,78 +165,87 @@ __device__ __forceinline__ void load_rows8(const ColPtrs &c, const RowFilter &f,
     }
 }
 
-// 8 rows per thread, every column read with 128-bit (64-bit for the u8 column) streaming loads.
+__device__ __forceinline__ void count_row(const RowRegs &r, int bshift, uint32_t *counters)
+{
+    if (!r.keep) return;
+    const uint64_t h = key_hash(r.a, r.b, r.proto);
+    atomicAdd(&counters[bshift >= 64 ? 0u : (uint32_t)(h >> bshift)], 1u);
+}
+
+// Writes this lane's row `r` and its pair partner's row, the even lane's first: the even lane (odd = 0) writes the low
+// 16 bytes (a, b) and the odd lane the high 16 bytes (value, t, proto) of both, so one warp store instruction covers 16
+// whole sectors.  Every lane must call this (the shuffles span the warp); a null destination skips only the stores, and
+// both lanes of a pair see the same one.
+__device__ __forceinline__ void pair_store(const RowRegs &r, Row32 *dst, uint32_t odd)
+{
+    const uint4 lo = make_uint4((uint32_t)r.a, (uint32_t)(r.a >> 32), (uint32_t)r.b, (uint32_t)(r.b >> 32));
+    const uint4 hi = make_uint4((uint32_t)r.value, (uint32_t)(r.value >> 32), r.t, r.proto);
+    const uint4 give = odd ? lo : hi;                  // the half of this lane's row that its partner writes
+    uint4 got;
+    got.x = __shfl_xor_sync(0xffffffffu, give.x, 1);
+    got.y = __shfl_xor_sync(0xffffffffu, give.y, 1);
+    got.z = __shfl_xor_sync(0xffffffffu, give.z, 1);
+    got.w = __shfl_xor_sync(0xffffffffu, give.w, 1);
+    Row32 *const pd = reinterpret_cast<Row32 *>(__shfl_xor_sync(0xffffffffu, reinterpret_cast<unsigned long long>(dst), 1));
+    Row32 *const d0 = odd ? pd : dst, *const d1 = odd ? dst : pd;
+    if (d0) stg128(reinterpret_cast<char *>(d0) + 16 * odd, odd ? got : lo);
+    if (d1) stg128(reinterpret_cast<char *>(d1) + 16 * odd, odd ? hi : got);
+}
+
+// 8 rows per lane, every column read with 128-bit (64-bit for the u8 column) streaming loads when all are 16-byte
+// aligned.  The scatter writes each row from a lane pair (pair_store), so its control flow is warp-uniform: the
+// grid-stride loop steps whole warps, and a lane whose rows lie (partly) past R still runs the iteration, with the
+// missing rows marked keep = false.  Lanes diverge only inside the loads and the destination lookup.
 template <bool SCATTER, bool VEC>
 __global__ void __launch_bounds__(256) partition_kernel(ColPtrs c, uint64_t R, RowFilter f, int bshift,
                                                         uint32_t *__restrict__ counters, Row32 *__restrict__ part,
                                                         const OptScatter opt)
 {
     const uint64_t ngroups = (R + 7) / 8;
-    const bool need_end = SCATTER || f.end_time != 0;
-    for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ngroups;
-         g += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t base = g * 8;
-        if (VEC && base + 8 <= R) {
-            uint4 z = make_uint4(0, 0, 0, 0);
-            uint4 sip0 = z, sip1 = z, dip0 = z, dip1 = z, fs0 = z, fs1 = z, fe0 = z, fe1 = z, sp = z, dp = z;
-            uint4 v0 = z, v1 = z, v2 = z, v3 = z;
-            uint2 pr = make_uint2(0, 0);
-            if (c.src_ip) { sip0 = ldg_stream128(c.src_ip + base); sip1 = ldg_stream128(c.src_ip + base + 4); }
-            if (c.dst_ip) { dip0 = ldg_stream128(c.dst_ip + base); dip1 = ldg_stream128(c.dst_ip + base + 4); }
-            if (c.flow_start) { fs0 = ldg_stream128(c.flow_start + base); fs1 = ldg_stream128(c.flow_start + base + 4); }
-            if (need_end) { fe0 = ldg_stream128(c.flow_end + base); fe1 = ldg_stream128(c.flow_end + base + 4); }
-            if (c.src_port) sp = ldg_stream128(c.src_port + base);
-            if (c.dst_port) dp = ldg_stream128(c.dst_port + base);
-            if (c.proto) pr = ldg_stream64(c.proto + base);
-            if (SCATTER) {
-                v0 = ldg_stream128(c.value + base); v1 = ldg_stream128(c.value + base + 2);
-                v2 = ldg_stream128(c.value + base + 4); v3 = ldg_stream128(c.value + base + 6);
-            }
-            const uint32_t sipv[8] = {sip0.x, sip0.y, sip0.z, sip0.w, sip1.x, sip1.y, sip1.z, sip1.w};
-            const uint32_t dipv[8] = {dip0.x, dip0.y, dip0.z, dip0.w, dip1.x, dip1.y, dip1.z, dip1.w};
-            const uint32_t fsv[8] = {fs0.x, fs0.y, fs0.z, fs0.w, fs1.x, fs1.y, fs1.z, fs1.w};
-            const uint32_t fev[8] = {fe0.x, fe0.y, fe0.z, fe0.w, fe1.x, fe1.y, fe1.z, fe1.w};
-            const uint32_t spw[4] = {sp.x, sp.y, sp.z, sp.w};
-            const uint32_t dpw[4] = {dp.x, dp.y, dp.z, dp.w};
-            const uint32_t vlo[8] = {v0.x, v0.z, v1.x, v1.z, v2.x, v2.z, v3.x, v3.z};
-            const uint32_t vhi[8] = {v0.y, v0.w, v1.y, v1.w, v2.y, v2.w, v3.y, v3.w};
-            RowRegs r[8];
+    const uint32_t lane = threadIdx.x & 31u;
+    for (uint64_t wg = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); wg < ngroups;
+         wg += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t base = (wg + lane) * 8;
+        if constexpr (!SCATTER) {          // no pair store: a lane counts only the rows it has
+            const bool need_end = f.end_time != 0;
+            if (VEC && base + 8 <= R) {
+                RowRegs r[8];
+                load_rows8<false>(c, f, base, need_end, r);
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const uint32_t sport = (spw[i >> 1] >> (16 * (i & 1))) & 0xffffu;
-                const uint32_t dport = (dpw[i >> 1] >> (16 * (i & 1))) & 0xffffu;
-                const uint32_t pw = i < 4 ? pr.x : pr.y;
-                r[i].a = pack64(dipv[i], sipv[i]);
-                r[i].b = pack64((sport << 16) | dport, fsv[i]);
-                r[i].proto = (pw >> (8 * (i & 3))) & 0xffu;
-                r[i].t = fev[i];
-                r[i].value = pack64(vlo[i], vhi[i]);
-                r[i].keep = row_keep(f, c, base + i, fsv[i], fev[i]);
-            }
-            if (SCATTER) {
-                // all eight cursor atomics in flight before the first dependent store
-                uint32_t pos[8], bkt[8];
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const uint64_t h = key_hash(r[i].a, r[i].b, r[i].proto);
-                    bkt[i] = bshift >= 64 ? 0u : (uint32_t)(h >> bshift);
-                    r[i].proto |= hash_tag(h, bshift) << 8;
-                    pos[i] = r[i].keep ? atomicAdd(&counters[bkt[i]], 1u) : 0xffffffffu;
-                }
-#pragma unroll
-                for (int i = 0; i < 8; i++)
-                    if (r[i].keep) place_row(r[i], bkt[i], pos[i], part, opt);
+                for (int i = 0; i < 8; i++) count_row(r[i], bshift, counters);
             } else {
-#pragma unroll
-                for (int i = 0; i < 8; i++) emit_row<SCATTER>(r[i], bshift, counters, part, opt);
+                const uint64_t end = base + 8 < R ? base + 8 : R;
+                for (uint64_t i = base; i < end; i++) {
+                    RowRegs r;
+                    load_row_scalar(c, f, i, false, r);
+                    count_row(r, bshift, counters);
+                }
             }
         } else {
-            const uint64_t end = base + 8 < R ? base + 8 : R;
-            for (uint64_t i = base; i < end; i++) {
-                RowRegs r;
-                load_row_scalar(c, f, i, SCATTER, r);
-                emit_row<SCATTER>(r, bshift, counters, part, opt);
+            RowRegs r[8];
+            if (VEC && base + 8 <= R) {
+                load_rows8<true>(c, f, base, true, r);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+                    r[i] = RowRegs{};
+                    if (base + i < R) load_row_scalar(c, f, base + i, true, r[i]);
+                }
             }
+            // all eight cursor atomics in flight before the first dependent lookup
+            uint32_t pos[8], bkt[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const uint64_t h = key_hash(r[i].a, r[i].b, r[i].proto);
+                bkt[i] = bshift >= 64 ? 0u : (uint32_t)(h >> bshift);
+                r[i].proto |= hash_tag(h, bshift) << 8;
+                pos[i] = r[i].keep ? atomicAdd(&counters[bkt[i]], 1u) : 0u;
+            }
+            Row32 *dst[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) dst[i] = r[i].keep ? row_dest(bkt[i], pos[i], part, opt) : nullptr;
+#pragma unroll
+            for (int i = 0; i < 8; i++) pair_store(r[i], dst[i], lane & 1u);
         }
     }
 }
@@ -1291,11 +1277,20 @@ static bool cols_aligned16(const ColPtrs &c)
            ok(c.proto) && ok(c.value);
 }
 
+// One wave of the CTAs that fit on the GPU at once (fewer for small tables); the grid-stride loop covers the rest.  More
+// CTAs than fit only queue behind the first wave: the scatter of 1e8 rows (2 CTAs of 256 threads per SM) took 3.40 ms on
+// an H100 at 700 W with one wave and 3.52 ms with four.
+template <bool SCATTER, bool VEC>
 static uint32_t partition_grid(uint64_t R)
 {
+    static const int per_sm = [] {
+        int n = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, partition_kernel<SCATTER, VEC>, 256, 0);
+        return n > 0 ? n : 1;
+    }();
     const uint64_t groups = (R + 7) / 8;
     const uint64_t want = (groups + 255) / 256;
-    const uint64_t cap = (uint64_t)num_sms() * 8;           // 8 resident CTAs of 256 threads per SM
+    const uint64_t cap = (uint64_t)num_sms() * per_sm;
     return (uint32_t)(want < cap ? (want ? want : 1) : cap);
 }
 
@@ -1305,9 +1300,9 @@ cudaError_t launch_hist(cudaStream_t st, const ColPtrs &c, uint64_t R, const Row
     const int bshift = 64 - logB;
     const OptScatter none{0, 0, nullptr, nullptr};
     if (cols_aligned16(c))
-        partition_kernel<false, true><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, hist, nullptr, none);
+        partition_kernel<false, true><<<partition_grid<false, true>(R), 256, 0, st>>>(c, R, f, bshift, hist, nullptr, none);
     else
-        partition_kernel<false, false><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, hist, nullptr, none);
+        partition_kernel<false, false><<<partition_grid<false, false>(R), 256, 0, st>>>(c, R, f, bshift, hist, nullptr, none);
     return cudaGetLastError();
 }
 
@@ -1318,9 +1313,9 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
     const int bshift = 64 - logB;
     const OptScatter opt{slot_cap, ovf_cap, ovf, ovf_count};
     if (cols_aligned16(c))
-        partition_kernel<true, true><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
+        partition_kernel<true, true><<<partition_grid<true, true>(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
     else
-        partition_kernel<true, false><<<partition_grid(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
+        partition_kernel<true, false><<<partition_grid<true, false>(R), 256, 0, st>>>(c, R, f, bshift, cursor, part, opt);
     return cudaGetLastError();
 }
 
