@@ -62,6 +62,7 @@ type AnomalyRow struct {
 type gpuJob struct {
 	job  *C.tad_job
 	cols C.tad_columns
+	fed  chan struct{} // StartStream: closed once the feeding goroutine no longer calls into the job (nil for Start)
 }
 
 type gpuJobRunner struct {
@@ -183,6 +184,149 @@ func (r *gpuJobRunner) Start(spec JobSpec, in *FlowColumns) error {
 	return nil
 }
 
+// BlockReader runs the job's SELECT once and calls emit for every block clickhouse-go hands over (the columns of one
+// block, same layout as FlowColumns).  StartStream calls it once per round: it must return the same rows every time
+// (a closed time window), in any order and block sizes.
+type BlockReader func(emit func(*FlowColumns) error) error
+
+// StartStream is Start for a table that never has to be in host memory at once (DESIGN.md section 10, single GPU): the
+// rows go to the engine block by block as the SELECT delivers them, through two library-owned pinned blocks filled
+// alternately, so block k+1 is decoded while block k is copied.  rowsHint is the SELECT count() (0 = unknown).  When the
+// engine needs another hash-range pass it asks for the rows again and the SELECT is re-run.  Blocks larger than
+// blockRows are cut.  Blocking: it returns when the input is complete.  The job is registered when it is submitted, so
+// State and Cancel reach it while its rows are still being read (Cancel makes the feeding call return); Results works
+// once the input is complete.
+func (r *gpuJobRunner) StartStream(spec JobSpec, rowsHint uint64, blockRows int, read BlockReader) error {
+	if blockRows <= 0 {
+		return fmt.Errorf("blockRows must be positive")
+	}
+	var bufs [2]C.tad_columns
+	freeBufs := func() {
+		C.tad_free_columns(r.ctx, &bufs[0])
+		C.tad_free_columns(r.ctx, &bufs[1])
+	}
+	for i := range bufs {
+		if rc := C.tad_alloc_columns(r.ctx, C.uint64_t(blockRows), C.TAD_MEM_HOST, &bufs[i]); rc != C.TAD_OK {
+			freeBufs()
+			return fmt.Errorf("tad_alloc_columns: %s", C.GoString(C.tad_strerror(rc)))
+		}
+		if len(spec.NSIgnore) > 0 {
+			if rc := C.tad_alloc_ns_columns(r.ctx, &bufs[i]); rc != C.TAD_OK {
+				freeBufs()
+				return fmt.Errorf("tad_alloc_ns_columns: %s", C.GoString(C.tad_strerror(rc)))
+			}
+		}
+	}
+	js := C.tad_job_spec{algo: algoCode(spec.Algo), start_time: C.uint32_t(spec.StartTime), end_time: C.uint32_t(spec.EndTime)}
+	if spec.SumReducer {
+		js.reducer = C.TAD_REDUCE_SUM
+	}
+	if len(spec.NSIgnore) > 0 {
+		js.n_ns_ignore = C.uint32_t(len(spec.NSIgnore))
+		js.ns_ignore = (*C.uint32_t)(unsafe.Pointer(&spec.NSIgnore[0]))
+	}
+	cid := C.CString(spec.ID)
+	C.strncpy(&js.id[0], cid, 39)
+	C.free(unsafe.Pointer(cid))
+	var job *C.tad_job
+	if rc := C.tad_submit_stream(r.ctx, &js, C.uint64_t(rowsHint), &job); rc != C.TAD_OK {
+		var st C.tad_status
+		C.tad_poll(job, &st)
+		C.tad_release(job)
+		freeBufs()
+		return illeagelArguementError{fmt.Errorf("%s", C.GoString(&st.err_msg[0]))}
+	}
+	gj := &gpuJob{job: job, fed: make(chan struct{})}
+	r.jobs.Store(spec.ID, gj)
+	// engine errors: a bad block or a source that changed between rounds is terminal (controller.go:505-514)
+	engineErr := func(call string, rc C.int) error {
+		var st C.tad_status
+		C.tad_poll(job, &st)
+		err := fmt.Errorf("%s: %s: %s", call, C.GoString(C.tad_strerror(rc)), C.GoString(&st.err_msg[0]))
+		if rc == C.TAD_ERR_INVALID_ARG {
+			return illeagelArguementError{err}
+		}
+		return err
+	}
+	failed := func(err error) error {
+		freeBufs() // push and end have returned: the engine no longer reads the blocks
+		if _, mine := r.jobs.LoadAndDelete(spec.ID); mine {
+			close(gj.fed)
+			C.tad_release(job) // cancels a job whose input has not ended
+		} else {
+			close(gj.fed) // Cancel took the job and releases it
+		}
+		return err
+	}
+	k := 0
+	push := func(in *FlowColumns, lo, n int) error {
+		if spec.StartTime != 0 && in.FlowStart == nil {
+			return illeagelArguementError{fmt.Errorf("invalid request: start_time needs the flow_start column")}
+		}
+		b := &bufs[k&1] // free again: the push of block k-1 has returned
+		k++
+		part := FlowColumns{}
+		cut32 := func(s []uint32) []uint32 { if s == nil { return nil }; return s[lo : lo+n] }
+		cut16 := func(s []uint16) []uint16 { if s == nil { return nil }; return s[lo : lo+n] }
+		part.SrcIP, part.DstIP, part.FlowStart, part.FlowEnd = cut32(in.SrcIP), cut32(in.DstIP), cut32(in.FlowStart), cut32(in.FlowEnd)
+		part.SrcPort, part.DstPort = cut16(in.SrcPort), cut16(in.DstPort)
+		if in.Proto != nil {
+			part.Proto = in.Proto[lo : lo+n]
+		}
+		part.Throughput = in.Throughput[lo : lo+n]
+		for _, err := range []error{
+			fillColumn((**uint32)(unsafe.Pointer(&b.src_ip)), part.SrcIP, n, "sourceIP", false),
+			fillColumn((**uint32)(unsafe.Pointer(&b.dst_ip)), part.DstIP, n, "destinationIP", false),
+			fillColumn((**uint16)(unsafe.Pointer(&b.src_port)), part.SrcPort, n, "sourceTransportPort", false),
+			fillColumn((**uint16)(unsafe.Pointer(&b.dst_port)), part.DstPort, n, "destinationTransportPort", false),
+			fillColumn((**uint8)(unsafe.Pointer(&b.proto)), part.Proto, n, "protocolIdentifier", false),
+			fillColumn((**uint32)(unsafe.Pointer(&b.flow_start)), part.FlowStart, n, "flowStartSeconds", false),
+			fillColumn((**uint32)(unsafe.Pointer(&b.flow_end)), part.FlowEnd, n, "flowEndSeconds", true),
+			fillColumn((**uint64)(unsafe.Pointer(&b.value)), part.Throughput, n, "throughput", true),
+		} {
+			if err != nil {
+				return err
+			}
+		}
+		if len(spec.NSIgnore) > 0 {
+			if err := fillColumn((**uint32)(unsafe.Pointer(&b.src_ns)), cut32(in.SrcNS), n, "sourcePodNamespace", true); err != nil {
+				return err
+			}
+			if err := fillColumn((**uint32)(unsafe.Pointer(&b.dst_ns)), cut32(in.DstNS), n, "destinationPodNamespace", true); err != nil {
+				return err
+			}
+		}
+		b.rows = C.uint64_t(n)
+		if rc := C.tad_stream_push(job, b); rc != C.TAD_OK {
+			return engineErr("tad_stream_push", rc)
+		}
+		return nil
+	}
+	for again := C.int32_t(1); again != 0; {
+		err := read(func(in *FlowColumns) error {
+			for lo := 0; lo < len(in.FlowEnd); lo += blockRows {
+				n := len(in.FlowEnd) - lo
+				if n > blockRows {
+					n = blockRows
+				}
+				if err := push(in, lo, n); err != nil {
+					return err
+				}
+			}
+			return nil
+		})
+		if err != nil {
+			return failed(err)
+		}
+		if rc := C.tad_stream_end(job, &again); rc != C.TAD_OK {
+			return failed(engineErr("tad_stream_end", rc))
+		}
+	}
+	freeBufs() // the input is complete: the engine no longer reads the blocks
+	close(gj.fed)
+	return nil
+}
+
 // State replaces GetSparkApplication + the Spark-UI stage scraping (controller.go:426-497).
 func (r *gpuJobRunner) State(id string) (state string, completed, total int, errMsg string) {
 	v, ok := r.jobs.Load(id)
@@ -232,6 +376,9 @@ func (r *gpuJobRunner) Cancel(id string) {
 	if v, ok := r.jobs.LoadAndDelete(id); ok {
 		j := v.(*gpuJob)
 		C.tad_cancel(j.job)
+		if j.fed != nil {
+			<-j.fed // a pending push or end returns TAD_ERR_CANCELLED; release only after the feeder has returned
+		}
 		C.tad_release(j.job)
 		C.tad_free_columns(r.ctx, &j.cols)
 	}

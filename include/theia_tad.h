@@ -214,6 +214,48 @@ int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
  * (TAD_ERR_STATE otherwise). */
 int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes);
 
+/* ---- Streamed input (single GPU) ---------------------------------------------------------------------------------
+ * The job's rows arrive as column blocks while it runs (a ClickHouse SELECT hands them over block by block), so the
+ * table never has to be in host memory at once and may hold more than 2^32 rows.  A ROUND is one complete delivery of
+ * the job's rows, in any order and any block sizes: tad_stream_push each block, then tad_stream_end.  When the job
+ * needs more than one hash-range pass (see tad_set_memory_budget), tad_stream_end sets *again = 1 and the caller
+ * delivers the same rows again; *again = 0 means the input is complete, and from then on tad_wait / tad_poll /
+ * tad_result / tad_job_memory behave as for any job.  There are as many rounds as a host-input job of the same rows
+ * makes sweeps over its table.
+ *
+ * Submit: rows_hint is the caller's estimate of one round's rows (its SELECT count()), 0 = unknown.  It only chooses the
+ * pass count and sizes the pass columns before the first round: a wrong hint may cost one round more, never a different
+ * result.  TAD_ERR_UNSUPPORTED when world_size > 1.  A context still runs one job at a time: a streamed job holds the
+ * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.
+ *
+ * Blocks: mem is TAD_MEM_HOST (any host memory; pinned buffers from tad_alloc_columns copy at the full PCIe rate) or
+ * TAD_MEM_DEVICE (read in place); fewer than 2^32 rows; flow_end and value are required; every block carries the same
+ * non-NULL columns as the job's first block (src_ns / dst_ns included).  A block that breaks one of these fails the job
+ * with TAD_ERR_INVALID_ARG.  A pushed block must stay valid and unchanged until the next tad_stream_push or
+ * tad_stream_end call on the job returns: the caller may fill block k+1 while block k is being copied.
+ *
+ * Each pass, not the job, must stay below 2^32-2 rows.  Every round must deliver, after the time-window and ns_ignore
+ * filters, as many rows of each low-hash-bit residue as the first round did; otherwise (the source changed between
+ * reads, e.g. an open-ended window over a table being appended to) the job fails with TAD_ERR_INVALID_ARG.  This is a
+ * check on counts, not on content.
+ *
+ * Status: rows_in and rows_kept count one round; phase times and device_ms sum over rounds and passes (the h2d phase of
+ * a streamed round includes the time the engine waited for its blocks); state is RUNNING while the job waits for input.
+ *
+ * Errors: push / end on a job not submitted with tad_submit_stream, or after its input is complete: TAD_ERR_STATE.
+ * After tad_cancel: TAD_ERR_CANCELLED, and the job is FAILED.  Once the job has failed, its error code.  tad_release of
+ * a job whose input has not ended cancels it.  The context stays usable for the next job in every case.
+ * tad_shutdown cancels a streamed job that waits for input; as for every job, release it before tad_shutdown.
+ *
+ * Threads: while the feeding thread is inside tad_stream_push or tad_stream_end, other threads may call tad_poll and
+ * tad_cancel on the job, but not tad_release: release it after the feeding thread has returned. */
+int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, tad_job **out);
+/* Hands one block of the current round to the job; returns once the engine has finished reading the previous block. */
+int tad_stream_push(tad_job *job, const tad_columns *block);
+/* Closes the round; returns once the engine has finished with the round's rows, with *again = 1 when the same rows
+ * must be pushed again for another pass, 0 when the input is complete.  again may be NULL. */
+int tad_stream_end(tad_job *job, int32_t *again);
+
 const char *tad_strerror(int err);
 int tad_abi_version(void);
 

@@ -20,7 +20,8 @@ TAD_REDUCE_MAX, TAD_REDUCE_SUM = 0, 1
 EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_alloc_columns",
            "tad_free_columns", "tad_submit", "tad_poll", "tad_wait", "tad_result", "tad_cancel",
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
-           "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory")
+           "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
+           "tad_stream_push", "tad_stream_end")
 
 
 class TadConfig(C.Structure):
@@ -78,6 +79,9 @@ def load():
     L.tad_free_columns.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_alloc_ns_columns.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_submit.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.POINTER(TadColumns), C.POINTER(C.c_void_p)]
+    L.tad_submit_stream.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(C.c_void_p)]
+    L.tad_stream_push.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
+    L.tad_stream_end.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
     L.tad_poll.argtypes = [C.c_void_p, C.POINTER(TadStatus)]
     L.tad_wait.argtypes = [C.c_void_p, C.c_int64, C.POINTER(TadStatus)]
     L.tad_result.argtypes = [C.c_void_p, C.POINTER(TadRows)]

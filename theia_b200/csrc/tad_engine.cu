@@ -147,6 +147,22 @@ struct tad_job {
     double t_submit = 0;
     uint32_t passes = 0;             // hash-range passes the job ran in (tad_job_memory)
     uint64_t peak_workspace = 0;     // largest device workspace the context held while the job ran
+    // streamed input (tad_submit_stream): the caller hands the worker one column block at a time, under `mu`.  `cols`
+    // then holds the first block: its non-NULL columns are the set every block must carry.
+    bool stream = false;
+    uint64_t rows_hint = 0;          // the caller's estimate of one round's rows (0 = unknown)
+    uint64_t round_rows = 0;         // rows of the first round (tad_status.rows_in)
+    struct {
+        tad_columns blk{};           // handed over, not yet taken by the worker
+        bool has_blk = false;
+        bool end_req = false;        // the caller closed the round; cleared when the worker finishes with it
+        bool round_done = false;     // the worker finished with the round; `again` is valid
+        bool again = false;
+        bool input_done = false;     // tad_stream_end returned again = 0
+        uint64_t pushed = 0, taken = 0, released = 0;   // blocks handed over / taken / no longer read by the engine
+        int err = 0;                 // a bad block: the worker fails the job with this code and message
+        char msg[200] = {0};
+    } in;
 };
 
 struct tad_ctx {
@@ -164,6 +180,7 @@ struct tad_ctx {
     std::deque<tad_job *> queue;
     std::thread worker;
     bool stop = false;
+    std::atomic<int> stopping{0};                   // tad_shutdown: a streamed job waiting for input is cancelled
     int debug_logb = -1;
     int debug_target = 0;      // TAD_GROUP_TARGET: mean rows per bucket (tuning)
     int num_sms = 132;
@@ -198,6 +215,7 @@ struct tad_ctx {
     size_t limit = 0;                               // while a job runs under a budget: ensure() never grows `held` past it
     DevBuf stage, pcnt;                             // pass mode: double-buffered host chunk staging; pass counters + cursor
     cudaEvent_t stage_ev[2]{};                      // staging half free again (the split kernel of its last chunk is done)
+    cudaEvent_t blk_ev[2]{};                        // streamed input: the engine has finished reading a caller's block
 };
 
 namespace {
@@ -1142,7 +1160,7 @@ size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_r
     for (int i = 0; i < 8; i++) z.col[i] = col_ptr(job->cols, i) ? col_bytes(i, col_rows) : 0;
     auto bufs = pipe_bufs(ctx, z);
     bufs.push_back({&ctx->stage, stage_bytes});
-    bufs.push_back({&ctx->pcnt, (kMaxPasses + 1) * 4});
+    bufs.push_back({&ctx->pcnt, (kMaxPasses + 1) * 8});
     return workspace_after(ctx, bufs, fresh);
 }
 
@@ -1159,16 +1177,84 @@ void add_pass(PassOut &acc, const PassOut &o)
     for (int i = 0; i < TAD_NPHASES; i++) acc.phase_ms[i] += o.phase_ms[i];
 }
 
-// A single-GPU job larger than `budget`, in hash-range passes (DESIGN.md section 9).  Pass (v, M) holds the rows whose
-// key hash has (h & (M - 1)) == v.  The first sweep counts the rows of every residue mod 64, which sizes every pass of
-// every M exactly; a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).
+// ---- streamed input: the worker's side of the hand-over (the caller's side is tad_stream_push / tad_stream_end) ----------
+// The next block of the current round; false once the caller has closed the round.
+bool next_block(tad_job *job, tad_columns &b)
+{
+    std::unique_lock<std::mutex> lk(job->mu);
+    for (;;) {
+        if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+        if (job->ctx->stopping.load()) fail(TAD_ERR_CANCELLED, "context is shutting down");
+        if (job->in.err) fail(job->in.err, "%s", job->in.msg);
+        if (job->in.has_blk) {
+            b = job->in.blk;
+            job->in.has_blk = false;
+            job->in.taken++;
+            job->cv.notify_all();
+            return true;
+        }
+        if (job->in.end_req) return false;
+        job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    }
+}
+
+// The engine no longer reads the first `n` blocks of the job: the pushes waiting for them may return.
+void release_blocks(tad_job *job, uint64_t n)
+{
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->in.released = n;
+    job->cv.notify_all();
+}
+
+// The worker has finished with the round: tad_stream_end returns `again`.
+void close_round(tad_job *job, bool again)
+{
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->in.released = job->in.taken;
+    job->in.end_req = false;
+    job->in.again = again;
+    job->in.round_done = true;
+    job->cv.notify_all();
+}
+
+// Device buffer grown to `bytes` with its first `keep` bytes carried over (ensure() frees before it allocates).
+void grow_keep(tad_ctx *ctx, DevBuf &b, size_t bytes, size_t keep, cudaStream_t st)
+{
+    if (bytes <= b.cap) return;
+    size_t want = alloc_bytes(bytes);
+    if (ctx->limit && ctx->held + want > ctx->limit) want = exact_bytes(bytes);
+    if (ctx->limit && ctx->held + want > ctx->limit)
+        fail(TAD_ERR_INTERNAL, "workspace would grow to %zu bytes, past the memory budget of %zu bytes", ctx->held + want, ctx->limit);
+    void *p = nullptr;
+    CU(cudaMalloc(&p, want));
+    ctx->held += want;
+    ctx->peak = std::max(ctx->peak, ctx->held);
+    if (keep) CU(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    if (b.p) CU(cudaFree(b.p));
+    ctx->held -= b.cap;
+    b.p = p;
+    b.cap = want;
+}
+
+constexpr uint64_t kMaxPassRows = (1ull << 32) - 2;   // the pipeline's offsets are u32: the row cap of one pass
+
+// A single-GPU job in hash-range passes (DESIGN.md sections 9 and 10).  Pass (v, M) holds the rows whose key hash has
+// (h & (M - 1)) == v.  The first sweep counts the rows of every residue mod 64, which sizes every pass of every M exactly;
+// a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).  A sweep reads
+// the job's columns (device-resident: one split launch; host: double-buffered chunks behind the copies) or, for a
+// streamed job, the blocks of one round.  Every later sweep must count what the first one counted.
 // Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
 uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
 {
     cudaStream_t st = ctx->stream;
+    const bool stream = job->stream;
+    // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
+    tad_columns pend{};
+    bool have_pend = stream && next_block(job, pend);
     const tad_columns &hc = job->cols;
-    const uint64_t R = hc.rows;
-    const bool host_input = hc.mem != TAD_MEM_DEVICE;
+    const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
+    const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
     const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
     auto staged = [&](int i) { return col_ptr(hc, i) && (i < 8 || ns); };
     // host input: double-buffered chunk staging, at most 1/16 of the budget
@@ -1176,30 +1262,38 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
     for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
     uint64_t chunk = 0;
     size_t half_bytes = 0;
-    if (host_input) {
+    if (host_input && row_bytes) {
         chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes))) & ~uint64_t(2047);
         for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
     }
     const size_t stage_bytes = 2 * half_bytes;
     // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits the budget
-    uint64_t lo = 0, hi = R;
+    uint64_t lo = 0, hi = stream ? kMaxPassRows : std::min(R, kMaxPassRows);
     while (lo < hi) {
         const uint64_t mid = lo + (hi - lo + 1) / 2;
         if (pass_need(ctx, job, mid, mid, false, stage_bytes, true) <= budget) lo = mid; else hi = mid - 1;
     }
     const uint64_t cap = lo;
     if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
+    uint32_t P = 1;
+    while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
+    // pass columns: a table's passes get `cap` rows; a streamed round's from the hint (or 1M rows without one), grown
+    // geometrically up to `cap` while the first round arrives
+    uint64_t colcap = stream ? std::min(cap, R ? R / P + R / P / 8 + 2048 : uint64_t(1) << 20) : cap;
     free_workspace(ctx);
     for (int i = 0; i < 8; i++)
-        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, cap));
-    if (stage_bytes) ensure(ctx, ctx->stage, stage_bytes);
-    ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 4);
+        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
+    if (stage_bytes && !stream) ensure(ctx, ctx->stage, stage_bytes);
+    ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 8);
     ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
     PassCols pcols{};
-    pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
-    pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
-    pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
-    pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
+    auto set_pcols = [&]() {
+        pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
+        pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
+        pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
+        pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
+    };
+    set_pcols();
     RowFilter f{};
     f.start_time = job->spec.start_time;
     f.end_time = job->spec.end_time;
@@ -1223,54 +1317,120 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
         default: c.dst_ns = (const uint32_t *)p; break;
         }
     };
-    uint32_t *d_cnt = static_cast<uint32_t *>(ctx->pcnt.p);          // [0, 64): rows per residue, [64]: pass cursor
-    const uint32_t *h_cnt = reinterpret_cast<const uint32_t *>(ctx->h_small);
-    // one sweep over the table: the rows of pass (v, M) -> the pass columns; returns the rows of the pass
-    auto sweep = [&](uint32_t v, uint32_t M) -> uint64_t {
-        CU(cudaMemsetAsync(d_cnt, 0, (kMaxPasses + 1) * 4, st));
-        CU(cudaEventRecord(ctx->ev[0], st));
-        if (!host_input) {
+    unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);   // [0, 64): rows per residue, [64]: pass cursor
+    const unsigned long long *h_cnt = ctx->h_small;
+    uint64_t nchunk = 0;             // host chunks staged in the current sweep
+    bool any_host = false;
+    // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M)
+    auto feed = [&](const tad_columns &b, uint32_t v, uint32_t M) {
+        const uint64_t n_all = b.rows;
+        if (n_all == 0) return;
+        if (b.mem == TAD_MEM_DEVICE) {
             ColPtrs c{};
-            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(hc, i));
-            CU(launch_pass_split(st, c, R, f, M - 1, v, pcols, (uint32_t)cap, d_cnt + kMaxPasses, d_cnt));
+            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(b, i));
+            CU(launch_pass_split(st, c, n_all, f, M - 1, v, pcols, (uint32_t)colcap, d_cnt + kMaxPasses, d_cnt));
             acc.launches++;
-        } else {
+            return;
+        }
+        any_host = true;
+        ensure(ctx, ctx->stage, stage_bytes);
+        for (uint64_t lo_r = 0; lo_r < n_all; lo_r += chunk, nchunk++) {
+            const uint64_t n = std::min<uint64_t>(chunk, n_all - lo_r);
+            const int h = (int)(nchunk & 1);
+            if (nchunk >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
+            ColPtrs c{};
+            char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+            for (int i = 0; i < 10; i++) {
+                if (!staged(i)) continue;
+                const size_t w = col_bytes(i, 1);
+                CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(b, i)) + lo_r * w, n * w, cudaMemcpyHostToDevice,
+                                   ctx->copy_stream));
+                set_col(c, i, dst);
+                dst += exact_bytes(col_bytes(i, chunk));
+            }
+            CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+            CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
+            CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)colcap, d_cnt + kMaxPasses, d_cnt));
+            acc.launches++;
+            CU(cudaEventRecord(ctx->stage_ev[h], st));
+        }
+    };
+    // first streamed round: make room in the pass columns for every row the next `n` input rows can add (`ub` bounds the
+    // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
+    uint64_t ub = 0;
+    auto room = [&](uint64_t n) {
+        if (colcap >= cap || ub + n <= colcap) { ub += n; return; }
+        CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        const uint64_t have = std::min<uint64_t>(ctx->h_small[128], colcap);
+        if (have + n > colcap) {
+            const uint64_t want = std::min(cap, std::max(2 * colcap, have + n));
+            for (int i = 0; i < 8; i++)
+                if (col_ptr(hc, i)) grow_keep(ctx, ctx->d_col[i], col_bytes(i, want), col_bytes(i, have), st);
+            colcap = want;
+            set_pcols();
+        }
+        ub = have + n;
+    };
+    uint64_t counts[kMaxPasses];
+    uint32_t sweeps = 0;
+    bool open = false;               // a streamed round is swept and its caller waits in tad_stream_end
+    // one sweep over the input: the rows of pass (v, M) -> the pass columns; returns the rows of the pass
+    auto sweep = [&](uint32_t v, uint32_t M) -> uint64_t {
+        CU(cudaMemsetAsync(d_cnt, 0, (kMaxPasses + 1) * 8, st));
+        CU(cudaEventRecord(ctx->ev[0], st));
+        nchunk = 0;
+        any_host = false;
+        if (host_input) {
             CU(cudaEventRecord(ctx->start_ev, st));
             CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
-            for (uint64_t k = 0; k * chunk < R; k++) {
-                const uint64_t lo_r = k * chunk, n = std::min<uint64_t>(chunk, R - lo_r);
-                const int h = (int)(k & 1);
-                if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
-                ColPtrs c{};
-                char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-                for (int i = 0; i < 10; i++) {
-                    if (!staged(i)) continue;
-                    const size_t w = col_bytes(i, 1);
-                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(hc, i)) + lo_r * w, n * w, cudaMemcpyHostToDevice,
-                                       ctx->copy_stream));
-                    set_col(c, i, dst);
-                    dst += exact_bytes(col_bytes(i, chunk));
+        }
+        if (!stream) {
+            feed(hc, v, M);
+        } else {
+            // the round's blocks; block k is released (its push returns) once block k+1 is enqueued and k's copy is done
+            uint64_t rows = 0, k = 0;
+            ub = 0;
+            tad_columns b{};
+            bool got = have_pend ? (b = pend, true) : next_block(job, b);
+            have_pend = false;
+            while (got) {
+                if (sweeps == 0) room(b.rows);
+                feed(b, v, M);
+                CU(cudaEventRecord(ctx->blk_ev[k & 1], b.mem == TAD_MEM_DEVICE ? st : ctx->copy_stream));
+                if (k > 0) {
+                    CU(cudaEventSynchronize(ctx->blk_ev[(k - 1) & 1]));
+                    uint64_t taken;
+                    {
+                        std::lock_guard<std::mutex> lk(job->mu);
+                        taken = job->in.taken;
+                    }
+                    release_blocks(job, taken - 1);
                 }
-                CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
-                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-                CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)cap, d_cnt + kMaxPasses, d_cnt));
-                acc.launches++;
-                CU(cudaEventRecord(ctx->stage_ev[h], st));
+                rows += b.rows;
+                k++;
+                got = next_block(job, b);
             }
+            if (sweeps == 0) job->round_rows = rows;
+            open = true;
         }
         CU(cudaEventRecord(ctx->ev[1], st));
-        CU(cudaMemcpyAsync(ctx->h_small, d_cnt, (kMaxPasses + 1) * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ctx->h_small, d_cnt, (kMaxPasses + 1) * 8, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         float ms = 0;
         CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        acc.phase_ms[host_input ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;      // the split runs behind the copies
+        acc.phase_ms[any_host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;      // the split runs behind the copies
         acc.device_ms += ms;
+        if (sweeps > 0)
+            for (int j = 0; j < kMaxPasses; j++)
+                if (h_cnt[j] != counts[j])
+                    fail(TAD_ERR_INVALID_ARG, "sweep %u of the input delivered %llu filtered rows of hash residue %d, the first "
+                         "delivered %llu: the source changed between reads", sweeps + 1, (unsigned long long)h_cnt[j], j,
+                         (unsigned long long)counts[j]);
+        sweeps++;
         return h_cnt[kMaxPasses];
     };
-    uint32_t P = 1;
-    while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
     const uint64_t got0 = sweep(0, P);
-    uint64_t counts[kMaxPasses];
     for (int j = 0; j < kMaxPasses; j++) counts[j] = h_cnt[j];
     auto pass_rows = [&](uint32_t v, uint32_t M) {
         uint64_t n = 0;
@@ -1283,6 +1443,13 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
         return m;
     };
     const uint32_t P0 = P;
+    if (stream) {
+        // an overestimated hint must not cost a round per surplus pass: plan from the rows the first round delivered,
+        // as an exact hint would have, at the price of that one round (loaded is then false unless P comes back to P0)
+        uint32_t Pr = 1;
+        while (Pr < (uint32_t)kMaxPasses && job->round_rows / Pr > cap / 8 * 7) Pr *= 2;
+        P = std::min(P, Pr);
+    }
     while (P < (uint32_t)kMaxPasses && largest(P) > cap) P *= 2;
     auto too_big = [&](uint64_t rows) {
         fail(TAD_ERR_NOMEM, "one 1/%d hash range of the table (%llu rows) needs %zu bytes of device workspace; the memory "
@@ -1290,9 +1457,18 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
              pass_need(ctx, job, rows, rows, false, stage_bytes, true), (unsigned long long)budget);
     };
     if (largest(P) > cap) too_big(largest(kMaxPasses));
-    bool loaded = P == P0 && got0 <= cap;         // pass (0, P) is in the pass columns already
+    bool loaded = P == P0 && got0 <= colcap;     // pass (0, P) is in the pass columns already
     std::deque<std::pair<uint32_t, uint32_t>> todo;
     for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
+    // a streamed round stays open until the engine knows whether another sweep (round) follows
+    auto finish_round = [&]() {
+        if (!open) return;
+        bool more = false;
+        for (const auto &e : todo) more = more || pass_rows(e.first, e.second) > 0;
+        close_round(job, more);
+        open = false;
+    };
+    if (!loaded) finish_round();
     std::vector<PassOut> outs;
     uint32_t passes = 0;
     try {
@@ -1301,8 +1477,17 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
             const uint32_t v = todo.front().first, M = todo.front().second;
             todo.pop_front();
             const uint64_t rows = pass_rows(v, M);
-            if (!loaded && rows) sweep(v, M);
+            if (!loaded && rows) {
+                if (stream && rows > colcap) {          // later rounds: the counts size the pass columns exactly
+                    for (int i = 0; i < 8; i++)
+                        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, rows));
+                    colcap = rows;
+                    set_pcols();
+                }
+                sweep(v, M);
+            }
             loaded = false;
+            bool split_pass = false;
             if (rows) {
                 tad_columns pc{};
                 pc.rows = pc.capacity = rows;
@@ -1333,12 +1518,15 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
                     if (M >= (uint32_t)kMaxPasses) too_big(rows);
                     todo.push_front({v + M, 2 * M});
                     todo.push_front({v, 2 * M});
-                    continue;
+                    split_pass = true;
                 }
-                add_pass(acc, o);
-                outs.push_back(o);
+                if (!split_pass) {
+                    add_pass(acc, o);
+                    outs.push_back(o);
+                }
             }
-            passes++;
+            if (!split_pass) passes++;
+            finish_round();
         }
         // one contiguous result block, pass after pass
         const OutLayout HL = out_layout(acc.out_rows ? acc.out_rows : 1);
@@ -1363,20 +1551,28 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
 void run_job(tad_ctx *ctx, tad_job *job)
 {
     CU(cudaSetDevice(ctx->cfg.device));
-    const tad_columns &hc = job->cols;
-    const uint64_t R = hc.rows;
+    const tad_columns &hc = job->cols;     // a streamed job's first push writes it: not read here for streams
+    const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
-    if (ctx->cfg.world_size == 1 && R > 0) {
+    auto context_budget = [&]() -> uint64_t {
+        if (const uint64_t set = ctx->budget.load()) return set;
+        size_t free_b = 0, total_b = 0;
+        CU(cudaMemGetInfo(&free_b, &total_b));
+        return free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
+    };
+    if (job->stream) {
+        // streamed input always runs through the pass columns (one pass when it fits), under the budget
+        set_progress(job, TAD_STATE_RUNNING, 0);
+        budget = context_budget();
+        ctx->limit = budget;
+        free_workspace(ctx);
+        split = true;
+    } else if (ctx->cfg.world_size == 1 && R > 0) {
         const uint64_t set = ctx->budget.load();
-        budget = set;
-        if (!set) {
-            size_t free_b = 0, total_b = 0;
-            CU(cudaMemGetInfo(&free_b, &total_b));
-            budget = free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
-        }
+        budget = context_budget();
         PipeShape s;
         s.rows = R;
         s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
@@ -1413,7 +1609,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
     {
         std::lock_guard<std::mutex> lk(job->mu);
         tad_status &s = job->st;
-        s.rows_in = R;
+        s.rows_in = job->stream ? job->round_rows : R;
         s.rows_kept = acc.kept;
         s.rows_owned = acc.owned;
         s.points = acc.points;
@@ -1504,6 +1700,103 @@ int validate(const tad_job_spec *spec, const tad_columns *cols, char *msg, size_
     return TAD_OK;
 }
 
+// Validates and enqueues a job (tad_submit, tad_submit_stream).  An invalid job is returned FAILED, like the controller
+// (controller.go:505-514): illegal arguments are terminal, never retried.
+int submit_job(tad_ctx *ctx, tad_job *job, const tad_job_spec *spec, const tad_columns *cols, tad_job **out)
+{
+    job->ctx = ctx;
+    job->spec = *spec;
+    job->spec.id[sizeof(job->spec.id) - 1] = 0;
+    job->cols = *cols;
+    job->t_submit = now_ms();
+    job->st.total_stages = kTotalStages;
+    *out = job;
+    char msg[200];
+    int rc = validate(spec, cols, msg, sizeof(msg));
+    if (rc == TAD_OK && job->stream && ctx->cfg.world_size > 1) {
+        snprintf(msg, sizeof(msg), "streamed input runs on a single GPU only");
+        rc = TAD_ERR_UNSUPPORTED;
+    }
+    if (rc != TAD_OK) {
+        job->st.state = TAD_STATE_FAILED;
+        job->st.error = rc;
+        snprintf(job->st.err_msg, sizeof(job->st.err_msg), "error in creating AnomalyDetector: %s", msg);
+        return rc;
+    }
+    if (spec->n_ns_ignore) job->ns_ignore.assign(spec->ns_ignore, spec->ns_ignore + spec->n_ns_ignore);
+    job->spec.ns_ignore = nullptr;
+    job->st.state = TAD_STATE_SCHEDULED;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->stop) {
+            job->st.state = TAD_STATE_FAILED;
+            job->st.error = TAD_ERR_STATE;
+            snprintf(job->st.err_msg, sizeof(job->st.err_msg), "context is shutting down");
+            return TAD_ERR_STATE;
+        }
+        ctx->queue.push_back(job);
+    }
+    ctx->cv.notify_one();
+    return TAD_OK;
+}
+
+bool finished(const tad_job *job) { return job->st.state == TAD_STATE_COMPLETED || job->st.state == TAD_STATE_FAILED; }
+
+// Fails a streamed job from the caller's side (a bad block) and waits until the worker has reported it FAILED.
+int stream_abort(tad_job *job, std::unique_lock<std::mutex> &lk, int code, const char *msg)
+{
+    if (!job->in.err) {
+        job->in.err = code;
+        snprintf(job->in.msg, sizeof(job->in.msg), "%s", msg);
+    }
+    job->cv.notify_all();
+    while (!finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    return code;
+}
+
+// Whether a push or end call is legal now: TAD_ERR_STATE on a job without streamed input or after its input is complete;
+// TAD_ERR_CANCELLED (once the job is FAILED) after tad_cancel; the job's error once it has failed.
+int stream_gate(tad_job *job, std::unique_lock<std::mutex> &lk)
+{
+    if (!job->stream || job->in.input_done) return TAD_ERR_STATE;
+    if (job->cancel.load()) {
+        while (!finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+        return TAD_ERR_CANCELLED;
+    }
+    if (finished(job)) return job->st.error ? job->st.error : TAD_ERR_STATE;
+    return TAD_OK;
+}
+
+// A streamed block: host or device memory, fewer than 2^32 rows, flow_end and value, and the first block's column set.
+int check_block(const tad_job *job, const tad_columns *b, char *msg, size_t n)
+{
+    if (b->mem != TAD_MEM_HOST && b->mem != TAD_MEM_DEVICE) {
+        snprintf(msg, n, "invalid request: bad column memory kind");
+        return TAD_ERR_INVALID_ARG;
+    }
+    if (b->rows >= (1ull << 32)) {
+        snprintf(msg, n, "invalid request: a streamed block has fewer than 2^32 rows");
+        return TAD_ERR_INVALID_ARG;
+    }
+    if (!b->flow_end || !b->value) {
+        snprintf(msg, n, "invalid request: flow_end and value columns are required");
+        return TAD_ERR_INVALID_ARG;
+    }
+    if (job->in.pushed == 0) {
+        if (job->spec.start_time && !b->flow_start) {
+            snprintf(msg, n, "invalid request: start_time needs the flow_start column");
+            return TAD_ERR_INVALID_ARG;
+        }
+        return TAD_OK;
+    }
+    for (int i = 0; i < 10; i++)
+        if ((col_ptr(job->cols, i) != nullptr) != (col_ptr(*b, i) != nullptr)) {
+            snprintf(msg, n, "invalid request: a streamed block carries another set of columns than the job's first block");
+            return TAD_ERR_INVALID_ARG;
+        }
+    return TAD_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1552,6 +1845,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     for (int i = 0; ok && i < kMaxChunks; i++) ok = cudaEventCreateWithFlags(&ctx->chunk_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->start_ev, cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
+    for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->blk_ev[i], cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && i <= kMaxXChunks; i++) ok = cudaEventCreateWithFlags(&ctx->x_ev[i], cudaEventDisableTiming) == cudaSuccess;
     if (const char *e = getenv("TAD_OPTIMISTIC")) ctx->optimistic = atoi(e);
     // defaults = the fastest measured configuration per world size (DESIGN.md section 6): peer pull everywhere, the exact fallback
@@ -1592,6 +1886,7 @@ void tad_shutdown(tad_ctx *ctx)
         std::lock_guard<std::mutex> lk(ctx->mu);
         ctx->stop = true;
     }
+    ctx->stopping.store(1);
     ctx->cv.notify_all();
     if (ctx->worker.joinable()) ctx->worker.join();
     cudaSetDevice(ctx->cfg.device);
@@ -1617,6 +1912,8 @@ void tad_shutdown(tad_ctx *ctx)
     if (ctx->start_ev) cudaEventDestroy(ctx->start_ev);
     for (int i = 0; i < 2; i++)
         if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
+    for (int i = 0; i < 2; i++)
+        if (ctx->blk_ev[i]) cudaEventDestroy(ctx->blk_ev[i]);
     for (int i = 0; i <= kMaxXChunks; i++)
         if (ctx->x_ev[i]) cudaEventDestroy(ctx->x_ev[i]);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
@@ -1680,37 +1977,56 @@ int tad_free_columns(tad_ctx *ctx, tad_columns *cols)
 int tad_submit(tad_ctx *ctx, const tad_job_spec *spec, const tad_columns *cols, tad_job **out)
 {
     if (!ctx || !spec || !cols || !out) return TAD_ERR_INVALID_ARG;
+    return submit_job(ctx, new tad_job(), spec, cols, out);
+}
+
+int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, tad_job **out)
+{
+    if (!ctx || !spec || !out) return TAD_ERR_INVALID_ARG;
     tad_job *job = new tad_job();
-    job->ctx = ctx;
-    job->spec = *spec;
-    job->spec.id[sizeof(job->spec.id) - 1] = 0;
-    job->cols = *cols;
-    job->t_submit = now_ms();
-    job->st.total_stages = kTotalStages;
-    *out = job;
+    job->stream = true;
+    job->rows_hint = rows_hint;
+    tad_columns none{};
+    return submit_job(ctx, job, spec, &none, out);
+}
+
+int tad_stream_push(tad_job *job, const tad_columns *block)
+{
+    if (!job || !block) return TAD_ERR_INVALID_ARG;
+    std::unique_lock<std::mutex> lk(job->mu);
+    int rc = stream_gate(job, lk);
+    if (rc != TAD_OK) return rc;
     char msg[200];
-    int rc = validate(spec, cols, msg, sizeof(msg));
-    if (rc != TAD_OK) {
-        // like the controller (controller.go:505-514): illegal arguments are terminal FAILED, never retried
-        job->st.state = TAD_STATE_FAILED;
-        job->st.error = rc;
-        snprintf(job->st.err_msg, sizeof(job->st.err_msg), "error in creating AnomalyDetector: %s", msg);
-        return rc;
-    }
-    if (spec->n_ns_ignore) job->ns_ignore.assign(spec->ns_ignore, spec->ns_ignore + spec->n_ns_ignore);
-    job->spec.ns_ignore = nullptr;
-    job->st.state = TAD_STATE_SCHEDULED;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->stop) {
-            job->st.state = TAD_STATE_FAILED;
-            job->st.error = TAD_ERR_STATE;
-            snprintf(job->st.err_msg, sizeof(job->st.err_msg), "context is shutting down");
-            return TAD_ERR_STATE;
-        }
-        ctx->queue.push_back(job);
-    }
-    ctx->cv.notify_one();
+    rc = check_block(job, block, msg, sizeof(msg));
+    if (rc != TAD_OK) return stream_abort(job, lk, rc, msg);
+    if (job->in.pushed == 0) job->cols = *block;       // the column set of the job
+    // one block of look-ahead: hand this one over once the worker has taken the previous one, then return once the
+    // engine no longer reads the previous one
+    while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (finished(job)) return job->st.error;
+    job->in.blk = *block;
+    job->in.has_blk = true;
+    const uint64_t k = job->in.pushed++;
+    job->cv.notify_all();
+    while (job->in.released < k && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    return finished(job) ? job->st.error : TAD_OK;
+}
+
+int tad_stream_end(tad_job *job, int32_t *again)
+{
+    if (!job) return TAD_ERR_INVALID_ARG;
+    std::unique_lock<std::mutex> lk(job->mu);
+    int rc = stream_gate(job, lk);
+    if (rc != TAD_OK) return rc;
+    while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (finished(job)) return job->st.error;
+    job->in.end_req = true;
+    job->cv.notify_all();
+    while (!job->in.round_done && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (!job->in.round_done) return job->st.error;
+    job->in.round_done = false;
+    job->in.input_done = !job->in.again;
+    if (again) *again = job->in.again ? 1 : 0;
     return TAD_OK;
 }
 
@@ -1749,7 +2065,9 @@ int tad_result(tad_job *job, tad_rows *rows)
 int tad_cancel(tad_job *job)
 {
     if (!job) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
     job->cancel.store(1);
+    job->cv.notify_all();        // a worker waiting for streamed input
     return TAD_OK;
 }
 
@@ -1780,6 +2098,7 @@ int tad_release(tad_job *job)
         const int s = job->st.state;
         if (s == TAD_STATE_SCHEDULED || s == TAD_STATE_RUNNING) {
             job->cancel.store(1);
+            job->cv.notify_all();
             while (!(job->st.state == TAD_STATE_COMPLETED || job->st.state == TAD_STATE_FAILED))
                 job->cv.wait_for(lk, std::chrono::milliseconds(1));
         }

@@ -262,12 +262,12 @@ __global__ void __launch_bounds__(256) partition_kernel(ColPtrs c, uint64_t R, R
 // ----------------------------------------------------------------------------------------
 template <bool VEC>
 __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t pass_mask, uint32_t pass_val,
-                                                         PassCols o, uint32_t cap, uint32_t *__restrict__ cursor,
-                                                         uint32_t *__restrict__ counts)
+                                                         PassCols o, uint32_t cap, unsigned long long *__restrict__ cursor,
+                                                         unsigned long long *__restrict__ counts)
 {
     __shared__ uint32_t s_cnt[kMaxPasses];
     __shared__ uint32_t s_warp[8];
-    __shared__ uint32_t s_base;
+    __shared__ unsigned long long s_base;     // 64-bit: one sweep of a streamed round may exceed 2^32 rows
     for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x) s_cnt[i] = 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint64_t ntiles = (R + 2047) / 2048;
@@ -305,10 +305,10 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
         if (threadIdx.x == 0) {
             uint32_t t = 0;
             for (int w = 0; w < 8; w++) { const uint32_t x = s_warp[w]; s_warp[w] = t; t += x; }
-            s_base = t ? atomicAdd(cursor, t) : 0u;
+            s_base = t ? atomicAdd(cursor, (unsigned long long)t) : 0ull;
         }
         __syncthreads();
-        uint32_t pos = s_base + s_warp[warp] + incl - n;
+        uint64_t pos = s_base + s_warp[warp] + incl - n;
         // a warp's kept rows land in one contiguous stretch of every column
 #pragma unroll
         for (int i = 0; i < 8; i++) {
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
         __syncthreads();           // s_warp / s_base are rewritten by the next tile
     }
     for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x)
-        if (s_cnt[i]) atomicAdd(&counts[i], s_cnt[i]);
+        if (s_cnt[i]) atomicAdd(&counts[i], (unsigned long long)s_cnt[i]);
 }
 
 // ----------------------------------------------------------------------------------------
@@ -1320,7 +1320,8 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 }
 
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
-                              uint32_t pass_val, const PassCols &out, uint32_t cap, uint32_t *cursor, uint32_t *counts)
+                              uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
+                              unsigned long long *counts)
 {
     if (R == 0) return cudaSuccess;
     const uint64_t tiles = (R + 2047) / 2048;

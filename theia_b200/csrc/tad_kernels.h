@@ -14,6 +14,7 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 // Hash-range passes: the rows of `c` that pass the stage-A filters and whose key hash has (h & pass_mask) == pass_val
 // are appended at out[*cursor ...) (rows past `cap` are dropped, *cursor still counts them); counts[kMaxPasses] gains
 // the filtered rows of every low-hash-bit residue.  Null key columns of `out` are skipped (they read as 0 anyway).
+// The cursor and counts are 64-bit: one sweep over a streamed round may hold more than 2^32 rows.
 constexpr int kMaxPasses = 64;
 struct PassCols {
     uint32_t *src_ip, *dst_ip, *flow_start, *flow_end;
@@ -22,7 +23,8 @@ struct PassCols {
     uint64_t *value;
 };
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
-                              uint32_t pass_val, const PassCols &out, uint32_t cap, uint32_t *cursor, uint32_t *counts);
+                              uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
+                              unsigned long long *counts);
 cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *offsets, uint32_t *cursor, uint32_t B,
                                uint32_t cap, uint32_t *big_list, uint32_t *big_base, uint32_t *cls_list /* 3 x B or null */,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);

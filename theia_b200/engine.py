@@ -6,6 +6,10 @@
     st = job.wait()                               # or poll(): state / completed_stages / total_stages
     rows = job.result()                           # dict of numpy arrays (tadetector columns)
     job.release(); cols.free(); eng.close()
+
+Streamed input (the table arrives block by block and is never held whole):
+
+    res, st = eng.run_stream(lambda: read_blocks(), algo="EWMA", rows_hint=n)   # re-reads while another pass needs it
 """
 from __future__ import annotations
 
@@ -153,6 +157,55 @@ class Job:
             self.h = None
 
 
+def _block_columns(block):
+    """(TadColumns, objects to keep alive) of one streamed block: a numpy dict (any host memory; a missing or None
+    column is NULL), Columns or DeviceColumns."""
+    if isinstance(block, (Columns, DeviceColumns)):
+        return block.c, block
+    c = L.TadColumns()
+    n = len(block["flow_end"])
+    c.rows = c.capacity = n
+    c.mem = L.TAD_MEM_HOST
+    keep = []
+    for name, dt in _COLS + _NS_COLS:
+        a = block.get(name)
+        if a is None:
+            continue
+        a = np.ascontiguousarray(a, dtype=dt)
+        if len(a) != n:
+            raise ValueError("column %s has %d values, flow_end has %d" % (name, len(a), n))
+        keep.append(a)
+        setattr(c, name, a.ctypes.data if n else C.addressof(_EMPTY))
+    return c, keep
+
+
+_EMPTY = C.c_uint64(0)     # a non-NULL address for the columns of an empty numpy block
+
+
+class StreamJob(Job):
+    """A job fed with column blocks (tad_submit_stream): push() every block of a round, then end(); while end() returns
+    True the engine needs the same rows once more."""
+
+    def __init__(self, eng, handle, keep):
+        super().__init__(eng, handle, keep)
+        self._last = None
+
+    def push(self, block):
+        c, keep = _block_columns(block)
+        rc = self.eng.lib.tad_stream_push(self.h, C.byref(c))
+        if rc != 0:
+            raise TadError(rc, self.poll()["err_msg"])
+        self._last = (c, keep)        # the engine may read this block until the next push or end returns
+
+    def end(self) -> bool:
+        again = C.c_int32()
+        rc = self.eng.lib.tad_stream_end(self.h, C.byref(again))
+        if rc != 0:
+            raise TadError(rc, self.poll()["err_msg"])
+        self._last = None
+        return bool(again.value)
+
+
 class TadEngine:
     def __init__(self, device: int = 0, world_size: int = 1, rank: int = 0, nccl_unique_id: bytes | None = None,
                  memory_budget: int | None = None):
@@ -192,8 +245,8 @@ class TadEngine:
     def columns_from_numpy(self, table: dict) -> Columns:
         return self.alloc_columns(max(1, len(table["flow_end"]))).fill(table)
 
-    def submit(self, cols, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
-               tad_id: str = "", emit_all: bool = False, ns_ignore=(), check: bool = True, global_rows: int = 0) -> Job:
+    @staticmethod
+    def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep):
         spec = L.TadJobSpec()
         spec.algo = L.ALGOS[algo] if isinstance(algo, str) else int(algo)
         spec.reducer = reducer
@@ -201,20 +254,37 @@ class TadEngine:
         spec.flags = L.TAD_FLAG_EMIT_ALL if emit_all else 0
         spec.id = tad_id.encode()[:39]
         spec.global_rows = int(global_rows)
-        keep = [cols]
         if len(ns_ignore):
             arr = np.asarray(ns_ignore, dtype=np.uint32)
             spec.n_ns_ignore = len(arr)
             spec.ns_ignore = arr.ctypes.data
             keep.append(arr)
-        h = C.c_void_p()
-        rc = self.lib.tad_submit(self.ctx, C.byref(spec), C.byref(cols.c), C.byref(h))
-        job = Job(self, h, keep)
+        return spec
+
+    def _checked(self, job, rc, check):
         if rc != 0 and check:
-            msg = job.poll()["err_msg"] if h else ""
+            msg = job.poll()["err_msg"] if job.h else ""
             job.release()
             raise TadError(rc, msg)
         return job
+
+    def submit(self, cols, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
+               tad_id: str = "", emit_all: bool = False, ns_ignore=(), check: bool = True, global_rows: int = 0) -> Job:
+        keep = [cols]
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep)
+        h = C.c_void_p()
+        rc = self.lib.tad_submit(self.ctx, C.byref(spec), C.byref(cols.c), C.byref(h))
+        return self._checked(Job(self, h, keep), rc, check)
+
+    def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
+                      ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
+                      check: bool = True) -> StreamJob:
+        """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown."""
+        keep = []
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep)
+        h = C.c_void_p()
+        rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
+        return self._checked(StreamJob(self, h, keep), rc, check)
 
     def run(self, table: dict, on_job=None, memory_budget: int | None = None, **kw):
         """Convenience: numpy table in, (result dict, status dict) out.  ``on_job(job)`` is called right after tad_submit
@@ -237,6 +307,27 @@ class TadEngine:
                 on_job(None)
             job.release()
             cols.free()
+
+    def run_stream(self, blocks_factory, memory_budget: int | None = None, **kw):
+        """Convenience: ``blocks_factory()`` yields one round's blocks (numpy dicts, Columns or DeviceColumns); it is
+        called once per round while the engine asks for the rows again.  Returns (result dict, status dict) like run();
+        the status also carries ``rounds`` and ``memory`` = Job.memory()."""
+        if memory_budget is not None:
+            self.set_memory_budget(memory_budget)
+        job = self.submit_stream(**kw)
+        try:
+            rounds, again = 0, True
+            while again:
+                for block in blocks_factory():
+                    job.push(block)
+                again = job.end()
+                rounds += 1
+            st = job.wait()
+            st["rounds"] = rounds
+            st["memory"] = job.memory()
+            return job.result(), st
+        finally:
+            job.release()
 
     def close(self):
         if self.ctx:
