@@ -89,6 +89,17 @@ func (r *gpuJobRunner) SetMemoryBudget(bytes uint64) error {
 	return nil
 }
 
+// SetHostBudget lets the runner's context pin up to `bytes` of host memory for its host row store (0 = none, the
+// default; nonzero values below 64 MiB are refused).  A streamed job that needs several hash-range passes then keeps its
+// rows there and StartStream runs its SELECT once; if the store would not hold the rows, the job asks for the rows again
+// as without a store.  It takes effect for jobs that start after the call.
+func (r *gpuJobRunner) SetHostBudget(bytes uint64) error {
+	if rc := C.tad_set_host_budget(r.ctx, C.uint64_t(bytes)); rc != C.TAD_OK {
+		return fmt.Errorf("tad_set_host_budget: %s", C.GoString(C.tad_strerror(rc)))
+	}
+	return nil
+}
+
 func algoCode(a string) C.int32_t {
 	switch a {
 	case "ARIMA":

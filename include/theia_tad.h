@@ -214,14 +214,30 @@ int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
  * (TAD_ERR_STATE otherwise). */
 int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes);
 
+/* Pinned host memory this context may hold for its host row store (bytes).  0 (default) = no store.  With a store, a
+ * streamed job (tad_submit_stream) that needs more than one hash-range pass keeps its first round's filtered rows in
+ * pinned host pages (32 bytes per row) and loads every pass from them, so the caller delivers its rows once whatever the
+ * pass count.  If the store would outgrow the budget, or the memory cannot be pinned, the job drops the store and goes on
+ * as without one: that round only counts its rows and further rounds are asked for.  tad_submit jobs and streamed jobs
+ * that run in one pass never use it.  The context keeps its pages for the next job up to the budget; pages above a
+ * lowered budget are freed before the next job, and tad_shutdown frees them all.  Applies to jobs that start after the
+ * call: a job reads the budget once, when the context starts running it (for a streamed job on an idle context that is
+ * at submit, before its first block).  Single GPU only (TAD_ERR_UNSUPPORTED when world_size > 1); TAD_ERR_INVALID_ARG
+ * for a nonzero value below 64 MiB. */
+int tad_set_host_budget(tad_ctx *ctx, uint64_t bytes);
+/* For a COMPLETED job: the rows that went through the host row store (0 if it was not used) and the most store bytes the
+ * context held while the job ran (TAD_ERR_STATE otherwise). */
+int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host_bytes);
+
 /* ---- Streamed input (single GPU) ---------------------------------------------------------------------------------
  * The job's rows arrive as column blocks while it runs (a ClickHouse SELECT hands them over block by block), so the
  * table never has to be in host memory at once and may hold more than 2^32 rows.  A ROUND is one complete delivery of
  * the job's rows, in any order and any block sizes: tad_stream_push each block, then tad_stream_end.  When the job
  * needs more than one hash-range pass (see tad_set_memory_budget), tad_stream_end sets *again = 1 and the caller
  * delivers the same rows again; *again = 0 means the input is complete, and from then on tad_wait / tad_poll /
- * tad_result / tad_job_memory behave as for any job.  There are as many rounds as a host-input job of the same rows
- * makes sweeps over its table.
+ * tad_result / tad_job_memory behave as for any job.  Without a host row store there are as many rounds as a host-input
+ * job of the same rows makes sweeps over its table.  With one (tad_set_host_budget), a round that went to the store
+ * ends with *again = 0: the passes are loaded from the store.
  *
  * Submit: rows_hint is the caller's estimate of one round's rows (its SELECT count()), 0 = unknown.  It only chooses the
  * pass count and sizes the pass columns before the first round: a wrong hint may cost one round more, never a different
@@ -234,10 +250,10 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * with TAD_ERR_INVALID_ARG.  A pushed block must stay valid and unchanged until the next tad_stream_push or
  * tad_stream_end call on the job returns: the caller may fill block k+1 while block k is being copied.
  *
- * Each pass, not the job, must stay below 2^32-2 rows.  Every round must deliver, after the time-window and ns_ignore
- * filters, as many rows of each low-hash-bit residue as the first round did; otherwise (the source changed between
- * reads, e.g. an open-ended window over a table being appended to) the job fails with TAD_ERR_INVALID_ARG.  This is a
- * check on counts, not on content.
+ * Each pass, not the job, must stay below 2^32-2 rows.  When there is more than one round, every round must deliver,
+ * after the time-window and ns_ignore filters, as many rows of each low-hash-bit residue as the first round did;
+ * otherwise (the source changed between reads, e.g. an open-ended window over a table being appended to) the job fails
+ * with TAD_ERR_INVALID_ARG.  This is a check on counts, not on content.
  *
  * Status: rows_in and rows_kept count one round; phase times and device_ms sum over rounds and passes (the h2d phase of
  * a streamed round includes the time the engine waited for its blocks); state is RUNNING while the job waits for input.

@@ -21,7 +21,7 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_free_columns", "tad_submit", "tad_poll", "tad_wait", "tad_result", "tad_cancel",
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
-           "tad_stream_push", "tad_stream_end")
+           "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory")
 
 
 class TadConfig(C.Structure):
@@ -90,6 +90,8 @@ def load():
     L.tad_get_unique_id.argtypes = [C.c_void_p, C.c_size_t]
     L.tad_set_memory_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+    L.tad_set_host_budget.argtypes = [C.c_void_p, C.c_uint64]
+    L.tad_job_host_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.tad_ch_string_index.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
     L.tad_ch_parse_ipv4.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
     L.tad_ch_format_ipv4.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]

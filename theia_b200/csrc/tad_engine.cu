@@ -152,6 +152,8 @@ struct tad_job {
     bool stream = false;
     uint64_t rows_hint = 0;          // the caller's estimate of one round's rows (0 = unknown)
     uint64_t round_rows = 0;         // rows of the first round (tad_status.rows_in)
+    uint64_t stored_rows = 0;        // rows the host row store held for the passes (tad_job_host_memory)
+    uint64_t peak_host = 0;          // most store bytes the context held while the job ran
     struct {
         tad_columns blk{};           // handed over, not yet taken by the worker
         bool has_blk = false;
@@ -216,6 +218,17 @@ struct tad_ctx {
     DevBuf stage, pcnt;                             // pass mode: double-buffered host chunk staging; pass counters + cursor
     cudaEvent_t stage_ev[2]{};                      // staging half free again (the split kernel of its last chunk is done)
     cudaEvent_t blk_ev[2]{};                        // streamed input: the engine has finished reading a caller's block
+    // host row store (DESIGN.md section 11): pinned pages that keep a streamed round's rows for the job's passes
+    std::atomic<uint64_t> host_budget{0};           // tad_set_host_budget; 0 = no store
+    std::vector<PinnedBlock> store_slabs;           // pinned slabs of up to 64 MiB, carved into pages
+    std::vector<char *> store_free;                 // pages holding no job's rows
+    size_t store_page = 0;                          // page bytes
+    size_t store_held = 0, store_peak = 0;          // pinned bytes of the slabs; their most since the running job started
+    DevBuf ostage;                                  // out-stage: two halves of packed rows, count matrix, scan scratch, chunk counts
+    cudaStream_t d2h_stream = nullptr;              // copies from the out-stage to the store
+    cudaEvent_t ost_ev[2]{};                        // out-stage half free again (its copies to the store are done)
+    cudaEvent_t cnt_ev[2]{};                        // a chunk's residue counts have reached h_chunk
+    uint32_t *h_chunk = nullptr;                    // pinned, 2 x 64: rows per residue of the last two chunks
 };
 
 namespace {
@@ -293,9 +306,16 @@ std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
                                &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx, &ctx->dbi, &ctx->exch,
                                &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total, &ctx->entries,
                                &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
-                               &ctx->stage, &ctx->pcnt};
+                               &ctx->stage, &ctx->pcnt, &ctx->ostage};
     for (int i = 0; i < 10; i++) v.push_back(&ctx->d_col[i]);
     return v;
+}
+
+void free_buf(tad_ctx *ctx, DevBuf &b)
+{
+    if (b.p) CU(cudaFree(b.p));
+    ctx->held -= b.cap;
+    b = DevBuf{};
 }
 
 void free_workspace(tad_ctx *ctx)
@@ -334,6 +354,80 @@ void give_pinned(tad_ctx *ctx, PinnedBlock b)
     std::lock_guard<std::mutex> lk(ctx->pool_mu);
     ctx->pinned_pool.push_back(b);
 }
+
+// ---- host row store pages (worker thread only) ------------------------------------------------------------------------
+constexpr uint64_t kStoreSlab = 64ull << 20;
+
+// budget / 1024 rounded to a MiB, within [1, 64] MiB: the 64 partly filled pages (one per residue) waste at most 1/16
+size_t store_page_bytes(uint64_t budget)
+{
+    const uint64_t mib = (budget / 1024 + (1u << 19)) >> 20;
+    return (size_t)std::min<uint64_t>(64, std::max<uint64_t>(1, mib)) << 20;
+}
+
+// Before a job: the slabs above the budget are freed (all of them when the page size changes) and every page is free.
+// Returns the budget it read: the job's host budget, so that the page size and the budget the job fills stay one pair
+// whatever tad_set_host_budget does while the job runs.
+uint64_t store_trim(tad_ctx *ctx)
+{
+    const uint64_t budget = ctx->host_budget.load();
+    const size_t page = budget ? store_page_bytes(budget) : 0;
+    while (!ctx->store_slabs.empty() && (page != ctx->store_page || ctx->store_held > budget)) {
+        cudaFreeHost(ctx->store_slabs.back().p);
+        ctx->store_held -= ctx->store_slabs.back().cap;
+        ctx->store_slabs.pop_back();
+    }
+    ctx->store_page = page;
+    ctx->store_free.clear();
+    for (const PinnedBlock &s : ctx->store_slabs)
+        for (size_t o = 0; o + page <= s.cap; o += page) ctx->store_free.push_back(static_cast<char *>(s.p) + o);
+    ctx->store_peak = ctx->store_held;
+    return budget;
+}
+
+// A free page; a new slab when none is left.  Null when the slab would pass the budget or cannot be pinned.
+char *store_take_page(tad_ctx *ctx, uint64_t budget)
+{
+    if (ctx->store_free.empty()) {
+        const size_t page = ctx->store_page;
+        const uint64_t room = budget > ctx->store_held ? budget - ctx->store_held : 0;
+        const size_t n = (size_t)std::min<uint64_t>(kStoreSlab / page, room / page);
+        if (n == 0) return nullptr;
+        PinnedBlock s;
+        s.cap = n * page;
+        NumaScope numa(ctx->numa);
+        if (cudaHostAlloc(&s.p, s.cap, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            return nullptr;
+        }
+        ctx->store_slabs.push_back(s);
+        ctx->store_held += s.cap;
+        ctx->store_peak = std::max(ctx->store_peak, ctx->store_held);
+        for (size_t o = 0; o < s.cap; o += page) ctx->store_free.push_back(static_cast<char *>(s.p) + o);
+    }
+    char *p = ctx->store_free.back();
+    ctx->store_free.pop_back();
+    return p;
+}
+
+// One job's rows in the store: per low-hash-bit residue, a list of pages filled in order.  The pages go back to the
+// context when the job ends, however it ends.
+struct RowStore {
+    tad_ctx *ctx;
+    std::vector<char *> pages[kMaxPasses];
+    uint64_t rows[kMaxPasses] = {};
+    explicit RowStore(tad_ctx *c) : ctx(c) {}
+    void clear()
+    {
+        cudaStreamSynchronize(ctx->d2h_stream);       // no copy into a page is still in flight
+        for (int j = 0; j < kMaxPasses; j++) {
+            ctx->store_free.insert(ctx->store_free.end(), pages[j].begin(), pages[j].end());
+            pages[j].clear();
+            rows[j] = 0;
+        }
+    }
+    ~RowStore() { clear(); }
+};
 
 void set_progress(tad_job *job, int state, int completed)
 {
@@ -1164,6 +1258,17 @@ size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_r
     return workspace_after(ctx, bufs, fresh);
 }
 
+// Workspace of a round packed into the host row store, on an empty workspace: the pass columns (`col_rows` rows each),
+// the host chunk staging, the pass counters and the out-stage.  The out-stage is freed before the first pass runs, so
+// the planner sizes the passes without it and uses the store only where this fits the budget at the planned cap.
+size_t store_round_need(tad_ctx *ctx, const tad_job *job, uint64_t col_rows, size_t stage_bytes, size_t ostage_bytes)
+{
+    std::vector<std::pair<DevBuf *, size_t>> bufs = {{&ctx->stage, stage_bytes}, {&ctx->pcnt, (kMaxPasses + 1) * 8},
+                                                     {&ctx->ostage, ostage_bytes}};
+    for (int i = 0; i < 8; i++) bufs.push_back({&ctx->d_col[i], col_ptr(job->cols, i) ? col_bytes(i, col_rows) : 0});
+    return workspace_after(ctx, bufs, true);
+}
+
 void add_pass(PassOut &acc, const PassOut &o)
 {
     acc.kept += o.kept;
@@ -1245,7 +1350,7 @@ constexpr uint64_t kMaxPassRows = (1ull << 32) - 2;   // the pipeline's offsets 
 // the job's columns (device-resident: one split launch; host: double-buffered chunks behind the copies) or, for a
 // streamed job, the blocks of one round.  Every later sweep must count what the first one counted.
 // Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
-uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
+uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_budget_set, PassOut &acc)
 {
     cudaStream_t st = ctx->stream;
     const bool stream = job->stream;
@@ -1274,6 +1379,14 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
         if (pass_need(ctx, job, mid, mid, false, stage_bytes, true) <= budget) lo = mid; else hi = mid - 1;
     }
     const uint64_t cap = lo;
+    // host row store (streamed input with a host budget, read once per job by store_trim): out-stage of two halves of
+    // `chunk` packed rows.  The plan above does not depend on it; the store is used only where the out-stage fits next
+    // to the round's buffers at `cap`.
+    const size_t pack_scratch = stream && chunk && host_budget_set ? exact_bytes(residue_pack_scratch_bytes(chunk)) : 0;
+    const size_t ostage_bytes = pack_scratch ? 2 * chunk * sizeof(Row32) + pack_scratch + 256 : 0;
+    const uint64_t host_budget =
+        ostage_bytes && store_round_need(ctx, job, cap, stage_bytes, ostage_bytes) <= budget ? host_budget_set : 0;
+    if (host_budget && ctx->store_page == 0) fail(TAD_ERR_INTERNAL, "host row store without a page size");
     if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
     uint32_t P = 1;
     while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
@@ -1321,6 +1434,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
     const unsigned long long *h_cnt = ctx->h_small;
     uint64_t nchunk = 0;             // host chunks staged in the current sweep
     bool any_host = false;
+    bool count_only = false;         // the host row store fell back mid-round: the rest of the round is only counted
     // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M)
     auto feed = [&](const tad_columns &b, uint32_t v, uint32_t M) {
         const uint64_t n_all = b.rows;
@@ -1328,7 +1442,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
         if (b.mem == TAD_MEM_DEVICE) {
             ColPtrs c{};
             for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(b, i));
-            CU(launch_pass_split(st, c, n_all, f, M - 1, v, pcols, (uint32_t)colcap, d_cnt + kMaxPasses, d_cnt));
+            CU(launch_pass_split(st, c, n_all, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
+                                 d_cnt));
             acc.launches++;
             return;
         }
@@ -1350,19 +1465,23 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
             }
             CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
             CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-            CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)colcap, d_cnt + kMaxPasses, d_cnt));
+            CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
+                                 d_cnt));
             acc.launches++;
             CU(cudaEventRecord(ctx->stage_ev[h], st));
         }
     };
     // first streamed round: make room in the pass columns for every row the next `n` input rows can add (`ub` bounds the
     // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
-    uint64_t ub = 0;
+    // With a host budget, rows that would pass `cap` go to the host row store instead: false, `have` = the rows the
+    // pass columns hold.
+    uint64_t ub = 0, have = 0;
     auto room = [&](uint64_t n) {
-        if (colcap >= cap || ub + n <= colcap) { ub += n; return; }
+        if ((colcap >= cap && !host_budget) || ub + n <= colcap) { ub += n; return true; }
         CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        const uint64_t have = std::min<uint64_t>(ctx->h_small[128], colcap);
+        have = std::min<uint64_t>(ctx->h_small[128], colcap);
+        if (host_budget && have + n > cap) return false;
         if (have + n > colcap) {
             const uint64_t want = std::min(cap, std::max(2 * colcap, have + n));
             for (int i = 0; i < 8; i++)
@@ -1371,6 +1490,181 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
             set_pcols();
         }
         ub = have + n;
+        return true;
+    };
+    // ---- host row store (DESIGN.md section 11) ------------------------------------------------------------------------
+    // The first round's blocks are packed into the staging halves; every full half (and the last, partial one) is
+    // counted, scanned and scattered per residue into an out-stage half, whose residue segments are then copied to the
+    // residue's pages on the D2H stream.  The passes load their residues from the pages.
+    RowStore rs(ctx);
+    bool store = false;              // the current round goes to the store
+    bool stored = false;             // the store holds the whole first round: the passes load from it
+    bool dropped = false;            // the store fell back in the first round: it only counted
+    uint64_t fill = 0, nhalf = 0, npack = 0;   // rows in the staging half being filled; halves filled; out-stage halves used
+    int opend = -1;                  // out-stage half whose copies to the store are not issued yet
+    Row32 *ost[2] = {nullptr, nullptr};
+    void *pscratch = nullptr;
+    uint32_t *d_chunk = nullptr;
+    auto pass_cols_of = [&](uint64_t lo) {        // the pass columns from row `lo`, as kernel input
+        ColPtrs c{};
+        for (int i = 0; i < 8; i++)
+            if (col_ptr(hc, i)) set_col(c, i, static_cast<const char *>(ctx->d_col[i].p) + col_bytes(i, lo));
+        return c;
+    };
+    auto store_drop = [&]() {        // fallback: pages back to the context, the rest of the round is only counted
+        CU(cudaStreamSynchronize(st));          // no pack reads the staging halves any more
+        rs.clear();
+        store = false;
+        count_only = true;
+        opend = -1;
+    };
+    // copies of out-stage half `o`'s residue segments to the pages; false when the store would pass its budget
+    auto store_out = [&](int o) {
+        const uint64_t page_rows = ctx->store_page / sizeof(Row32);
+        CU(cudaEventSynchronize(ctx->cnt_ev[o]));
+        CU(cudaStreamWaitEvent(ctx->d2h_stream, ctx->cnt_ev[o], 0));
+        const uint32_t *n = ctx->h_chunk + kMaxPasses * o;
+        uint64_t at = 0;
+        for (int j = 0; j < kMaxPasses; j++) {
+            for (uint64_t left = n[j]; left;) {
+                const uint64_t used = rs.rows[j] % page_rows;
+                if (used == 0) {
+                    char *p = store_take_page(ctx, host_budget);
+                    if (!p) return false;
+                    rs.pages[j].push_back(p);
+                }
+                const uint64_t k = std::min(left, page_rows - used);
+                CU(cudaMemcpyAsync(rs.pages[j].back() + used * sizeof(Row32), ost[o] + at, k * sizeof(Row32),
+                                   cudaMemcpyDeviceToHost, ctx->d2h_stream));
+                rs.rows[j] += k;
+                at += k;
+                left -= k;
+            }
+        }
+        CU(cudaEventRecord(ctx->ost_ev[o], ctx->d2h_stream));
+        return true;
+    };
+    // count / scan / scatter `n` <= chunk device rows into the next out-stage half, then issue the copies of the previous
+    // one (its counts are back by now; this chunk's copies are on the bus meanwhile).  `totals`: count them for the job.
+    auto pack = [&](const ColPtrs &c, uint64_t n, bool totals) {
+        const int o = (int)(npack++ & 1);
+        CU(cudaStreamWaitEvent(st, ctx->ost_ev[o], 0));      // the copies that last read out-stage half o are done
+        CU(launch_residue_pack(st, c, n, f, pscratch, pack_scratch, d_chunk, totals ? d_cnt : nullptr, ost[o]));
+        acc.launches += 3;
+        CU(cudaMemcpyAsync(ctx->h_chunk + kMaxPasses * o, d_chunk, kMaxPasses * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaEventRecord(ctx->cnt_ev[o], st));
+        if (opend >= 0 && !store_out(opend)) { store_drop(); return; }
+        opend = o;
+    };
+    auto pack_half = [&]() {         // the staging half being filled
+        const int h = (int)(nhalf++ & 1);
+        ColPtrs c{};
+        char *src = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+        for (int i = 0; i < 10; i++) {
+            if (!staged(i)) continue;
+            set_col(c, i, src);
+            src += exact_bytes(col_bytes(i, chunk));
+        }
+        CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+        CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
+        pack(c, fill, true);
+        CU(cudaEventRecord(ctx->stage_ev[h], st));
+        fill = 0;
+    };
+    auto start_store = [&]() {
+        ensure(ctx, ctx->stage, stage_bytes);
+        ensure(ctx, ctx->ostage, ostage_bytes);
+        char *p = static_cast<char *>(ctx->ostage.p);
+        ost[0] = reinterpret_cast<Row32 *>(p);
+        ost[1] = reinterpret_cast<Row32 *>(p + chunk * sizeof(Row32));
+        pscratch = p + 2 * chunk * sizeof(Row32);
+        d_chunk = reinterpret_cast<uint32_t *>(p + 2 * chunk * sizeof(Row32) + pack_scratch);
+        store = true;
+    };
+    // the pass columns overflow in the first round: their `have` rows go to the store first (counted already)
+    auto switch_to_store = [&]() {
+        start_store();
+        for (uint64_t lo = 0; lo < have && store; lo += chunk) pack(pass_cols_of(lo), std::min(chunk, have - lo), false);
+    };
+    // one block into the staging halves (a D2D copy for a device block); a full half is packed.  The rest of a block
+    // the store fell back in is counted.
+    auto put = [&](const tad_columns &b) {
+        uint64_t lo = 0;
+        any_host = true;             // the round's time is the copies' (h2d phase), as for a sweep of host blocks
+        while (lo < b.rows && store) {
+            if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+            const int h = (int)(nhalf & 1);
+            if (fill == 0) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // its last pack is done
+            const uint64_t n = std::min(chunk - fill, b.rows - lo);
+            char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+            for (int i = 0; i < 10; i++) {
+                if (!staged(i)) continue;
+                const size_t w = col_bytes(i, 1);
+                CU(cudaMemcpyAsync(dst + fill * w, static_cast<const char *>(col_ptr(b, i)) + lo * w, n * w,
+                                   b.mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                                   ctx->copy_stream));
+                dst += exact_bytes(col_bytes(i, chunk));
+            }
+            fill += n;
+            lo += n;
+            if (fill == chunk) pack_half();
+        }
+        if (lo < b.rows) {
+            tad_columns rest = b;
+            rest.rows -= lo;
+            void **cols[10] = {(void **)&rest.src_ip, (void **)&rest.dst_ip, (void **)&rest.src_port, (void **)&rest.dst_port,
+                               (void **)&rest.proto, (void **)&rest.flow_start, (void **)&rest.flow_end, (void **)&rest.value,
+                               (void **)&rest.src_ns, (void **)&rest.dst_ns};
+            for (int i = 0; i < 10; i++)
+                if (*cols[i]) *cols[i] = static_cast<char *>(*cols[i]) + col_bytes(i, lo);
+            feed(rest, 0, P);
+        }
+    };
+    // end of the store's round: the last half, the last copies; the out-stage is not needed any more
+    auto end_store = [&]() {
+        if (store && fill) pack_half();
+        if (store && opend >= 0 && !store_out(opend)) store_drop();
+        if (store) {
+            if (opend >= 0) CU(cudaStreamWaitEvent(st, ctx->ost_ev[opend], 0));
+            stored = true;
+            store = false;
+        }
+        CU(cudaStreamSynchronize(st));
+        free_buf(ctx, ctx->ostage);
+        dropped = count_only;
+        count_only = false;          // later rounds split their pass into the pass columns
+    };
+    // pass (v, M) from the store into the pass columns, through the staging halves
+    auto load = [&](uint32_t v, uint32_t M) {
+        const uint64_t page_rows = ctx->store_page / sizeof(Row32), piece = half_bytes / sizeof(Row32);
+        CU(cudaEventRecord(ctx->ev[0], st));
+        CU(cudaEventRecord(ctx->start_ev, st));
+        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
+        uint64_t at = 0, k = 0;
+        for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M)
+            for (size_t pg = 0; pg < rs.pages[j].size(); pg++) {
+                const uint64_t in_pg = std::min(page_rows, rs.rows[j] - pg * page_rows);
+                for (uint64_t r0 = 0; r0 < in_pg; r0 += piece, k++) {
+                    const uint64_t n = std::min(piece, in_pg - r0);
+                    const int h = (int)(k & 1);
+                    Row32 *dst = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->stage.p) + h * half_bytes);
+                    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));    // its last unpack is done
+                    CU(cudaMemcpyAsync(dst, rs.pages[j][pg] + r0 * sizeof(Row32), n * sizeof(Row32),
+                                       cudaMemcpyHostToDevice, ctx->copy_stream));
+                    CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+                    CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
+                    CU(launch_store_unpack(st, dst, n, pcols, at));
+                    acc.launches++;
+                    CU(cudaEventRecord(ctx->stage_ev[h], st));
+                    at += n;
+                }
+            }
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaStreamSynchronize(st));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        acc.phase_ms[TAD_PHASE_H2D] += ms;
+        acc.device_ms += ms;
     };
     uint64_t counts[kMaxPasses];
     uint32_t sweeps = 0;
@@ -1394,10 +1688,17 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
             tad_columns b{};
             bool got = have_pend ? (b = pend, true) : next_block(job, b);
             have_pend = false;
+            if (sweeps == 0 && host_budget && P > 1) start_store();     // the hint plans passes: the round goes to the store
             while (got) {
-                if (sweeps == 0) room(b.rows);
-                feed(b, v, M);
-                CU(cudaEventRecord(ctx->blk_ev[k & 1], b.mem == TAD_MEM_DEVICE ? st : ctx->copy_stream));
+                if (sweeps == 0 && host_budget && !store && !count_only && !room(b.rows)) switch_to_store();
+                else if (sweeps == 0 && !host_budget) room(b.rows);
+                const bool to_store = store;
+                if (store) put(b); else feed(b, v, M);
+                if (to_store && !store) {            // the store fell back inside this block: its rest was split on st
+                    CU(cudaEventRecord(ctx->start_ev, st));
+                    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
+                }
+                CU(cudaEventRecord(ctx->blk_ev[k & 1], b.mem == TAD_MEM_DEVICE && !to_store ? st : ctx->copy_stream));
                 if (k > 0) {
                     CU(cudaEventSynchronize(ctx->blk_ev[(k - 1) & 1]));
                     uint64_t taken;
@@ -1412,6 +1713,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
                 got = next_block(job, b);
             }
             if (sweeps == 0) job->round_rows = rows;
+            if (sweeps == 0 && ctx->ostage.p) end_store();
             open = true;
         }
         CU(cudaEventRecord(ctx->ev[1], st));
@@ -1448,7 +1750,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
         // as an exact hint would have, at the price of that one round (loaded is then false unless P comes back to P0)
         uint32_t Pr = 1;
         while (Pr < (uint32_t)kMaxPasses && job->round_rows / Pr > cap / 8 * 7) Pr *= 2;
-        P = std::min(P, Pr);
+        P = stored ? Pr : std::min(P, Pr);      // stored: no round to save, so a low hint does not keep P either
     }
     while (P < (uint32_t)kMaxPasses && largest(P) > cap) P *= 2;
     auto too_big = [&](uint64_t rows) {
@@ -1457,17 +1759,19 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
              pass_need(ctx, job, rows, rows, false, stage_bytes, true), (unsigned long long)budget);
     };
     if (largest(P) > cap) too_big(largest(kMaxPasses));
-    bool loaded = P == P0 && got0 <= colcap;     // pass (0, P) is in the pass columns already
+    bool loaded = !stored && !dropped && P == P0 && got0 <= colcap;     // pass (0, P) is in the pass columns already
     std::deque<std::pair<uint32_t, uint32_t>> todo;
     for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
     // a streamed round stays open until the engine knows whether another sweep (round) follows
     auto finish_round = [&]() {
         if (!open) return;
         bool more = false;
-        for (const auto &e : todo) more = more || pass_rows(e.first, e.second) > 0;
+        for (const auto &e : todo) more = more || (!stored && pass_rows(e.first, e.second) > 0);
         close_round(job, more);
         open = false;
     };
+    if (stored)
+        for (int j = 0; j < kMaxPasses; j++) job->stored_rows += rs.rows[j];
     if (!loaded) finish_round();
     std::vector<PassOut> outs;
     uint32_t passes = 0;
@@ -1484,7 +1788,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
                     colcap = rows;
                     set_pcols();
                 }
-                sweep(v, M);
+                if (stored) load(v, M); else sweep(v, M);
             }
             loaded = false;
             bool split_pass = false;
@@ -1554,6 +1858,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
     const tad_columns &hc = job->cols;     // a streamed job's first push writes it: not read here for streams
     const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
+    const uint64_t host_budget = store_trim(ctx);      // the job's one read of the host budget
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
@@ -1603,7 +1908,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
             split = true;
         }
     }
-    if (split) passes = run_passes(ctx, job, budget, acc);
+    if (split) passes = run_passes(ctx, job, budget, host_budget, acc);
     publish_rows(job, acc.block, acc.out_rows);
     ctx->limit = 0;
     {
@@ -1624,6 +1929,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
         s.state = TAD_STATE_COMPLETED;
         job->passes = passes;
         job->peak_workspace = ctx->peak;
+        job->peak_host = ctx->store_peak;
         job->cv.notify_all();     // last touch of `job` by the worker (tad_release may free it now)
     }
 }
@@ -1648,6 +1954,7 @@ void worker_main(tad_ctx *ctx)
             // nothing of this job may still be reading the caller's columns once it is reported FAILED
             cudaStreamSynchronize(ctx->copy_stream);
             cudaStreamSynchronize(ctx->stream);
+            cudaStreamSynchronize(ctx->d2h_stream);
             cudaGetLastError();
             std::lock_guard<std::mutex> lk(job->mu);
             job->st.state = TAD_STATE_FAILED;
@@ -1842,6 +2149,9 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     NumaScope numa_scope(ctx->numa);
     bool ok = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) == cudaSuccess;
     ok = ok && cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking) == cudaSuccess;
+    for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->ost_ev[i], cudaEventDisableTiming) == cudaSuccess;
+    for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->cnt_ev[i], cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && i < kMaxChunks; i++) ok = cudaEventCreateWithFlags(&ctx->chunk_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->start_ev, cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
@@ -1863,6 +2173,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_small, 256 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
+    ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     if (!ok) {
         tad_shutdown(ctx);      // releases whatever was created
         return TAD_ERR_CUDA;
@@ -1903,6 +2214,8 @@ void tad_shutdown(tad_ctx *ctx)
     for (DevBuf *b : workspace_bufs(ctx))
         if (b->p) cudaFree(b->p);
     for (auto &b : ctx->pinned_pool) cudaFreeHost(b.p);
+    for (auto &b : ctx->store_slabs) cudaFreeHost(b.p);
+    if (ctx->h_chunk) cudaFreeHost(ctx->h_chunk);
     if (ctx->h_stats) cudaFreeHost(ctx->h_stats);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
     for (int i = 0; i < kMaxEvents; i++)
@@ -1914,9 +2227,14 @@ void tad_shutdown(tad_ctx *ctx)
         if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
     for (int i = 0; i < 2; i++)
         if (ctx->blk_ev[i]) cudaEventDestroy(ctx->blk_ev[i]);
+    for (int i = 0; i < 2; i++) {
+        if (ctx->ost_ev[i]) cudaEventDestroy(ctx->ost_ev[i]);
+        if (ctx->cnt_ev[i]) cudaEventDestroy(ctx->cnt_ev[i]);
+    }
     for (int i = 0; i <= kMaxXChunks; i++)
         if (ctx->x_ev[i]) cudaEventDestroy(ctx->x_ev[i]);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
+    if (ctx->d2h_stream) cudaStreamDestroy(ctx->d2h_stream);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -2087,6 +2405,25 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
     if (job->st.state != TAD_STATE_COMPLETED) return TAD_ERR_STATE;
     if (passes) *passes = job->passes;
     if (peak_workspace_bytes) *peak_workspace_bytes = job->peak_workspace;
+    return TAD_OK;
+}
+
+int tad_set_host_budget(tad_ctx *ctx, uint64_t bytes)
+{
+    if (!ctx) return TAD_ERR_INVALID_ARG;
+    if (ctx->cfg.world_size > 1) return TAD_ERR_UNSUPPORTED;
+    if (bytes && bytes < kBudgetFloor) return TAD_ERR_INVALID_ARG;
+    ctx->host_budget.store(bytes);
+    return TAD_OK;
+}
+
+int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host_bytes)
+{
+    if (!job) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->st.state != TAD_STATE_COMPLETED) return TAD_ERR_STATE;
+    if (stored_rows) *stored_rows = job->stored_rows;
+    if (peak_host_bytes) *peak_host_bytes = job->peak_host;
     return TAD_OK;
 }
 

@@ -332,6 +332,99 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
 }
 
 // ----------------------------------------------------------------------------------------
+// Host row store (DESIGN.md section 11): a streamed round's filtered rows are packed per low-hash-bit residue into
+// 32-byte records (Row32 without the hash tag) and copied to pinned host pages, one copy per residue segment.  One chunk
+// (at most a staging half of rows) at a time: count per (residue, tile), exclusive scan over the residue-major count
+// matrix, scatter.  The scatter reads the chunk a second time; HBM reads it far faster than PCIe delivers it.
+// ----------------------------------------------------------------------------------------
+__device__ __forceinline__ void load_tile_rows(const ColPtrs &c, const RowFilter &f, uint64_t R, uint64_t base, bool vec,
+                                               RowRegs (&r)[8])
+{
+    if (vec && base + 8 <= R) {
+        load_rows8<true>(c, f, base, true, r);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            r[i] = RowRegs{};
+            if (base + i < R) load_row_scalar(c, f, base + i, true, r[i]);
+        }
+    }
+}
+
+// cnt[j * ntiles + tile] = filtered rows of residue j in 2048-row tile `tile`; chunk[j] and totals[j] (null: skipped) gain
+// the residue's rows.  The residue is counted as pass_split_kernel counts it.
+template <bool VEC>
+__global__ void __launch_bounds__(256) residue_count_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t ntiles,
+                                                            uint32_t *__restrict__ cnt, uint32_t *__restrict__ chunk,
+                                                            unsigned long long *__restrict__ totals)
+{
+    __shared__ uint32_t s_cnt[kMaxPasses];
+    const int tid = threadIdx.x;
+    uint32_t tot = 0;              // thread tid < kMaxPasses: this CTA's rows of residue tid
+    for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        if (tid < kMaxPasses) s_cnt[tid] = 0;
+        __syncthreads();
+        RowRegs r[8];
+        load_tile_rows(c, f, R, (uint64_t)tile * 2048 + (uint64_t)tid * 8, VEC, r);
+#pragma unroll
+        for (int i = 0; i < 8; i++)
+            if (r[i].keep) atomicAdd(&s_cnt[(uint32_t)key_hash(r[i].a, r[i].b, r[i].proto) & (kMaxPasses - 1)], 1u);
+        __syncthreads();
+        if (tid < kMaxPasses) {    // the same thread clears s_cnt[tid] at the top of the next tile
+            cnt[(size_t)tid * ntiles + tile] = s_cnt[tid];
+            tot += s_cnt[tid];
+        }
+    }
+    if (tid < kMaxPasses && tot) {
+        atomicAdd(&chunk[tid], tot);
+        if (totals) atomicAdd(&totals[tid], (unsigned long long)tot);
+    }
+}
+
+// Every filtered row to out[off[j * ntiles + tile] + its rank among the tile's rows of residue j], ranked through shared
+// counters.  Rows are written from lane pairs (pair_store): every lane of a CTA runs every tile.
+template <bool VEC>
+__global__ void __launch_bounds__(256) residue_scatter_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t ntiles,
+                                                              const uint32_t *__restrict__ off, Row32 *__restrict__ out)
+{
+    __shared__ uint32_t s_off[kMaxPasses];
+    const int tid = threadIdx.x;
+    for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        if (tid < kMaxPasses) s_off[tid] = off[(size_t)tid * ntiles + tile];
+        __syncthreads();
+        RowRegs r[8];
+        load_tile_rows(c, f, R, (uint64_t)tile * 2048 + (uint64_t)tid * 8, VEC, r);
+        Row32 *dst[8];
+#pragma unroll
+        for (int i = 0; i < 8; i++)
+            dst[i] = r[i].keep
+                         ? out + atomicAdd(&s_off[(uint32_t)key_hash(r[i].a, r[i].b, r[i].proto) & (kMaxPasses - 1)], 1u)
+                         : nullptr;
+#pragma unroll
+        for (int i = 0; i < 8; i++) pair_store(r[i], dst[i], tid & 1);
+        __syncthreads();           // s_off is rewritten by the next tile
+    }
+}
+
+// Stored rows in[0, n) -> the pass columns at row `at`.  Null key columns are skipped (their stored fields are zero).
+__global__ void __launch_bounds__(256) store_unpack_kernel(const Row32 *__restrict__ in, uint64_t n, PassCols o, uint64_t at)
+{
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint4 lo = ldg_stream128(in + i);
+        const uint4 hi = ldg_stream128(reinterpret_cast<const char *>(in + i) + 16);
+        const uint64_t p = at + i;
+        if (o.src_ip) o.src_ip[p] = lo.y;                // a = src_ip << 32 | dst_ip
+        if (o.dst_ip) o.dst_ip[p] = lo.x;
+        if (o.src_port) o.src_port[p] = (uint16_t)(lo.z >> 16);   // b = flow_start << 32 | src_port << 16 | dst_port
+        if (o.dst_port) o.dst_port[p] = (uint16_t)lo.z;
+        if (o.flow_start) o.flow_start[p] = lo.w;
+        if (o.proto) o.proto[p] = (uint8_t)hi.w;
+        o.flow_end[p] = hi.z;
+        o.value[p] = pack64(hi.x, hi.y);
+    }
+}
+
+// ----------------------------------------------------------------------------------------
 // multi-CTA exclusive scans (bucket offsets; series base per bucket).  The grid never exceeds the
 // SM count with one 1024-thread CTA each, so all CTAs are co-resident and a CTA may spin on the
 // partial sums its lower-numbered peers publish (flags carry a per-launch epoch: no memset).
@@ -1331,6 +1424,55 @@ cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, con
         pass_split_kernel<true><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
     else
         pass_split_kernel<false><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
+    return cudaGetLastError();
+}
+
+// scratch of launch_residue_pack: count matrix, its exclusive scan, CUB temp storage
+static size_t residue_items(uint64_t rows) { return (size_t)kMaxPasses * ((rows + 2047) / 2048); }
+static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+size_t residue_pack_scratch_bytes(uint64_t max_rows)
+{
+    const size_t n = residue_items(max_rows);
+    size_t temp = 0;
+    exclusive_scan_u32(nullptr, temp, nullptr, nullptr, (int)n, 0);
+    return 2 * align256(n * 4) + align256(temp);
+}
+
+cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, void *scratch,
+                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out)
+{
+    cudaError_t e = cudaMemsetAsync(chunk, 0, kMaxPasses * sizeof(uint32_t), st);
+    if (e != cudaSuccess || R == 0) return e;
+    const uint32_t ntiles = (uint32_t)((R + 2047) / 2048);
+    const size_t n = residue_items(R);
+    uint32_t *cnt = static_cast<uint32_t *>(scratch);
+    uint32_t *off = reinterpret_cast<uint32_t *>(static_cast<char *>(scratch) + align256(n * 4));
+    void *temp = static_cast<char *>(scratch) + 2 * align256(n * 4);
+    size_t temp_bytes = 0;
+    if ((e = exclusive_scan_u32(nullptr, temp_bytes, nullptr, nullptr, (int)n, st)) != cudaSuccess) return e;
+    if (2 * align256(n * 4) + temp_bytes > scratch_bytes) return cudaErrorInvalidValue;
+    const uint32_t lim = (uint32_t)num_sms() * 8;
+    const uint32_t grid = ntiles < lim ? ntiles : lim;
+    const bool vec = cols_aligned16(c);
+    if (vec)
+        residue_count_kernel<true><<<grid, 256, 0, st>>>(c, R, f, ntiles, cnt, chunk, totals);
+    else
+        residue_count_kernel<false><<<grid, 256, 0, st>>>(c, R, f, ntiles, cnt, chunk, totals);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = exclusive_scan_u32(temp, temp_bytes, cnt, off, (int)n, st)) != cudaSuccess) return e;
+    if (vec)
+        residue_scatter_kernel<true><<<grid, 256, 0, st>>>(c, R, f, ntiles, off, out);
+    else
+        residue_scatter_kernel<false><<<grid, 256, 0, st>>>(c, R, f, ntiles, off, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_store_unpack(cudaStream_t st, const Row32 *in, uint64_t n, const PassCols &out, uint64_t at)
+{
+    if (n == 0) return cudaSuccess;
+    const uint64_t want = (n + 255) / 256, lim = (uint64_t)num_sms() * 8;
+    store_unpack_kernel<<<(uint32_t)(want < lim ? want : lim), 256, 0, st>>>(in, n, out, at);
     return cudaGetLastError();
 }
 

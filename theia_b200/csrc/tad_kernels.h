@@ -25,6 +25,15 @@ struct PassCols {
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
                               uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
                               unsigned long long *counts);
+// Host row store: the rows of `c` that pass the stage-A filters, packed as Row32 records without the hash tag, grouped
+// by low-hash-bit residue (residue 0 first) into out[0, rows kept).  chunk[kMaxPasses] (u32, zeroed here) receives the
+// rows of every residue and totals[kMaxPasses] (null: skipped) gains them.  R <= the max_rows the scratch was sized for;
+// three launches.
+size_t residue_pack_scratch_bytes(uint64_t max_rows);
+cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, void *scratch,
+                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out);
+// Stored rows in[0, n) -> out columns at rows [at, at + n); null key columns are skipped.  One launch.
+cudaError_t launch_store_unpack(cudaStream_t st, const Row32 *in, uint64_t n, const PassCols &out, uint64_t at);
 cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *offsets, uint32_t *cursor, uint32_t B,
                                uint32_t cap, uint32_t *big_list, uint32_t *big_base, uint32_t *cls_list /* 3 x B or null */,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);
@@ -61,6 +70,8 @@ size_t spill_scratch_bytes(uint64_t big_rows);
 // Sort a capacity-class bucket list ascending (CUB radix sort over `key_bits` bits); scratch from sort_lists_scratch_bytes(max n).
 size_t sort_lists_scratch_bytes(uint32_t max_items);
 cudaError_t sort_bucket_list(cudaStream_t st, uint32_t *list, uint32_t n, int key_bits, void *scratch, size_t scratch_bytes);
+// CUB exclusive sum of n u32 (temp == nullptr: only sets temp_bytes)
+cudaError_t exclusive_scan_u32(void *temp, size_t &temp_bytes, const uint32_t *in, uint32_t *out, int n, cudaStream_t st);
 // Optimistic partition (seg.stride != 0): a listed bucket holds min(count, stride) rows in its slot and the rest in
 // ovf[0, n_ovf) (every overflow row belongs to a listed bucket).
 cudaError_t run_spill(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets, const uint32_t *big_list,

@@ -10,6 +10,7 @@
 Streamed input (the table arrives block by block and is never held whole):
 
     res, st = eng.run_stream(lambda: read_blocks(), algo="EWMA", rows_hint=n)   # re-reads while another pass needs it
+    eng.set_host_budget(4 << 30)    # or keep the rows in pinned host memory between passes: read once
 """
 from __future__ import annotations
 
@@ -141,12 +142,18 @@ class Job:
         return out
 
     def memory(self) -> dict:
-        """Of a COMPLETED job: the hash-range passes it ran in and the largest device workspace the context held."""
+        """Of a COMPLETED job: the hash-range passes it ran in, the largest device workspace the context held, the rows
+        that went through the host row store and the most store bytes the context held."""
         passes, peak = C.c_uint32(), C.c_uint64()
         rc = self.eng.lib.tad_job_memory(self.h, C.byref(passes), C.byref(peak))
         if rc != 0:
             raise TadError(rc, "tad_job_memory")
-        return {"passes": passes.value, "peak_workspace_bytes": peak.value}
+        stored, peak_host = C.c_uint64(), C.c_uint64()
+        rc = self.eng.lib.tad_job_host_memory(self.h, C.byref(stored), C.byref(peak_host))
+        if rc != 0:
+            raise TadError(rc, "tad_job_host_memory")
+        return {"passes": passes.value, "peak_workspace_bytes": peak.value, "stored_rows": stored.value,
+                "peak_host_bytes": peak_host.value}
 
     def cancel(self):
         self.eng.lib.tad_cancel(self.h)
@@ -208,7 +215,7 @@ class StreamJob(Job):
 
 class TadEngine:
     def __init__(self, device: int = 0, world_size: int = 1, rank: int = 0, nccl_unique_id: bytes | None = None,
-                 memory_budget: int | None = None):
+                 memory_budget: int | None = None, host_budget: int | None = None):
         self.lib = L.load()
         cfg = L.TadConfig()
         cfg.device, cfg.world_size, cfg.rank = device, world_size, rank
@@ -224,6 +231,15 @@ class TadEngine:
         self.ctx = ctx
         if memory_budget is not None:
             self.set_memory_budget(memory_budget)
+        if host_budget is not None:
+            self.set_host_budget(host_budget)
+
+    def set_host_budget(self, nbytes: int):
+        """Pinned host bytes the context may hold for its host row store (0 = none): a streamed job that needs several
+        passes then keeps its rows there and is delivered once."""
+        rc = self.lib.tad_set_host_budget(self.ctx, int(nbytes))
+        if rc != 0:
+            raise TadError(rc, "tad_set_host_budget(%d)" % nbytes)
 
     def set_memory_budget(self, nbytes: int):
         """Device bytes the context's workspace may hold (0 = free memory at job start); larger jobs run in passes."""
