@@ -8,6 +8,7 @@
 //   entries  : one 32 B SeriesEntry per connection, written IN PLACE over the dead part[]
 //              region of its bucket (a bucket is fully staged in shared memory before its
 //              entries are written)
+//   EWMA writes csr_v/t and entries for spilled buckets only: the group kernel scores the others.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -110,6 +111,8 @@ enum {
     ST_OVF,             // optimistic partition: rows that did not fit their bucket's fixed-capacity slot
     ST_LOCALKEPT,       // multi-GPU optimistic partition: rows of THIS rank that passed the filters (ST_KEPT = rows owned);
                         // must follow ST_OVF: the two travel in one 8-byte all-gather
+    ST_GSERIES,         // EWMA: series / points of the buckets the group kernel scored in place (ST_SERIES / ST_POINTS
+    ST_GPOINTS,         // then count the spilled buckets only); adjacent: zeroed together before every scoring attempt
     ST_COUNT
 };
 

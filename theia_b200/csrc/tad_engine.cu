@@ -1095,10 +1095,13 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         ensure(ctx, ctx->csr_p, z.csr_p);
         csr_p = (uint32_t *)ctx->csr_p.p;
     }
+    // EWMA is scored inside the group kernel (launch_group_ewma, in the detect loop below): only the spilled buckets go
+    // through the per-series arrays, the series scan and the detect kernel
+    const bool fused = sp.algo == TAD_ALGO_EWMA;
+    const uint32_t n_cls[3] = {ctx->h_stats[ST_NCLS0], ctx->h_stats[ST_NCLS1], ctx->h_stats[ST_NCLS2]};
     mark(-1);
     {
         int l = 0;
-        const uint32_t n_cls[3] = {ctx->h_stats[ST_NCLS0], ctx->h_stats[ST_NCLS1], ctx->h_stats[ST_NCLS2]};
         if (ctx->sort_classes) {
             // class lists in ascending bucket order: concurrently running CTAs then touch neighbouring slots / csr stretches
             const size_t need = sort_lists_scratch_bytes(Bl);
@@ -1108,8 +1111,10 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             for (int k = 0; k < 3; k++)
                 if (n_cls[k] > 1) { CU(sort_bucket_list(st, cls_list + (size_t)k * Bl, n_cls[k], bits, ctx->sortb.p, ctx->sortb.cap)); launches += 3; }
         }
-        CU(launch_group(st, seg, entries, offsets, Bl, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb, sp.reducer, &l));
-        launches += l;
+        if (!fused) {
+            CU(launch_group(st, seg, entries, offsets, Bl, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb, sp.reducer, &l));
+            launches += l;
+        }
     }
     mark(TAD_PHASE_GROUP);
     if (n_big) {
@@ -1124,17 +1129,22 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     }
     ensure(ctx, ctx->sbase, z.sbase);      // series base per bucket + bucket hint per 32 series
     uint32_t *sbase = (uint32_t *)ctx->sbase.p;
-    CU(launch_series_scan(st, nsb, npb, sbase, Bl, d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
-    CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    check_cancel();
-    const uint32_t S = ctx->h_stats[ST_SERIES];
-    const uint64_t points = ctx->h_stats[ST_POINTS];
-    set_progress(job, TAD_STATE_RUNNING, 4);
+    uint32_t S = 0;                        // series of the detect kernels (EWMA: of the spilled buckets)
+    uint64_t points = 0;
+    if (!fused || n_big) {
+        CU(launch_series_scan(st, nsb, npb, sbase, Bl, d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
+        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        check_cancel();
+        S = ctx->h_stats[ST_SERIES];
+        points = ctx->h_stats[ST_POINTS];
+    }
+    if (!fused) set_progress(job, TAD_STATE_RUNNING, 4);
 
     // ---- detect -----------------------------------------------------------------------------
     const bool emit_all = (sp.flags & TAD_FLAG_EMIT_ALL) != 0;
-    uint64_t out_cap = out_cap_guess(points, emit_all);
+    // EWMA: the points are counted by the scoring kernel itself, so the first guess comes from the rows
+    uint64_t out_cap = out_cap_guess(fused ? owned : points, emit_all);
     uint64_t out_rows = 0;
     OutLayout L{};
     OutCols oc{};
@@ -1148,7 +1158,14 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         oc = out_cols(ctx->outb.p, L);
         CU(cudaMemsetAsync(d_stats + ST_OUTCOUNT, 0, 4, st));
         mark(-1);
-        if (sp.algo == TAD_ALGO_EWMA) {
+        if (fused) {
+            // the group kernel never writes over the rows it reads: a rerun with larger capacity scores them again
+            CU(cudaMemsetAsync(d_stats + ST_GSERIES, 0, 8, st));
+            int l = 0;
+            CU(launch_group_ewma(st, seg, offsets, Bl, cls_list, n_cls, sp.reducer,
+                                 GroupScore{oc, (uint32_t)out_cap, d_stats, emit_all}, &l));
+            launches += l;
+            mark(TAD_PHASE_GROUP);
             CU(launch_detect_ewma(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, oc, (uint32_t)out_cap, d_stats, emit_all));
             launches += S ? 1 : 0;
         } else if (sp.algo == TAD_ALGO_DBSCAN) {
@@ -1177,6 +1194,12 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         if (attempt == 2) fail(TAD_ERR_INTERNAL, "result capacity did not converge");
     }
     check_cancel();
+    uint64_t series_all = S, points_all = points;
+    if (fused) {
+        series_all += ctx->h_stats[ST_GSERIES];
+        points_all += ctx->h_stats[ST_GPOINTS];
+        set_progress(job, TAD_STATE_RUNNING, 4);
+    }
     set_progress(job, TAD_STATE_RUNNING, 5);
     if (sync_at_end) {
         // end-of-job barrier of the peer-pull path: my slots and counters may be overwritten (next job) only after every
@@ -1218,8 +1241,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     if (first_k >= 0 && last_k > first_k) CU(cudaEventElapsedTime(&total, ctx->ev[first_k], ctx->ev[last_k]));
     out.kept = kept;
     out.owned = owned;
-    out.points = points;
-    out.series = S;
+    out.points = points_all;
+    out.series = series_all;
     out.out_rows = out_rows;
     out.spill_rows = big_rows;
     out.launches = launches;

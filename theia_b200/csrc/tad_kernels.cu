@@ -9,9 +9,12 @@
 //   group    (K3)  one CTA per bucket: TMA bulk load into shared memory, hash-group by
 //                  key, O(n) bucket-sort of each series by flowEndSeconds, reduce duplicates,
 //                  write per-series arrays + series entries                   reads 32, writes 12 B/row
-//   sscan    (K3b) exclusive scan of series-per-bucket
+//                  EWMA: score every series in shared memory instead (stddev_samp + EWMA + flag) and write
+//                  the result rows; no arrays, no entries                     reads 32 B/row, writes 46 B/result row
+//   sscan    (K3b) exclusive scan of series-per-bucket (EWMA: only when a bucket spilled)
 //   detect   (K4)  one thread per series, read straight from the per-series arrays: stddev_samp
-//                  (Welford, sequential FP64), EWMA / DBSCAN score + flag, queued emission  reads 8-12 B/row
+//                  (Welford, sequential FP64), EWMA (spilled buckets only) / DBSCAN score + flag,
+//                  queued emission                                            reads 8-12 B/row
 //
 // All FP64 arithmetic on the score path uses explicit round-to-nearest intrinsics in the
 // exact operation order of the reference UDFs (anomaly_detection.py:146-212) so that the
@@ -600,6 +603,47 @@ __global__ void __launch_bounds__(1024) series_scan_kernel(const uint32_t *__res
 }
 
 // ----------------------------------------------------------------------------------------
+// Division by the running count on the Welford critical path (fused EWMA group kernel and detect kernels)
+// ----------------------------------------------------------------------------------------
+// d / k with k a small integer is computed as
+// q0 = d * r (r = RN(1/k) from a table filled with __drcp_rn) plus ONE FMA residual correction
+// q1 = fma(fma(-k, q0, d), r, q0).  That is the correctly rounded quotient: q0 is within 1.5 ulp of z = d/k, so the
+// residual k (z - q0) is exact, and q0 + residual * r = z + (z - q0) * eps with |eps| <= 2^-53 -- a perturbation
+// below 2^-52 ulp(z) -- while z itself keeps a distance of at least ulp(z) / (2k) from every rounding boundary
+// (d - k * midpoint is a non-zero multiple of ulp(z)/2).  So RN(q0 + residual * r) = RN(z) for every k < 2^50.
+// Checked against `/` on 6e8 random and 1.2e9 near-midpoint operands (profiles/microbench/divcheck.c); three
+// dependent operations instead of the ~30 of the generic __ddiv_rn sequence.
+constexpr uint32_t kRcpTable = 4096;
+__device__ double g_rcp[kRcpTable + 1];
+
+__global__ void rcp_table_kernel()
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k <= kRcpTable) g_rcp[k] = k ? __drcp_rn((double)k) : 0.0;
+}
+
+// Fused EWMA: stddev_samp of one time-sorted series v[0, c) of shared memory (Welford, as detect_ewma_direct_kernel), with
+// the EWMA value of every point to e[0, c).  The two chains do not depend on each other; v and e do not overlap, so the
+// loads of an unrolled group are all issued before its chain starts.
+__device__ __forceinline__ double ewma_series(const unsigned long long *__restrict__ v, double *__restrict__ e, uint32_t c)
+{
+    double cnt = 0.0, avg = 0.0, m2 = 0.0, prev = 0.0;
+#pragma unroll 4
+    for (uint32_t i = 0; i < c; i++) {
+        const double x = __ull2double_rn(v[i]), r = g_rcp[i + 1];
+        cnt = __dadd_rn(cnt, 1.0);
+        const double d = __dsub_rn(x, avg);
+        const double q0 = __dmul_rn(d, r);
+        const double dn = __fma_rn(__fma_rn(-cnt, q0, d), r, q0);
+        avg = __dadd_rn(avg, dn);
+        m2 = __dadd_rn(m2, __dmul_rn(d, __dsub_rn(d, dn)));
+        prev = __dadd_rn(__dmul_rn(0.5, prev), __dmul_rn(0.5, x));
+        e[i] = prev;
+    }
+    return c >= 2 ? __dsqrt_rn(__ddiv_rn(m2, __dsub_rn(cnt, 1.0))) : __longlong_as_double(0x7ff8000000000000LL);
+}
+
+// ----------------------------------------------------------------------------------------
 // K3: per-bucket group + time sort in shared memory
 // ----------------------------------------------------------------------------------------
 template <int CAP, int NT>
@@ -611,7 +655,29 @@ struct GroupSmem {
     alignas(8) unsigned long long mbar;
     uint32_t warp_sums[32];
     uint32_t total;
+    uint32_t qcount, qbase;                   // fused EWMA: queued result rows, first output row of the CTA
 };
+// Five CTAs of the smallest class share an SM (228 KB, 1 KB reserved per CTA) with room for the fused instance's 256 B
+// segment table; the two queue words above sit in what was the struct's tail padding.
+static_assert(sizeof(GroupSmem<1024, 256>) == 45312, "the smallest capacity class must keep five CTAs per SM");
+
+// What the group kernel does with a bucket once its series are grouped, time-sorted and reduced.
+enum GroupMode : int {
+    kGroupArrays = 0,     // per-series arrays + series entries for a detect kernel (ARIMA)
+    kGroupRank = 1,       // the same plus every point's value rank inside its series (DBSCAN)
+    kGroupEwma = 2,       // EWMA scored in place: result rows only, no arrays, entries or nsb / npb
+};
+
+// Fused EWMA: where each source segment's rows of the bucket start (`first`, in the segment) and where they were
+// placed inside the staged bucket (`pre`), so that a staged row index maps back to its row in global memory.
+struct SegTable {
+    uint32_t first[kMaxSeg], pre[kMaxSeg];
+};
+__device__ __forceinline__ SegTable &seg_table()
+{
+    __shared__ SegTable t;               // allocated only in the kernels that call this (the fused instances)
+    return t;
+}
 
 template <int NT>
 __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *warp_sums, uint32_t *total)
@@ -679,14 +745,17 @@ __device__ __forceinline__ uint32_t count_lt_u64(const unsigned long long *a, ui
 
 constexpr int kSlotHashBits = 13;      // hash-tag bits that pick the shared-memory slot (largest table: 2 * kGroupCap)
 
-template <int CAP, int NT, bool VRANK>
-__global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntry *__restrict__ entries,
+// Fused instances: as many CTAs per SM as the shared memory allows (five of the smallest class: at most 48 registers),
+// which also lets ptxas keep the larger classes free of spills.  The other instances keep their plain bound.
+template <int CAP, int NT, int MODE>
+__global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : CAP == kGroupCapSmall ? 5 : CAP == kGroupCapMid ? 2 : 1) group_kernel(const SegDesc seg, SeriesEntry *__restrict__ entries,
                                                    const uint32_t *__restrict__ offsets, const uint32_t *__restrict__ bucket_list,
                                                    uint32_t lo_rows,
                                                    uint64_t *__restrict__ csr_v, uint32_t *__restrict__ csr_t,
                                                    uint32_t *__restrict__ csr_p, uint32_t *__restrict__ nsb,
-                                                   uint32_t *__restrict__ npb, int reducer)
+                                                   uint32_t *__restrict__ npb, int reducer, const GroupScore score)
 {
+    constexpr bool VRANK = MODE == kGroupRank, FUSED = MODE == kGroupEwma;
     using S = GroupSmem<CAP, NT>;
     constexpr int HT = S::HT;
     constexpr int RPT = CAP / NT;      // rows per thread
@@ -725,7 +794,12 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
         if (sc)
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                          :: "r"(smem_u32(s.x) + (inc - sc) * 32u), "l"(seg.base[tid] + so), "r"(sc * 32u), "r"(bar) : "memory");
+        if constexpr (FUSED) {
+            seg_table().first[tid] = so;
+            seg_table().pre[tid] = inc - sc;
+        }
     }
+    if (FUSED && tid == 0) s.qcount = 0u;
 #pragma unroll
     for (int i = 0; i < SPT; i++) s.ht[tid + i * NT] = 0u;
     __syncthreads();
@@ -789,14 +863,17 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
             if (w & 0xffffu) {
                 const uint32_t ex = pre + loc[i];
                 const uint32_t so = ex & 0xffffu, k = ex >> 16, cnt = w >> 16, rep = (w & 0xffffu) - 1u;
-                const uint4 kk = x4[2 * rep];
-                const uint32_t pp = x4[2 * rep + 1].w;
+                uint4 kk{};
+                uint32_t pp = 0;
+                if constexpr (!FUSED) { kk = x4[2 * rep]; pp = x4[2 * rep + 1].w; }
                 s.soff[base + i] = (uint16_t)so;
                 s.ht[base + i] = (cnt << 16) | k;
-                // series entry, in place over the (already staged) bucket rows
-                uint4 *e4 = reinterpret_cast<uint4 *>(ent + k);
-                e4[0] = kk;
-                e4[1] = make_uint4(pp & 0xffu, cnt, off_b + so, 0u);
+                if constexpr (!FUSED) {
+                    // series entry, in place over the (already staged) bucket rows
+                    uint4 *e4 = reinterpret_cast<uint4 *>(ent + k);
+                    e4[0] = kk;
+                    e4[1] = make_uint4(pp & 0xffu, cnt, off_b + so, 0u);
+                }
             }
         }
     }
@@ -807,7 +884,9 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
     uint32_t *tout = ts + CAP;                                          // times, final order
     unsigned long long *vout = reinterpret_cast<unsigned long long *>(s.x + 8 * CAP);
     uint16_t *pslot = reinterpret_cast<uint16_t *>(s.x + 16 * CAP);   // VRANK: slot of the series at each position
+    uint16_t *keyrow = pslot;                                           // FUSED: a staged row of every series (its key)
     uint16_t *pout = reinterpret_cast<uint16_t *>(s.x + 18 * CAP);    // VRANK: value rank -> time index
+    uint16_t *pser = pout;                                              // FUSED: series index at each position
     uint32_t *binc = reinterpret_cast<uint32_t *>(s.x + 20 * CAP);    // per-bin counts -> exclusive offsets
     uint32_t *tmin = reinterpret_cast<uint32_t *>(s.x + 24 * CAP);    // per series index
     uint32_t *tmax = reinterpret_cast<uint32_t *>(s.x + 28 * CAP);
@@ -825,6 +904,8 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
             const uint32_t k = s.ht[mySP[j] & 0xffffu] & 0xffffu;
             atomicMin(&tmin[k], myT[j]);
             atomicMax(&tmax[k], myT[j]);
+            // the row that arrived first at its slot: every row of a series carries the same key
+            if (FUSED && (mySP[j] >> 16) == 0u) keyrow[k] = (uint16_t)r;
         }
     }
     __syncthreads();
@@ -887,6 +968,7 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
             tout[pos] = t;
             vout[pos] = myV[j];
             if (VRANK) pslot[pos] = (uint16_t)slot;
+            if (FUSED) pser[pos] = (uint16_t)s.ht[slot];
             mySP[j] = pos | ((pos > s.soff[slot] ? 1u : 0u) << 31);
         }
     }
@@ -923,7 +1005,7 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
             }
             if (wr + 1 != cnt) {
                 removed += cnt - (wr + 1);
-                ent[w & 0xffffu].n = wr + 1;
+                if (!FUSED) ent[w & 0xffffu].n = wr + 1;
                 s.ht[sl] = ((wr + 1) << 16) | (w & 0xffffu);
             }
         }
@@ -931,6 +1013,74 @@ __global__ void __launch_bounds__(NT) group_kernel(const SegDesc seg, SeriesEntr
         const uint32_t pre = block_exclusive_scan<NT>(removed, s.warp_sums, &s.total);
         (void)pre;
         points = n - s.total;
+    }
+
+    if constexpr (FUSED) {
+        // ---- E: EWMA scored in place ------------------------------------------------------------------------------
+        // The same FP64 operations in the same order as detect_ewma_direct_kernel.  One thread per series runs the
+        // Welford chain and, next to it, the EWMA chain (which does not depend on it), keeping the EWMA value of every
+        // point; the flags then need only a compare against the series' stddev, one thread per point.  Free shared
+        // memory from here on: ts [0, 4 CAP), binc [20 CAP, 24 CAP), tmin / tmax [24 CAP, 32 CAP), and ht / soff once
+        // sinfo is built.
+        static_assert(CAP <= (int)kRcpTable, "every count of the Welford chain must have its reciprocal in the table");
+        uint32_t *queue = ts;                                                 // point | series << 16 | flag << 31
+        uint32_t *sinfo = binc;                                               // per series: first point | points << 16
+        double *ewma = reinterpret_cast<double *>(s.x + 24 * CAP);            // EWMA value at every point
+        double *sdv = reinterpret_cast<double *>(s.ht);                       // per series: stddev_samp
+#pragma unroll
+        for (int i = 0; i < SPT; i++) {
+            const uint32_t w = s.ht[tid * SPT + i];
+            if (w >> 16) sinfo[w & 0xffffu] = s.soff[tid * SPT + i] | (w & 0xffff0000u);
+        }
+        __syncthreads();
+        for (uint32_t k = tid; k < ns; k += NT) {
+            const uint32_t si = sinfo[k], so = si & 0xffffu;
+            sdv[k] = ewma_series(vout + so, ewma + so, si >> 16);
+        }
+        __syncthreads();
+        for (uint32_t p = tid; p < n; p += NT) {
+            const uint32_t k = pser[p], si = sinfo[k], c = si >> 16;
+            if (p - (si & 0xffffu) >= c) continue;                           // hole left by the duplicate reduce
+            const bool has_sd = c >= 2;
+            if (!has_sd && !score.emit_all) continue;
+            const bool flag = has_sd && (fabs(__dsub_rn(__ull2double_rn(vout[p]), ewma[p])) > sdv[k]);
+            if (flag || score.emit_all) queue[atomicAdd(&s.qcount, 1u)] = p | (k << 16) | (flag ? 0x80000000u : 0u);
+        }
+        __syncthreads();
+        if (tid == 0) {
+            s.qbase = s.qcount ? atomicAdd(&score.stats[ST_OUTCOUNT], s.qcount) : 0u;
+            atomicAdd(&score.stats[ST_GSERIES], ns);
+            atomicAdd(&score.stats[ST_GPOINTS], points);
+        }
+        __syncthreads();
+        // ---- emission: one result row per thread and step, every column written coalesced.  The key is read back from
+        // the bucket's source rows (intact: this instance writes nothing over its input), which the bulk copy has just
+        // brought through L2.
+        const uint32_t base = s.qbase;
+        const uint32_t nq = base < score.out_cap ? min(s.qcount, score.out_cap - base) : 0u;
+        const OutCols &o = score.out;
+        const SegTable &sgt = seg_table();
+        for (uint32_t j = tid; j < nq; j += NT) {
+            const uint32_t q = queue[j], p = q & 0xffffu, k = (q >> 16) & 0x7fffu, r = keyrow[k];
+            int sg = 0;
+            while (sg + 1 < seg.nseg && sgt.pre[sg + 1] <= r) sg++;
+            const Row32 *row = seg.base[sg] + sgt.first[sg] + (r - sgt.pre[sg]);
+            const uint4 kk = *reinterpret_cast<const uint4 *>(row);
+            const uint32_t pp = reinterpret_cast<const uint32_t *>(row)[7];
+            const uint32_t idx = base + j;
+            o.src_ip[idx] = kk.y;                       // a = src_ip << 32 | dst_ip
+            o.dst_ip[idx] = kk.x;
+            o.flow_start[idx] = kk.w;                   // b = flow_start << 32 | src_port << 16 | dst_port
+            o.src_port[idx] = (uint16_t)(kk.z >> 16);
+            o.dst_port[idx] = (uint16_t)kk.z;
+            o.proto[idx] = (uint8_t)pp;
+            o.flow_end[idx] = tout[p];
+            o.stddev[idx] = sdv[k];
+            o.algo_calc[idx] = ewma[p];
+            o.throughput[idx] = __ull2double_rn(vout[p]);
+            o.anomaly[idx] = (q >> 31) ? 1 : 0;
+        }
+        return;
     }
 
     if (VRANK) {
@@ -999,23 +1149,6 @@ __device__ __forceinline__ void write_out(const OutCols &o, uint32_t idx, const 
     o.algo_calc[idx] = calc;
     o.throughput[idx] = x;
     o.anomaly[idx] = flag ? 1 : 0;
-}
-
-// Division by the running count on the Welford critical path.  d / k with k a small integer is computed as
-// q0 = d * r (r = RN(1/k) from a table filled with __drcp_rn) plus ONE FMA residual correction
-// q1 = fma(fma(-k, q0, d), r, q0).  That is the correctly rounded quotient: q0 is within 1.5 ulp of z = d/k, so the
-// residual k (z - q0) is exact, and q0 + residual * r = z + (z - q0) * eps with |eps| <= 2^-53 -- a perturbation
-// below 2^-52 ulp(z) -- while z itself keeps a distance of at least ulp(z) / (2k) from every rounding boundary
-// (d - k * midpoint is a non-zero multiple of ulp(z)/2).  So RN(q0 + residual * r) = RN(z) for every k < 2^50.
-// Checked against `/` on 6e8 random and 1.2e9 near-midpoint operands (profiles/microbench/divcheck.c); three
-// dependent operations instead of the ~30 of the generic __ddiv_rn sequence.
-constexpr uint32_t kRcpTable = 4096;
-__device__ double g_rcp[kRcpTable + 1];
-
-__global__ void rcp_table_kernel()
-{
-    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k <= kRcpTable) g_rcp[k] = k ? __drcp_rn((double)k) : 0.0;
 }
 
 // stddev_samp as Spark's CentralMomentAgg computes it (Welford), sequential in time order.  The reciprocals
@@ -1494,15 +1627,15 @@ cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *
     return cudaGetLastError();
 }
 
-template <int CAP, int NT, bool VRANK>
+template <int CAP, int NT, int MODE>
 static cudaError_t launch_group_class(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets,
                                       const uint32_t *bucket_list, uint32_t n_buckets, uint32_t lo_rows,
                                       uint64_t *csr_v, uint32_t *csr_t, uint32_t *csr_p, uint32_t *nsb, uint32_t *npb,
-                                      int reducer)
+                                      int reducer, const GroupScore &score)
 {
     using S = GroupSmem<CAP, NT>;
     static std::atomic<bool> configured{false};
-    auto kern = group_kernel<CAP, NT, VRANK>;
+    auto kern = group_kernel<CAP, NT, MODE>;
     if (!configured.load(std::memory_order_acquire)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(S));
         if (e != cudaSuccess) return e;
@@ -1510,7 +1643,7 @@ static cudaError_t launch_group_class(cudaStream_t st, const SegDesc &seg, Serie
     }
     if (n_buckets == 0) return cudaSuccess;
     kern<<<n_buckets, NT, sizeof(S), st>>>(seg, entries, offsets, bucket_list, lo_rows, csr_v, csr_t, csr_p, nsb, npb,
-                                           reducer);
+                                           reducer, score);
     return cudaGetLastError();
 }
 
@@ -1518,26 +1651,27 @@ static cudaError_t launch_group_class(cudaStream_t st, const SegDesc &seg, Serie
 // highest occupancy.  Each class is launched over ITS OWN bucket list (built by the bucket scan), one CTA per
 // listed bucket -- launching all B CTAs per class and exiting early costs ~0.5 ms per class at 180 KB of shared
 // memory per CTA.  Empty buckets keep the zeroes the caller memset into nsb / npb.
-template <bool VRANK>
+template <int MODE>
 static cudaError_t launch_group_all(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets,
                                     uint32_t B, const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v,
-                                    uint32_t *csr_t, uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, int *launches)
+                                    uint32_t *csr_t, uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer,
+                                    const GroupScore &score, int *launches)
 {
     *launches = 0;
     cudaError_t e = cudaSuccess;
     if (n_cls[2]) {
-        e = launch_group_class<kGroupCap, 512, VRANK>(st, seg, entries, offsets, cls_list + 2 * (size_t)B, n_cls[2], kGroupCapMid,
-                                                      csr_v, csr_t, csr_p, nsb, npb, reducer);
+        e = launch_group_class<kGroupCap, 512, MODE>(st, seg, entries, offsets, cls_list + 2 * (size_t)B, n_cls[2], kGroupCapMid,
+                                                     csr_v, csr_t, csr_p, nsb, npb, reducer, score);
         ++*launches;
     }
     if (e == cudaSuccess && n_cls[1]) {
-        e = launch_group_class<kGroupCapMid, 256, VRANK>(st, seg, entries, offsets, cls_list + B, n_cls[1], kGroupCapSmall,
-                                                         csr_v, csr_t, csr_p, nsb, npb, reducer);
+        e = launch_group_class<kGroupCapMid, 256, MODE>(st, seg, entries, offsets, cls_list + B, n_cls[1], kGroupCapSmall,
+                                                        csr_v, csr_t, csr_p, nsb, npb, reducer, score);
         ++*launches;
     }
     if (e == cudaSuccess) {
-        e = launch_group_class<kGroupCapSmall, 256, VRANK>(st, seg, entries, offsets, cls_list, n_cls[0], 0, csr_v, csr_t,
-                                                           csr_p, nsb, npb, reducer);
+        e = launch_group_class<kGroupCapSmall, 256, MODE>(st, seg, entries, offsets, cls_list, n_cls[0], 0, csr_v, csr_t,
+                                                          csr_p, nsb, npb, reducer, score);
         *launches += n_cls[0] ? 1 : 0;
     }
     return e;
@@ -1547,10 +1681,11 @@ cudaError_t launch_group(cudaStream_t st, const SegDesc &seg, SeriesEntry *entri
                          const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v, uint32_t *csr_t,
                          uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, int *launches)
 {
-    return csr_p ? launch_group_all<true>(st, seg, entries, offsets, B, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb,
-                                          reducer, launches)
-                 : launch_group_all<false>(st, seg, entries, offsets, B, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb,
-                                           reducer, launches);
+    const GroupScore none{};
+    return csr_p ? launch_group_all<kGroupRank>(st, seg, entries, offsets, B, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb,
+                                                reducer, none, launches)
+                 : launch_group_all<kGroupArrays>(st, seg, entries, offsets, B, cls_list, n_cls, csr_v, csr_t, csr_p, nsb,
+                                                  npb, reducer, none, launches);
 }
 
 cudaError_t launch_series_scan(cudaStream_t st, const uint32_t *nsb, const uint32_t *npb, uint32_t *sbase, uint32_t B,
@@ -1567,6 +1702,14 @@ static void ensure_rcp_table(cudaStream_t st)
         rcp_table_kernel<<<(kRcpTable + 256) / 256, 256, 0, st>>>();
         cudaStreamSynchronize(st);      // once per process: other contexts (streams) of this device read the table too
     });
+}
+
+cudaError_t launch_group_ewma(cudaStream_t st, const SegDesc &seg, const uint32_t *offsets, uint32_t B, const uint32_t *cls_list,
+                              const uint32_t n_cls[3], int reducer, const GroupScore &score, int *launches)
+{
+    ensure_rcp_table(st);
+    return launch_group_all<kGroupEwma>(st, seg, nullptr, offsets, B, cls_list, n_cls, nullptr, nullptr, nullptr, nullptr,
+                                        nullptr, reducer, score, launches);
 }
 
 cudaError_t launch_detect_ewma(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase, uint32_t B,

@@ -45,6 +45,19 @@ size_t scan_sync_bytes();   // zero-initialised once; epoch must be > 0 and diff
 cudaError_t launch_group(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets, uint32_t B,
                          const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v, uint32_t *csr_t,
                          uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, int *launches);
+// EWMA scored inside the group kernel: every bucket of the class lists is grouped, time-sorted, reduced and scored in
+// shared memory, and its flagged points (every point with emit_all) go straight to out[0, out_cap); rows past out_cap are
+// counted, not written.  stats[ST_OUTCOUNT] gains the result rows, stats[ST_GSERIES] / [ST_GPOINTS] the series and points.
+// Writes no series entries, per-series arrays or nsb / npb, and never writes over the bucket rows it reads, so a relaunch
+// with the three counters zeroed gives the same rows.
+struct GroupScore {
+    OutCols out;
+    uint32_t out_cap;
+    uint32_t *stats;
+    int emit_all;
+};
+cudaError_t launch_group_ewma(cudaStream_t st, const SegDesc &seg, const uint32_t *offsets, uint32_t B, const uint32_t *cls_list,
+                              const uint32_t n_cls[3], int reducer, const GroupScore &score, int *launches);
 cudaError_t launch_series_scan(cudaStream_t st, const uint32_t *nsb, const uint32_t *npb, uint32_t *sbase, uint32_t B,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);
 cudaError_t launch_detect_ewma(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase, uint32_t B,
