@@ -244,6 +244,42 @@ class Dictionary:
             remap[k] = j
         return remap[codes]
 
+    def encode_block(self, col: "BlockText", idx) -> np.ndarray:
+        """ids of the rows ``idx`` of one block's String column.  Only the block's distinct names that those rows use are
+        looked up (or added), so a name keeps its id across blocks and rounds and no Python string is made per row."""
+        sel = col.ids[idx]
+        used = np.zeros(len(col.names), dtype=bool)
+        used[sel] = True
+        remap = np.zeros(len(col.names), dtype=np.uint32)
+        for k in np.flatnonzero(used):
+            u = col.names[k]
+            j = self.ids.get(u)
+            if j is None:
+                j = self.ids[u] = len(self.names)
+                self.names.append(u)
+            remap[k] = j
+        return remap[sel]
+
+
+class BlockText:
+    """A String column of one Native block as the library's per-block dictionary (``StringColumn.codes()``): ``ids`` per
+    row and the block's distinct ``names``.  Predicates and the job's Dictionary only ever look at the names."""
+
+    def __init__(self, col):
+        self.ids, names = col.codes()
+        self.names = names
+
+    def __len__(self):
+        return len(self.ids)
+
+
+def _text_test(col, test) -> np.ndarray:
+    """``test`` (a vectorised predicate over a numpy str array) for every row of a text column: applied to the column
+    itself, or for a BlockText to its distinct names and spread to the rows through the ids."""
+    if isinstance(col, BlockText):
+        return test(np.asarray(col.names, dtype=str))[col.ids]
+    return test(np.asarray(col).astype(str))
+
 
 def _host_mask(flows: dict, plan: QueryPlan, branch: Branch, pod_label, pod_name, pod_namespace, external_ip,
                svc_port_name) -> np.ndarray:
@@ -253,34 +289,72 @@ def _host_mask(flows: dict, plan: QueryPlan, branch: Branch, pod_label, pod_name
     if plan.agg_flow == "pod":
         side = "destination" if branch.direction == "inbound" else "source"
         if pod_label:
-            lab = np.asarray(flows[side + "PodLabels"]).astype(str)
-            m &= np.char.find(np.char.lower(lab), pod_label.lower()) >= 0        # ilike '%label%'
+            m &= _text_test(flows[side + "PodLabels"],
+                            lambda lab: np.char.find(np.char.lower(lab), pod_label.lower()) >= 0)   # ilike '%label%'
         elif pod_name:
-            m &= np.asarray(flows[side + "PodName"]).astype(str) == pod_name
+            m &= _text_test(flows[side + "PodName"], lambda s: s == pod_name)
         else:
-            m &= np.asarray(flows[side + "PodLabels"]).astype(str) != ""
+            m &= _text_test(flows[side + "PodLabels"], lambda s: s != "")
         if pod_namespace and (pod_label or pod_name):
-            m &= np.asarray(flows[side + "PodNamespace"]).astype(str) == pod_namespace
+            m &= _text_test(flows[side + "PodNamespace"], lambda s: s == pod_namespace)
     elif plan.agg_flow == "external":
         m &= np.asarray(flows["flowType"]) == 3
         if external_ip:
-            dst = np.asarray(flows["destinationIP"])
-            if dst.dtype.kind in "iu":                                # already the u32 key column (Native transport)
+            dst = flows["destinationIP"]
+            if not isinstance(dst, BlockText) and np.asarray(dst).dtype.kind in "iu":   # u32 key column (Native transport)
                 try:
-                    m &= dst == ip_to_u32([external_ip])[0]
+                    m &= np.asarray(dst) == ip_to_u32([external_ip])[0]
                 except ValueError:
                     m &= False                                        # an IPv6 literal never equals an IPv4 column
             else:
-                m &= dst.astype(str) == external_ip                   # destinationIP = '...' (:590-592)
+                m &= _text_test(dst, lambda s: s == external_ip)      # destinationIP = '...' (:590-592)
     elif plan.agg_flow == "svc":
-        svc = np.asarray(flows["destinationServicePortName"]).astype(str)
-        m &= (svc == svc_port_name) if svc_port_name else (svc != "")
+        m &= _text_test(flows["destinationServicePortName"], (lambda s: s == svc_port_name) if svc_port_name
+                        else (lambda s: s != ""))
     if plan.start_time and "flow_start" not in branch.key and flows.get("flowStartSeconds") is not None:
         # external / svc: flowStartSeconds >= start is a WHERE condition (anomaly_detection.py:581-583) on a column
         # that is not part of the key, so it cannot ride the engine's key column: filter here.  A table that does
         # not carry the column came from raw_select_sql, whose WHERE clause already applied the same condition.
         m &= np.asarray(flows["flowStartSeconds"]).astype(np.int64) >= _epoch(plan.start_time)
     return m
+
+
+def _dictionary_ids(col, idx, dictionary: Dictionary) -> np.ndarray:
+    if isinstance(col, BlockText):
+        return dictionary.encode_block(col, idx)
+    return dictionary.encode(np.asarray(col)[idx])
+
+
+def _branch_columns(flows: dict, plan: QueryPlan, br: Branch, masks: tuple, dicts: dict, ns_dict: Dictionary,
+                    ipv4_as_u32: bool) -> dict:
+    """One branch's engine columns from a flows table or one block of it: the host predicates, then key slots,
+    ``flow_end`` / ``value`` and, with an ignore list, the namespace ids.  ``ipv4_as_u32``: an address column of IPv4 text
+    becomes its u32 value (a whole table); otherwise text addresses go through the dictionary like every other String
+    key, which keeps a name's id the same in every block of a stream."""
+    idx = np.flatnonzero(_host_mask(flows, plan, br, *masks))
+    cols = {}
+    for slot in KEY_SLOTS:
+        src = br.key.get(slot)
+        if src is None:
+            cols[slot] = None
+        elif isinstance(src, tuple):
+            cols[slot] = np.full(len(idx), src[1], dtype=np.uint32)
+        elif isinstance(flows[src], BlockText):
+            cols[slot] = dicts[slot].encode_block(flows[src], idx)
+        else:
+            raw = np.asarray(flows[src])[idx]
+            if src in ("sourceIP", "destinationIP") and ipv4_as_u32:
+                cols[slot] = encode_ip_column(raw, dicts[slot])
+            elif raw.dtype.kind in "iu":
+                cols[slot] = raw
+            else:
+                cols[slot] = dicts[slot].encode(raw)
+    cols["flow_end"] = np.asarray(flows["flowEndSeconds"])[idx]
+    cols["value"] = np.asarray(flows["throughput"])[idx]
+    if plan.ns_ignore:
+        cols["src_ns"] = _dictionary_ids(flows["sourcePodNamespace"], idx, ns_dict)
+        cols["dst_ns"] = _dictionary_ids(flows["destinationPodNamespace"], idx, ns_dict)
+    return cols
 
 
 def anomaly_detection(engine, algo_type: str, flows: dict, start_time: str = "", end_time: str = "", tad_id: str = "",
@@ -304,31 +378,8 @@ def run_engine(engine, algo_type: str, flows: dict, start_time: str = "", end_ti
                       pod_namespace)
     dicts = {slot: Dictionary() for slot in KEY_SLOTS}
     ns_dict = Dictionary()
-    parts = []
-    for br in plan.branches:
-        mask = _host_mask(flows, plan, br, pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
-        idx = np.flatnonzero(mask)
-        cols = {}
-        for slot in KEY_SLOTS:
-            src = br.key.get(slot)
-            if src is None:
-                cols[slot] = None
-            elif isinstance(src, tuple):
-                cols[slot] = np.full(len(idx), src[1], dtype=np.uint32)
-            else:
-                raw = np.asarray(flows[src])[idx]
-                if src in ("sourceIP", "destinationIP"):
-                    cols[slot] = encode_ip_column(raw, dicts[slot])
-                elif raw.dtype.kind in "iu":
-                    cols[slot] = raw
-                else:
-                    cols[slot] = dicts[slot].encode(raw)
-        cols["flow_end"] = np.asarray(flows["flowEndSeconds"])[idx]
-        cols["value"] = np.asarray(flows["throughput"])[idx]
-        if plan.ns_ignore:
-            cols["src_ns"] = ns_dict.encode(np.asarray(flows["sourcePodNamespace"])[idx])
-            cols["dst_ns"] = ns_dict.encode(np.asarray(flows["destinationPodNamespace"])[idx])
-        parts.append(cols)
+    masks = (pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
+    parts = [_branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=True) for br in plan.branches]
     table = {}
     for k in parts[0]:
         if any(p[k] is None for p in parts):
@@ -344,6 +395,69 @@ def run_engine(engine, algo_type: str, flows: dict, start_time: str = "", end_ti
     kw = {} if on_job is None else {"on_job": on_job}      # progress hook of the controller (tad_poll while the job runs)
     got, st = engine.run(table, algo=algo_type, reducer=plan.reducer, start_time=start,
                          end_time=_epoch(plan.end_time), tad_id=tad_id, ns_ignore=ignore_ids, **kw)
+    return got, st, plan, dicts
+
+
+def _block_table(block: dict) -> dict:
+    """A decoded Native block (``{column: numpy array or StringColumn}``) with every String column as a BlockText."""
+    out = {}
+    for k, v in block.items():
+        if isinstance(v, tuple):
+            raise NotImplementedError("Nullable columns are not part of the flows schema")
+        out[k] = BlockText(v) if hasattr(v, "codes") else v
+    return out
+
+
+def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_time: str = "", tad_id: str = "",
+                      ns_ignore_list=(), agg_flow=None, pod_label=None, external_ip=None, svc_port_name=None,
+                      pod_name=None, pod_namespace=None, rows_hint: int = 0, on_job=None):
+    """:func:`run_engine` over streamed input: ``blocks()`` yields one round of decoded Native blocks
+    (``{column: numpy array or clickhouse_native.StringColumn}``, as ``read_blocks`` / ``read_blocks_stream`` yield them)
+    and is called again for every round the engine asks for.  Each block's branches are pushed as they are built (two
+    blocks per source block in ``pod`` mode); blocks are never concatenated, and only the engine's one block of
+    look-ahead stays referenced.  String keys, text addresses included, go through the job's dictionaries, so a value has
+    the same id in every block and round; the namespace dictionary starts with the ignore list, whose ids the job spec
+    needs at submit.  ``rows_hint``: one round's rows (0 = unknown).  Returns (result SoA, status, plan, dictionaries)."""
+    if algo_type not in VALID_ALGOS:
+        raise ValueError("Algorithm should be in {}".format(" or ".join(VALID_ALGOS)))
+    plan = plan_query(start_time, end_time, ns_ignore_list, agg_flow, pod_label, external_ip, svc_port_name, pod_name,
+                      pod_namespace)
+    dicts = {slot: Dictionary() for slot in KEY_SLOTS}
+    ns_dict = Dictionary()
+    ignore = [str(x) for x in plan.ns_ignore]
+    ns_dict.encode(np.asarray(ignore, dtype=object))
+    ignore_ids = sorted({ns_dict.ids[x] for x in ignore})
+    masks = (pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
+    # as in run_engine: the window's lower bound reaches the engine only through a flow_start key column
+    start = _epoch(plan.start_time) if all("flow_start" in br.key for br in plan.branches) else 0
+    job = engine.submit_stream(algo=algo_type, reducer=plan.reducer, start_time=start, end_time=_epoch(plan.end_time),
+                               tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint))
+    if on_job is not None:
+        on_job(job)
+    try:
+        rounds, again = 0, True
+        while again:
+            for block in blocks():
+                flows = _block_table(block)
+                del block
+                for br in plan.branches:
+                    cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False)
+                    if len(cols["flow_end"]):
+                        job.push(cols)
+                    del cols
+                del flows
+            again = job.end()
+            rounds += 1
+        st = job.wait()
+        st["rounds"] = rounds
+        got = job.result()
+    except BaseException:
+        job.cancel()
+        raise
+    finally:
+        if on_job is not None:
+            on_job(None)
+        job.release()
     return got, st, plan, dicts
 
 
@@ -549,6 +663,10 @@ class ClickHouseHTTP:
                 m = re.search(r"Code:\s*(\d+)", text)
                 raise ClickHouseError(int(m.group(1)) if m else -1, text)
 
+    def count(self, sql: str) -> int:
+        """The value of a ``SELECT count() ...`` (the rows hint of a streamed job)."""
+        return int(self._post(sql.rstrip() + " FORMAT TabSeparated").strip() or 0)
+
     def insert_native(self, table: str, block: bytes) -> None:
         self._post("INSERT INTO %s FORMAT Native" % table, block)
 
@@ -581,13 +699,60 @@ def raw_select_sql(plan: QueryPlan, pod_label=None, pod_name=None, pod_namespace
         # of text -- text addresses cap the host-side ingest at ~1e7 rows/s per core.  IPv4StringToNum throws on anything
         # else, so a dual-stack table fails the query and the job is rerun in text mode.
         cols = ["IPv4StringToNum({0}) AS {0}".format(c) if c in ("sourceIP", "destinationIP") else c for c in cols]
-    sql = "SELECT {} FROM {}".format(", ".join(cols), TABLE_NAME)
+    return "SELECT {} FROM {}".format(", ".join(cols), TABLE_NAME) + _window_where(plan)
+
+
+def _window_where(plan: QueryPlan) -> str:
     where = []
     if plan.start_time:
         where.append("flowStartSeconds >= '{}'".format(plan.start_time))
     if plan.end_time:
         where.append("flowEndSeconds < '{}'".format(plan.end_time))
-    return sql + (" WHERE " + " AND ".join(where) if where else "")
+    return " WHERE " + " AND ".join(where) if where else ""
+
+
+def count_sql(plan: QueryPlan) -> str:
+    """``SELECT count()`` over the window :func:`raw_select_sql` reads: the rows of one streamed round, before the host
+    predicates (an upper bound, which the engine accepts as a hint)."""
+    return "SELECT count() FROM {}".format(TABLE_NAME) + _window_where(plan)
+
+
+def _select_blocks(transport, sql: str):
+    """Factory of one round of the SELECT's decoded Native blocks; every call issues the SELECT again."""
+    from . import clickhouse_native as chn
+
+    def blocks():
+        if hasattr(transport, "select_native_stream"):
+            decoded = chn.read_blocks_stream(transport.select_native_stream(sql))
+        else:
+            decoded = chn.read_blocks(transport.select_native(sql))
+        for cols, _types, _rows in decoded:
+            yield cols
+    return blocks
+
+
+def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str):
+    """main()'s job on streamed input (TAD_STREAM_INPUT=1): (result SoA, plan, dictionaries)."""
+    hint = 0
+    if hasattr(transport, "count"):
+        hint = int(transport.count(count_sql(plan))) * len(plan.branches)    # pod: every row feeds both branches
+    if os.getenv("TAD_HOST_BUDGET") is not None:
+        engine.set_host_budget(int(os.getenv("TAD_HOST_BUDGET")))
+
+    def run(ipv4_pushdown):
+        sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=ipv4_pushdown)
+        return run_engine_stream(engine, a["algo"], _select_blocks(transport, sql), a["start_time"], a["end_time"], tad_id,
+                                 a["ns_ignore_list"], a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
+                                 a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None, rows_hint=hint)
+    try:
+        got, _st, plan, dicts = run(pushdown)
+    except Exception as e:
+        if not pushdown or not _is_ipv4_pushdown_failure(e):
+            raise
+        # ClickHouse may reject a non-IPv4 address after some blocks were pushed: that job was cancelled and released
+        logger.info("IPv4 push-down failed (non-IPv4 addresses?): rerunning the job with the addresses as text")
+        got, _st, plan, dicts = run(False)
+    return got, plan, dicts
 
 
 def main(argv=None, engine=None, transport=None) -> int:
@@ -612,25 +777,29 @@ def main(argv=None, engine=None, transport=None) -> int:
         plan = plan_query(a["start_time"], a["end_time"], a["ns_ignore_list"], a["agg_flow"], a["pod_label"], a["external_ip"],
                           a["svc_port_name"], a["pod_name"], a["pod_namespace"])
         pushdown = os.getenv("TAD_IPV4_PUSHDOWN", "0") == "1"
-        sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=pushdown)
-        def read(q):          # block-by-block while the response arrives when the transport can stream, else the whole body
-            if hasattr(transport, "select_native_stream"):
-                return chn.flows_from_native(transport.select_native_stream(q))
-            return chn.flows_from_native(transport.select_native(q))
-        try:
-            flows = read(sql)
-        except Exception as e:
-            if not pushdown or not _is_ipv4_pushdown_failure(e):
-                raise
-            logger.info("IPv4 push-down failed (non-IPv4 addresses?): reading the addresses as text")
-            sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"])
-            flows = read(sql)
-        for c in (x.split(" AS ")[-1] for x in sql[len("SELECT "):sql.index(" FROM ")].split(", ")):   # empty table: no block at all
-            flows.setdefault(c, np.zeros(0, dtype=np.uint64 if c == "throughput" else np.uint32))
-        tad_id = a["id"] or str(uuid.uuid4())                               # write_anomaly_detection_result (:715-718)
-        got, _st, plan, dicts = run_engine(engine, a["algo"], flows, a["start_time"], a["end_time"], tad_id, a["ns_ignore_list"],
-                                           a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
-                                           a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None)
+        if os.getenv("TAD_STREAM_INPUT", "0") == "1":       # blocks pushed to a streamed job as they are decoded
+            tad_id = a["id"] or str(uuid.uuid4())
+            got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id)
+        else:
+            sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=pushdown)
+            def read(q):          # block-by-block while the response arrives when the transport can stream, else the whole body
+                if hasattr(transport, "select_native_stream"):
+                    return chn.flows_from_native(transport.select_native_stream(q))
+                return chn.flows_from_native(transport.select_native(q))
+            try:
+                flows = read(sql)
+            except Exception as e:
+                if not pushdown or not _is_ipv4_pushdown_failure(e):
+                    raise
+                logger.info("IPv4 push-down failed (non-IPv4 addresses?): reading the addresses as text")
+                sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"])
+                flows = read(sql)
+            for c in (x.split(" AS ")[-1] for x in sql[len("SELECT "):sql.index(" FROM ")].split(", ")):   # empty table: no block at all
+                flows.setdefault(c, np.zeros(0, dtype=np.uint64 if c == "throughput" else np.uint32))
+            tad_id = a["id"] or str(uuid.uuid4())                               # write_anomaly_detection_result (:715-718)
+            got, _st, plan, dicts = run_engine(engine, a["algo"], flows, a["start_time"], a["end_time"], tad_id, a["ns_ignore_list"],
+                                               a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
+                                               a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None)
         if len(got["flow_end"]):                                           # column-wise: no Python object per result row
             block = chn.tadetector_block_from_result(got, plan, dicts, a["algo"], tad_id)
         else:                                                               # the NO ANOMALY DETECTED sentinel (:395-420)
