@@ -272,6 +272,36 @@ int tad_stream_push(tad_job *job, const tad_columns *block);
  * must be pushed again for another pass, 0 when the input is complete.  again may be NULL. */
 int tad_stream_end(tad_job *job, int32_t *again);
 
+/* ---- Text key slots of streamed blocks ---------------------------------------------------------------------------
+ * Replaces: the host dictionary pass over sourceIP / destinationIP String columns (create_table.sh:38-39) that turns
+ * IPv6 and other non-IPv4 text into key ids before tad_stream_push.  A text column is a Native String column exactly as
+ * it sits in the block: `rows` x (VarUInt length, bytes), `nbytes` long, and marks[k] = the byte offset of row 32k
+ * (ceil(rows / 32) marks, marks[0] = 0).  The engine decodes it and dictionary-encodes it on the GPU into job-stable u32
+ * ids, dense and in order of first appearance (over the round's rows, in push order, then row order: the ids a host
+ * dictionary built the same way gives), so every round and pass of a job keys the same name alike.  The dictionary and
+ * the text staging count against tad_set_memory_budget and in tad_job_memory's peak; a first round whose dictionary
+ * leaves no room for its pass columns only counts its rows (one more round is asked for), and a dictionary that does not
+ * fit by itself fails the job with TAD_ERR_NOMEM. */
+typedef struct {
+    const uint8_t *bytes;      /* the column's bytes (host memory)                                                   */
+    uint64_t nbytes;
+    const uint64_t *marks;     /* ceil(rows / 32) byte offsets: of rows 0, 32, 64, ...                               */
+} tad_text_column;
+/* tad_stream_push with src_ip / dst_ip given as text: a NULL text pointer means that slot comes from `block` as for
+ * tad_stream_push; a slot given as text must have its u32 column NULL.  Which slots are text is part of the job's column
+ * set: every block must make its first block's choice.  Text is accepted in host blocks (mem = TAD_MEM_HOST) only.  A
+ * block that breaks one of these, marks that decrease or pass nbytes, or (found on the GPU, reported by this call or a
+ * later push / end call) VarUInt lengths that do not end exactly at the next mark fail the job with
+ * TAD_ERR_INVALID_ARG.  TAD_ERR_UNSUPPORTED for a job not submitted with tad_submit_stream (tad_submit_stream itself is
+ * single-GPU only).  The block and its text columns must stay valid and unchanged until the next push or end call
+ * returns.  Errors and threads otherwise as for tad_stream_push. */
+int tad_stream_push_text(tad_job *job, const tad_columns *block, const tad_text_column *src_ip,
+                         const tad_text_column *dst_ip);
+/* For a COMPLETED job: the dictionary of text slot `slot` (0 = src_ip, 1 = dst_ip): the name of id k is
+ * bytes[offsets[k] .. offsets[k + 1]), *count names, in host memory owned by the job until tad_release.
+ * TAD_ERR_STATE before completion and for a slot the job did not take as text.  Any thread. */
+int tad_job_names(tad_job *job, int32_t slot, const uint8_t **bytes, const uint64_t **offsets, uint32_t *count);
+
 const char *tad_strerror(int err);
 int tad_abi_version(void);
 
@@ -298,6 +328,11 @@ int tad_ch_parse_ipv4(const uint8_t *buf, const uint64_t *offsets, const uint32_
 /* u32 -> String column bytes (VarUInt length + "a.b.c.d" per row) for the tadetector INSERT (create_table.sh:363-384).
  * Needs at most 16 bytes per row; TAD_ERR_INVALID_ARG if out_cap is too small. */
 int tad_ch_format_ipv4(const uint32_t *ips, uint64_t rows, uint8_t *out, size_t out_cap, size_t *written);
+/* Dictionary ids -> String column bytes (VarUInt length + name per row) for the tadetector INSERT, the name of id k being
+ * bytes[offsets[k] .. offsets[k + 1]) (tad_job_names).  TAD_ERR_INVALID_ARG for an id >= count or when out_cap is too
+ * small; *written = the bytes written. */
+int tad_ch_format_names(const uint8_t *bytes, const uint64_t *offsets, uint32_t count, const uint32_t *ids, uint64_t rows,
+                        uint8_t *out, size_t out_cap, size_t *written);
 
 /* Dense dictionary ids (order of first appearance) for a String column: ids[i] in [0, *n_unique); first_row[k] is the
  * row at which id k first occurs (the caller reads the k-th name from there).  first_row needs room for `rows` entries.

@@ -21,7 +21,8 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_free_columns", "tad_submit", "tad_poll", "tad_wait", "tad_result", "tad_cancel",
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
-           "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory")
+           "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
+           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names")
 
 
 class TadConfig(C.Structure):
@@ -34,6 +35,10 @@ class TadColumns(C.Structure):
                 ("src_ip", C.c_void_p), ("dst_ip", C.c_void_p), ("src_port", C.c_void_p), ("dst_port", C.c_void_p),
                 ("proto", C.c_void_p), ("flow_start", C.c_void_p), ("flow_end", C.c_void_p), ("value", C.c_void_p),
                 ("src_ns", C.c_void_p), ("dst_ns", C.c_void_p)]
+
+
+class TadTextColumn(C.Structure):
+    _fields_ = [("bytes", C.c_void_p), ("nbytes", C.c_uint64), ("marks", C.c_void_p)]
 
 
 class TadJobSpec(C.Structure):
@@ -82,6 +87,8 @@ def load():
     L.tad_submit_stream.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(C.c_void_p)]
     L.tad_stream_push.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_stream_end.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+    L.tad_stream_push_text.argtypes = [C.c_void_p, C.POINTER(TadColumns), C.POINTER(TadTextColumn), C.POINTER(TadTextColumn)]
+    L.tad_job_names.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
     L.tad_poll.argtypes = [C.c_void_p, C.POINTER(TadStatus)]
     L.tad_wait.argtypes = [C.c_void_p, C.c_int64, C.POINTER(TadStatus)]
     L.tad_result.argtypes = [C.c_void_p, C.POINTER(TadRows)]
@@ -95,6 +102,8 @@ def load():
     L.tad_ch_string_index.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
     L.tad_ch_parse_ipv4.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
     L.tad_ch_format_ipv4.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.tad_ch_format_names.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t,
+                                      C.POINTER(C.c_size_t)]
     L.tad_ch_dictionary.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
     _lib = L
     return L

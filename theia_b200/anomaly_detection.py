@@ -326,16 +326,17 @@ def _dictionary_ids(col, idx, dictionary: Dictionary) -> np.ndarray:
 
 
 def _branch_columns(flows: dict, plan: QueryPlan, br: Branch, masks: tuple, dicts: dict, ns_dict: Dictionary,
-                    ipv4_as_u32: bool) -> dict:
+                    ipv4_as_u32: bool, text_slots=()) -> dict:
     """One branch's engine columns from a flows table or one block of it: the host predicates, then key slots,
     ``flow_end`` / ``value`` and, with an ignore list, the namespace ids.  ``ipv4_as_u32``: an address column of IPv4 text
     becomes its u32 value (a whole table); otherwise text addresses go through the dictionary like every other String
-    key, which keeps a name's id the same in every block of a stream."""
+    key, which keeps a name's id the same in every block of a stream.  ``text_slots``: key slots the engine encodes from
+    the block's text itself (left None here)."""
     idx = np.flatnonzero(_host_mask(flows, plan, br, *masks))
     cols = {}
     for slot in KEY_SLOTS:
         src = br.key.get(slot)
-        if src is None:
+        if src is None or slot in text_slots:
             cols[slot] = None
         elif isinstance(src, tuple):
             cols[slot] = np.full(len(idx), src[1], dtype=np.uint32)
@@ -410,14 +411,20 @@ def _block_table(block: dict) -> dict:
 
 def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_time: str = "", tad_id: str = "",
                       ns_ignore_list=(), agg_flow=None, pod_label=None, external_ip=None, svc_port_name=None,
-                      pod_name=None, pod_namespace=None, rows_hint: int = 0, on_job=None):
+                      pod_name=None, pod_namespace=None, rows_hint: int = 0, on_job=None, device_text: bool = False):
     """:func:`run_engine` over streamed input: ``blocks()`` yields one round of decoded Native blocks
     (``{column: numpy array or clickhouse_native.StringColumn}``, as ``read_blocks`` / ``read_blocks_stream`` yield them)
     and is called again for every round the engine asks for.  Each block's branches are pushed as they are built (two
     blocks per source block in ``pod`` mode); blocks are never concatenated, and only the engine's one block of
     look-ahead stays referenced.  String keys, text addresses included, go through the job's dictionaries, so a value has
     the same id in every block and round; the namespace dictionary starts with the ignore list, whose ids the job spec
-    needs at submit.  ``rows_hint``: one round's rows (0 = unknown).  Returns (result SoA, status, plan, dictionaries)."""
+    needs at submit.  ``rows_hint``: one round's rows (0 = unknown).  Returns (result SoA, status, plan, dictionaries).
+
+    ``device_text``: in connection mode, the two address columns go to the engine as the block's String column bytes
+    (``StringColumn.text()``, tad_stream_push_text) and are dictionary-encoded on the GPU; their dictionaries come back
+    as ``clickhouse_native.Names`` (tad_job_names).  Connection mode is the one mode whose host mask keeps every row and
+    reads no key text; the pod / svc / external modes keep their host encoding whatever ``device_text`` says."""
+    from .clickhouse_native import Names
     if algo_type not in VALID_ALGOS:
         raise ValueError("Algorithm should be in {}".format(" or ".join(VALID_ALGOS)))
     plan = plan_query(start_time, end_time, ns_ignore_list, agg_flow, pod_label, external_ip, svc_port_name, pod_name,
@@ -430,6 +437,8 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
     masks = (pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
     # as in run_engine: the window's lower bound reaches the engine only through a flow_start key column
     start = _epoch(plan.start_time) if all("flow_start" in br.key for br in plan.branches) else 0
+    text = {"src_ip": "sourceIP", "dst_ip": "destinationIP"} if device_text and not plan.agg_flow else {}
+    pushed_text = False
     job = engine.submit_stream(algo=algo_type, reducer=plan.reducer, start_time=start, end_time=_epoch(plan.end_time),
                                tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint))
     if on_job is not None:
@@ -438,12 +447,17 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
         rounds, again = 0, True
         while again:
             for block in blocks():
-                flows = _block_table(block)
+                raw = {slot: block[c] for slot, c in text.items()}
+                flows = _block_table({k: v for k, v in block.items() if k not in text.values()})
                 del block
                 for br in plan.branches:
-                    cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False)
+                    cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False, text_slots=raw)
                     if len(cols["flow_end"]):
-                        job.push(cols)
+                        if raw:
+                            job.push(cols, text={slot: col.text() for slot, col in raw.items()})
+                            pushed_text = True
+                        else:
+                            job.push(cols)
                     del cols
                 del flows
             again = job.end()
@@ -451,6 +465,9 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
         st = job.wait()
         st["rounds"] = rounds
         got = job.result()
+        if pushed_text:
+            for slot in text:
+                dicts[slot] = Names(*job.names(slot))
     except BaseException:
         job.cancel()
         raise
@@ -731,8 +748,9 @@ def _select_blocks(transport, sql: str):
     return blocks
 
 
-def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str):
-    """main()'s job on streamed input (TAD_STREAM_INPUT=1): (result SoA, plan, dictionaries)."""
+def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str, device_text: bool = False):
+    """main()'s job on streamed input (TAD_STREAM_INPUT=1): (result SoA, plan, dictionaries).  ``device_text``
+    (TAD_DEVICE_TEXT=1, text addresses only): run_engine_stream's ``device_text``."""
     hint = 0
     if hasattr(transport, "count"):
         hint = int(transport.count(count_sql(plan))) * len(plan.branches)    # pod: every row feeds both branches
@@ -743,7 +761,8 @@ def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, t
         sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=ipv4_pushdown)
         return run_engine_stream(engine, a["algo"], _select_blocks(transport, sql), a["start_time"], a["end_time"], tad_id,
                                  a["ns_ignore_list"], a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
-                                 a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None, rows_hint=hint)
+                                 a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None, rows_hint=hint,
+                                 device_text=device_text and not ipv4_pushdown)
     try:
         got, _st, plan, dicts = run(pushdown)
     except Exception as e:
@@ -779,7 +798,9 @@ def main(argv=None, engine=None, transport=None) -> int:
         pushdown = os.getenv("TAD_IPV4_PUSHDOWN", "0") == "1"
         if os.getenv("TAD_STREAM_INPUT", "0") == "1":       # blocks pushed to a streamed job as they are decoded
             tad_id = a["id"] or str(uuid.uuid4())
-            got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id)
+            # TAD_DEVICE_TEXT=1: the address text of a connection-mode job is dictionary-encoded on the GPU (no push-down)
+            device_text = os.getenv("TAD_DEVICE_TEXT", "0") == "1" and not pushdown
+            got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id, device_text)
         else:
             sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=pushdown)
             def read(q):          # block-by-block while the response arrives when the transport can stream, else the whole body

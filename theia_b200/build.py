@@ -6,7 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtheia_tad.so")
-SOURCES = ["tad_kernels.cu", "tad_spill.cu", "tad_scan.cu", "tad_arima.cu", "tad_engine.cu", "tad_nccl.cu", "tad_chnative.cu"]
+SOURCES = ["tad_kernels.cu", "tad_spill.cu", "tad_scan.cu", "tad_arima.cu", "tad_engine.cu", "tad_nccl.cu", "tad_chnative.cu",
+           "tad_text.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wno-format-truncation"]
 

@@ -44,8 +44,9 @@ _FIXED = {
 class StringColumn:
     """A String column kept as (buffer, offsets, lengths): rows are decoded only when asked for."""
 
-    def __init__(self, buf, offsets: np.ndarray, lengths: np.ndarray):
+    def __init__(self, buf, offsets: np.ndarray, lengths: np.ndarray, start: int = 0, end: int | None = None):
         self.buf, self.offsets, self.lengths = buf, offsets, lengths
+        self.start, self.end = start, end       # the column's byte span in ``buf`` (as read from a block)
 
     def __len__(self):
         return len(self.offsets)
@@ -71,6 +72,18 @@ class StringColumn:
             if rc != 0:
                 raise ValueError("tad_ch_parse_ipv4 failed (%d)" % rc)
         return out, ok.astype(bool)
+
+    def text(self):
+        """(column bytes, marks): the column exactly as it sits in its Native block, and the byte offset of rows 0, 32,
+        64, ... in it -- a text key slot of ``StreamJob.push`` (tad_stream_push_text).  Both come from the index the
+        reader already built."""
+        end = self.end if self.end is not None else (int(self.offsets[-1]) + int(self.lengths[-1]) if len(self) else self.start)
+        data = np.frombuffer(self.buf, dtype=np.uint8)[self.start:end]
+        lens = self.lengths[::32].astype(np.uint64)
+        vlen = np.ones(len(lens), dtype=np.uint64)
+        for bits in (7, 14, 21, 28):
+            vlen += lens >= np.uint64(1 << bits)
+        return data, self.offsets[::32] - vlen - np.uint64(self.start)
 
     def codes(self):
         """(ids, names): dense dictionary ids in order of first appearance -- the shim's per-job string dictionary
@@ -133,7 +146,7 @@ def _read_data(buf, p: int, typ: str, rows: int):
                                             C.byref(used))
         if rc != 0:
             raise ValueError("truncated or malformed String column")
-        return StringColumn(buf, offsets + np.uint64(p), lengths), p + used.value
+        return StringColumn(buf, offsets + np.uint64(p), lengths, p, p + used.value), p + used.value
     m = re.fullmatch(r"FixedString\((\d+)\)", typ)
     if m:
         w = int(m.group(1))
@@ -364,6 +377,31 @@ def _string_column_bytes(values=None, const=None, rows=0, ids=None, names=None) 
     return b"".join(enc[np.asarray(ids, dtype=np.int64)].tolist())
 
 
+class Names:
+    """A dictionary as one byte array and offsets (``StreamJob.names``): the name of id k is data[offsets[k]:offsets[k+1]]."""
+
+    def __init__(self, data, offsets):
+        self.data = np.ascontiguousarray(data, dtype=np.uint8)
+        self.offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+
+
+def format_names(names: Names, ids) -> bytes:
+    """String column bytes of ``names`` at ``ids`` (tad_ch_format_names): no Python object per name or row."""
+    ids = np.ascontiguousarray(ids, dtype=np.uint32)
+    count = len(names.offsets) - 1
+    # capacity only: an id past the dictionary is rejected by the library call
+    lens = np.diff(names.offsets)[np.minimum(ids, count - 1)] if len(ids) and count > 0 else np.zeros(1, dtype=np.uint64)
+    cap = int(lens.sum()) + 10 * len(ids) + 1
+    out = np.empty(cap, dtype=np.uint8)
+    used = C.c_size_t(0)
+    data = names.data if len(names.data) else np.zeros(1, dtype=np.uint8)
+    rc = _lib.load().tad_ch_format_names(data.ctypes.data, names.offsets.ctypes.data, count, ids.ctypes.data, len(ids),
+                                         out.ctypes.data, cap, C.byref(used))
+    if rc != 0:
+        raise ValueError("tad_ch_format_names failed (%d): an id past the dictionary" % rc)
+    return out[:used.value].tobytes()
+
+
 def tadetector_block_from_result(got: dict, plan, dicts: dict, algo_type: str, tad_id: str) -> bytes:
     """The same INSERT body as ``tadetector_block(_result_rows(...))`` (theia_b200/anomaly_detection.py), built column-wise
     from the engine's result arrays: no per-row dicts, so a job with millions of anomalous points stays array-speed.  The
@@ -375,6 +413,8 @@ def tadetector_block_from_result(got: dict, plan, dicts: dict, algo_type: str, t
 
     def ip_col(slot):
         d = dicts[slot]
+        if isinstance(d, Names):                                # a device dictionary (text key slot)
+            return ("names", got[slot], d)
         if d.names:                                             # the column went through the dictionary (non-IPv4 text)
             return ("ids", np.asarray(got[slot]), list(d.names))
         return ("ipv4", np.ascontiguousarray(got[slot], dtype=np.uint32), None)
@@ -414,6 +454,8 @@ def tadetector_block_from_result(got: dict, plan, dicts: dict, algo_type: str, t
                 out.append(b"\x00" * n)                          # '' : the table default
             elif spec[0] == "const":
                 out.append(_string_column_bytes(const=spec[1], rows=n))
+            elif spec[0] == "names":
+                out.append(format_names(spec[2], spec[1]))
             elif spec[0] == "ipv4":
                 buf = np.empty(16 * n + 16, dtype=np.uint8)
                 used = C.c_size_t(0)

@@ -101,6 +101,31 @@ int tad_ch_format_ipv4(const uint32_t *ips, uint64_t rows, uint8_t *out, size_t 
     return TAD_OK;
 }
 
+int tad_ch_format_names(const uint8_t *bytes, const uint64_t *offsets, uint32_t count, const uint32_t *ids, uint64_t rows,
+                        uint8_t *out, size_t out_cap, size_t *written)
+{
+    if ((rows && (!ids || !offsets || !bytes)) || (!out && out_cap) || !written) return TAD_ERR_INVALID_ARG;
+    size_t p = 0;
+    for (uint64_t i = 0; i < rows; i++) {
+        const uint32_t id = ids[i];
+        if (id >= count || offsets[id + 1] < offsets[id]) return TAD_ERR_INVALID_ARG;
+        uint64_t n = offsets[id + 1] - offsets[id];
+        uint8_t len[10];
+        int k = 0;
+        do {
+            len[k++] = (uint8_t)((n & 0x7f) | (n >= 0x80 ? 0x80 : 0));
+            n >>= 7;
+        } while (n);
+        n = offsets[id + 1] - offsets[id];
+        if (out_cap - p < k || out_cap - p - k < n) return TAD_ERR_INVALID_ARG;
+        memcpy(out + p, len, k);
+        if (n) memcpy(out + p + k, bytes + offsets[id], n);
+        p += k + n;
+    }
+    *written = p;
+    return TAD_OK;
+}
+
 int tad_ch_dictionary(const uint8_t *buf, const uint64_t *offsets, const uint32_t *lengths, uint64_t rows, uint32_t *ids,
                       uint64_t *first_row, uint32_t *n_unique)
 {

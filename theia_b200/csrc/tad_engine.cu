@@ -21,6 +21,7 @@
 #include "../../include/theia_tad.h"
 #include "tad_kernels.h"
 #include "tad_nccl.h"
+#include "tad_text.h"
 
 using namespace tad;
 
@@ -161,10 +162,16 @@ struct tad_job {
         bool round_done = false;     // the worker finished with the round; `again` is valid
         bool again = false;
         bool input_done = false;     // tad_stream_end returned again = 0
+        tad_text_column txt[2]{};    // the handed-over block's text slots (tad_stream_push_text)
         uint64_t pushed = 0, taken = 0, released = 0;   // blocks handed over / taken / no longer read by the engine
         int err = 0;                 // a bad block: the worker fails the job with this code and message
         char msg[200] = {0};
     } in;
+    // text key slots (tad_stream_push_text): src_ip / dst_ip arrive as Native String bytes and are dictionary-encoded
+    // on the device; set by the first block.  On completion each slot's dictionary is copied here (tad_job_names).
+    bool text[2] = {false, false};
+    std::vector<uint8_t> names[2];
+    std::vector<uint64_t> names_off[2];
 };
 
 struct tad_ctx {
@@ -229,6 +236,13 @@ struct tad_ctx {
     cudaEvent_t ost_ev[2]{};                        // out-stage half free again (its copies to the store are done)
     cudaEvent_t cnt_ev[2]{};                        // a chunk's residue counts have reached h_chunk
     uint32_t *h_chunk = nullptr;                    // pinned, 2 x 64: rows per residue of the last two chunks
+    // text key slots (DESIGN.md section 10, "Text keys on the device"): one dictionary per slot, alive for one job
+    struct TextSlot {
+        DevBuf slots, minrow, slot_id, arena, off, hash, state;
+        uint32_t cap = 0;                           // table slots (0: no dictionary yet)
+        uint64_t names_ub = 0, bytes_ub = 0;        // upper bounds of its names / arena bytes, exact after each readback
+    } tdict[2];
+    DevBuf tstage, tscratch;                        // a chunk's marks and text bytes; the encode scratch
 };
 
 namespace {
@@ -306,7 +320,9 @@ std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
                                &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx, &ctx->dbi, &ctx->exch,
                                &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total, &ctx->entries,
                                &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
-                               &ctx->stage, &ctx->pcnt, &ctx->ostage};
+                               &ctx->stage, &ctx->pcnt, &ctx->ostage, &ctx->tstage, &ctx->tscratch};
+    for (auto &t : ctx->tdict)
+        for (DevBuf *b : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) v.push_back(b);
     for (int i = 0; i < 10; i++) v.push_back(&ctx->d_col[i]);
     return v;
 }
@@ -325,6 +341,7 @@ void free_workspace(tad_ctx *ctx)
         ctx->held -= b->cap;
         *b = DevBuf{};
     }
+    for (auto &t : ctx->tdict) t.cap = 0;
 }
 
 PinnedBlock take_pinned(tad_ctx *ctx, size_t bytes)
@@ -470,6 +487,9 @@ void *col_ptr(const tad_columns &c, int idx)
     default: return c.dst_ns;
     }
 }
+
+// Whether a job's rows carry key/value column i: its first block's column, or a text slot encoded into it on the device.
+bool has_col(const tad_job *job, int i) { return col_ptr(job->cols, i) || (i < 2 && job->text[i]); }
 
 struct OutLayout {
     size_t off[11];
@@ -1274,7 +1294,7 @@ size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_r
     s.owned = s.series = rows;
     s.out_cap = out_cap_guess(rows, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
     PipeSizes z = pipe_sizes(s);
-    for (int i = 0; i < 8; i++) z.col[i] = col_ptr(job->cols, i) ? col_bytes(i, col_rows) : 0;
+    for (int i = 0; i < 8; i++) z.col[i] = has_col(job, i) ? col_bytes(i, col_rows) : 0;
     auto bufs = pipe_bufs(ctx, z);
     bufs.push_back({&ctx->stage, stage_bytes});
     bufs.push_back({&ctx->pcnt, (kMaxPasses + 1) * 8});
@@ -1288,7 +1308,7 @@ size_t store_round_need(tad_ctx *ctx, const tad_job *job, uint64_t col_rows, siz
 {
     std::vector<std::pair<DevBuf *, size_t>> bufs = {{&ctx->stage, stage_bytes}, {&ctx->pcnt, (kMaxPasses + 1) * 8},
                                                      {&ctx->ostage, ostage_bytes}};
-    for (int i = 0; i < 8; i++) bufs.push_back({&ctx->d_col[i], col_ptr(job->cols, i) ? col_bytes(i, col_rows) : 0});
+    for (int i = 0; i < 8; i++) bufs.push_back({&ctx->d_col[i], has_col(job, i) ? col_bytes(i, col_rows) : 0});
     return workspace_after(ctx, bufs, true);
 }
 
@@ -1307,7 +1327,7 @@ void add_pass(PassOut &acc, const PassOut &o)
 
 // ---- streamed input: the worker's side of the hand-over (the caller's side is tad_stream_push / tad_stream_end) ----------
 // The next block of the current round; false once the caller has closed the round.
-bool next_block(tad_job *job, tad_columns &b)
+bool next_block(tad_job *job, tad_columns &b, tad_text_column *txt)
 {
     std::unique_lock<std::mutex> lk(job->mu);
     for (;;) {
@@ -1316,6 +1336,8 @@ bool next_block(tad_job *job, tad_columns &b)
         if (job->in.err) fail(job->in.err, "%s", job->in.msg);
         if (job->in.has_blk) {
             b = job->in.blk;
+            txt[0] = job->in.txt[0];
+            txt[1] = job->in.txt[1];
             job->in.has_blk = false;
             job->in.taken++;
             job->cv.notify_all();
@@ -1379,36 +1401,49 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     const bool stream = job->stream;
     // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
     tad_columns pend{};
-    bool have_pend = stream && next_block(job, pend);
+    tad_text_column pend_txt[2]{};
+    bool have_pend = stream && next_block(job, pend, pend_txt);
     const tad_columns &hc = job->cols;
     const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
     const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
     const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
-    auto staged = [&](int i) { return col_ptr(hc, i) && (i < 8 || ns); };
+    auto staged = [&](int i) { return has_col(job, i) && (i < 8 || ns); };
     // host input: double-buffered chunk staging, at most 1/16 of the budget
     size_t row_bytes = 0;
     for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
+    // text key slots: per staged row, kTextRowBytes of text staging (any IPv6 text) and the encode scratch
+    const bool text = job->text[0] || job->text[1];
+    constexpr size_t kTextRowBytes = 48;
+    const size_t text_row = text ? kTextRowBytes + text_scratch_bytes(1u << 20) / (1u << 20) + 1 : 0;
     uint64_t chunk = 0;
-    size_t half_bytes = 0;
+    size_t half_bytes = 0, tmarks = 0, text_bytes = 0;
     if (host_input && row_bytes) {
-        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes))) & ~uint64_t(2047);
+        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes + text_row))) & ~uint64_t(2047);
         for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
     }
-    const size_t stage_bytes = 2 * half_bytes;
-    // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits the budget
-    uint64_t lo = 0, hi = stream ? kMaxPassRows : std::min(R, kMaxPassRows);
-    while (lo < hi) {
-        const uint64_t mid = lo + (hi - lo + 1) / 2;
-        if (pass_need(ctx, job, mid, mid, false, stage_bytes, true) <= budget) lo = mid; else hi = mid - 1;
+    if (text && chunk) {
+        tmarks = exact_bytes((chunk / 32 + 2) * 8);
+        text_bytes = alloc_bytes(tmarks + chunk * kTextRowBytes) + alloc_bytes(text_scratch_bytes(chunk));
     }
-    const uint64_t cap = lo;
+    const size_t stage_bytes = 2 * half_bytes;
+    const size_t plan_stage = stage_bytes + text_bytes;      // the text staging is planned as part of the staging
+    // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits `b`
+    auto pass_cap = [&](uint64_t b) {
+        uint64_t lo = 0, hi = stream ? kMaxPassRows : std::min(R, kMaxPassRows);
+        while (lo < hi) {
+            const uint64_t mid = lo + (hi - lo + 1) / 2;
+            if (pass_need(ctx, job, mid, mid, false, plan_stage, true) <= b) lo = mid; else hi = mid - 1;
+        }
+        return lo;
+    };
+    uint64_t cap = pass_cap(budget);
     // host row store (streamed input with a host budget, read once per job by store_trim): out-stage of two halves of
     // `chunk` packed rows.  The plan above does not depend on it; the store is used only where the out-stage fits next
     // to the round's buffers at `cap`.
     const size_t pack_scratch = stream && chunk && host_budget_set ? exact_bytes(residue_pack_scratch_bytes(chunk)) : 0;
     const size_t ostage_bytes = pack_scratch ? 2 * chunk * sizeof(Row32) + pack_scratch + 256 : 0;
     const uint64_t host_budget =
-        ostage_bytes && store_round_need(ctx, job, cap, stage_bytes, ostage_bytes) <= budget ? host_budget_set : 0;
+        ostage_bytes && store_round_need(ctx, job, cap, plan_stage, ostage_bytes) <= budget ? host_budget_set : 0;
     if (host_budget && ctx->store_page == 0) fail(TAD_ERR_INTERNAL, "host row store without a page size");
     if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
     uint32_t P = 1;
@@ -1418,8 +1453,12 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     uint64_t colcap = stream ? std::min(cap, R ? R / P + R / P / 8 + 2048 : uint64_t(1) << 20) : cap;
     free_workspace(ctx);
     for (int i = 0; i < 8; i++)
-        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
+        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
     if (stage_bytes && !stream) ensure(ctx, ctx->stage, stage_bytes);
+    if (text_bytes) {
+        ensure(ctx, ctx->tstage, tmarks + chunk * kTextRowBytes);
+        ensure(ctx, ctx->tscratch, text_scratch_bytes(chunk));
+    }
     ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 8);
     ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
     PassCols pcols{};
@@ -1458,8 +1497,181 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     uint64_t nchunk = 0;             // host chunks staged in the current sweep
     bool any_host = false;
     bool count_only = false;         // the host row store fell back mid-round: the rest of the round is only counted
-    // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M)
-    auto feed = [&](const tad_columns &b, uint32_t v, uint32_t M) {
+    uint32_t sweeps = 0;
+    bool store = false;              // the current round goes to the host row store
+    uint64_t ub = 0, have = 0;       // first streamed round: bound of the rows in the pass columns; rows they hold
+    // ---- text key slots (DESIGN.md section 10, "Text keys on the device") ---------------------------------------------
+    // A host chunk's text slot is copied (its marks, then the bytes of its 32-row segments) into the text staging and
+    // encoded into the chunk's staged u32 key column on the copy stream, ahead of the chunk's split or pack.  The
+    // dictionaries live for the whole job, so ids are the same in every round.
+    bool text_dropped = false;       // the dictionaries took the first round's pass columns' room: that round only counted
+    auto dict_bytes = [&]() {
+        size_t b = 0;
+        for (auto &t : ctx->tdict)
+            for (DevBuf *x : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) b += x->cap;
+        return b;
+    };
+    // the first round's pass columns are freed for the dictionaries: the round only counts (or goes on to the store)
+    auto drop_pass_cols = [&]() {
+        CU(cudaStreamSynchronize(st));
+        for (int i = 0; i < 8; i++) free_buf(ctx, ctx->d_col[i]);
+        colcap = ub = 0;
+        set_pcols();
+        text_dropped = true;
+        if (!store) count_only = true;
+    };
+    // room for `extra` more dictionary bytes under the budget: in the first round the pass columns give way
+    auto dict_room = [&](size_t extra) {
+        if (!ctx->limit || ctx->held + extra <= ctx->limit) return;
+        if (sweeps == 0 && !text_dropped) drop_pass_cols();
+        if (ctx->held + extra > ctx->limit)
+            fail(TAD_ERR_NOMEM, "the text key dictionaries need %zu bytes of device workspace (%zu held); with the job's "
+                 "staging that passes the memory budget of %llu bytes", dict_bytes() + extra, dict_bytes(),
+                 (unsigned long long)budget);
+    };
+    auto dict_of = [&](int t) {
+        auto &d = ctx->tdict[t];
+        return TextDict{(unsigned long long *)d.slots.p, (uint32_t *)d.minrow.p, (uint32_t *)d.slot_id.p, d.cap,
+                        (uint8_t *)d.arena.p, (uint64_t *)d.off.p, (uint64_t *)d.hash.p, (unsigned long long *)d.state.p,
+                        sweeps > 0 ? 1u : 0u};
+    };
+    // the dictionaries' names and bytes (exact again), and their decode error flags
+    auto text_sync = [&]() {
+        for (int t = 0; t < 2; t++)
+            if (ctx->tdict[t].state.p)
+                CU(cudaMemcpyAsync(ctx->h_small + 192 + 8 * t, ctx->tdict[t].state.p, 8 * 8, cudaMemcpyDeviceToHost,
+                                   ctx->copy_stream));
+        CU(cudaStreamSynchronize(ctx->copy_stream));
+        for (int t = 0; t < 2; t++) {
+            auto &d = ctx->tdict[t];
+            if (!d.state.p) continue;
+            const unsigned long long *w = ctx->h_small + 192 + 8 * t;
+            if (w[2])
+                fail(TAD_ERR_INVALID_ARG, "invalid request: the %s text column of a streamed block does not match its marks "
+                     "(a VarUInt length runs past a mark or the column's end)", t ? "dst_ip" : "src_ip");
+            if (w[5])
+                fail(TAD_ERR_INVALID_ARG, "a later round of the input brought a %s name the first round did not: the "
+                     "source changed between reads", t ? "dst_ip" : "src_ip");
+            d.names_ub = w[0];
+            d.bytes_ub = w[1];
+        }
+    };
+    auto grow_dict_buf = [&](DevBuf &b, size_t bytes, size_t keep) {
+        if (bytes <= b.cap) return;
+        // geometric growth where the budget allows it, else the exact size
+        if (!ctx->limit || ctx->held + exact_bytes(2 * b.cap) <= ctx->limit) bytes = std::max(bytes, 2 * b.cap);
+        dict_room(exact_bytes(bytes));
+        grow_keep(ctx, b, bytes, keep, ctx->copy_stream);
+    };
+    // slot t's dictionary takes `n` more rows of `span` text bytes: its load stays at or below 1/2 counting every row as
+    // a new name
+    auto text_grow = [&](int t, uint64_t n, uint64_t span) {
+        auto &d = ctx->tdict[t];
+        auto ok = [&]() {
+            const uint64_t nn = d.names_ub + n;
+            return d.cap && 2 * nn <= d.cap && d.arena.cap >= d.bytes_ub + span && d.off.cap >= (nn + 1) * 8 &&
+                   d.hash.cap >= nn * 8;
+        };
+        if (!ok()) {
+            if (!d.state.p) {                     // the job's first text chunk of this slot
+                d.names_ub = d.bytes_ub = 0;
+                dict_room(exact_bytes(64));
+                ensure(ctx, d.state, 64);
+                CU(cudaMemsetAsync(d.state.p, 0, 64, ctx->copy_stream));
+                grow_dict_buf(d.off, 4096, 0);
+                CU(cudaMemsetAsync(d.off.p, 0, 8, ctx->copy_stream));
+            } else {
+                text_sync();
+            }
+            const uint64_t names = d.names_ub, bytes = d.bytes_ub, nn = names + n;
+            if (nn > (1ull << 30))
+                fail(TAD_ERR_INVALID_ARG, "invalid request: a text key slot may hold at most 2^30 distinct names");
+            grow_dict_buf(d.off, (nn + 1) * 8, (names + 1) * 8);
+            grow_dict_buf(d.hash, std::max<uint64_t>(nn, 512) * 8, names * 8);
+            grow_dict_buf(d.arena, std::max<uint64_t>(bytes + span, 4096), bytes);
+            if (!d.cap || 2 * nn > d.cap) {       // a larger table, the names re-inserted on the device
+                uint64_t c = 1024;                // nn <= 2^30: c <= 2^31
+                while (c < 2 * nn) c *= 2;
+                dict_room(exact_bytes((size_t)c * 8) + 2 * exact_bytes((size_t)c * 4));
+                DevBuf ns, nm, ni;
+                ensure(ctx, ns, (size_t)c * 8);
+                ensure(ctx, nm, (size_t)c * 4);
+                ensure(ctx, ni, (size_t)c * 4);
+                TextDict old = dict_of(t), nd = old;
+                nd.slots = (unsigned long long *)ns.p;
+                nd.minrow = (uint32_t *)nm.p;
+                nd.slot_id = (uint32_t *)ni.p;
+                nd.cap = (uint32_t)c;
+                CU(launch_text_clear(ctx->copy_stream, nd));
+                CU(launch_text_rehash(ctx->copy_stream, old, nd, names));
+                acc.launches += names ? 1 : 0;
+                CU(cudaStreamSynchronize(ctx->copy_stream));
+                free_buf(ctx, d.slots);
+                free_buf(ctx, d.minrow);
+                free_buf(ctx, d.slot_id);
+                d.slots = ns;
+                d.minrow = nm;
+                d.slot_id = ni;
+                d.cap = (uint32_t)c;
+            }
+        }
+        d.names_ub += n;
+        d.bytes_ub += span;
+    };
+    // segment s's first byte in text slot t of a block of `rows` rows (the column's end for s = its segment count)
+    auto mark_at = [](const tad_text_column &tx, uint64_t rows, uint64_t s) {
+        return s < (rows + 31) / 32 ? tx.marks[s] : tx.nbytes;
+    };
+    // rows [lo, lo + n) of a block, cut at a mark where a slot's text does not fit the text staging; the staging grows
+    // for a single segment larger than it
+    auto text_fit = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n) {
+        for (int t = 0; t < 2; t++) {
+            if (!job->text[t]) continue;
+            const uint64_t s0 = lo / 32;
+            uint64_t s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
+            const uint64_t room_b = ctx->tstage.cap - tmarks, a = mark_at(tx[t], rows, s0);
+            if (mark_at(tx[t], rows, s1) - a <= room_b) continue;
+            const uint64_t one = mark_at(tx[t], rows, s0 + 1) - a;
+            if (one > room_b) {
+                CU(cudaStreamSynchronize(ctx->copy_stream));
+                if (!fits(ctx, ctx->tstage, tmarks + one))
+                    fail(TAD_ERR_NOMEM, "32 rows of a text column hold %llu bytes: more than the memory budget of %llu "
+                         "bytes leaves for the text staging", (unsigned long long)one, (unsigned long long)budget);
+                ensure(ctx, ctx->tstage, tmarks + one);
+                s1 = s0 + 1;
+            } else {
+                uint64_t l = s0 + 1, h = s1;
+                while (l < h) {
+                    const uint64_t mid = l + (h - l + 1) / 2;
+                    if (mark_at(tx[t], rows, mid) - a <= room_b) l = mid; else h = mid - 1;
+                }
+                s1 = l;
+            }
+            n = std::min(n, s1 * 32 - lo);
+        }
+        return n;
+    };
+    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids at dst[t] (device u32)
+    auto text_encode = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, char *const *dst) {
+        for (int t = 0; t < 2; t++) {
+            if (!job->text[t]) continue;
+            const uint64_t s0 = lo / 32, s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
+            const uint64_t a = mark_at(tx[t], rows, s0), span = mark_at(tx[t], rows, s1) - a;
+            // the first round builds the dictionary; later rounds look names up in it and add none (a frozen table
+            // needs no room: a missing name fails the round)
+            if (sweeps == 0 || !ctx->tdict[t].state.p) text_grow(t, n, span);
+            char *m = static_cast<char *>(ctx->tstage.p);
+            CU(cudaMemcpyAsync(m, tx[t].marks + s0, (s1 - s0) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
+            if (span) CU(cudaMemcpyAsync(m + tmarks, tx[t].bytes + a, span, cudaMemcpyHostToDevice, ctx->copy_stream));
+            CU(launch_text_encode(ctx->copy_stream, dict_of(t), reinterpret_cast<const uint8_t *>(m + tmarks), span,
+                                  reinterpret_cast<const uint64_t *>(m), (uint32_t)(s1 - s0), s0 * 32, rows, lo, n,
+                                  ctx->tscratch.p, ctx->tscratch.cap, reinterpret_cast<uint32_t *>(dst[t])));
+            acc.launches += kTextLaunches;
+        }
+    };
+    // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M).  Text slots: `tx`, of
+    // which the block's rows are rows [origin, origin + b.rows).
+    auto feed = [&](const tad_columns &b, uint32_t v, uint32_t M, const tad_text_column *tx, uint64_t origin) {
         const uint64_t n_all = b.rows;
         if (n_all == 0) return;
         if (b.mem == TAD_MEM_DEVICE) {
@@ -1472,20 +1684,26 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         }
         any_host = true;
         ensure(ctx, ctx->stage, stage_bytes);
-        for (uint64_t lo_r = 0; lo_r < n_all; lo_r += chunk, nchunk++) {
-            const uint64_t n = std::min<uint64_t>(chunk, n_all - lo_r);
+        for (uint64_t lo_r = 0, n; lo_r < n_all; lo_r += n, nchunk++) {
+            n = std::min<uint64_t>(chunk, n_all - lo_r);
+            if (text) n = text_fit(tx, origin + n_all, origin + lo_r, n);
             const int h = (int)(nchunk & 1);
             if (nchunk >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
             ColPtrs c{};
             char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+            char *ids[2] = {nullptr, nullptr};
             for (int i = 0; i < 10; i++) {
                 if (!staged(i)) continue;
                 const size_t w = col_bytes(i, 1);
-                CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(b, i)) + lo_r * w, n * w, cudaMemcpyHostToDevice,
-                                   ctx->copy_stream));
+                if (i < 2 && job->text[i])
+                    ids[i] = dst;
+                else
+                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(b, i)) + lo_r * w, n * w,
+                                       cudaMemcpyHostToDevice, ctx->copy_stream));
                 set_col(c, i, dst);
                 dst += exact_bytes(col_bytes(i, chunk));
             }
+            if (text) text_encode(tx, origin + n_all, origin + lo_r, n, ids);
             CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
             CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
             CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
@@ -1498,7 +1716,6 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
     // With a host budget, rows that would pass `cap` go to the host row store instead: false, `have` = the rows the
     // pass columns hold.
-    uint64_t ub = 0, have = 0;
     auto room = [&](uint64_t n) {
         if ((colcap >= cap && !host_budget) || ub + n <= colcap) { ub += n; return true; }
         CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
@@ -1507,8 +1724,16 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         if (host_budget && have + n > cap) return false;
         if (have + n > colcap) {
             const uint64_t want = std::min(cap, std::max(2 * colcap, have + n));
+            if (text && ctx->limit) {        // beside the dictionaries the columns may not grow: the round only counts
+                size_t grow = 0;
+                for (int i = 0; i < 8; i++) grow += has_col(job, i) ? exact_bytes(col_bytes(i, want)) : 0;
+                if (ctx->held + grow > ctx->limit) {
+                    drop_pass_cols();
+                    return true;
+                }
+            }
             for (int i = 0; i < 8; i++)
-                if (col_ptr(hc, i)) grow_keep(ctx, ctx->d_col[i], col_bytes(i, want), col_bytes(i, have), st);
+                if (has_col(job, i)) grow_keep(ctx, ctx->d_col[i], col_bytes(i, want), col_bytes(i, have), st);
             colcap = want;
             set_pcols();
         }
@@ -1520,7 +1745,6 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     // counted, scanned and scattered per residue into an out-stage half, whose residue segments are then copied to the
     // residue's pages on the D2H stream.  The passes load their residues from the pages.
     RowStore rs(ctx);
-    bool store = false;              // the current round goes to the store
     bool stored = false;             // the store holds the whole first round: the passes load from it
     bool dropped = false;            // the store fell back in the first round: it only counted
     uint64_t fill = 0, nhalf = 0, npack = 0;   // rows in the staging half being filled; halves filled; out-stage halves used
@@ -1531,7 +1755,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     auto pass_cols_of = [&](uint64_t lo) {        // the pass columns from row `lo`, as kernel input
         ColPtrs c{};
         for (int i = 0; i < 8; i++)
-            if (col_ptr(hc, i)) set_col(c, i, static_cast<const char *>(ctx->d_col[i].p) + col_bytes(i, lo));
+            if (has_col(job, i)) set_col(c, i, static_cast<const char *>(ctx->d_col[i].p) + col_bytes(i, lo));
         return c;
     };
     auto store_drop = [&]() {        // fallback: pages back to the context, the rest of the round is only counted
@@ -1606,28 +1830,40 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     };
     // the pass columns overflow in the first round: their `have` rows go to the store first (counted already)
     auto switch_to_store = [&]() {
+        // the out-stage was planned without the dictionaries: where it does not fit beside them, the round only counts
+        if (text && ctx->limit &&
+            ctx->held + exact_bytes(ostage_bytes) + (stage_bytes > ctx->stage.cap ? exact_bytes(stage_bytes) : 0) > ctx->limit) {
+            count_only = true;
+            return;
+        }
         start_store();
         for (uint64_t lo = 0; lo < have && store; lo += chunk) pack(pass_cols_of(lo), std::min(chunk, have - lo), false);
     };
     // one block into the staging halves (a D2D copy for a device block); a full half is packed.  The rest of a block
     // the store fell back in is counted.
-    auto put = [&](const tad_columns &b) {
+    auto put = [&](const tad_columns &b, const tad_text_column *tx) {
         uint64_t lo = 0;
         any_host = true;             // the round's time is the copies' (h2d phase), as for a sweep of host blocks
         while (lo < b.rows && store) {
             if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
             const int h = (int)(nhalf & 1);
             if (fill == 0) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // its last pack is done
-            const uint64_t n = std::min(chunk - fill, b.rows - lo);
+            uint64_t n = std::min(chunk - fill, b.rows - lo);
+            if (text) n = text_fit(tx, b.rows, lo, n);
             char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+            char *ids[2] = {nullptr, nullptr};
             for (int i = 0; i < 10; i++) {
                 if (!staged(i)) continue;
                 const size_t w = col_bytes(i, 1);
-                CU(cudaMemcpyAsync(dst + fill * w, static_cast<const char *>(col_ptr(b, i)) + lo * w, n * w,
-                                   b.mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
-                                   ctx->copy_stream));
+                if (i < 2 && job->text[i])
+                    ids[i] = dst + fill * w;
+                else
+                    CU(cudaMemcpyAsync(dst + fill * w, static_cast<const char *>(col_ptr(b, i)) + lo * w, n * w,
+                                       b.mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                                       ctx->copy_stream));
                 dst += exact_bytes(col_bytes(i, chunk));
             }
+            if (text) text_encode(tx, b.rows, lo, n, ids);
             fill += n;
             lo += n;
             if (fill == chunk) pack_half();
@@ -1640,7 +1876,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                                (void **)&rest.src_ns, (void **)&rest.dst_ns};
             for (int i = 0; i < 10; i++)
                 if (*cols[i]) *cols[i] = static_cast<char *>(*cols[i]) + col_bytes(i, lo);
-            feed(rest, 0, P);
+            feed(rest, 0, P, tx, lo);
         }
     };
     // end of the store's round: the last half, the last copies; the out-stage is not needed any more
@@ -1690,7 +1926,6 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         acc.device_ms += ms;
     };
     uint64_t counts[kMaxPasses];
-    uint32_t sweeps = 0;
     bool open = false;               // a streamed round is swept and its caller waits in tad_stream_end
     // one sweep over the input: the rows of pass (v, M) -> the pass columns; returns the rows of the pass
     auto sweep = [&](uint32_t v, uint32_t M) -> uint64_t {
@@ -1703,20 +1938,21 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
         }
         if (!stream) {
-            feed(hc, v, M);
+            feed(hc, v, M, nullptr, 0);
         } else {
             // the round's blocks; block k is released (its push returns) once block k+1 is enqueued and k's copy is done
             uint64_t rows = 0, k = 0;
             ub = 0;
             tad_columns b{};
-            bool got = have_pend ? (b = pend, true) : next_block(job, b);
+            tad_text_column tx[2]{};
+            bool got = have_pend ? (b = pend, tx[0] = pend_txt[0], tx[1] = pend_txt[1], true) : next_block(job, b, tx);
             have_pend = false;
             if (sweeps == 0 && host_budget && P > 1) start_store();     // the hint plans passes: the round goes to the store
             while (got) {
                 if (sweeps == 0 && host_budget && !store && !count_only && !room(b.rows)) switch_to_store();
-                else if (sweeps == 0 && !host_budget) room(b.rows);
+                else if (sweeps == 0 && !host_budget && !count_only) room(b.rows);
                 const bool to_store = store;
-                if (store) put(b); else feed(b, v, M);
+                if (store) put(b, tx); else feed(b, v, M, tx, 0);
                 if (to_store && !store) {            // the store fell back inside this block: its rest was split on st
                     CU(cudaEventRecord(ctx->start_ev, st));
                     CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
@@ -1733,7 +1969,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 }
                 rows += b.rows;
                 k++;
-                got = next_block(job, b);
+                got = next_block(job, b, tx);
             }
             if (sweeps == 0) job->round_rows = rows;
             if (sweeps == 0 && ctx->ostage.p) end_store();
@@ -1746,6 +1982,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
         acc.phase_ms[any_host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;      // the split runs behind the copies
         acc.device_ms += ms;
+        if (text) text_sync();
         if (sweeps > 0)
             for (int j = 0; j < kMaxPasses; j++)
                 if (h_cnt[j] != counts[j])
@@ -1757,6 +1994,15 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     };
     const uint64_t got0 = sweep(0, P);
     for (int j = 0; j < kMaxPasses; j++) counts[j] = h_cnt[j];
+    if (text) {
+        count_only = false;
+        // the passes run beside the dictionaries
+        const size_t held_dict = dict_bytes();
+        cap = pass_cap(budget > held_dict ? budget - held_dict : 0);
+        if (cap == 0)
+            fail(TAD_ERR_NOMEM, "the text key dictionaries hold %zu bytes: beside them the memory budget of %llu bytes does "
+                 "not hold one row of a pass", held_dict, (unsigned long long)budget);
+    }
     auto pass_rows = [&](uint32_t v, uint32_t M) {
         uint64_t n = 0;
         for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M) n += counts[j];
@@ -1779,7 +2025,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     auto too_big = [&](uint64_t rows) {
         fail(TAD_ERR_NOMEM, "one 1/%d hash range of the table (%llu rows) needs %zu bytes of device workspace; the memory "
              "budget is %llu bytes", kMaxPasses, (unsigned long long)rows,
-             pass_need(ctx, job, rows, rows, false, stage_bytes, true), (unsigned long long)budget);
+             pass_need(ctx, job, rows, rows, false, plan_stage, true), (unsigned long long)budget);
     };
     if (largest(P) > cap) too_big(largest(kMaxPasses));
     bool loaded = !stored && !dropped && P == P0 && got0 <= colcap;     // pass (0, P) is in the pass columns already
@@ -1807,7 +2053,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             if (!loaded && rows) {
                 if (stream && rows > colcap) {          // later rounds: the counts size the pass columns exactly
                     for (int i = 0; i < 8; i++)
-                        if (col_ptr(hc, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, rows));
+                        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, rows));
                     colcap = rows;
                     set_pcols();
                 }
@@ -1819,9 +2065,9 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 tad_columns pc{};
                 pc.rows = pc.capacity = rows;
                 pc.mem = TAD_MEM_DEVICE;
-                pc.src_ip = col_ptr(hc, 0) ? pcols.src_ip : nullptr; pc.dst_ip = col_ptr(hc, 1) ? pcols.dst_ip : nullptr;
-                pc.src_port = col_ptr(hc, 2) ? pcols.src_port : nullptr; pc.dst_port = col_ptr(hc, 3) ? pcols.dst_port : nullptr;
-                pc.proto = col_ptr(hc, 4) ? pcols.proto : nullptr; pc.flow_start = col_ptr(hc, 5) ? pcols.flow_start : nullptr;
+                pc.src_ip = has_col(job, 0) ? pcols.src_ip : nullptr; pc.dst_ip = has_col(job, 1) ? pcols.dst_ip : nullptr;
+                pc.src_port = has_col(job, 2) ? pcols.src_port : nullptr; pc.dst_port = has_col(job, 3) ? pcols.dst_port : nullptr;
+                pc.proto = has_col(job, 4) ? pcols.proto : nullptr; pc.flow_start = has_col(job, 5) ? pcols.flow_start : nullptr;
                 pc.flow_end = pcols.flow_end; pc.value = pcols.value;
                 // optimistic partition where its slot buffer fits next to what the context holds; else the exact one, on
                 // a workspace cleared of earlier passes' buffers if need be (the planner sized `cap` for that)
@@ -1830,7 +2076,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                     for (DevBuf *b : workspace_bufs(ctx)) {
                         // kept: the pass columns, staging, counters and the ns_ignore list the sweeps read
                         if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore ||
-                            (b >= ctx->d_col && b < ctx->d_col + 8))
+                            (b >= ctx->d_col && b < ctx->d_col + 8) || b == &ctx->tstage || b == &ctx->tscratch ||
+                            (text && (void *)b >= (void *)ctx->tdict && (void *)b < (void *)(ctx->tdict + 2)))
                             continue;
                         if (b->p) CU(cudaFree(b->p));
                         ctx->held -= b->cap;
@@ -1871,6 +2118,23 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     } catch (...) {
         for (PassOut &o : outs) give_pinned(ctx, o.block);
         throw;
+    }
+    // each text slot's dictionary to host memory the job owns (tad_job_names); the device copy goes with the workspace
+    for (int t = 0; t < 2; t++) {
+        if (!job->text[t]) continue;
+        auto &d = ctx->tdict[t];
+        uint64_t names = 0, bytes = 0;
+        if (d.state.p) {
+            text_sync();
+            names = d.names_ub;
+            bytes = d.bytes_ub;
+        }
+        job->names[t].resize(bytes);
+        job->names_off[t].assign(names + 1, 0);
+        if (bytes) CU(cudaMemcpy(job->names[t].data(), d.arena.p, bytes, cudaMemcpyDeviceToHost));
+        if (names) CU(cudaMemcpy(job->names_off[t].data(), d.off.p, (names + 1) * 8, cudaMemcpyDeviceToHost));
+        for (DevBuf *x : {&d.slots, &d.minrow, &d.slot_id, &d.arena, &d.off, &d.hash, &d.state}) free_buf(ctx, *x);
+        d.cap = 0;
     }
     return passes;
 }
@@ -1979,6 +2243,14 @@ void worker_main(tad_ctx *ctx)
             cudaStreamSynchronize(ctx->stream);
             cudaStreamSynchronize(ctx->d2h_stream);
             cudaGetLastError();
+            for (auto &t : ctx->tdict) {       // a dictionary lives for one job
+                for (DevBuf *b : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) {
+                    if (b->p) cudaFree(b->p);
+                    ctx->held -= b->cap;
+                    *b = DevBuf{};
+                }
+                t.cap = 0;
+            }
             std::lock_guard<std::mutex> lk(job->mu);
             job->st.state = TAD_STATE_FAILED;
             job->st.error = f.code;
@@ -2097,9 +2369,40 @@ int stream_gate(tad_job *job, std::unique_lock<std::mutex> &lk)
     return TAD_OK;
 }
 
-// A streamed block: host or device memory, fewer than 2^32 rows, flow_end and value, and the first block's column set.
-int check_block(const tad_job *job, const tad_columns *b, char *msg, size_t n)
+// A streamed block: host or device memory, fewer than 2^32 rows, flow_end and value, and the first block's column set,
+// text slots included.  A text slot: host memory, its u32 column NULL, one mark per 32 rows from 0, not decreasing, none
+// past the column's end.
+int check_block(const tad_job *job, const tad_columns *b, const tad_text_column *const *txt, char *msg, size_t n)
 {
+    for (int t = 0; t < 2; t++) {
+        const tad_text_column *x = txt[t];
+        if (!x) continue;
+        if (b->mem != TAD_MEM_HOST) {
+            snprintf(msg, n, "invalid request: text key columns are accepted in host blocks only");
+            return TAD_ERR_INVALID_ARG;
+        }
+        if (col_ptr(*b, t)) {
+            snprintf(msg, n, "invalid request: a slot given as text must have its u32 column NULL");
+            return TAD_ERR_INVALID_ARG;
+        }
+        const uint64_t nseg = (b->rows + 31) / 32;
+        if ((x->nbytes && !x->bytes) || (nseg && !x->marks) || (nseg && x->marks[0] != 0)) {
+            snprintf(msg, n, "invalid request: a text column needs its bytes and one mark per 32 rows, the first 0");
+            return TAD_ERR_INVALID_ARG;
+        }
+        for (uint64_t s = 0; s < nseg; s++)
+            if (x->marks[s] > x->nbytes || (s && x->marks[s] < x->marks[s - 1])) {
+                snprintf(msg, n, "invalid request: the marks of a text column decrease or pass its end");
+                return TAD_ERR_INVALID_ARG;
+            }
+    }
+    if (job->in.pushed > 0)
+        for (int t = 0; t < 2; t++)
+            if (job->text[t] != (txt[t] != nullptr)) {
+                snprintf(msg, n, "invalid request: a streamed block gives %s as %s, the job's first block did not",
+                         t ? "dst_ip" : "src_ip", txt[t] ? "text" : "u32");
+                return TAD_ERR_INVALID_ARG;
+            }
     if (b->mem != TAD_MEM_HOST && b->mem != TAD_MEM_DEVICE) {
         snprintf(msg, n, "invalid request: bad column memory kind");
         return TAD_ERR_INVALID_ARG;
@@ -2331,21 +2634,30 @@ int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint
     return submit_job(ctx, job, spec, &none, out);
 }
 
-int tad_stream_push(tad_job *job, const tad_columns *block)
+int tad_stream_push(tad_job *job, const tad_columns *block) { return tad_stream_push_text(job, block, nullptr, nullptr); }
+
+int tad_stream_push_text(tad_job *job, const tad_columns *block, const tad_text_column *src_ip, const tad_text_column *dst_ip)
 {
     if (!job || !block) return TAD_ERR_INVALID_ARG;
+    if ((src_ip || dst_ip) && !job->stream) return TAD_ERR_UNSUPPORTED;
     std::unique_lock<std::mutex> lk(job->mu);
     int rc = stream_gate(job, lk);
     if (rc != TAD_OK) return rc;
     char msg[200];
-    rc = check_block(job, block, msg, sizeof(msg));
+    const tad_text_column *txt[2] = {src_ip, dst_ip};
+    rc = check_block(job, block, txt, msg, sizeof(msg));
     if (rc != TAD_OK) return stream_abort(job, lk, rc, msg);
-    if (job->in.pushed == 0) job->cols = *block;       // the column set of the job
+    if (job->in.pushed == 0) {                         // the column set of the job
+        job->cols = *block;
+        for (int t = 0; t < 2; t++) job->text[t] = txt[t] != nullptr;
+    }
+
     // one block of look-ahead: hand this one over once the worker has taken the previous one, then return once the
     // engine no longer reads the previous one
     while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
     if (finished(job)) return job->st.error;
     job->in.blk = *block;
+    for (int t = 0; t < 2; t++) job->in.txt[t] = txt[t] ? *txt[t] : tad_text_column{};
     job->in.has_blk = true;
     const uint64_t k = job->in.pushed++;
     job->cv.notify_all();
@@ -2428,6 +2740,17 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
     if (job->st.state != TAD_STATE_COMPLETED) return TAD_ERR_STATE;
     if (passes) *passes = job->passes;
     if (peak_workspace_bytes) *peak_workspace_bytes = job->peak_workspace;
+    return TAD_OK;
+}
+
+int tad_job_names(tad_job *job, int32_t slot, const uint8_t **bytes, const uint64_t **offsets, uint32_t *count)
+{
+    if (!job || slot < 0 || slot > 1 || !bytes || !offsets || !count) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->st.state != TAD_STATE_COMPLETED || !job->text[slot]) return TAD_ERR_STATE;
+    *bytes = job->names[slot].data();
+    *offsets = job->names_off[slot].data();
+    *count = (uint32_t)(job->names_off[slot].size() - 1);
     return TAD_OK;
 }
 

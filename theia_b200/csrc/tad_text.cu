@@ -1,0 +1,257 @@
+// Text key slots on the device (tad_text.h): decode of Native String column bytes, and the job's dictionary of names.
+// A translation unit of its own, so that no existing kernel's unit gains a CUB instance or a constant.
+#include <cub/device/device_scan.cuh>
+
+#include "tad_text.h"
+
+namespace tad {
+
+namespace {
+
+constexpr unsigned long long kEmpty = ~0ull;
+constexpr uint32_t kNone = 0xffffffffu;
+constexpr uint64_t kByteBits = 40;           // scan word: new names << 40 | their bytes (a chunk has < 2^24 rows)
+constexpr int kThreads = 256;
+
+__device__ __forceinline__ uint64_t name_hash(const uint8_t *s, uint32_t len)
+{
+    uint64_t h = 1469598103934665603ull;     // FNV-1a, then a fold so that the low (slot) bits see the high bytes
+    for (uint32_t k = 0; k < len; k++) h = (h ^ s[k]) * 1099511628211ull;
+    return h ^ (h >> 29);
+}
+
+__device__ __forceinline__ bool same_bytes(const uint8_t *a, uint32_t na, const uint8_t *b, uint32_t nb)
+{
+    if (na != nb) return false;
+    for (uint32_t k = 0; k < na; k++)
+        if (a[k] != b[k]) return false;
+    return true;
+}
+
+struct ChunkScratch {
+    uint32_t *off, *len, *slot_of;
+    unsigned long long *scan_in, *scan_out;
+    void *cub_tmp;
+    size_t cub_bytes;
+};
+
+size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+size_t cub_scan_bytes(uint64_t n)
+{
+    size_t b = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, b, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, (int)n);
+    return b;
+}
+
+ChunkScratch carve(void *scratch, uint64_t n)
+{
+    char *p = static_cast<char *>(scratch);
+    ChunkScratch c;
+    c.off = reinterpret_cast<uint32_t *>(p); p += align256(n * 4);
+    c.len = reinterpret_cast<uint32_t *>(p); p += align256(n * 4);
+    c.slot_of = reinterpret_cast<uint32_t *>(p); p += align256(n * 4);
+    c.scan_in = reinterpret_cast<unsigned long long *>(p); p += align256(n * 8);
+    c.scan_out = reinterpret_cast<unsigned long long *>(p); p += align256(n * 8);
+    c.cub_tmp = p;
+    c.cub_bytes = cub_scan_bytes(n);
+    return c;
+}
+
+// One thread per 32-row segment: walk its rows' VarUInt lengths inside [mark, next mark) and record the (offset,
+// length) of the rows in [lo, lo + n).  Every byte read is checked against the segment's end, which is checked against
+// the span: a malformed column can set the error flag, never read outside the span.
+__global__ void text_decode_kernel(const uint8_t *__restrict__ text, uint64_t span, const uint64_t *__restrict__ marks,
+                                   uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo, uint64_t n,
+                                   uint32_t *__restrict__ off, uint32_t *__restrict__ len, unsigned long long *state)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= nseg) return;
+    const uint64_t base = marks[0];
+    const uint64_t r0 = seg0_row + 32ull * k, r1 = min(r0 + 32, block_rows);
+    uint64_t pos = marks[k] - base;
+    const uint64_t end = k + 1 < nseg ? marks[k + 1] - base : span;
+    bool ok = pos <= end && end <= span;
+    for (uint64_t r = r0; ok && r < r1; r++) {
+        uint64_t v = 0;
+        int shift = 0;
+        for (;;) {                                   // VarUInt: 7 bits per byte, least significant group first
+            if (pos >= end || shift > 63) { ok = false; break; }
+            const uint8_t b = text[pos++];
+            v |= (uint64_t)(b & 0x7f) << shift;
+            if (!(b & 0x80)) break;
+            shift += 7;
+        }
+        if (!ok || v > end - pos) { ok = false; break; }
+        if (r >= lo && r < lo + n) {
+            off[r - lo] = (uint32_t)pos;
+            len[r - lo] = (uint32_t)v;
+        }
+        pos += v;
+    }
+    ok = ok && pos == end;
+    if (!ok) {
+        atomicOr(state + 2, 1ull);
+        for (uint64_t r = max(r0, lo); r < min(r1, lo + n); r++) {
+            off[r - lo] = 0;
+            len[r - lo] = 0;
+        }
+    }
+}
+
+// One thread per row: find the row's name.  A name with an id writes it; a new name claims an empty slot (or meets the
+// row that claimed it in this chunk) and records its smallest row there.
+__global__ void text_probe_kernel(TextDict d, const uint8_t *__restrict__ text, const uint32_t *__restrict__ off,
+                                  const uint32_t *__restrict__ len, uint64_t n, uint32_t *__restrict__ slot_of,
+                                  uint32_t *__restrict__ ids)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t *s = text + off[i];
+    const uint32_t m = len[i];
+    const uint64_t h = name_hash(s, m);
+    const uint32_t tag = (uint32_t)(h >> 32), mask = d.cap - 1;
+    uint32_t p = (uint32_t)h & mask;
+    for (;;) {
+        unsigned long long cur = *(volatile unsigned long long *)(d.slots + p);
+        if (cur == kEmpty && d.frozen) {             // a later round's name the first round did not bring
+            atomicOr(d.state + 5, 1ull);
+            slot_of[i] = kNone;
+            ids[i] = 0;
+            return;
+        }
+        if (cur == kEmpty) {
+            const unsigned long long mine = (unsigned long long)tag << 32 | kTextPending | (uint32_t)i;
+            cur = atomicCAS(d.slots + p, kEmpty, mine);
+            if (cur == kEmpty) {
+                slot_of[i] = p;
+                atomicMin(d.minrow + p, (uint32_t)i);
+                return;
+            }
+        }
+        if ((uint32_t)(cur >> 32) == tag) {
+            const uint32_t ref = (uint32_t)cur;
+            if (ref & kTextPending) {
+                const uint32_t r = ref & ~kTextPending;
+                if (same_bytes(s, m, text + off[r], len[r])) {
+                    slot_of[i] = p;
+                    atomicMin(d.minrow + p, (uint32_t)i);
+                    return;
+                }
+            } else if (same_bytes(s, m, d.arena + d.off[ref], (uint32_t)(d.off[ref + 1] - d.off[ref]))) {
+                slot_of[i] = kNone;
+                ids[i] = ref;
+                return;
+            }
+        }
+        p = (p + 1) & mask;
+    }
+}
+
+// The first row of each new name: (1 << 40 | its length), every other row 0.
+__global__ void text_first_kernel(TextDict d, const uint32_t *__restrict__ slot_of, const uint32_t *__restrict__ len,
+                                  uint64_t n, unsigned long long *__restrict__ scan_in)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t p = slot_of[i];
+    scan_in[i] = p != kNone && d.minrow[p] == (uint32_t)i ? (1ull << kByteBits) | len[i] : 0ull;
+}
+
+// The first row of each new name takes id names + rank, copies its bytes to the arena and publishes the id in its slot.
+__global__ void text_assign_kernel(TextDict d, const uint8_t *__restrict__ text, const uint32_t *__restrict__ off,
+                                   const uint32_t *__restrict__ len, const uint32_t *__restrict__ slot_of,
+                                   const unsigned long long *__restrict__ scan_in,
+                                   const unsigned long long *__restrict__ scan_out, uint64_t n)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long x = scan_out[i], v = scan_in[i];
+    if (i == n - 1) {
+        d.state[3] = (x + v) >> kByteBits;
+        d.state[4] = (x + v) & ((1ull << kByteBits) - 1);
+    }
+    if (!v) return;
+    const uint32_t id = (uint32_t)(d.state[0] + (x >> kByteBits));
+    const uint64_t at = d.state[1] + (x & ((1ull << kByteBits) - 1));
+    const uint8_t *s = text + off[i];
+    const uint32_t m = len[i];
+    for (uint32_t k = 0; k < m; k++) d.arena[at + k] = s[k];
+    d.off[id] = at;
+    const uint64_t h = name_hash(s, m);
+    d.hash[id] = h;
+    const uint32_t p = slot_of[i];
+    d.slot_id[p] = id;
+    d.slots[p] = (h >> 32) << 32 | id;
+}
+
+// Every row that reached a pending slot reads the id published there; the slot is reset for the next chunk.
+__global__ void text_resolve_kernel(TextDict d, const uint32_t *__restrict__ slot_of, uint64_t n, uint32_t *__restrict__ ids)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) {
+        d.state[0] += d.state[3];
+        d.state[1] += d.state[4];
+        d.off[d.state[0]] = d.state[1];
+    }
+    if (i >= n) return;
+    const uint32_t p = slot_of[i];
+    if (p == kNone) return;
+    ids[i] = d.slot_id[p];
+    d.minrow[p] = kNone;
+}
+
+__global__ void text_rehash_kernel(TextDict d, const uint64_t *__restrict__ hash, uint64_t names)
+{
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= names) return;
+    const uint64_t h = hash[k];
+    const uint32_t mask = d.cap - 1;
+    uint32_t p = (uint32_t)h & mask;
+    const unsigned long long e = (h >> 32) << 32 | k;
+    while (atomicCAS(d.slots + p, kEmpty, e) != kEmpty) p = (p + 1) & mask;
+}
+
+unsigned grid(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
+
+}  // namespace
+
+size_t text_scratch_bytes(uint64_t n)
+{
+    n = n ? n : 1;
+    return 3 * align256(n * 4) + 2 * align256(n * 8) + align256(cub_scan_bytes(n));
+}
+
+cudaError_t launch_text_clear(cudaStream_t st, const TextDict &d)
+{
+    cudaError_t e = cudaMemsetAsync(d.slots, 0xff, (size_t)d.cap * sizeof(unsigned long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d.minrow, 0xff, (size_t)d.cap * sizeof(uint32_t), st);
+    return e;
+}
+
+cudaError_t launch_text_rehash(cudaStream_t st, const TextDict &old, const TextDict &d, uint64_t names)
+{
+    if (!names) return cudaSuccess;
+    text_rehash_kernel<<<grid(names), kThreads, 0, st>>>(d, old.hash, names);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_text_encode(cudaStream_t st, const TextDict &d, const uint8_t *text, uint64_t span_bytes,
+                               const uint64_t *marks, uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo,
+                               uint64_t n, void *scratch, size_t scratch_bytes, uint32_t *ids)
+{
+    if (n == 0) return cudaSuccess;
+    if (scratch_bytes < text_scratch_bytes(n) || n >= (1ull << 24)) return cudaErrorInvalidValue;
+    ChunkScratch c = carve(scratch, n);
+    text_decode_kernel<<<(nseg + 127) / 128, 128, 0, st>>>(text, span_bytes, marks, nseg, seg0_row, block_rows, lo, n, c.off,
+                                                          c.len, d.state);
+    text_probe_kernel<<<grid(n), kThreads, 0, st>>>(d, text, c.off, c.len, n, c.slot_of, ids);
+    text_first_kernel<<<grid(n), kThreads, 0, st>>>(d, c.slot_of, c.len, n, c.scan_in);
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(c.cub_tmp, c.cub_bytes, c.scan_in, c.scan_out, (int)n, st);
+    if (e != cudaSuccess) return e;
+    text_assign_kernel<<<grid(n), kThreads, 0, st>>>(d, text, c.off, c.len, c.slot_of, c.scan_in, c.scan_out, n);
+    text_resolve_kernel<<<grid(n), kThreads, 0, st>>>(d, c.slot_of, n, ids);
+    return cudaGetLastError();
+}
+
+}  // namespace tad

@@ -1,0 +1,49 @@
+// Text key slots of streamed host blocks (tad_stream_push_text): ClickHouse Native String column bytes decoded and
+// dictionary-encoded on the device into job-stable u32 ids (implemented in tad_text.cu; DESIGN.md section 10).
+#pragma once
+#include <cstddef>
+#include <cstdint>
+
+#include <cuda_runtime.h>
+
+namespace tad {
+
+// The device dictionary of one text slot.  Open addressing over a 64-bit FNV-1a hash of the bytes: a slot holds
+// (high 32 hash bits << 32) | ref, where ref is a name id, or kTextPending | row for a name first seen in the chunk being
+// encoded.  A lookup compares the bytes whenever the tag matches.  Names are kept once each in `arena`, in id order:
+// name k is arena[off[k], off[k + 1]).  state[0] = names, state[1] = arena bytes, state[2] = decode error flag,
+// state[3..4] = the current chunk's new names / bytes, state[5] = a name was missing from a frozen dictionary.
+struct TextDict {
+    unsigned long long *slots;   // cap
+    uint32_t *minrow;            // cap: smallest row of the chunk that reached a pending slot (UINT32_MAX: none)
+    uint32_t *slot_id;           // cap: the id a pending slot's first row published
+    uint32_t cap;                // power of two
+    uint8_t *arena;
+    uint64_t *off;               // names + 1
+    uint64_t *hash;              // names: each name's hash, for the rehash
+    unsigned long long *state;   // 8 words
+    uint32_t frozen;             // the dictionary is complete: a name not in it sets state[5] and is not added
+};
+
+// Scratch of one chunk of `n` rows: per row (offset, length) into the staged text, the pending slot it reached, and the
+// (new-name count << 40 | bytes) scan.  text_scratch_bytes(n) sizes it.
+size_t text_scratch_bytes(uint64_t n);
+
+// A fresh table of `cap` slots (every slot empty, minrow all ones).  Two launches.
+cudaError_t launch_text_clear(cudaStream_t st, const TextDict &d);
+// Every name of `old` (its `names` ids) re-inserted into the empty table `d` (same arena).  One launch.
+cudaError_t launch_text_rehash(cudaStream_t st, const TextDict &old, const TextDict &d, uint64_t names);
+
+// Rows [lo, lo + n) of a block, as the bytes of its 32-row segments s0 .. s0 + nseg - 1: `text` holds the span from
+// the start of segment s0 (span_bytes), `marks` the block's marks of those segments (absolute, marks[0] = the span's
+// start), block_rows the block's rows.  Each row's id (order of first appearance over the dictionary's life) goes to
+// ids[0, n).  A segment whose VarUInt lengths do not end exactly at the next mark (or the span's end), or that would read
+// past the span, sets state[2] and encodes its rows as the empty name.  Seven launches (two of them the CUB scan).
+cudaError_t launch_text_encode(cudaStream_t st, const TextDict &d, const uint8_t *text, uint64_t span_bytes,
+                               const uint64_t *marks, uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo,
+                               uint64_t n, void *scratch, size_t scratch_bytes, uint32_t *ids);
+
+constexpr uint32_t kTextPending = 0x80000000u;
+constexpr int kTextLaunches = 7;
+
+}  // namespace tad

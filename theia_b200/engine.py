@@ -197,12 +197,44 @@ class StreamJob(Job):
         super().__init__(eng, handle, keep)
         self._last = None
 
-    def push(self, block):
+    def push(self, block, text=None):
+        """``text``: {"src_ip" / "dst_ip": (column bytes, marks)} -- those slots as Native String column bytes with the
+        byte offset of every 32nd row (tad_stream_push_text), encoded into job-wide ids on the GPU."""
         c, keep = _block_columns(block)
-        rc = self.eng.lib.tad_stream_push(self.h, C.byref(c))
+        if text:
+            tx = []
+            for slot in ("src_ip", "dst_ip"):
+                if slot not in text:
+                    tx.append(None)
+                    continue
+                data, marks = text[slot]
+                data = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data
+                marks = np.ascontiguousarray(marks, dtype=np.uint64)
+                t = L.TadTextColumn()
+                t.bytes = data.ctypes.data if len(data) else C.addressof(_EMPTY)
+                t.nbytes = len(data)
+                t.marks = marks.ctypes.data if len(marks) else C.addressof(_EMPTY)
+                keep = [keep, data, marks]
+                tx.append(t)
+            keep = [keep, tx]
+            rc = self.eng.lib.tad_stream_push_text(self.h, C.byref(c), *(C.byref(t) if t is not None else None for t in tx))
+        else:
+            rc = self.eng.lib.tad_stream_push(self.h, C.byref(c))
         if rc != 0:
             raise TadError(rc, self.poll()["err_msg"])
         self._last = (c, keep)        # the engine may read this block until the next push or end returns
+
+    def names(self, slot: str):
+        """Of a COMPLETED job: the dictionary of a text slot as numpy (bytes, offsets): id k is bytes[offsets[k]:offsets[k+1]]."""
+        b, o, n = C.c_void_p(), C.c_void_p(), C.c_uint32()
+        rc = self.eng.lib.tad_job_names(self.h, ("src_ip", "dst_ip").index(slot), C.byref(b), C.byref(o), C.byref(n))
+        if rc != 0:
+            raise TadError(rc, "tad_job_names")
+        offsets = np.ctypeslib.as_array((C.c_uint64 * (n.value + 1)).from_address(o.value)).copy()
+        nbytes = int(offsets[-1])
+        data = np.frombuffer((C.c_char * nbytes).from_address(b.value), dtype=np.uint8).copy() if nbytes else \
+            np.zeros(0, dtype=np.uint8)
+        return data, offsets
 
     def end(self) -> bool:
         again = C.c_int32()
