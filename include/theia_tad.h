@@ -302,6 +302,41 @@ int tad_stream_push_text(tad_job *job, const tad_columns *block, const tad_text_
  * TAD_ERR_STATE before completion and for a slot the job did not take as text.  Any thread. */
 int tad_job_names(tad_job *job, int32_t slot, const uint8_t **bytes, const uint64_t **offsets, uint32_t *count);
 
+/* ---- Row predicates of a streamed job's text slots ---------------------------------------------------------------
+ * Replaces: the String predicates of the aggregated-flow queries (anomaly_detection.py:566-609), which the host can no
+ * longer apply once a block hands its String key columns over as text.  The engine evaluates them on the GPU, once per
+ * distinct name while the first round builds the dictionaries, and drops the rows that fail:
+ *   TAD_NAME_ANY        every name                                                      (no predicate on the slot)
+ *   TAD_NAME_EQ         the name's bytes equal the pattern's                  podName = x, podNamespace = x (:566-575),
+ *                                                                             destinationServicePortName = x (:598-602),
+ *                                                                             destinationIP = x (:590-592)
+ *   TAD_NAME_NONEMPTY   a name of length > 0                                  podLabels <> '' (:577-578),
+ *                                                                             destinationServicePortName <> '' (:603-604)
+ *   TAD_NAME_ICONTAINS  pattern.lower() in name.lower(), as Python has it     ilike(podLabels, '%x%') (:560-565), with
+ *                       for a UTF-8 name and an ASCII pattern: A-Z fold to    '%' and '_' in x taken literally, as the
+ *                       a-z; U+0130 (C4 B0) folds to 'i' followed by          host mirror takes them
+ *                       U+0307, U+212A (E2 84 AA) to 'k' (the only two non-ASCII code points that lower-case to ASCII);
+ *                       every other byte compares exactly.  A pattern byte >= 0x80 is TAD_ERR_INVALID_ARG at submit.
+ *   proto_eq            -1 = none; 0..255: keep only rows whose proto byte equals it    flowType = 3 (:587-589)
+ * A row is kept when every slot's predicate holds for its name, proto_eq holds, and the time-window and ns_ignore filters
+ * hold.  Dropped rows count as filtered: rows_kept, the per-residue round-consistency counts and the host row store see
+ * only kept rows.  The dictionaries still hold every name of the job's rows (tad_job_names), kept or not.
+ *
+ * TAD_ERR_INVALID_ARG, the context usable afterwards in every case: at submit for a bad op, a NULL pattern with a nonzero
+ * length, an ICONTAINS pattern byte >= 0x80 or proto_eq outside -1..255 (the job is returned FAILED); at the first push
+ * (the job fails) for a predicate on a slot the first block does not give as text, or proto_eq without a proto column or
+ * without any text slot.  Single GPU and host blocks only, as for tad_stream_push_text. */
+enum { TAD_NAME_ANY = 0, TAD_NAME_EQ = 1, TAD_NAME_NONEMPTY = 2, TAD_NAME_ICONTAINS = 3 };
+typedef struct {
+    int32_t op[2];              /* per text slot (0 = src_ip, 1 = dst_ip): TAD_NAME_*                                    */
+    const uint8_t *pattern[2];  /* EQ / ICONTAINS; copied by the call                                                    */
+    uint32_t pattern_len[2];
+    int32_t proto_eq;           /* -1 = none; 0..255: keep only rows whose proto byte equals it                          */
+} tad_stream_filter;
+/* tad_submit_stream with row predicates; a NULL filter is tad_submit_stream. */
+int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, const tad_stream_filter *filter,
+                               tad_job **out);
+
 const char *tad_strerror(int err);
 int tad_abi_version(void);
 

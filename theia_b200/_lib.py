@@ -22,7 +22,8 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
            "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
-           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names")
+           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered")
+TAD_NAME_OPS = {"any": 0, "eq": 1, "nonempty": 2, "icontains": 3}
 
 
 class TadConfig(C.Structure):
@@ -39,6 +40,10 @@ class TadColumns(C.Structure):
 
 class TadTextColumn(C.Structure):
     _fields_ = [("bytes", C.c_void_p), ("nbytes", C.c_uint64), ("marks", C.c_void_p)]
+
+
+class TadStreamFilter(C.Structure):
+    _fields_ = [("op", C.c_int32 * 2), ("pattern", C.c_void_p * 2), ("pattern_len", C.c_uint32 * 2), ("proto_eq", C.c_int32)]
 
 
 class TadJobSpec(C.Structure):
@@ -85,6 +90,9 @@ def load():
     L.tad_alloc_ns_columns.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_submit.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.POINTER(TadColumns), C.POINTER(C.c_void_p)]
     L.tad_submit_stream.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(C.c_void_p)]
+    L.tad_submit_stream_filtered.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(TadStreamFilter),
+                                             C.POINTER(C.c_void_p)]
+    L.tad_debug_name_match.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     L.tad_stream_push.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_stream_end.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
     L.tad_stream_push_text.argtypes = [C.c_void_p, C.POINTER(TadColumns), C.POINTER(TadTextColumn), C.POINTER(TadTextColumn)]

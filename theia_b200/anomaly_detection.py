@@ -326,13 +326,16 @@ def _dictionary_ids(col, idx, dictionary: Dictionary) -> np.ndarray:
 
 
 def _branch_columns(flows: dict, plan: QueryPlan, br: Branch, masks: tuple, dicts: dict, ns_dict: Dictionary,
-                    ipv4_as_u32: bool, text_slots=()) -> dict:
+                    ipv4_as_u32: bool, text_slots=(), keep_all: bool = False) -> dict:
     """One branch's engine columns from a flows table or one block of it: the host predicates, then key slots,
     ``flow_end`` / ``value`` and, with an ignore list, the namespace ids.  ``ipv4_as_u32``: an address column of IPv4 text
     becomes its u32 value (a whole table); otherwise text addresses go through the dictionary like every other String
     key, which keeps a name's id the same in every block of a stream.  ``text_slots``: key slots the engine encodes from
-    the block's text itself (left None here)."""
-    idx = np.flatnonzero(_host_mask(flows, plan, br, *masks))
+    the block's text itself (left None here).  ``keep_all``: every row, the host predicates left to the engine."""
+    if keep_all:
+        idx = np.arange(len(flows["flowEndSeconds"]))
+    else:
+        idx = np.flatnonzero(_host_mask(flows, plan, br, *masks))
     cols = {}
     for slot in KEY_SLOTS:
         src = br.key.get(slot)
@@ -423,7 +426,9 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
     ``device_text``: in connection mode, the two address columns go to the engine as the block's String column bytes
     (``StringColumn.text()``, tad_stream_push_text) and are dictionary-encoded on the GPU; their dictionaries come back
     as ``clickhouse_native.Names`` (tad_job_names).  Connection mode is the one mode whose host mask keeps every row and
-    reads no key text; the pod / svc / external modes keep their host encoding whatever ``device_text`` says."""
+    reads no key text; with ``device_text=True`` the pod / svc / external modes keep their host encoding.
+    ``device_text="all"``: those modes push their String keys as text too, every row of a block, and the engine
+    evaluates their string predicates on the GPU (tad_submit_stream_filtered; :func:`_device_text_branches`)."""
     from .clickhouse_native import Names
     if algo_type not in VALID_ALGOS:
         raise ValueError("Algorithm should be in {}".format(" or ".join(VALID_ALGOS)))
@@ -437,24 +442,46 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
     masks = (pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
     # as in run_engine: the window's lower bound reaches the engine only through a flow_start key column
     start = _epoch(plan.start_time) if all("flow_start" in br.key for br in plan.branches) else 0
-    text = {"src_ip": "sourceIP", "dst_ip": "destinationIP"} if device_text and not plan.agg_flow else {}
+    branch_text, text_filter = [{} for _ in plan.branches], None
+    head, rest = [], None
+    if device_text == "all":
+        # the first round's first block is read before the submit: whether the mode's keys can go as text depends on it
+        rest = iter(blocks())
+        head.append(next(rest, None))
+        branch_text, text_filter = _device_text_branches(plan, head[0], *masks)
+    elif device_text and not plan.agg_flow:
+        branch_text = [{"src_ip": "sourceIP", "dst_ip": "destinationIP"}]
+    text_cols = {c for bt in branch_text for c in bt.values()}
+
+    def round0():
+        while head:
+            b = head.pop()
+            if b is not None:
+                yield b
+        yield from (blocks() if rest is None else rest)
+
+    # the namespace columns of an ignore list stay host-encoded, also where they are a text key
+    host_cols = {"sourcePodNamespace", "destinationPodNamespace"} if plan.ns_ignore else set()
     pushed_text = False
+    kw = {} if text_filter is None else {"text_filter": text_filter}
     job = engine.submit_stream(algo=algo_type, reducer=plan.reducer, start_time=start, end_time=_epoch(plan.end_time),
-                               tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint))
+                               tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint), **kw)
     if on_job is not None:
         on_job(job)
     try:
         rounds, again = 0, True
         while again:
-            for block in blocks():
-                raw = {slot: block[c] for slot, c in text.items()}
-                flows = _block_table({k: v for k, v in block.items() if k not in text.values()})
+            for block in (round0() if rounds == 0 else blocks()):
+                raw = {c: block[c] for c in text_cols}
+                flows = _block_table({k: v for k, v in block.items() if k not in text_cols or k in host_cols})
                 del block
-                for br in plan.branches:
-                    cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False, text_slots=raw)
+                for br, bt in zip(plan.branches, branch_text):
+                    slots = {slot: raw[c] for slot, c in bt.items()}
+                    cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False, text_slots=slots,
+                                           keep_all=text_filter is not None)
                     if len(cols["flow_end"]):
-                        if raw:
-                            job.push(cols, text={slot: col.text() for slot, col in raw.items()})
+                        if slots:
+                            job.push(cols, text={slot: col.text() for slot, col in slots.items()})
                             pushed_text = True
                         else:
                             job.push(cols)
@@ -466,7 +493,7 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
         st["rounds"] = rounds
         got = job.result()
         if pushed_text:
-            for slot in text:
+            for slot in {s for bt in branch_text for s in bt}:
                 dicts[slot] = Names(*job.names(slot))
     except BaseException:
         job.cancel()
@@ -476,6 +503,39 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
             on_job(None)
         job.release()
     return got, st, plan, dicts
+
+
+def _device_text_branches(plan: QueryPlan, first, pod_label, pod_name, pod_namespace, external_ip, svc_port_name):
+    """``device_text="all"``: per branch the key slots the engine takes as text ({slot: flows column}) and the job's row
+    predicates (engine.submit_stream's ``text_filter``; None in connection mode, which has none).  A mode whose
+    conditions the engine cannot express keeps its host encoding (no text, no predicates): a non-ASCII ``--pod-label``
+    (the GPU's ILIKE folds ASCII patterns only), or blocks that carry ``flowStartSeconds`` where it is not a key (its
+    lower bound is a host predicate then; ``first`` is the job's first block, None for an empty round)."""
+    host = [{} for _ in plan.branches], None
+    if not plan.agg_flow:
+        return [{"src_ip": "sourceIP", "dst_ip": "destinationIP"}], None
+    if plan.start_time and first is not None and "flowStartSeconds" in first and \
+            any("flow_start" not in br.key for br in plan.branches):
+        return host
+    if plan.agg_flow == "external":
+        flt = {"proto_eq": 3}
+        if external_ip:
+            flt["dst_ip"] = ("eq", external_ip.encode())
+        return [{"dst_ip": "destinationIP"}], flt
+    if plan.agg_flow == "svc":
+        return [{"src_ip": "destinationServicePortName"}], \
+            {"src_ip": ("eq", svc_port_name.encode()) if svc_port_name else ("nonempty", b"")}
+    if pod_label and not pod_label.isascii():
+        return host
+    if pod_label:
+        flt = {"dst_ip": ("icontains", pod_label.encode())}
+    elif pod_name:
+        flt = {"dst_ip": ("eq", pod_name.encode())}
+    else:
+        flt = {"dst_ip": ("nonempty", b"")}
+    if pod_namespace and (pod_label or pod_name):
+        flt["src_ip"] = ("eq", pod_namespace.encode())
+    return [{"src_ip": br.key["src_ip"], "dst_ip": br.key["dst_ip"]} for br in plan.branches], flt
 
 
 def _ip_text(dictionary: "Dictionary", v: int) -> str:
@@ -750,7 +810,7 @@ def _select_blocks(transport, sql: str):
 
 def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str, device_text: bool = False):
     """main()'s job on streamed input (TAD_STREAM_INPUT=1): (result SoA, plan, dictionaries).  ``device_text``
-    (TAD_DEVICE_TEXT=1, text addresses only): run_engine_stream's ``device_text``."""
+    (TAD_DEVICE_TEXT=1: True, text addresses only; TAD_DEVICE_TEXT=all: "all"): run_engine_stream's ``device_text``."""
     hint = 0
     if hasattr(transport, "count"):
         hint = int(transport.count(count_sql(plan))) * len(plan.branches)    # pod: every row feeds both branches
@@ -762,7 +822,7 @@ def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, t
         return run_engine_stream(engine, a["algo"], _select_blocks(transport, sql), a["start_time"], a["end_time"], tad_id,
                                  a["ns_ignore_list"], a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
                                  a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None, rows_hint=hint,
-                                 device_text=device_text and not ipv4_pushdown)
+                                 device_text=False if ipv4_pushdown else device_text)
     try:
         got, _st, plan, dicts = run(pushdown)
     except Exception as e:
@@ -798,8 +858,9 @@ def main(argv=None, engine=None, transport=None) -> int:
         pushdown = os.getenv("TAD_IPV4_PUSHDOWN", "0") == "1"
         if os.getenv("TAD_STREAM_INPUT", "0") == "1":       # blocks pushed to a streamed job as they are decoded
             tad_id = a["id"] or str(uuid.uuid4())
-            # TAD_DEVICE_TEXT=1: the address text of a connection-mode job is dictionary-encoded on the GPU (no push-down)
-            device_text = os.getenv("TAD_DEVICE_TEXT", "0") == "1" and not pushdown
+            # TAD_DEVICE_TEXT=1: the address text of a connection-mode job is dictionary-encoded on the GPU (no push-down);
+            # TAD_DEVICE_TEXT=all: every mode's String keys, its string predicates evaluated on the GPU
+            device_text = {"1": True, "all": "all"}.get(os.getenv("TAD_DEVICE_TEXT", "0"), False) if not pushdown else False
             got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id, device_text)
         else:
             sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=pushdown)

@@ -419,18 +419,32 @@ def tadetector_block_from_result(got: dict, plan, dicts: dict, algo_type: str, t
             return ("ids", np.asarray(got[slot]), list(d.names))
         return ("ipv4", np.ascontiguousarray(got[slot], dtype=np.uint32), None)
 
+    def name_col(slot):
+        d = dicts[slot]
+        if isinstance(d, Names):
+            return ("names", got[slot], d)
+        return ("ids", np.asarray(got[slot]), list(d.names))
+
+    def labels_col(slot):
+        d, ids = dicts[slot], np.asarray(got[slot])
+        if isinstance(d, Names):                # cleaned once per distinct name the result uses
+            used, inv = np.unique(ids, return_inverse=True)
+            names = [remove_meaningless_labels(bytes(d.data[int(d.offsets[k]):int(d.offsets[k + 1])]).decode())
+                     for k in used]
+            return ("ids", inv.reshape(-1), names)
+        return ("ids", ids, [remove_meaningless_labels(x) for x in d.names])
+
     if plan.agg_flow == "pod":
-        cols["podNamespace"] = ("ids", np.asarray(got["src_ip"]), list(dicts["src_ip"].names))
-        second = list(dicts["dst_ip"].names)
+        cols["podNamespace"] = name_col("src_ip")
         if plan.branches[0].group[1] == "podLabels":
-            cols["podLabels"] = ("ids", np.asarray(got["dst_ip"]), [remove_meaningless_labels(x) for x in second])
+            cols["podLabels"] = labels_col("dst_ip")
         else:
-            cols["podName"] = ("ids", np.asarray(got["dst_ip"]), second)
+            cols["podName"] = name_col("dst_ip")
         cols["direction"] = ("ids", (np.asarray(got["proto"]) != 0).astype(np.int64), ["inbound", "outbound"])
     elif plan.agg_flow == "external":
         cols["destinationIP"] = ip_col("dst_ip")
     elif plan.agg_flow == "svc":
-        cols["destinationServicePortName"] = ("ids", np.asarray(got["src_ip"]), list(dicts["src_ip"].names))
+        cols["destinationServicePortName"] = name_col("src_ip")
     else:
         cols["sourceIP"], cols["destinationIP"] = ip_col("src_ip"), ip_col("dst_ip")
         cols["sourceTransportPort"] = ("num", got["src_port"], None)

@@ -172,6 +172,11 @@ struct tad_job {
     bool text[2] = {false, false};
     std::vector<uint8_t> names[2];
     std::vector<uint64_t> names_off[2];
+    // row predicates (tad_submit_stream_filtered): per text slot a TAD_NAME_* op and its pattern, and proto_eq (-1: none)
+    int32_t name_op[2] = {TAD_NAME_ANY, TAD_NAME_ANY};
+    std::vector<uint8_t> name_pat[2];
+    int32_t proto_eq = -1;
+    bool filtered() const { return name_op[0] != TAD_NAME_ANY || name_op[1] != TAD_NAME_ANY || proto_eq >= 0; }
 };
 
 struct tad_ctx {
@@ -239,8 +244,10 @@ struct tad_ctx {
     // text key slots (DESIGN.md section 10, "Text keys on the device"): one dictionary per slot, alive for one job
     struct TextSlot {
         DevBuf slots, minrow, slot_id, arena, off, hash, state;
+        DevBuf keep, pat;                           // a filtered job: the predicate's byte per name; its pattern
         uint32_t cap = 0;                           // table slots (0: no dictionary yet)
         uint64_t names_ub = 0, bytes_ub = 0;        // upper bounds of its names / arena bytes, exact after each readback
+        std::vector<DevBuf *> bufs() { return {&slots, &minrow, &slot_id, &arena, &off, &hash, &state, &keep, &pat}; }
     } tdict[2];
     DevBuf tstage, tscratch;                        // a chunk's marks and text bytes; the encode scratch
 };
@@ -322,7 +329,7 @@ std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
                                &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
                                &ctx->stage, &ctx->pcnt, &ctx->ostage, &ctx->tstage, &ctx->tscratch};
     for (auto &t : ctx->tdict)
-        for (DevBuf *b : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) v.push_back(b);
+        for (DevBuf *b : t.bufs()) v.push_back(b);
     for (int i = 0; i < 10; i++) v.push_back(&ctx->d_col[i]);
     return v;
 }
@@ -1508,7 +1515,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     auto dict_bytes = [&]() {
         size_t b = 0;
         for (auto &t : ctx->tdict)
-            for (DevBuf *x : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) b += x->cap;
+            for (DevBuf *x : t.bufs()) b += x->cap;
         return b;
     };
     // the first round's pass columns are freed for the dictionaries: the round only counts (or goes on to the store)
@@ -1570,7 +1577,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         auto ok = [&]() {
             const uint64_t nn = d.names_ub + n;
             return d.cap && 2 * nn <= d.cap && d.arena.cap >= d.bytes_ub + span && d.off.cap >= (nn + 1) * 8 &&
-                   d.hash.cap >= nn * 8;
+                   d.hash.cap >= nn * 8 && (!job->name_op[t] || d.keep.cap >= nn);
         };
         if (!ok()) {
             if (!d.state.p) {                     // the job's first text chunk of this slot
@@ -1580,6 +1587,11 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 CU(cudaMemsetAsync(d.state.p, 0, 64, ctx->copy_stream));
                 grow_dict_buf(d.off, 4096, 0);
                 CU(cudaMemsetAsync(d.off.p, 0, 8, ctx->copy_stream));
+                if (const size_t m = job->name_pat[t].size()) {     // the predicate's pattern, for the match kernel
+                    dict_room(exact_bytes(m));
+                    ensure(ctx, d.pat, m);
+                    CU(cudaMemcpyAsync(d.pat.p, job->name_pat[t].data(), m, cudaMemcpyHostToDevice, ctx->copy_stream));
+                }
             } else {
                 text_sync();
             }
@@ -1588,6 +1600,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 fail(TAD_ERR_INVALID_ARG, "invalid request: a text key slot may hold at most 2^30 distinct names");
             grow_dict_buf(d.off, (nn + 1) * 8, (names + 1) * 8);
             grow_dict_buf(d.hash, std::max<uint64_t>(nn, 512) * 8, names * 8);
+            if (job->name_op[t]) grow_dict_buf(d.keep, std::max<uint64_t>(nn, 4096), names);
             grow_dict_buf(d.arena, std::max<uint64_t>(bytes + span, 4096), bytes);
             if (!d.cap || 2 * nn > d.cap) {       // a larger table, the names re-inserted on the device
                 uint64_t c = 1024;                // nn <= 2^30: c <= 2^31
@@ -1651,8 +1664,13 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         }
         return n;
     };
-    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids at dst[t] (device u32)
-    auto text_encode = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, char *const *dst) {
+    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids at dst[t] (device u32).  A filtered job then
+    // marks the rows its predicates drop (the first round also evaluates them on the names the chunk added); `proto` is
+    // the chunk's staged proto column.
+    const bool filt = job->filtered();
+    const int mark = filt ? (job->text[0] ? 1 : 2) : 0;          // the slot whose ids carry the drop bit
+    auto text_encode = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, char *const *dst,
+                           const char *proto) {
         for (int t = 0; t < 2; t++) {
             if (!job->text[t]) continue;
             const uint64_t s0 = lo / 32, s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
@@ -1667,6 +1685,24 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                                   reinterpret_cast<const uint64_t *>(m), (uint32_t)(s1 - s0), s0 * 32, rows, lo, n,
                                   ctx->tscratch.p, ctx->tscratch.cap, reinterpret_cast<uint32_t *>(dst[t])));
             acc.launches += kTextLaunches;
+            if (job->name_op[t] && sweeps == 0) {     // an open dictionary: its new names get their predicate byte
+                auto &d = ctx->tdict[t];
+                CU(launch_text_match(ctx->copy_stream, dict_of(t), (uint8_t *)d.keep.p, job->name_op[t],
+                                     (const uint8_t *)d.pat.p, (uint32_t)job->name_pat[t].size(), n));
+                acc.launches++;
+            }
+        }
+        if (filt) {
+            TextMark m{};
+            for (int t = 0; t < 2; t++) {
+                m.ids[t] = reinterpret_cast<const uint32_t *>(dst[t]);
+                m.keep[t] = job->name_op[t] ? (const uint8_t *)ctx->tdict[t].keep.p : nullptr;
+            }
+            m.proto = reinterpret_cast<const uint8_t *>(proto);
+            m.proto_eq = job->proto_eq;
+            m.mark = reinterpret_cast<uint32_t *>(dst[mark - 1]);
+            CU(launch_text_mark(ctx->copy_stream, m, n));
+            acc.launches++;
         }
     };
     // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M).  Text slots: `tx`, of
@@ -1691,7 +1727,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             if (nchunk >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
             ColPtrs c{};
             char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-            char *ids[2] = {nullptr, nullptr};
+            char *ids[2] = {nullptr, nullptr}, *proto = nullptr;
             for (int i = 0; i < 10; i++) {
                 if (!staged(i)) continue;
                 const size_t w = col_bytes(i, 1);
@@ -1700,14 +1736,15 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 else
                     CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(b, i)) + lo_r * w, n * w,
                                        cudaMemcpyHostToDevice, ctx->copy_stream));
+                if (i == 4) proto = dst;
                 set_col(c, i, dst);
                 dst += exact_bytes(col_bytes(i, chunk));
             }
-            if (text) text_encode(tx, origin + n_all, origin + lo_r, n, ids);
+            if (text) text_encode(tx, origin + n_all, origin + lo_r, n, ids, proto);
             CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
             CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
             CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
-                                 d_cnt));
+                                 d_cnt, mark));
             acc.launches++;
             CU(cudaEventRecord(ctx->stage_ev[h], st));
         }
@@ -1793,10 +1830,12 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     };
     // count / scan / scatter `n` <= chunk device rows into the next out-stage half, then issue the copies of the previous
     // one (its counts are back by now; this chunk's copies are on the bus meanwhile).  `totals`: count them for the job.
+    // `totals` also tells staged rows (marked rows of a filtered job among them) from the pass columns' clean ones.
     auto pack = [&](const ColPtrs &c, uint64_t n, bool totals) {
         const int o = (int)(npack++ & 1);
         CU(cudaStreamWaitEvent(st, ctx->ost_ev[o], 0));      // the copies that last read out-stage half o are done
-        CU(launch_residue_pack(st, c, n, f, pscratch, pack_scratch, d_chunk, totals ? d_cnt : nullptr, ost[o]));
+        CU(launch_residue_pack(st, c, n, f, pscratch, pack_scratch, d_chunk, totals ? d_cnt : nullptr, ost[o],
+                               totals ? mark : 0));
         acc.launches += 3;
         CU(cudaMemcpyAsync(ctx->h_chunk + kMaxPasses * o, d_chunk, kMaxPasses * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaEventRecord(ctx->cnt_ev[o], st));
@@ -1851,7 +1890,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             uint64_t n = std::min(chunk - fill, b.rows - lo);
             if (text) n = text_fit(tx, b.rows, lo, n);
             char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-            char *ids[2] = {nullptr, nullptr};
+            char *ids[2] = {nullptr, nullptr}, *proto = nullptr;
             for (int i = 0; i < 10; i++) {
                 if (!staged(i)) continue;
                 const size_t w = col_bytes(i, 1);
@@ -1861,9 +1900,10 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                     CU(cudaMemcpyAsync(dst + fill * w, static_cast<const char *>(col_ptr(b, i)) + lo * w, n * w,
                                        b.mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
                                        ctx->copy_stream));
+                if (i == 4) proto = dst + fill * w;
                 dst += exact_bytes(col_bytes(i, chunk));
             }
-            if (text) text_encode(tx, b.rows, lo, n, ids);
+            if (text) text_encode(tx, b.rows, lo, n, ids, proto);
             fill += n;
             lo += n;
             if (fill == chunk) pack_half();
@@ -2133,7 +2173,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         job->names_off[t].assign(names + 1, 0);
         if (bytes) CU(cudaMemcpy(job->names[t].data(), d.arena.p, bytes, cudaMemcpyDeviceToHost));
         if (names) CU(cudaMemcpy(job->names_off[t].data(), d.off.p, (names + 1) * 8, cudaMemcpyDeviceToHost));
-        for (DevBuf *x : {&d.slots, &d.minrow, &d.slot_id, &d.arena, &d.off, &d.hash, &d.state}) free_buf(ctx, *x);
+        for (DevBuf *x : d.bufs()) free_buf(ctx, *x);
         d.cap = 0;
     }
     return passes;
@@ -2244,7 +2284,7 @@ void worker_main(tad_ctx *ctx)
             cudaStreamSynchronize(ctx->d2h_stream);
             cudaGetLastError();
             for (auto &t : ctx->tdict) {       // a dictionary lives for one job
-                for (DevBuf *b : {&t.slots, &t.minrow, &t.slot_id, &t.arena, &t.off, &t.hash, &t.state}) {
+                for (DevBuf *b : t.bufs()) {
                     if (b->p) cudaFree(b->p);
                     ctx->held -= b->cap;
                     *b = DevBuf{};
@@ -2416,6 +2456,16 @@ int check_block(const tad_job *job, const tad_columns *b, const tad_text_column 
         return TAD_ERR_INVALID_ARG;
     }
     if (job->in.pushed == 0) {
+        for (int t = 0; t < 2; t++)
+            if (job->name_op[t] != TAD_NAME_ANY && !txt[t]) {
+                snprintf(msg, n, "invalid request: a row predicate on %s, which the first block does not give as text",
+                         t ? "dst_ip" : "src_ip");
+                return TAD_ERR_INVALID_ARG;
+            }
+        if (job->proto_eq >= 0 && (!b->proto || (!txt[0] && !txt[1]))) {
+            snprintf(msg, n, "invalid request: proto_eq needs the proto column and a text key slot");
+            return TAD_ERR_INVALID_ARG;
+        }
         if (job->spec.start_time && !b->flow_start) {
             snprintf(msg, n, "invalid request: start_time needs the flow_start column");
             return TAD_ERR_INVALID_ARG;
@@ -2630,6 +2680,46 @@ int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint
     tad_job *job = new tad_job();
     job->stream = true;
     job->rows_hint = rows_hint;
+    tad_columns none{};
+    return submit_job(ctx, job, spec, &none, out);
+}
+
+int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, const tad_stream_filter *filter,
+                               tad_job **out)
+{
+    if (!filter) return tad_submit_stream(ctx, spec, rows_hint, out);
+    if (!ctx || !spec || !out) return TAD_ERR_INVALID_ARG;
+    const char *bad = nullptr;
+    for (int t = 0; t < 2 && !bad; t++) {
+        const int op = filter->op[t];
+        const uint32_t m = filter->pattern_len[t];
+        if (op < TAD_NAME_ANY || op > TAD_NAME_ICONTAINS) bad = "a row predicate op is not a TAD_NAME_* value";
+        else if (m && !filter->pattern[t]) bad = "a row predicate pattern is NULL with a nonzero length";
+        else if (op == TAD_NAME_ICONTAINS)
+            for (uint32_t k = 0; k < m && !bad; k++)
+                if (filter->pattern[t][k] >= 0x80) bad = "an ICONTAINS pattern holds a byte >= 0x80 (ASCII only)";
+    }
+    if (!bad && (filter->proto_eq < -1 || filter->proto_eq > 255)) bad = "proto_eq is outside -1..255";
+    tad_job *job = new tad_job();
+    job->stream = true;
+    job->rows_hint = rows_hint;
+    if (bad) {                   // returned FAILED, as submit_job returns an invalid job
+        job->ctx = ctx;
+        job->spec = *spec;
+        job->st.total_stages = kTotalStages;
+        job->st.state = TAD_STATE_FAILED;
+        job->st.error = TAD_ERR_INVALID_ARG;
+        snprintf(job->st.err_msg, sizeof(job->st.err_msg), "error in creating AnomalyDetector: invalid request: %s", bad);
+        *out = job;
+        return TAD_ERR_INVALID_ARG;
+    }
+    for (int t = 0; t < 2; t++) {
+        job->name_op[t] = filter->op[t];
+        // only EQ and ICONTAINS read a pattern
+        if (filter->op[t] == TAD_NAME_EQ || filter->op[t] == TAD_NAME_ICONTAINS)
+            job->name_pat[t].assign(filter->pattern[t], filter->pattern[t] + filter->pattern_len[t]);
+    }
+    job->proto_eq = filter->proto_eq;
     tad_columns none{};
     return submit_job(ctx, job, spec, &none, out);
 }

@@ -24,6 +24,7 @@
 #include <atomic>
 #include <cstdio>
 #include <mutex>
+#include <type_traits>
 
 namespace tad {
 
@@ -263,7 +264,22 @@ __global__ void __launch_bounds__(256) partition_kernel(ColPtrs c, uint64_t R, R
 // counted under its low kMaxPasses hash bits, so the first sweep gives the exact size of every pass of any P <= 64.
 // Rows past `cap` are counted but not written: the host then replans and sweeps again.
 // ----------------------------------------------------------------------------------------
-template <bool VEC>
+// Rows of a filtered streamed job whose text predicates failed carry bit 31 in the id of the job's first text slot
+// (tad_text.h, kTextDropped): MARK = 1 for src_ip, 2 for dst_ip, 0 for a job without predicates.  Such a row is dropped as
+// the stage-A filters drop one; every row that stays carries a clean id, so its key is unchanged.
+template <int MARK>
+__device__ __forceinline__ void drop_marked(RowRegs (&r)[8])
+{
+    if constexpr (MARK != 0) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const uint32_t id = MARK == 1 ? (uint32_t)(r[i].a >> 32) : (uint32_t)r[i].a;
+            r[i].keep = r[i].keep && !(id >> 31);
+        }
+    }
+}
+
+template <bool VEC, int MARK>
 __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t pass_mask, uint32_t pass_val,
                                                          PassCols o, uint32_t cap, unsigned long long *__restrict__ cursor,
                                                          unsigned long long *__restrict__ counts)
@@ -287,6 +303,7 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
                 else r[i].keep = false;
             }
         }
+        drop_marked<MARK>(r);
         uint32_t mine = 0;
 #pragma unroll
         for (int i = 0; i < 8; i++) {
@@ -356,7 +373,7 @@ __device__ __forceinline__ void load_tile_rows(const ColPtrs &c, const RowFilter
 
 // cnt[j * ntiles + tile] = filtered rows of residue j in 2048-row tile `tile`; chunk[j] and totals[j] (null: skipped) gain
 // the residue's rows.  The residue is counted as pass_split_kernel counts it.
-template <bool VEC>
+template <bool VEC, int MARK>
 __global__ void __launch_bounds__(256) residue_count_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t ntiles,
                                                             uint32_t *__restrict__ cnt, uint32_t *__restrict__ chunk,
                                                             unsigned long long *__restrict__ totals)
@@ -369,6 +386,7 @@ __global__ void __launch_bounds__(256) residue_count_kernel(ColPtrs c, uint64_t 
         __syncthreads();
         RowRegs r[8];
         load_tile_rows(c, f, R, (uint64_t)tile * 2048 + (uint64_t)tid * 8, VEC, r);
+        drop_marked<MARK>(r);
 #pragma unroll
         for (int i = 0; i < 8; i++)
             if (r[i].keep) atomicAdd(&s_cnt[(uint32_t)key_hash(r[i].a, r[i].b, r[i].proto) & (kMaxPasses - 1)], 1u);
@@ -386,7 +404,7 @@ __global__ void __launch_bounds__(256) residue_count_kernel(ColPtrs c, uint64_t 
 
 // Every filtered row to out[off[j * ntiles + tile] + its rank among the tile's rows of residue j], ranked through shared
 // counters.  Rows are written from lane pairs (pair_store): every lane of a CTA runs every tile.
-template <bool VEC>
+template <bool VEC, int MARK>
 __global__ void __launch_bounds__(256) residue_scatter_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t ntiles,
                                                               const uint32_t *__restrict__ off, Row32 *__restrict__ out)
 {
@@ -397,6 +415,7 @@ __global__ void __launch_bounds__(256) residue_scatter_kernel(ColPtrs c, uint64_
         __syncthreads();
         RowRegs r[8];
         load_tile_rows(c, f, R, (uint64_t)tile * 2048 + (uint64_t)tid * 8, VEC, r);
+        drop_marked<MARK>(r);
         Row32 *dst[8];
 #pragma unroll
         for (int i = 0; i < 8; i++)
@@ -1547,16 +1566,25 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
                               uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
-                              unsigned long long *counts)
+                              unsigned long long *counts, int mark)
 {
     if (R == 0) return cudaSuccess;
     const uint64_t tiles = (R + 2047) / 2048;
     const uint64_t lim = (uint64_t)num_sms() * 8;
     const uint32_t grid = (uint32_t)(tiles < lim ? tiles : lim);
-    if (cols_aligned16(c))
-        pass_split_kernel<true><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
-    else
-        pass_split_kernel<false><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
+    auto go = [&](auto vec, auto mk) {
+        pass_split_kernel<decltype(vec)::value, decltype(mk)::value><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out,
+                                                                                          cap, cursor, counts);
+    };
+    const bool vec = cols_aligned16(c);
+    using T = std::true_type;
+    using F = std::false_type;
+    using M0 = std::integral_constant<int, 0>;
+    using M1 = std::integral_constant<int, 1>;
+    using M2 = std::integral_constant<int, 2>;
+    if (mark == 1) vec ? go(T{}, M1{}) : go(F{}, M1{});
+    else if (mark == 2) vec ? go(T{}, M2{}) : go(F{}, M2{});
+    else vec ? go(T{}, M0{}) : go(F{}, M0{});
     return cudaGetLastError();
 }
 
@@ -1573,7 +1601,7 @@ size_t residue_pack_scratch_bytes(uint64_t max_rows)
 }
 
 cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, void *scratch,
-                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out)
+                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out, int mark)
 {
     cudaError_t e = cudaMemsetAsync(chunk, 0, kMaxPasses * sizeof(uint32_t), st);
     if (e != cudaSuccess || R == 0) return e;
@@ -1588,17 +1616,29 @@ cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, c
     const uint32_t lim = (uint32_t)num_sms() * 8;
     const uint32_t grid = ntiles < lim ? ntiles : lim;
     const bool vec = cols_aligned16(c);
-    if (vec)
-        residue_count_kernel<true><<<grid, 256, 0, st>>>(c, R, f, ntiles, cnt, chunk, totals);
-    else
-        residue_count_kernel<false><<<grid, 256, 0, st>>>(c, R, f, ntiles, cnt, chunk, totals);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = exclusive_scan_u32(temp, temp_bytes, cnt, off, (int)n, st)) != cudaSuccess) return e;
-    if (vec)
-        residue_scatter_kernel<true><<<grid, 256, 0, st>>>(c, R, f, ntiles, off, out);
-    else
-        residue_scatter_kernel<false><<<grid, 256, 0, st>>>(c, R, f, ntiles, off, out);
-    return cudaGetLastError();
+    auto count = [&](auto v, auto mk) {
+        residue_count_kernel<decltype(v)::value, decltype(mk)::value><<<grid, 256, 0, st>>>(c, R, f, ntiles, cnt, chunk, totals);
+    };
+    auto scatter = [&](auto v, auto mk) {
+        residue_scatter_kernel<decltype(v)::value, decltype(mk)::value><<<grid, 256, 0, st>>>(c, R, f, ntiles, off, out);
+    };
+    // both kernels for one (VEC, MARK) pair, the scan between them
+    auto pack = [&](auto v, auto mk) -> cudaError_t {
+        count(v, mk);
+        cudaError_t e2 = cudaGetLastError();
+        if (e2 != cudaSuccess) return e2;
+        if ((e2 = exclusive_scan_u32(temp, temp_bytes, cnt, off, (int)n, st)) != cudaSuccess) return e2;
+        scatter(v, mk);
+        return cudaGetLastError();
+    };
+    using T = std::true_type;
+    using F = std::false_type;
+    using M0 = std::integral_constant<int, 0>;
+    using M1 = std::integral_constant<int, 1>;
+    using M2 = std::integral_constant<int, 2>;
+    if (mark == 1) return vec ? pack(T{}, M1{}) : pack(F{}, M1{});
+    if (mark == 2) return vec ? pack(T{}, M2{}) : pack(F{}, M2{});
+    return vec ? pack(T{}, M0{}) : pack(F{}, M0{});
 }
 
 cudaError_t launch_store_unpack(cudaStream_t st, const Row32 *in, uint64_t n, const PassCols &out, uint64_t at)

@@ -15,6 +15,8 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 // are appended at out[*cursor ...) (rows past `cap` are dropped, *cursor still counts them); counts[kMaxPasses] gains
 // the filtered rows of every low-hash-bit residue.  Null key columns of `out` are skipped (they read as 0 anyway).
 // The cursor and counts are 64-bit: one sweep over a streamed round may hold more than 2^32 rows.
+// `mark` (here and in launch_residue_pack): 1 / 2 = a row whose src_ip / dst_ip id has bit 31 set (a failed text
+// predicate, tad_text.h) is dropped as well; 0 = no such bit.
 constexpr int kMaxPasses = 64;
 struct PassCols {
     uint32_t *src_ip, *dst_ip, *flow_start, *flow_end;
@@ -24,14 +26,14 @@ struct PassCols {
 };
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
                               uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
-                              unsigned long long *counts);
+                              unsigned long long *counts, int mark = 0);
 // Host row store: the rows of `c` that pass the stage-A filters, packed as Row32 records without the hash tag, grouped
 // by low-hash-bit residue (residue 0 first) into out[0, rows kept).  chunk[kMaxPasses] (u32, zeroed here) receives the
 // rows of every residue and totals[kMaxPasses] (null: skipped) gains them.  R <= the max_rows the scratch was sized for;
 // three launches.
 size_t residue_pack_scratch_bytes(uint64_t max_rows);
 cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, void *scratch,
-                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out);
+                                size_t scratch_bytes, uint32_t *chunk, unsigned long long *totals, Row32 *out, int mark = 0);
 // Stored rows in[0, n) -> out columns at rows [at, at + n); null key columns are skipped.  One launch.
 cudaError_t launch_store_unpack(cudaStream_t st, const Row32 *in, uint64_t n, const PassCols &out, uint64_t at);
 cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *offsets, uint32_t *cursor, uint32_t B,

@@ -20,7 +20,7 @@ __device__ __forceinline__ uint64_t name_hash(const uint8_t *s, uint32_t len)
     return h ^ (h >> 29);
 }
 
-__device__ __forceinline__ bool same_bytes(const uint8_t *a, uint32_t na, const uint8_t *b, uint32_t nb)
+__host__ __device__ __forceinline__ bool same_bytes(const uint8_t *a, uint32_t na, const uint8_t *b, uint32_t nb)
 {
     if (na != nb) return false;
     for (uint32_t k = 0; k < na; k++)
@@ -212,9 +212,94 @@ __global__ void text_rehash_kernel(TextDict d, const uint64_t *__restrict__ hash
     while (atomicCAS(d.slots + p, kEmpty, e) != kEmpty) p = (p + 1) & mask;
 }
 
+// Folded unit of s at byte k for the case-insensitive test (Python's str.lower() as far as it can meet an ASCII
+// pattern): A-Z -> a-z; U+0130 (C4 B0) -> 'i' and then a non-ASCII unit (its U+0307); U+212A (E2 84 AA) -> 'k'; every
+// other byte as it is.  `adv` = the bytes consumed; `last` = the unit ends the ASCII run (U+0130's combining dot follows).
+__host__ __device__ __forceinline__ uint8_t fold_unit(const uint8_t *s, uint32_t n, uint32_t k, uint32_t &adv, bool &last)
+{
+    const uint8_t c = s[k];
+    adv = 1;
+    last = false;
+    if (c >= 'A' && c <= 'Z') return (uint8_t)(c + 32);
+    if (c == 0xC4 && k + 1 < n && s[k + 1] == 0xB0) { adv = 2; last = true; return 'i'; }
+    if (c == 0xE2 && k + 2 < n && s[k + 1] == 0x84 && s[k + 2] == 0xAA) { adv = 3; return 'k'; }
+    return c;
+}
+
+// pattern.lower() in name.lower() for a UTF-8 name and an ASCII pattern.  Lower-cased non-ASCII code points other than
+// U+0130 and U+212A stay non-ASCII, so they can never meet a pattern byte and compare exactly.
+__host__ __device__ __forceinline__ bool name_icontains(const uint8_t *s, uint32_t n, const uint8_t *p, uint32_t m)
+{
+    if (m == 0) return true;
+    for (uint32_t start = 0; start < n; start++) {
+        uint32_t k = start, j = 0;
+        while (j < m && k < n) {
+            uint32_t adv;
+            bool last;
+            const uint8_t u = fold_unit(s, n, k, adv, last);
+            const uint8_t q = p[j] >= 'A' && p[j] <= 'Z' ? (uint8_t)(p[j] + 32) : p[j];
+            if (u != q) break;
+            j++;
+            k += adv;
+            if (last) break;
+        }
+        if (j == m) return true;
+    }
+    return false;
+}
+
+// The name predicate of a text slot (tad_stream_filter): TAD_NAME_ANY / EQ / NONEMPTY / ICONTAINS.
+__host__ __device__ __forceinline__ bool name_match(int op, const uint8_t *s, uint32_t n, const uint8_t *p, uint32_t m)
+{
+    switch (op) {
+    case kNameEq: return same_bytes(s, n, p, m);
+    case kNameNonEmpty: return n > 0;
+    case kNameIContains: return name_icontains(s, n, p, m);
+    default: return true;
+    }
+}
+
+// One thread per name the chunk may have added: the chunk's new names are ids [state[0] - state[3], state[0]).
+__global__ void text_match_kernel(TextDict d, uint8_t *__restrict__ keep, int op, const uint8_t *__restrict__ pat,
+                                  uint32_t pat_len, uint64_t n)
+{
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const uint64_t names = d.state[0], added = d.state[3];
+    if (k >= added) return;
+    const uint64_t id = names - added + k;
+    const uint64_t a = d.off[id];
+    keep[id] = name_match(op, d.arena + a, (uint32_t)(d.off[id + 1] - a), pat, pat_len) ? 1 : 0;
+}
+
+__global__ void text_mark_kernel(TextMark m, uint64_t n)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool keep = m.proto_eq < 0 || m.proto[i] == (uint8_t)m.proto_eq;
+    for (int t = 0; t < 2; t++)
+        if (m.keep[t]) keep = keep && m.keep[t][m.ids[t][i]];
+    if (!keep) m.mark[i] |= kTextDropped;
+}
+
 unsigned grid(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 }  // namespace
+
+cudaError_t launch_text_match(cudaStream_t st, const TextDict &d, uint8_t *keep, int op, const uint8_t *pat,
+                              uint32_t pat_len, uint64_t n)
+{
+    if (n == 0) return cudaSuccess;
+    text_match_kernel<<<grid(n), kThreads, 0, st>>>(d, keep, op, pat, pat_len, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_text_mark(cudaStream_t st, const TextMark &m, uint64_t n)
+{
+    if (n == 0) return cudaSuccess;
+    text_mark_kernel<<<grid(n), kThreads, 0, st>>>(m, n);
+    return cudaGetLastError();
+}
 
 size_t text_scratch_bytes(uint64_t n)
 {
@@ -255,3 +340,11 @@ cudaError_t launch_text_encode(cudaStream_t st, const TextDict &d, const uint8_t
 }
 
 }  // namespace tad
+
+// The device's name predicate run on the host, for the tests: 1 when `name` passes op / pattern, 0 when not, -1 for a bad op.
+extern "C" int tad_debug_name_match(int op, const uint8_t *name, uint32_t name_len, const uint8_t *pattern,
+                                    uint32_t pattern_len)
+{
+    if (op < tad::kNameAny || op > tad::kNameIContains) return -1;
+    return tad::name_match(op, name, name_len, pattern, pattern_len) ? 1 : 0;
+}

@@ -46,4 +46,27 @@ cudaError_t launch_text_encode(cudaStream_t st, const TextDict &d, const uint8_t
 constexpr uint32_t kTextPending = 0x80000000u;
 constexpr int kTextLaunches = 7;
 
+// Row predicates of a filtered streamed job (tad_stream_filter).  Name ops, as TAD_NAME_* of include/theia_tad.h:
+constexpr int kNameAny = 0, kNameEq = 1, kNameNonEmpty = 2, kNameIContains = 3;
+// A dropped row carries this bit in the id of the job's first text slot (ids are < 2^30); the split and pack kernels'
+// marked instances drop it.
+constexpr uint32_t kTextDropped = 0x80000000u;
+
+// keep[id] = the predicate `op` / pattern (device memory) on name id, for the names the chunk just encoded added to `d`
+// (ids [state[0] - state[3], state[0]); `n`, the chunk's rows, bounds their count).  Only while the dictionary is open.
+// One launch.
+cudaError_t launch_text_match(cudaStream_t st, const TextDict &d, uint8_t *keep, int op, const uint8_t *pat,
+                              uint32_t pat_len, uint64_t n);
+
+// One chunk's row predicates: a slot with keep[t] set fails a row whose name's keep byte is 0; proto_eq >= 0 fails a row
+// whose proto byte differs.  A failed row gets kTextDropped in mark[i] (the first text slot's ids).  One launch.
+struct TextMark {
+    const uint32_t *ids[2];
+    const uint8_t *keep[2];
+    const uint8_t *proto;
+    int32_t proto_eq;
+    uint32_t *mark;
+};
+cudaError_t launch_text_mark(cudaStream_t st, const TextMark &m, uint64_t n);
+
 }  // namespace tad

@@ -326,12 +326,28 @@ class TadEngine:
 
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
-                      check: bool = True) -> StreamJob:
-        """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown."""
+                      check: bool = True, text_filter=None) -> StreamJob:
+        """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
+        ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
+        (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
+        for every row."""
         keep = []
         spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep)
         h = C.c_void_p()
-        rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
+        if text_filter is None:
+            rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
+        else:
+            flt = L.TadStreamFilter()
+            for t, slot in enumerate(("src_ip", "dst_ip")):
+                op, pat = text_filter.get(slot, ("any", b""))
+                flt.op[t] = L.TAD_NAME_OPS[op] if isinstance(op, str) else int(op)
+                pat = bytes(pat)
+                buf = C.create_string_buffer(pat, len(pat) or 1)
+                keep.append(buf)
+                flt.pattern[t] = C.cast(buf, C.c_void_p).value
+                flt.pattern_len[t] = len(pat)
+            flt.proto_eq = int(text_filter.get("proto_eq", -1))
+            rc = self.lib.tad_submit_stream_filtered(self.ctx, C.byref(spec), int(rows_hint), C.byref(flt), C.byref(h))
         return self._checked(StreamJob(self, h, keep), rc, check)
 
     def run(self, table: dict, on_job=None, memory_budget: int | None = None, **kw):
