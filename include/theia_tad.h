@@ -197,9 +197,26 @@ int tad_wait(tad_job *job, int64_t timeout_ms, tad_status *status);
 /* Replaces: SELECT ... FROM tadetector WHERE id = ? (rest.go:249-315) for a finished job. */
 int tad_result(tad_job *job, tad_rows *rows);
 
-/* Replaces: DeleteSparkApplication (controller.go:385-424). */
+/* Replaces: DeleteSparkApplication (controller.go:385-424).  tad_cancel returns at once; the job then fails with
+ * TAD_ERR_CANCELLED at its next check.  An ARIMA job on one GPU checks inside its fit kernel: every warp stops at its
+ * next evaluation round and drops the fits in flight, so the job stops within one likelihood evaluation of the longest
+ * prefix being fitted, whatever the series' length (within one phase of the pipeline otherwise, and at the end of the job
+ * when world_size > 1).  tad_release of a job that
+ * has not finished cancels it and waits until it has failed; the context then runs the next queued job. */
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
+
+/* Replaces: nothing finer than GetSparkAppProgress's completed / total stages (pkg/controller/util.go:129-159), which
+ * tad_poll reports; this counts the work inside the stages, so a long ARIMA fit phase shows that it moves.  Any state,
+ * any thread, like tad_poll.  Non-ARIMA jobs: fits 0 / 0.  The counts never decrease, except that a pass which is split
+ * after its fit phase gives its fits back. */
+typedef struct {
+    uint32_t passes_done;   /* hash-range passes whose pipeline has finished                          */
+    uint32_t passes;        /* passes planned so far (grows when a pass splits)                        */
+    uint64_t fits_done;     /* ARIMA prefix fits finished, summed over the passes so far               */
+    uint64_t fits_total;    /* ARIMA prefix fits of the passes whose fit phase has started              */
+} tad_progress;
+int tad_job_progress(tad_job *job, tad_progress *p);
 
 /* Device memory this context's workspace may hold (bytes).  0 (default) = what is free on the device when a job starts,
  * plus what the context already holds, less a headroom of 512 MiB.  A job that does not fit runs in hash-range passes:

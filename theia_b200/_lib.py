@@ -22,7 +22,7 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
            "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
-           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered")
+           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered", "tad_job_progress")
 TAD_NAME_OPS = {"any": 0, "eq": 1, "nonempty": 2, "icontains": 3}
 
 
@@ -58,6 +58,10 @@ class TadStatus(C.Structure):
                 ("points", C.c_uint64), ("series", C.c_uint64), ("result_rows", C.c_uint64), ("spill_rows", C.c_uint64),
                 ("gpu_launches", C.c_uint64), ("device_ms", C.c_double), ("total_ms", C.c_double),
                 ("phase_ms", C.c_double * TAD_NPHASES)]
+
+
+class TadProgress(C.Structure):
+    _fields_ = [("passes_done", C.c_uint32), ("passes", C.c_uint32), ("fits_done", C.c_uint64), ("fits_total", C.c_uint64)]
 
 
 class TadRows(C.Structure):
@@ -103,6 +107,7 @@ def load():
     L.tad_cancel.argtypes = [C.c_void_p]
     L.tad_release.argtypes = [C.c_void_p]
     L.tad_get_unique_id.argtypes = [C.c_void_p, C.c_size_t]
+    L.tad_job_progress.argtypes = [C.c_void_p, C.POINTER(TadProgress)]
     L.tad_set_memory_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     L.tad_set_host_budget.argtypes = [C.c_void_p, C.c_uint64]

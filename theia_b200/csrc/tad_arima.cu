@@ -556,14 +556,12 @@ __host__ __device__ void arima_fit(const ArimaObj &o, double x[3])
 // ------------------------------------------------------------------------------------------
 // kernels
 // ------------------------------------------------------------------------------------------
-// one thread per series: validity, Box-Cox lambda, transformed series into yb[]
-__global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
-                                                           const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
-                                                           const uint64_t *__restrict__ csr_v, double *__restrict__ yb,
-                                                           double *__restrict__ lam)
+// one series: validity, Box-Cox lambda, transformed series into yb[]; returns its prefix fits (n - 3 with a lambda, else 0)
+__device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
+                                                        const uint32_t *__restrict__ sbase, uint32_t B, uint32_t i,
+                                                        const uint64_t *__restrict__ csr_v, double *__restrict__ yb,
+                                                        double *__restrict__ lam)
 {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= S) return;
     const SeriesEntry e = load_entry(entries, offsets, sbase, B, i);
     const uint64_t *v = csr_v + e.off;
     double *y = yb + e.off;
@@ -578,7 +576,7 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
         y[q] = lx;
         sumlog += lx;
     }
-    if (!valid || constant) { lam[i] = NAN; return; }
+    if (!valid || constant) { lam[i] = NAN; return 0; }
     const double l = boxcox_mle_lambda(y, n, sumlog);
     bool finite = isfinite(l);
     for (uint32_t q = 0; q < n && finite; q++) {
@@ -586,6 +584,19 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
         finite = isfinite(y[q]);
     }
     lam[i] = finite ? l : NAN;                             // overflowing transform -> the series yields no rows
+    return finite ? n - 3 : 0u;
+}
+
+// one thread per series; *fits_total gains the prefix fits of the series (one atomic per warp)
+__global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
+                                                           const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
+                                                           const uint64_t *__restrict__ csr_v, double *__restrict__ yb,
+                                                           double *__restrict__ lam, uint32_t *__restrict__ fits_total)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t fits = i < S ? arima_boxcox_series(entries, offsets, sbase, B, i, csr_v, yb, lam) : 0u;
+    fits = __reduce_add_sync(0xffffffffu, fits);          // the grid covers whole warps
+    if ((threadIdx.x & 31) == 0 && fits) atomicAdd(fits_total, fits);
 }
 
 // Prefix fits (pred[] in Box-Cox space), evaluation-synchronous, one warp per series: the fits t = n-1 .. 3 form a job
@@ -594,10 +605,15 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
 // on its own prefix and parameters -- then each lane advances its own optimiser state (lbfgs_advance) to the next trial
 // point; a lane whose fit has ended writes its forecast and takes the next job.  Per fit the arithmetic is the same as
 // in arima_fit: only the scheduling differs.
+// Cancel: lane 0 reads *cancel in every round (a volatile load from L2, so every round reads it anew) and the next round
+// starts with it; once it is nonzero the warp leaves at once, dropping the fits in flight unfinished -- a cancelled job
+// fails without reading pred[].  So the wait is bounded by one round (one evaluation of the longest prefix in flight),
+// not by one fit (tens of rounds) or one series.  *fits_done gains the fits finished, one atomic per warp and round.
 __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                              const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
                                                              const double *__restrict__ yb, const double *__restrict__ lam,
-                                                             double *__restrict__ pred)
+                                                             double *__restrict__ pred, const volatile uint32_t *cancel,
+                                                             uint32_t *__restrict__ fits_done)
 {
     const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
@@ -612,7 +628,11 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
     ArimaObj o{y, 0};
     double u[3] = {0.0, 0.0, 0.0};
     Lbfgs st;
+    // lane 0: the cancel word as read in the previous round; the first read is here, so that a warp which starts after
+    // the cancel fits nothing
+    uint32_t stop = lane == 0 ? *cancel : 0u;
     for (;;) {
+        if (__shfl_sync(0xffffffffu, stop, 0)) break;      // cancelled: the fits in flight are dropped
         // ---- hand the next jobs to the idle lanes --------------------------------------------
         const uint32_t idle = __ballot_sync(0xffffffffu, !busy);
         if (idle && next >= 3) {
@@ -626,19 +646,24 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
             next -= __popc(idle);
         }
         if (!__any_sync(0xffffffffu, busy)) break;
+        // the next round's cancel word, read here so that its latency overlaps the evaluation
+        if (lane == 0) stop = *cancel;
         // ---- all busy lanes evaluate together -------------------------------------------------
         double f = 0.0, g[3] = {0.0, 0.0, 0.0};
         if (busy) arima_fg(o, u, f, g);
         __syncwarp();
         // ---- every lane advances its own optimiser --------------------------------------------
+        bool ended = false;
         if (busy && lbfgs_advance(st, u, f, g)) {
             double phi, theta, s2, fc = 0.0;
             arima_transform(u, phi, theta, s2);
             arima_loglike(o, phi, theta, s2, &fc);
             p[o.n] = fc;
             busy = false;
+            ended = true;
         }
-        __syncwarp();
+        const uint32_t fin = __ballot_sync(0xffffffffu, ended);
+        if (lane == 0 && fin) atomicAdd(fits_done, (uint32_t)__popc(fin));
     }
 }
 
@@ -738,18 +763,23 @@ __global__ void __launch_bounds__(NT) detect_arima_kernel(const SeriesEntry *__r
     }
 }
 
-cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                                uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, double *scratch_y,
-                                double *scratch_pred, double *scratch_lam, bool fit, const OutCols &out, uint32_t out_cap,
-                                uint32_t *stats, int emit_all)
+cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
+                             uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits)
 {
     if (S == 0) return cudaSuccess;
-    if (fit) {
-        arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam);
-        const uint64_t threads = (uint64_t)S * 32;
-        arima_fit_sync_kernel<<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                                scratch_lam, scratch_pred);
-    }
+    arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam, fits);
+    const uint64_t threads = (uint64_t)S * 32;
+    arima_fit_sync_kernel<<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
+                                                                            scratch_lam, scratch_pred, cancel, fits + 1);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
+                                uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, const double *scratch_pred,
+                                const double *scratch_lam, const OutCols &out, uint32_t out_cap, uint32_t *stats, int emit_all)
+{
+    if (S == 0) return cudaSuccess;
     constexpr int NT = 128;
     detect_arima_kernel<NT><<<(S + NT - 1) / NT, NT, 0, st>>>(entries, offsets, sbase, B, S, csr_v, csr_t, scratch_pred,
                                                              scratch_lam, out, out_cap, stats, emit_all);

@@ -115,6 +115,9 @@ enum {
     ST_GPOINTS,         // then count the spilled buckets only); adjacent: zeroed together before every scoring attempt
     ST_COUNT
 };
+// ARIMA fit launch, outside the ST_COUNT readback: [ST_FITS, +2) the fit counters (launch_arima_fit's fits[0..1]), which
+// the worker copies back while the fit kernel runs, and [ST_FITS + 2] the kernel's cancel word
+constexpr int ST_FITS = 32;
 
 constexpr int kGroupCap = 4096;       // rows a bucket may hold to take the shared-memory path (largest class)
 constexpr int kGroupCapMid = 2048;    // second capacity class

@@ -147,6 +147,7 @@ struct tad_job {
     tad_rows rows{};
     double t_submit = 0;
     uint32_t passes = 0;             // hash-range passes the job ran in (tad_job_memory)
+    tad_progress prog{};             // passes and ARIMA fits so far (tad_job_progress), under `mu`
     uint64_t peak_workspace = 0;     // largest device workspace the context held while the job ran
     // streamed input (tad_submit_stream): the caller hands the worker one column block at a time, under `mu`.  `cols`
     // then holds the first block: its non-NULL columns are the set every block must carry.
@@ -205,6 +206,11 @@ struct tad_ctx {
     unsigned long long *h_small = nullptr;   // pinned, 256 x u64
     uint32_t scan_epoch = 0;
     uint32_t *h_stats = nullptr;   // pinned readback of the device scalars
+    // ARIMA fit launch (wait_arima_fit): pinned [0, 2): the fit counters while the kernel runs, [2, 4): once it has ended,
+    // [4]: 1, the value a cancel copies into the kernel's cancel word
+    uint32_t *h_fits = nullptr;
+    cudaEvent_t fit_ev[2]{};        // [0]: the fit counters are reset; [1]: the fit kernel has ended
+    cudaEvent_t fits_ev = nullptr;  // a copy of the fit counters has reached h_fits
     std::mutex pool_mu;
     std::vector<PinnedBlock> pinned_pool;
     NcclComm nccl;
@@ -458,6 +464,80 @@ void set_progress(tad_job *job, int state, int completed)
     std::lock_guard<std::mutex> lk(job->mu);
     job->st.state = state;
     job->st.completed_stages = std::max(job->st.completed_stages, completed);    // passes rerun the stages
+}
+
+tad_progress progress_of(tad_job *job)
+{
+    std::lock_guard<std::mutex> lk(job->mu);
+    return job->prog;
+}
+
+// tad_job_progress's pass counts.  fits_before: the job's counts before a pass that has just been split, which gives its
+// fits back (its halves fit the same series again); null: the fit counts stay.
+void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progress *fits_before = nullptr)
+{
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->prog.passes_done = done;
+    job->prog.passes = planned;
+    if (fits_before) {
+        job->prog.fits_done = fits_before->fits_done;
+        job->prog.fits_total = fits_before->fits_total;
+    }
+}
+
+// The ARIMA fit launch of a pass (launch_arima_fit with d_fits = its counters and cancel word, enqueued on ctx->stream behind
+// their reset and fit_ev[0]), waited for without blocking behind it: the worker polls an event recorded after the fit
+// kernel, copies tad_cancel into the kernel's cancel word (single GPU only: on several GPUs a rank that left early would
+// strand its peers at the end-of-job all-gather) and about every 50 ms copies the pass's fit counters back; both copies
+// run on the copy stream, beside the kernel.  The counters are published added to the job's counts before the pass.
+// Returns once the kernel has ended, its final counts published.
+void wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits)
+{
+    uint64_t done0, total0;
+    {
+        std::lock_guard<std::mutex> lk(job->mu);
+        done0 = job->prog.fits_done;
+        total0 = job->prog.fits_total;
+    }
+    auto publish = [&](const uint32_t *h) {
+        std::lock_guard<std::mutex> lk(job->mu);
+        job->prog.fits_total = total0 + h[0];
+        job->prog.fits_done = done0 + h[1];
+    };
+    const bool cancellable = ctx->cfg.world_size == 1;
+    CU(cudaEventRecord(ctx->fit_ev[1], ctx->stream));
+    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));     // no copy touches the words before their reset
+    bool copying = false, cancelled = false;
+    double next_copy = now_ms();
+    for (;;) {
+        if (cancellable && !cancelled && job->cancel.load()) {
+            CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 4, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+            cancelled = true;
+        }
+        const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
+        if (e != cudaErrorNotReady) {
+            CU(e);
+            break;
+        }
+        if (copying) {
+            const cudaError_t c = cudaEventQuery(ctx->fits_ev);
+            if (c != cudaErrorNotReady) {
+                CU(c);
+                publish(ctx->h_fits);
+                copying = false;
+            }
+        }
+        if (!copying && now_ms() >= next_copy) {
+            CU(cudaMemcpyAsync(ctx->h_fits, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
+            CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
+            copying = true;
+            next_copy = now_ms() + 50.0;
+        }
+        std::this_thread::sleep_for(std::chrono::milliseconds(1));
+    }
+    CU(cudaMemcpyAsync(ctx->h_fits + 2, d_fits, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    publish(ctx->h_fits + 2);
 }
 
 int pick_logb(const tad_ctx *ctx, uint64_t rows)
@@ -1205,9 +1285,16 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             ensure(ctx, ctx->ar_y, z.ar_y);
             ensure(ctx, ctx->ar_pred, z.ar_pred);
             ensure(ctx, ctx->ar_lam, z.ar_lam);
-            CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (double *)ctx->ar_y.p,
-                                   (double *)ctx->ar_pred.p, (double *)ctx->ar_lam.p, attempt == 0, oc, (uint32_t)out_cap,
-                                   d_stats, emit_all));
+            if (attempt == 0 && S) {
+                CU(cudaMemsetAsync(d_stats + ST_FITS, 0, 12, st));      // fit counters and cancel word
+                CU(cudaEventRecord(ctx->fit_ev[0], st));
+                CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, (double *)ctx->ar_y.p, (double *)ctx->ar_pred.p,
+                                    (double *)ctx->ar_lam.p, d_stats + ST_FITS + 2, d_stats + ST_FITS));
+                wait_arima_fit(ctx, job, d_stats + ST_FITS);
+                if (ctx->cfg.world_size == 1) check_cancel();      // pred[] is incomplete: no detect
+            }
+            CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
+                                   (const double *)ctx->ar_lam.p, oc, (uint32_t)out_cap, d_stats, emit_all));
             launches += S ? (attempt == 0 ? 3 : 1) : 0;
         } else {
             fail(TAD_ERR_UNSUPPORTED, "algorithm %d is not implemented by this build", sp.algo);
@@ -2083,10 +2170,12 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         for (int j = 0; j < kMaxPasses; j++) job->stored_rows += rs.rows[j];
     if (!loaded) finish_round();
     std::vector<PassOut> outs;
-    uint32_t passes = 0;
+    uint32_t passes = 0, planned = P;
+    set_passes(job, 0, planned);
     try {
         while (!todo.empty()) {
             if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+            const tad_progress before = progress_of(job);
             const uint32_t v = todo.front().first, M = todo.front().second;
             todo.pop_front();
             const uint64_t rows = pass_rows(v, M);
@@ -2140,6 +2229,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 }
             }
             if (!split_pass) passes++;
+            else planned++;
+            set_passes(job, passes, planned, split_pass ? &before : nullptr);
             finish_round();
         }
         // one contiguous result block, pass after pass
@@ -2227,11 +2318,15 @@ void run_job(tad_ctx *ctx, tad_job *job)
     PassOut acc;
     uint32_t passes = 1;
     if (!split) {
+        set_passes(job, 0, 1);
         try {
             run_pipeline(ctx, job, hc, true, force_exact, acc);
+            set_passes(job, 1, 1);
         } catch (const PassSplit &) {          // thrown only under a budget
             CU(cudaStreamSynchronize(ctx->stream));
             acc = PassOut{};
+            const tad_progress none{};
+            set_passes(job, 0, 1, &none);
             split = true;
         }
     }
@@ -2550,6 +2645,10 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_small, 256 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
+    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 5 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
+    if (ok) ctx->h_fits[4] = 1;
+    for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->fit_ev[i], cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && cudaEventCreateWithFlags(&ctx->fits_ev, cudaEventDisableTiming) == cudaSuccess;
     if (!ok) {
         tad_shutdown(ctx);      // releases whatever was created
         return TAD_ERR_CUDA;
@@ -2594,6 +2693,10 @@ void tad_shutdown(tad_ctx *ctx)
     if (ctx->h_chunk) cudaFreeHost(ctx->h_chunk);
     if (ctx->h_stats) cudaFreeHost(ctx->h_stats);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
+    if (ctx->h_fits) cudaFreeHost(ctx->h_fits);
+    for (int i = 0; i < 2; i++)
+        if (ctx->fit_ev[i]) cudaEventDestroy(ctx->fit_ev[i]);
+    if (ctx->fits_ev) cudaEventDestroy(ctx->fits_ev);
     for (int i = 0; i < kMaxEvents; i++)
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
     for (int i = 0; i < kMaxChunks; i++)
@@ -2811,6 +2914,14 @@ int tad_cancel(tad_job *job)
     std::lock_guard<std::mutex> lk(job->mu);
     job->cancel.store(1);
     job->cv.notify_all();        // a worker waiting for streamed input
+    return TAD_OK;
+}
+
+int tad_job_progress(tad_job *job, tad_progress *p)
+{
+    if (!job || !p) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    *p = job->prog;
     return TAD_OK;
 }
 

@@ -70,12 +70,18 @@ cudaError_t launch_detect_dbscan(cudaStream_t st, const SeriesEntry *entries, co
                                  uint32_t *scratch_pc, uint8_t *scratch_flag, const OutCols &out, uint32_t out_cap,
                                  uint32_t *stats, int emit_all);
 
-// ARIMA (tad_arima.cu): Box-Cox + per-prefix ARIMA(1,1,1) MLE fits (when `fit`) then score/flag/compact.
+// ARIMA (tad_arima.cu): launch_arima_fit runs Box-Cox + the per-prefix ARIMA(1,1,1) MLE fits into scratch_pred (two
+// launches), launch_detect_arima then scores / flags / compacts (one launch, rerun alone when the result grows).
 // scratch_y / scratch_pred: one double per point slot; scratch_lam: one double per series.
+// cancel: a device word the fit kernel reads in every round; nonzero = every warp leaves at its next round and drops the
+// fits in flight, so pred[] is then incomplete.  fits[0] gains the prefix fits of the series, fits[1] the fits finished
+// (u32: one fit per point, fewer than 2^32 points per pass).
+cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
+                             uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits);
 cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                                uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, double *scratch_y,
-                                double *scratch_pred, double *scratch_lam, bool fit, const OutCols &out, uint32_t out_cap,
-                                uint32_t *stats, int emit_all);
+                                uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, const double *scratch_pred,
+                                const double *scratch_lam, const OutCols &out, uint32_t out_cap, uint32_t *stats, int emit_all);
 
 // Oversized buckets (more rows than the shared-memory capacity): global-memory path.
 // Sorts the rows of all listed buckets by (hash, key, time), reduces duplicates and writes the

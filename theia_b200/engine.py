@@ -155,7 +155,17 @@ class Job:
         return {"passes": passes.value, "peak_workspace_bytes": peak.value, "stored_rows": stored.value,
                 "peak_host_bytes": peak_host.value}
 
+    def progress(self) -> dict:
+        """In any state (tad_job_progress): the hash-range passes finished and planned so far, and the ARIMA prefix fits
+        finished and those of the passes whose fit phase has started (0 / 0 for the other algorithms)."""
+        p = L.TadProgress()
+        rc = self.eng.lib.tad_job_progress(self.h, C.byref(p))
+        if rc != 0:
+            raise TadError(rc, "tad_job_progress")
+        return {"passes_done": p.passes_done, "passes": p.passes, "fits_done": p.fits_done, "fits_total": p.fits_total}
+
     def cancel(self):
+        """tad_cancel: returns at once; an ARIMA job on one GPU stops within one evaluation round of its fit kernel."""
         self.eng.lib.tad_cancel(self.h)
 
     def release(self):
