@@ -201,7 +201,7 @@ int tad_result(tad_job *job, tad_rows *rows);
  * TAD_ERR_CANCELLED at its next check.  An ARIMA job on one GPU checks inside its fit kernel: every warp stops at its
  * next evaluation round and drops the fits in flight, so the job stops within one likelihood evaluation of the longest
  * prefix being fitted, whatever the series' length (within one phase of the pipeline otherwise, and at the end of the job
- * when world_size > 1).  tad_release of a job that
+ * when world_size > 1, or of the current pass under a memory budget).  tad_release of a job that
  * has not finished cancels it and waits until it has failed; the context then runs the next queued job. */
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
@@ -224,11 +224,21 @@ int tad_job_progress(tad_job *job, tad_progress *p);
  * whole pipeline; the result rows are the same rows a one-pass run gives.  Host-resident input is read over PCIe once
  * per pass.  A job fails with TAD_ERR_NOMEM only when a 1/64 hash range of it does not fit.  Caller-owned columns and
  * pinned host memory are not counted.  If the budget drops below what the context holds, the workspace is freed before
- * the next job.  Applies to jobs that start after the call; single GPU only (TAD_ERR_UNSUPPORTED when world_size > 1);
- * TAD_ERR_INVALID_ARG below the floor of 64 MiB. */
+ * the next job.  Applies to jobs that start after the call; TAD_ERR_INVALID_ARG below the floor of 64 MiB.
+ *
+ * Several GPUs (world_size > 1): 0 means "no planning", not free memory: a job without a budget runs exactly as it does
+ * without this call (no planning collective, launch or sync).  With one, the ranks run the same passes over their shards
+ * at once: they agree on the pass count from every rank's rows and budget (one blocking all-gather at job start) and the
+ * first sweep's per-owner counts, and every pass ends with an 8-byte all-gather on which they split it or stop together.
+ * The ranks may set different values, each rank's workspace staying inside its own, but every rank of a job must have a
+ * nonzero budget or none (like the run-time switches every rank must see alike).  The job fails with TAD_ERR_NOMEM on
+ * every rank, naming the rank and the bytes, when a 1/64 hash range does not fit one rank, and a tad_cancel on any rank
+ * fails the job with TAD_ERR_CANCELLED on every rank, at the end of the current pass (a job cancelled before it started
+ * still meets its peers once).  The contexts stay usable in both cases.  The exported partition buffer of earlier jobs is
+ * freed at the start of such a job.  Host or device columns as for tad_submit; streamed input is single GPU only. */
 int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
-/* For a COMPLETED job: the passes it ran in and the largest device workspace the context held while it ran
- * (TAD_ERR_STATE otherwise). */
+/* For a COMPLETED job: the passes it ran in (the same count on every rank of a multi-GPU job) and the largest device
+ * workspace the context held while it ran (TAD_ERR_STATE otherwise). */
 int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes);
 
 /* Pinned host memory this context may hold for its host row store (bytes).  0 (default) = no store.  With a store, a

@@ -575,6 +575,22 @@ void *col_ptr(const tad_columns &c, int idx)
     }
 }
 
+void set_col(ColPtrs &c, int i, const void *p)
+{
+    switch (i) {
+    case 0: c.src_ip = (const uint32_t *)p; break;
+    case 1: c.dst_ip = (const uint32_t *)p; break;
+    case 2: c.src_port = (const uint16_t *)p; break;
+    case 3: c.dst_port = (const uint16_t *)p; break;
+    case 4: c.proto = (const uint8_t *)p; break;
+    case 5: c.flow_start = (const uint32_t *)p; break;
+    case 6: c.flow_end = (const uint32_t *)p; break;
+    case 7: c.value = (const uint64_t *)p; break;
+    case 8: c.src_ns = (const uint32_t *)p; break;
+    default: c.dst_ns = (const uint32_t *)p; break;
+    }
+}
+
 // Whether a job's rows carry key/value column i: its first block's column, or a text slot encoded into it on the device.
 bool has_col(const tad_job *job, int i) { return col_ptr(job->cols, i) || (i < 2 && job->text[i]); }
 
@@ -707,7 +723,17 @@ struct PassOut {
 // The pipeline (ingest, partition, exchange, group, detect, egress) over `hc`.  `filters`: apply the job's time window
 // and ns_ignore list (passes were filtered by the split kernel already).  `force_exact`: the exact partition even where
 // the optimistic slot buffer would be used (the planner found it does not fit the budget).
-void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filters, bool force_exact, PassOut &out)
+// `pass`: one pass of a multi-GPU job in passes (run_passes_multi), null otherwise.  Its sizes come from the all-gathered
+// counts, so they are the same on every rank: the bucket count follows its global rows and the NCCL exchange's chunk count
+// its largest shard.  The pipeline then leaves every decision that changes which collectives a rank issues to the
+// driver's end-of-pass all-gather: a cancel does not throw here, and the peer-pull end barrier is that all-gather, so a
+// rank that throws PassSplit has issued every collective its peers have.
+struct AgreedPass {
+    uint64_t global_rows;            // the pass's rows over all ranks
+    uint64_t max_rows;               // the most rows one rank holds in the pass
+};
+void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filters, bool force_exact, PassOut &out,
+                  const AgreedPass *pass = nullptr)
 {
     const tad_job_spec &sp = job->spec;
     const uint64_t R = hc.rows;
@@ -722,7 +748,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         }
     };
     auto check_cancel = [&]() {
-        if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+        if (!pass && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
     };
 
     CU(cudaSetDevice(ctx->cfg.device));
@@ -806,7 +832,9 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     uint64_t R_total = R;
     ensure(ctx, ctx->small, 4096);
     unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
-    if (world > 1 && sp.global_rows) {
+    if (world > 1 && pass) {
+        R_total = pass->global_rows;   // the pass's total from the all-gathered counts
+    } else if (world > 1 && sp.global_rows) {
         R_total = sp.global_rows;      // the host counted the table: no start-of-job collective, no host sync
     } else if (world > 1) {
         // global row count -> same bucket count on every rank
@@ -976,7 +1004,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     const size_t x_need = x_cnt_bytes + (size_t)B * slotM * sizeof(Row32);
     bool sync_at_end = false;
     if (world > 1 && ctx->peer_pull && ctx->optimistic && R_total > 0 && (uint64_t)B * slotM <= (1ull << 31) &&
-        x_need <= ctx->x_budget) {
+        x_need <= ctx->x_budget && !force_exact) {
         ensure_exported(x_need);
         uint32_t *xcursor = static_cast<uint32_t *>(ctx->xbuf.p);
         Row32 *xpart = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->xbuf.p) + x_cnt_bytes);
@@ -1069,7 +1097,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         // With peer pull (default) the exact partition is written into the EXPORTED buffer and the owners' group kernels read
         // their segments straight out of the peers' copies: no receive buffer, no all-to-all (and no chunking: K = 1).
         const bool pull = ctx->peer_pull != 0 && ctx->exact_pull != 0;
-        const int K = pull ? 1 : (R >= ctx->exchange_min_rows && (world == 2 || ctx->exchange_chunks_forced)) ? ctx->exchange_chunks : 1;
+        const uint64_t k_rows = pass ? pass->max_rows : R;      // a pass: the same chunk count on every rank
+        const int K = pull ? 1 : (k_rows >= ctx->exchange_min_rows && (world == 2 || ctx->exchange_chunks_forced)) ? ctx->exchange_chunks : 1;
         auto xlo = [&](int cidx) -> uint64_t {
             if (cidx <= 0) return 0;
             if (cidx >= K) return R;
@@ -1315,7 +1344,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         set_progress(job, TAD_STATE_RUNNING, 4);
     }
     set_progress(job, TAD_STATE_RUNNING, 5);
-    if (sync_at_end) {
+    if (sync_at_end && !pass) {
         // end-of-job barrier of the peer-pull path: my slots and counters may be overwritten (next job) only after every
         // peer's group kernel has read them; its wait is the ranks' arrival skew, accounted as TAD_PHASE_SYNC
         mark(-1);
@@ -1417,6 +1446,23 @@ void add_pass(PassOut &acc, const PassOut &o)
     acc.launches += o.launches;
     acc.device_ms += o.device_ms;
     for (int i = 0; i < TAD_NPHASES; i++) acc.phase_ms[i] += o.phase_ms[i];
+}
+
+// The passes' result rows as one contiguous block, pass after pass (acc.out_rows rows); the passes' blocks go back.
+void join_passes(tad_ctx *ctx, std::vector<PassOut> &outs, PassOut &acc)
+{
+    const OutLayout HL = out_layout(acc.out_rows ? acc.out_rows : 1);
+    acc.block = take_pinned(ctx, HL.total);
+    uint64_t at = 0;
+    for (PassOut &o : outs) {
+        const OutLayout PL = out_layout(o.out_rows ? o.out_rows : 1);
+        for (int i = 0; i < 11; i++)
+            memcpy(static_cast<char *>(acc.block.p) + HL.off[i] + at * kOutWidth[i],
+                   static_cast<const char *>(o.block.p) + PL.off[i], kOutWidth[i] * o.out_rows);
+        at += o.out_rows;
+        give_pinned(ctx, o.block);
+        o.block = PinnedBlock{};
+    }
 }
 
 // ---- streamed input: the worker's side of the hand-over (the caller's side is tad_stream_push / tad_stream_end) ----------
@@ -1572,20 +1618,6 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
         f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
     }
-    auto set_col = [](ColPtrs &c, int i, const void *p) {
-        switch (i) {
-        case 0: c.src_ip = (const uint32_t *)p; break;
-        case 1: c.dst_ip = (const uint32_t *)p; break;
-        case 2: c.src_port = (const uint16_t *)p; break;
-        case 3: c.dst_port = (const uint16_t *)p; break;
-        case 4: c.proto = (const uint8_t *)p; break;
-        case 5: c.flow_start = (const uint32_t *)p; break;
-        case 6: c.flow_end = (const uint32_t *)p; break;
-        case 7: c.value = (const uint64_t *)p; break;
-        case 8: c.src_ns = (const uint32_t *)p; break;
-        default: c.dst_ns = (const uint32_t *)p; break;
-        }
-    };
     unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);   // [0, 64): rows per residue, [64]: pass cursor
     const unsigned long long *h_cnt = ctx->h_small;
     uint64_t nchunk = 0;             // host chunks staged in the current sweep
@@ -2233,19 +2265,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             set_passes(job, passes, planned, split_pass ? &before : nullptr);
             finish_round();
         }
-        // one contiguous result block, pass after pass
-        const OutLayout HL = out_layout(acc.out_rows ? acc.out_rows : 1);
-        acc.block = take_pinned(ctx, HL.total);
-        uint64_t at = 0;
-        for (PassOut &o : outs) {
-            const OutLayout PL = out_layout(o.out_rows ? o.out_rows : 1);
-            for (int i = 0; i < 11; i++)
-                memcpy(static_cast<char *>(acc.block.p) + HL.off[i] + at * kOutWidth[i],
-                       static_cast<const char *>(o.block.p) + PL.off[i], kOutWidth[i] * o.out_rows);
-            at += o.out_rows;
-            give_pinned(ctx, o.block);
-            o.block = PinnedBlock{};
-        }
+        join_passes(ctx, outs, acc);
     } catch (...) {
         for (PassOut &o : outs) give_pinned(ctx, o.block);
         throw;
@@ -2270,9 +2290,422 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     return passes;
 }
 
+// ---- several GPUs in hash-range passes (DESIGN.md section 9, "Several GPUs") ---------------------------------------------
+// The sizes below depend only on values every rank shares (the pass's counts, the job, the world size and the run-time
+// switches every rank must see alike), so every rank computes them for every other rank.
+int log_world(const tad_ctx *ctx)
+{
+    int l = 0;
+    while ((1 << l) < ctx->cfg.world_size) l++;
+    return l;
+}
+
+uint32_t mp_buckets(const tad_ctx *ctx, uint64_t global)      // global buckets, as run_pipeline picks them
+{
+    return 1u << std::max(pick_logb(ctx, global), log_world(ctx));
+}
+
+uint32_t mp_slot(const tad_ctx *ctx) { return std::max<uint32_t>(256u, (uint32_t)kGroupCap / (uint32_t)ctx->cfg.world_size); }
+
+// Whether run_pipeline may take the optimistic slot path for a pass of `global` rows.
+bool mp_slots_allowed(const tad_ctx *ctx, uint64_t global)
+{
+    const uint64_t B = mp_buckets(ctx, global);
+    const size_t x = ((B * 4 + 65535) & ~size_t(65535)) + B * mp_slot(ctx) * sizeof(Row32);
+    return ctx->peer_pull && ctx->optimistic && global > 0 && B * mp_slot(ctx) <= (1ull << 31) && x <= ctx->x_budget;
+}
+
+// Exported-buffer bytes of a pass: the exact partition pulled by the peers (every rank's buffer holds the pass's largest
+// shard, `max_rows`) and, with `slots`, the optimistic slots of all B buckets.
+size_t mp_xbuf_bytes(const tad_ctx *ctx, uint64_t global, uint64_t max_rows, bool slots)
+{
+    const uint64_t B = mp_buckets(ctx, global);
+    const size_t cnt = (B * 4 + 65535) & ~size_t(65535);
+    size_t x = ctx->peer_pull && ctx->exact_pull ? cnt + std::max<uint64_t>(max_rows, 1) * sizeof(Row32) : 0;
+    if (slots && mp_slots_allowed(ctx, global)) x = std::max(x, cnt + B * mp_slot(ctx) * sizeof(Row32));
+    return x;
+}
+
+// The pipeline buffers one multi-GPU pass grows (the exported buffer apart), with upper bounds as pass_need: `rows` input
+// rows of this rank, `owned` rows it owns, `global` rows over all ranks; both partitions when `slots` (an overflow falls
+// back to the exact one).
+std::vector<std::pair<DevBuf *, size_t>> mp_pipe_bufs(tad_ctx *ctx, const tad_job *job, uint64_t global, uint64_t rows,
+                                                       uint64_t owned, bool slots)
+{
+    const size_t W = ctx->cfg.world_size;
+    PipeShape s;
+    s.rows = rows;
+    s.algo = job->spec.algo;
+    s.B = mp_buckets(ctx, global);
+    s.Bl = s.B >> log_world(ctx);
+    s.owned = s.series = owned;
+    s.out_cap = out_cap_guess(owned, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
+    PipeSizes z = pipe_sizes(s);
+    const bool pull = ctx->peer_pull && ctx->exact_pull;
+    const size_t K = pull ? 1 : ctx->exchange_chunks, B = s.B, Bl = s.Bl;
+    z.part = pull ? 0 : std::max<uint64_t>(rows, 1) * sizeof(Row32);
+    z.entries = std::max<uint64_t>(owned, 1) * sizeof(SeriesEntry);
+    z.hist = z.cursor = B * 4 * K;
+    z.offsets = (B + 1) * 4 * K;
+    auto v = pipe_bufs(ctx, z);
+    v.push_back({&ctx->hist_all, B * 4 * W * K});
+    v.push_back({&ctx->seg_off, (Bl + 1) * 4 * W * K});
+    v.push_back({&ctx->seg_total, Bl * 4});
+    v.push_back({&ctx->exch, pull ? 0 : std::max<uint64_t>(owned, 1) * sizeof(Row32)});
+    v.push_back({&ctx->xcnt, slots ? Bl * 4 * W : 0});
+    v.push_back({&ctx->xtotal, slots ? Bl * 4 : 0});
+    v.push_back({&ctx->sortb, ctx->sort_classes ? sort_lists_scratch_bytes((uint32_t)Bl) : 0});
+    return v;
+}
+
+size_t mp_pipe_bytes(tad_ctx *ctx, const tad_job *job, uint64_t global, uint64_t rows, uint64_t owned, bool slots)
+{
+    size_t b = 0;
+    for (const auto &x : mp_pipe_bufs(ctx, job, global, rows, owned, slots)) b += x.second ? alloc_bytes(x.second) : 0;
+    return b;
+}
+
+// A multi-GPU job under a memory budget.  Pass (v, P) holds the rows whose key hash has (h & (P-1)) == v on every rank at
+// once; the owner rank is chosen by the top hash bits, so each pass is an ordinary multi-GPU job over the ranks' pass
+// columns.  Every decision that changes which collectives a rank issues (the pass count, a split, the slot path, a cancel,
+// a NOMEM verdict) is taken on all-gathered data, identically on every rank:
+//   plan    one blocking all-gather of every rank's rows, pass capacity under its own budget, kept bytes and cancel flag;
+//   counts  the first sweep counts every filtered row under (owner rank, residue): all-gathered, they give every rank's
+//           input and owned rows of every pass for every P, so P is raised (pass 0 swept again, at most once) where some
+//           rank would not fit, and the job fails with TAD_ERR_NOMEM on every rank where a 1/64 range does not fit one;
+//   passes  run_pipeline at world_size > 1 over the pass columns, global_rows = the pass's total from the counts;
+//   end     every pass ends with an 8-byte all-gather of {split, cancelled}: a rank whose spill scratch or result buffer
+//           does not fit skips the rest of its pass but still gets there, and then every rank splits the pass or stops.
+uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
+{
+    cudaStream_t st = ctx->stream;
+    const int W = ctx->cfg.world_size, me = ctx->cfg.rank, logW = log_world(ctx);
+    const tad_columns &hc = job->cols;
+    const uint64_t R = hc.rows;
+    const bool host = hc.mem != TAD_MEM_DEVICE && R > 0;
+    const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
+    auto staged = [&](int i) { return col_ptr(hc, i) && (i < 8 || ns); };
+    size_t row_bytes = 0, half_bytes = 0;
+    for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
+    uint64_t chunk = 0;
+    if (host) {         // double-buffered chunk staging, at most 1/16 of the budget
+        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes))) & ~uint64_t(2047);
+        for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
+    }
+    const size_t stage_bytes = 2 * half_bytes;
+    const size_t NC = (size_t)W * kMaxPasses;               // one rank's (owner, residue) counters
+    const size_t pcnt_bytes = (NC * (W + 1) + 1) * 8;        // mine, every rank's (all-gathered), the pass cursor
+    set_progress(job, TAD_STATE_RUNNING, 0);
+
+    // ---- plan ----------------------------------------------------------------------------------------------------------
+    // what every pass keeps: pass columns of `n` rows, staging, counters, the ns_ignore list (and kFixedBytes)
+    auto kept_bytes = [&](uint64_t n) {
+        std::vector<std::pair<DevBuf *, size_t>> b = {{&ctx->stage, stage_bytes}, {&ctx->pcnt, pcnt_bytes},
+                                                      {&ctx->ns_ignore, ns ? job->ns_ignore.size() * 4 : 0}};
+        for (int i = 0; i < 8; i++) b.push_back({&ctx->d_col[i], has_col(job, i) ? col_bytes(i, n) : 0});
+        return workspace_after(ctx, b, true);
+    };
+    // rows one pass may hold on this rank: the largest n for which a pass whose input rows, owned rows and largest shard
+    // are all n fits the budget (exact partition)
+    auto need_n = [&](uint64_t n) {
+        const uint64_t g = n * (uint64_t)W;
+        return kept_bytes(std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) + alloc_bytes(mp_xbuf_bytes(ctx, g, n, false));
+    };
+    uint64_t lo = 0, hi = kMaxPassRows;
+    while (lo < hi) {
+        const uint64_t mid = lo + (hi - lo + 1) / 2;
+        if (need_n(mid) <= budget) lo = mid; else hi = mid - 1;
+    }
+    const uint64_t cap = lo, colcap = std::min(cap, R);
+
+    // The budget applies from the plan on: until then the context may still hold the exported buffer of an earlier job,
+    // larger than this budget, which only the plan all-gather lets it free.  No rank may fail on its own before it.
+    ctx->limit = 0;
+    ensure(ctx, ctx->small, 4096);
+    unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
+    // all-gather of h_small[0, n) into h_small[n, n + n * W); its time is the ranks' skew (phase sync)
+    double gather_ms = 0;
+    auto gather = [&](int n) {
+        CU(cudaMemcpyAsync(d_small, ctx->h_small, n * 8, cudaMemcpyHostToDevice, st));
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (nccl_allgather(&ctx->nccl, d_small, d_small + n, n * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaMemcpyAsync(ctx->h_small + n, d_small + n, (size_t)n * 8 * W, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        gather_ms += ms;
+    };
+    // the exported buffer of an earlier job is freed for the plan: unmap the peers' buffers now, free ours once every rank
+    // has (after the plan all-gather).  peers_mapped is the same on every rank.
+    const bool had_x = ctx->peers_mapped;
+    for (int r = 0; r < W && had_x; r++)
+        if (ctx->peer_x[r]) { CU(cudaIpcCloseMemHandle(ctx->peer_x[r])); ctx->peer_x[r] = nullptr; }
+    ctx->peers_mapped = false;
+    ctx->x_agreed = 0;
+    struct RankPlan {
+        uint64_t rows, cap, budget, kept;
+        bool cancel;
+    } rk[kMaxRanks];
+    memset(ctx->h_small, 0, 16 * 8);
+    ctx->h_small[0] = R;
+    ctx->h_small[1] = cap;
+    ctx->h_small[2] = budget;
+    ctx->h_small[3] = kept_bytes(colcap);
+    ctx->h_small[4] = job->cancel.load() ? 1 : 0;
+    gather(16);
+    uint64_t total = 0;
+    for (int r = 0; r < W; r++) {
+        const unsigned long long *w = ctx->h_small + 16 + 16 * r;
+        rk[r] = RankPlan{w[0], w[1], w[2], w[3], w[4] != 0};
+        total += w[0];
+    }
+    free_buf(ctx, ctx->xbuf);
+    ctx->limit = budget;
+    ctx->peak = ctx->held;
+    for (int r = 0; r < W; r++)
+        if (rk[r].cancel) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", r);
+    for (int r = 0; r < W; r++)
+        if (rk[r].cap == 0)
+            fail(TAD_ERR_NOMEM, "rank %d: a memory budget of %llu bytes does not hold one row of a pass", r,
+                 (unsigned long long)rk[r].budget);
+    // P from the rows: every rank's input and its share of the table within its capacity, with 1/8 head-room
+    auto guess_ok = [&](uint32_t p) {
+        for (int r = 0; r < W; r++)
+            if (std::max(rk[r].rows, (total + W - 1) / W) / p > rk[r].cap / 8 * 7) return false;
+        return true;
+    };
+    uint32_t P = 1;
+    while (P < (uint32_t)kMaxPasses && !guess_ok(P)) P *= 2;
+
+    // ---- pass columns and the sweep --------------------------------------------------------------------------------------
+    for (int i = 0; i < 8; i++)
+        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
+    if (stage_bytes) ensure(ctx, ctx->stage, stage_bytes);
+    ensure(ctx, ctx->pcnt, pcnt_bytes);
+    ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
+    PassCols pcols{};
+    pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
+    pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
+    pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
+    pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
+    RowFilter f{};
+    f.start_time = job->spec.start_time;
+    f.end_time = job->spec.end_time;
+    if (ns) {
+        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
+        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
+        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
+        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
+    }
+    unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);
+    unsigned long long *d_cursor = d_cnt + NC * (W + 1);
+    // the rows of pass (v, M) -> the pass columns, counted under (owner, residue); host input through the staging halves,
+    // the split of each chunk behind its copy
+    auto sweep = [&](uint32_t v, uint32_t M) {
+        CU(cudaMemsetAsync(d_cnt, 0, NC * 8, st));
+        CU(cudaMemsetAsync(d_cursor, 0, 8, st));
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (!host) {
+            ColPtrs c{};
+            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(hc, i));
+            CU(launch_pass_split(st, c, R, f, M - 1, v, pcols, (uint32_t)colcap, d_cursor, d_cnt, 0, logW));
+            acc.launches += R ? 1 : 0;
+        } else {
+            CU(cudaEventRecord(ctx->start_ev, st));
+            CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
+            uint64_t k = 0;
+            for (uint64_t at = 0, n; at < R; at += n, k++) {
+                n = std::min<uint64_t>(chunk, R - at);
+                const int h = (int)(k & 1);
+                if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
+                ColPtrs c{};
+                char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+                for (int i = 0; i < 10; i++) {
+                    if (!staged(i)) continue;
+                    const size_t w = col_bytes(i, 1);
+                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(hc, i)) + at * w, n * w, cudaMemcpyHostToDevice,
+                                       ctx->copy_stream));
+                    set_col(c, i, dst);
+                    dst += exact_bytes(col_bytes(i, chunk));
+                }
+                CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
+                CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)colcap, d_cursor, d_cnt, 0, logW));
+                acc.launches++;
+                CU(cudaEventRecord(ctx->stage_ev[h], st));
+            }
+        }
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaStreamSynchronize(st));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        acc.phase_ms[host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;     // the split runs behind the copies
+        acc.device_ms += ms;
+    };
+
+    // ---- counts ----------------------------------------------------------------------------------------------------------
+    sweep(0, P);
+    std::vector<uint64_t> cnt(NC * W);       // [source rank][owner rank][residue]
+    {
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (nccl_allgather(&ctx->nccl, d_cnt, d_cnt + NC, NC * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+        CU(cudaEventRecord(ctx->ev[1], st));
+        PinnedBlock hb = take_pinned(ctx, NC * W * 8);
+        const cudaError_t e1 = cudaMemcpyAsync(hb.p, d_cnt + NC, NC * W * 8, cudaMemcpyDeviceToHost, st);
+        const cudaError_t e2 = cudaStreamSynchronize(st);
+        if (e1 == cudaSuccess && e2 == cudaSuccess) memcpy(cnt.data(), hb.p, NC * W * 8);
+        give_pinned(ctx, hb);
+        CU(e1);
+        CU(e2);
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        gather_ms += ms;
+    }
+    struct PassDims {
+        uint64_t global = 0, max_rows = 0, rows[kMaxRanks] = {}, owned[kMaxRanks] = {};
+    };
+    auto dims = [&](uint32_t v, uint32_t M) {
+        PassDims d;
+        for (int s = 0; s < W; s++)
+            for (int o = 0; o < W; o++)
+                for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M) {
+                    const uint64_t n = cnt[((size_t)s * W + o) * kMaxPasses + j];
+                    d.rows[s] += n;
+                    d.owned[o] += n;
+                    d.global += n;
+                }
+        for (int s = 0; s < W; s++) d.max_rows = std::max(d.max_rows, d.rows[s]);
+        return d;
+    };
+    // the exported buffer grows to the largest any pass of the plan needs and is never shrunk inside the job
+    auto xbuf_of = [&](uint32_t M, bool slots) {
+        size_t x = 0;
+        for (uint32_t v = 0; v < M; v++) {
+            const PassDims d = dims(v, M);
+            if (d.global) x = std::max(x, mp_xbuf_bytes(ctx, d.global, d.max_rows, slots));
+        }
+        return x;
+    };
+    auto need = [&](int r, const PassDims &d, bool slots, size_t x) {
+        return rk[r].kept + mp_pipe_bytes(ctx, job, d.global, d.rows[r], d.owned[r], slots) + alloc_bytes(x);
+    };
+    int bad_r = 0;
+    uint32_t bad_v = 0;
+    // whether every pass of (., M) fits every rank
+    auto fits_all = [&](uint32_t M, bool slots) {
+        const size_t x = xbuf_of(M, slots);
+        for (uint32_t v = 0; v < M; v++) {
+            const PassDims d = dims(v, M);
+            if (!d.global) continue;
+            for (int r = 0; r < W; r++)
+                if (d.rows[r] > std::min(rk[r].cap, rk[r].rows) || d.owned[r] > kMaxPassRows ||
+                    need(r, d, slots, x) > rk[r].budget) {
+                    bad_r = r;
+                    bad_v = v;
+                    return false;
+                }
+        }
+        return true;
+    };
+    const uint32_t P0 = P;
+    while (P < (uint32_t)kMaxPasses && !fits_all(P, false)) P *= 2;
+    auto too_big = [&](int r, uint32_t v, uint32_t M) {
+        const PassDims d = dims(v, M);
+        fail(TAD_ERR_NOMEM, "rank %d: one 1/%u hash range of the table (%llu rows in, %llu owned) needs %zu bytes of device "
+             "workspace; its memory budget is %llu bytes", r, M, (unsigned long long)d.rows[r], (unsigned long long)d.owned[r],
+             need(r, d, false, xbuf_of(M, false)), (unsigned long long)rk[r].budget);
+    };
+    if (!fits_all(P, false)) too_big(bad_r, bad_v, P);
+    // the slot path where its exported buffer fits next to the workspace of every pass on every rank
+    const bool slots = ctx->peer_pull && ctx->optimistic && fits_all(P, true);
+    const size_t xplan = xbuf_of(P, slots);
+    bool loaded = P == P0;           // pass (0, P) is in the pass columns already
+
+    // ---- passes ----------------------------------------------------------------------------------------------------------
+    std::deque<std::pair<uint32_t, uint32_t>> todo;
+    for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
+    std::vector<PassOut> outs;
+    uint32_t passes = 0, planned = P;
+    set_passes(job, 0, planned);
+    try {
+        while (!todo.empty()) {
+            const uint32_t v = todo.front().first, M = todo.front().second;
+            todo.pop_front();
+            const PassDims d = dims(v, M);
+            if (!d.global) {              // the same on every rank: no collective
+                loaded = false;
+                set_passes(job, ++passes, planned);
+                continue;
+            }
+            if (!loaded) sweep(v, M);
+            loaded = false;
+            // the buffers of earlier passes go where this pass's growth would pass the budget
+            const size_t xgrow = alloc_bytes(xplan) > ctx->xbuf.cap ? alloc_bytes(xplan) - ctx->xbuf.cap : 0;
+            if (workspace_after(ctx, mp_pipe_bufs(ctx, job, d.global, d.rows[me], d.owned[me], slots), false) + xgrow > budget)
+                for (DevBuf *b : workspace_bufs(ctx)) {
+                    if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore || b == &ctx->small ||
+                        (b >= ctx->d_col && b < ctx->d_col + 8))
+                        continue;
+                    free_buf(ctx, *b);
+                }
+            tad_columns pc{};
+            pc.rows = pc.capacity = d.rows[me];
+            pc.mem = TAD_MEM_DEVICE;
+            pc.src_ip = has_col(job, 0) ? pcols.src_ip : nullptr; pc.dst_ip = has_col(job, 1) ? pcols.dst_ip : nullptr;
+            pc.src_port = has_col(job, 2) ? pcols.src_port : nullptr; pc.dst_port = has_col(job, 3) ? pcols.dst_port : nullptr;
+            pc.proto = has_col(job, 4) ? pcols.proto : nullptr; pc.flow_start = has_col(job, 5) ? pcols.flow_start : nullptr;
+            pc.flow_end = pcols.flow_end; pc.value = pcols.value;
+            const tad_progress before = progress_of(job);
+            PassOut o;
+            bool split_here = false;
+            try {
+                const AgreedPass ap{d.global, d.max_rows};
+                run_pipeline(ctx, job, pc, false, !slots, o, &ap);
+            } catch (const PassSplit &) {
+                CU(cudaStreamSynchronize(st));
+                split_here = true;
+            }
+            // ---- the agreed end of the pass: {split, cancelled} of every rank ----
+            ctx->h_small[0] = (split_here ? 1u : 0u) | (job->cancel.load() ? 2u : 0u);
+            gather(1);
+            int split_r = -1, cancel_r = -1;
+            for (int r = W - 1; r >= 0; r--) {
+                if (ctx->h_small[1 + r] & 1) split_r = r;
+                if (ctx->h_small[1 + r] & 2) cancel_r = r;
+            }
+            if (cancel_r >= 0 || split_r >= 0) {
+                give_pinned(ctx, o.block);
+                if (cancel_r >= 0) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", cancel_r);
+                if (M >= (uint32_t)kMaxPasses)
+                    fail(TAD_ERR_NOMEM, "rank %d: the oversized-bucket scratch or result buffer of a 1/%d hash range of the "
+                         "table (%llu rows owned) does not fit its memory budget of %llu bytes", split_r, kMaxPasses,
+                         (unsigned long long)d.owned[split_r], (unsigned long long)rk[split_r].budget);
+                todo.push_front({v + M, 2 * M});
+                todo.push_front({v, 2 * M});
+                set_passes(job, passes, ++planned, &before);
+                continue;
+            }
+            add_pass(acc, o);
+            outs.push_back(o);
+            set_passes(job, ++passes, planned);
+        }
+        join_passes(ctx, outs, acc);
+    } catch (...) {
+        for (PassOut &o : outs) give_pinned(ctx, o.block);
+        throw;
+    }
+    acc.phase_ms[TAD_PHASE_SYNC] += gather_ms;
+    acc.device_ms += gather_ms;
+    return passes;
+}
+
 void run_job(tad_ctx *ctx, tad_job *job)
 {
     CU(cudaSetDevice(ctx->cfg.device));
+    // several GPUs under a budget: every rank joins the plan all-gather, a job cancelled before it started too
+    const uint64_t multi_budget = ctx->cfg.world_size > 1 ? ctx->budget.load() : 0;
+    if (!multi_budget && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
     const tad_columns &hc = job->cols;     // a streamed job's first push writes it: not read here for streams
     const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
@@ -2293,6 +2726,9 @@ void run_job(tad_ctx *ctx, tad_job *job)
         ctx->limit = budget;
         free_workspace(ctx);
         split = true;
+    } else if (multi_budget) {
+        budget = multi_budget;          // run_passes_multi applies it once the plan has freed the exported buffer
+        free_workspace(ctx);
     } else if (ctx->cfg.world_size == 1 && R > 0) {
         const uint64_t set = ctx->budget.load();
         budget = context_budget();
@@ -2317,7 +2753,9 @@ void run_job(tad_ctx *ctx, tad_job *job)
     ctx->peak = ctx->held;
     PassOut acc;
     uint32_t passes = 1;
-    if (!split) {
+    if (multi_budget) {
+        passes = run_passes_multi(ctx, job, budget, acc);
+    } else if (!split) {
         set_passes(job, 0, 1);
         try {
             run_pipeline(ctx, job, hc, true, force_exact, acc);
@@ -2370,7 +2808,6 @@ void worker_main(tad_ctx *ctx)
             ctx->queue.pop_front();
         }
         try {
-            if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
             run_job(ctx, job);
         } catch (const JobFail &f) {
             // nothing of this job may still be reading the caller's columns once it is reported FAILED
@@ -2928,7 +3365,6 @@ int tad_job_progress(tad_job *job, tad_progress *p)
 int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes)
 {
     if (!ctx) return TAD_ERR_INVALID_ARG;
-    if (ctx->cfg.world_size > 1) return TAD_ERR_UNSUPPORTED;
     if (bytes && bytes < kBudgetFloor) return TAD_ERR_INVALID_ARG;
     ctx->budget.store(bytes);
     return TAD_OK;

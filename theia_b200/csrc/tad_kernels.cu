@@ -279,15 +279,19 @@ __device__ __forceinline__ void drop_marked(RowRegs (&r)[8])
     }
 }
 
-template <bool VEC, int MARK>
+// LOGW > 0 (several GPUs, 2^LOGW ranks): every filtered row is counted under (owner rank, residue) instead, owner = the
+// top LOGW hash bits as the pipeline assigns owners: counts[owner * kMaxPasses + residue], 64-bit counters in shared memory.
+template <bool VEC, int MARK, int LOGW>
 __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, RowFilter f, uint32_t pass_mask, uint32_t pass_val,
                                                          PassCols o, uint32_t cap, unsigned long long *__restrict__ cursor,
                                                          unsigned long long *__restrict__ counts)
 {
-    __shared__ uint32_t s_cnt[kMaxPasses];
+    using Cnt = std::conditional_t<(LOGW > 0), unsigned long long, uint32_t>;
+    constexpr int kCnt = kMaxPasses << LOGW;
+    __shared__ Cnt s_cnt[kCnt];
     __shared__ uint32_t s_warp[8];
     __shared__ unsigned long long s_base;     // 64-bit: one sweep of a streamed round may exceed 2^32 rows
-    for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x) s_cnt[i] = 0;
+    for (int i = threadIdx.x; i < kCnt; i += blockDim.x) s_cnt[i] = 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint64_t ntiles = (R + 2047) / 2048;
     __syncthreads();
@@ -308,8 +312,12 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
 #pragma unroll
         for (int i = 0; i < 8; i++) {
             if (!r[i].keep) continue;
-            const uint32_t h = (uint32_t)key_hash(r[i].a, r[i].b, r[i].proto);
-            atomicAdd(&s_cnt[h & (kMaxPasses - 1)], 1u);
+            const uint64_t h64 = key_hash(r[i].a, r[i].b, r[i].proto);
+            const uint32_t h = (uint32_t)h64;
+            if constexpr (LOGW > 0)
+                atomicAdd(&s_cnt[(uint32_t)(h64 >> (64 - LOGW)) * kMaxPasses + (h & (kMaxPasses - 1))], 1ull);
+            else
+                atomicAdd(&s_cnt[h & (kMaxPasses - 1)], 1u);
             if ((h & pass_mask) == pass_val) mine |= 1u << i;
         }
         // exclusive block scan of the per-thread counts
@@ -347,7 +355,7 @@ __global__ void __launch_bounds__(256) pass_split_kernel(ColPtrs c, uint64_t R, 
         }
         __syncthreads();           // s_warp / s_base are rewritten by the next tile
     }
-    for (int i = threadIdx.x; i < kMaxPasses; i += blockDim.x)
+    for (int i = threadIdx.x; i < kCnt; i += blockDim.x)
         if (s_cnt[i]) atomicAdd(&counts[i], (unsigned long long)s_cnt[i]);
 }
 
@@ -1566,15 +1574,16 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
                               uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
-                              unsigned long long *counts, int mark)
+                              unsigned long long *counts, int mark, int log_world)
 {
     if (R == 0) return cudaSuccess;
+    if (log_world < 0 || log_world > 3 || (log_world && mark)) return cudaErrorInvalidValue;
     const uint64_t tiles = (R + 2047) / 2048;
     const uint64_t lim = (uint64_t)num_sms() * 8;
     const uint32_t grid = (uint32_t)(tiles < lim ? tiles : lim);
-    auto go = [&](auto vec, auto mk) {
-        pass_split_kernel<decltype(vec)::value, decltype(mk)::value><<<grid, 256, 0, st>>>(c, R, f, pass_mask, pass_val, out,
-                                                                                          cap, cursor, counts);
+    auto go = [&](auto vec, auto mk, auto lw) {
+        pass_split_kernel<decltype(vec)::value, decltype(mk)::value, decltype(lw)::value><<<grid, 256, 0, st>>>(
+            c, R, f, pass_mask, pass_val, out, cap, cursor, counts);
     };
     const bool vec = cols_aligned16(c);
     using T = std::true_type;
@@ -1582,9 +1591,15 @@ cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, con
     using M0 = std::integral_constant<int, 0>;
     using M1 = std::integral_constant<int, 1>;
     using M2 = std::integral_constant<int, 2>;
-    if (mark == 1) vec ? go(T{}, M1{}) : go(F{}, M1{});
-    else if (mark == 2) vec ? go(T{}, M2{}) : go(F{}, M2{});
-    else vec ? go(T{}, M0{}) : go(F{}, M0{});
+    using W1 = std::integral_constant<int, 1>;
+    using W2 = std::integral_constant<int, 2>;
+    using W3 = std::integral_constant<int, 3>;
+    if (log_world == 1) vec ? go(T{}, M0{}, W1{}) : go(F{}, M0{}, W1{});
+    else if (log_world == 2) vec ? go(T{}, M0{}, W2{}) : go(F{}, M0{}, W2{});
+    else if (log_world == 3) vec ? go(T{}, M0{}, W3{}) : go(F{}, M0{}, W3{});
+    else if (mark == 1) vec ? go(T{}, M1{}, M0{}) : go(F{}, M1{}, M0{});
+    else if (mark == 2) vec ? go(T{}, M2{}, M0{}) : go(F{}, M2{}, M0{});
+    else vec ? go(T{}, M0{}, M0{}) : go(F{}, M0{}, M0{});
     return cudaGetLastError();
 }
 

@@ -17,6 +17,8 @@ cudaError_t launch_scatter(cudaStream_t st, const ColPtrs &c, uint64_t R, const 
 // The cursor and counts are 64-bit: one sweep over a streamed round may hold more than 2^32 rows.
 // `mark` (here and in launch_residue_pack): 1 / 2 = a row whose src_ip / dst_ip id has bit 31 set (a failed text
 // predicate, tad_text.h) is dropped as well; 0 = no such bit.
+// `log_world` 1..3 (2, 4 or 8 ranks; mark must be 0): counts[2^log_world x kMaxPasses] gains the filtered rows under
+// (owner rank, residue) instead, owner = the top log_world bits of the key hash, as the multi-GPU pipeline assigns owners.
 constexpr int kMaxPasses = 64;
 struct PassCols {
     uint32_t *src_ip, *dst_ip, *flow_start, *flow_end;
@@ -26,7 +28,7 @@ struct PassCols {
 };
 cudaError_t launch_pass_split(cudaStream_t st, const ColPtrs &c, uint64_t R, const RowFilter &f, uint32_t pass_mask,
                               uint32_t pass_val, const PassCols &out, uint32_t cap, unsigned long long *cursor,
-                              unsigned long long *counts, int mark = 0);
+                              unsigned long long *counts, int mark = 0, int log_world = 0);
 // Host row store: the rows of `c` that pass the stage-A filters, packed as Row32 records without the hash tag, grouped
 // by low-hash-bit residue (residue 0 first) into out[0, rows kept).  chunk[kMaxPasses] (u32, zeroed here) receives the
 // rows of every residue and totals[kMaxPasses] (null: skipped) gains them.  R <= the max_rows the scratch was sized for;

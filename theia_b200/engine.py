@@ -284,7 +284,8 @@ class TadEngine:
             raise TadError(rc, "tad_set_host_budget(%d)" % nbytes)
 
     def set_memory_budget(self, nbytes: int):
-        """Device bytes the context's workspace may hold (0 = free memory at job start); larger jobs run in passes."""
+        """Device bytes the context's workspace may hold; larger jobs run in passes.  0 = free memory at job start on one
+        GPU, no planning on a rank engine (world_size > 1), where every rank of a job must set a budget or none."""
         rc = self.lib.tad_set_memory_budget(self.ctx, int(nbytes))
         if rc != 0:
             raise TadError(rc, "tad_set_memory_budget(%d)" % nbytes)
