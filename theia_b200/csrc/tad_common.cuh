@@ -96,6 +96,18 @@ __host__ __device__ __forceinline__ uint64_t key_hash(uint64_t a, uint64_t b, ui
     return mix64(a ^ mix64(b + 0x9e3779b97f4a7c15ULL * (uint64_t)(proto + 1u)));
 }
 
+// Shared-memory capacity classes of the group kernel, smallest first: a bucket of 0 < n <= kGroupCap rows goes to the
+// first class whose capacity holds it.  Every class runs four rows per thread.  `ctas` is the CTAs per SM the fused
+// (EWMA) instance is built for (its __launch_bounds__); a static_assert on each class's shared-memory footprint keeps it
+// reachable.  The bucket scan, the class lists, the ST_NCLS* counters and the group launchers all derive from this table.
+struct GroupClass { int cap, threads, ctas; };
+constexpr int kGroupClasses = 4;
+__host__ __device__ constexpr GroupClass group_class(int c)
+{
+    return c == 0 ? GroupClass{1024, 256, 5} : c == 1 ? GroupClass{1536, 384, 3} : c == 2 ? GroupClass{2048, 512, 2}
+                                                                                        : GroupClass{4096, 1024, 1};
+}
+
 // device scalars the host reads back between phases
 enum {
     ST_KEPT = 0,        // rows that passed the stage-A filters
@@ -105,10 +117,8 @@ enum {
     ST_SERIES,          // total series
     ST_POINTS,          // total points after the reduce
     ST_OUTCOUNT,        // result rows produced (may exceed capacity -> rerun)
-    ST_NCLS0,           // buckets per shared-memory capacity class (1024 / 2048 / 4096 rows)
-    ST_NCLS1,
-    ST_NCLS2,
-    ST_OVF,             // optimistic partition: rows that did not fit their bucket's fixed-capacity slot
+    ST_NCLS0,           // [ST_NCLS0, +kGroupClasses): buckets per shared-memory capacity class (group_class)
+    ST_OVF = ST_NCLS0 + kGroupClasses,           // optimistic partition: rows that did not fit their bucket's fixed-capacity slot
     ST_LOCALKEPT,       // multi-GPU optimistic partition: rows of THIS rank that passed the filters (ST_KEPT = rows owned);
                         // must follow ST_OVF: the two travel in one 8-byte all-gather
     ST_GSERIES,         // EWMA: series / points of the buckets the group kernel scored in place (ST_SERIES / ST_POINTS
@@ -119,11 +129,8 @@ enum {
 // the worker copies back while the fit kernel runs, and [ST_FITS + 2] the kernel's cancel word
 constexpr int ST_FITS = 32;
 
-constexpr int kGroupCap = 4096;       // rows a bucket may hold to take the shared-memory path (largest class)
-constexpr int kGroupCapMid = 2048;    // second capacity class
-constexpr int kGroupCapSmall = 1024;  // first capacity class (highest occupancy)
+constexpr int kGroupCap = group_class(kGroupClasses - 1).cap;   // rows a bucket may hold to take the shared-memory path
 constexpr int kGroupTarget = 768;     // mean rows per bucket pick_logb aims for
-constexpr int kGroupHT = 2 * kGroupCap;
 
 
 // sbase[] layout (written by the series scan): [0, B] exclusive scan of series per bucket (sbase[B] = S), followed by the

@@ -675,7 +675,7 @@ PipeSizes pipe_sizes(const PipeShape &s)
     z.hist = z.cursor = z.big_list = B * 4;
     z.nsb = z.npb = (size_t)s.Bl * 4;
     z.offsets = z.big_base = (B + 1) * 4;
-    z.cls_list = B * 4 * 3;
+    z.cls_list = B * 4 * kGroupClasses;
     z.csr_v = cap_rows * 8 + 64;       // + one sector: the direct detector reads whole 32-byte sectors
     z.csr_t = cap_rows * 4;
     z.csr_p = z.dbx = s.algo == TAD_ALGO_DBSCAN ? cap_rows * 4 : 0;
@@ -1234,7 +1234,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     // EWMA is scored inside the group kernel (launch_group_ewma, in the detect loop below): only the spilled buckets go
     // through the per-series arrays, the series scan and the detect kernel
     const bool fused = sp.algo == TAD_ALGO_EWMA;
-    const uint32_t n_cls[3] = {ctx->h_stats[ST_NCLS0], ctx->h_stats[ST_NCLS1], ctx->h_stats[ST_NCLS2]};
+    uint32_t n_cls[kGroupClasses];                        // buckets of every capacity class
+    std::copy(ctx->h_stats + ST_NCLS0, ctx->h_stats + ST_NCLS0 + kGroupClasses, n_cls);
     mark(-1);
     {
         int l = 0;
@@ -1244,7 +1245,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             ensure(ctx, ctx->sortb, need);
             int bits = 1;
             while ((1u << bits) < Bl && bits < 32) bits++;
-            for (int k = 0; k < 3; k++)
+            for (int k = 0; k < kGroupClasses; k++)
                 if (n_cls[k] > 1) { CU(sort_bucket_list(st, cls_list + (size_t)k * Bl, n_cls[k], bits, ctx->sortb.p, ctx->sortb.cap)); launches += 3; }
         }
         if (!fused) {

@@ -25,6 +25,7 @@
 #include <cstdio>
 #include <mutex>
 #include <type_traits>
+#include <utility>
 
 namespace tad {
 
@@ -534,7 +535,7 @@ __device__ __forceinline__ void grid_prefix(ScanSync *sy, uint32_t epoch, const 
 __global__ void __launch_bounds__(1024) bucket_scan_kernel(const uint32_t *__restrict__ hist, uint32_t *__restrict__ offsets,
                                                            uint32_t *__restrict__ cursor, uint32_t B, uint32_t cap,
                                                            uint32_t *__restrict__ big_list, uint32_t *__restrict__ big_base,
-                                                           uint32_t *__restrict__ cls_list /* 3 x B, may be null */,
+                                                           uint32_t *__restrict__ cls_list /* kGroupClasses x B, may be null */,
                                                            uint32_t *__restrict__ stats, ScanSync *sy, uint32_t epoch)
 {
     __shared__ uint32_t total_s, nbig_s, bigrows_s, maxb_s;
@@ -572,9 +573,15 @@ __global__ void __launch_bounds__(1024) bucket_scan_kernel(const uint32_t *__res
         if (cls_list) {
             // bucket list of its shared-memory capacity class (order is irrelevant: one CTA per entry);
             // one atomic per (warp, class) instead of one per bucket
-            const uint32_t c = (h == 0 || h > cap) ? 3u : (h <= (uint32_t)kGroupCapSmall ? 0u : (h <= (uint32_t)kGroupCapMid ? 1u : 2u));
+            uint32_t c = kGroupClasses;
+            if (h != 0 && h <= cap) {
+                c = 0;
+#pragma unroll
+                for (int k = 0; k + 1 < kGroupClasses; k++) c += h > (uint32_t)group_class(k).cap ? 1u : 0u;
+                if (h > (uint32_t)kGroupCap) c = kGroupClasses;
+            }
             const unsigned peers = __match_any_sync(__activemask(), c);
-            if (c < 3u) {
+            if (c < (uint32_t)kGroupClasses) {
                 const int lane = threadIdx.x & 31, leader = __ffs(peers) - 1;
                 uint32_t base = 0;
                 if (lane == leader) base = atomicAdd(&stats[ST_NCLS0 + c], (uint32_t)__popc(peers));
@@ -675,7 +682,8 @@ __device__ __forceinline__ double ewma_series(const unsigned long long *__restri
 // ----------------------------------------------------------------------------------------
 template <int CAP, int NT>
 struct GroupSmem {
-    static constexpr int HT = 2 * CAP;
+    static constexpr int HT = 2 * CAP;        // need not be a power of two: slots are picked by multiply-shift
+    static_assert(CAP % NT == 0 && HT % NT == 0, "every thread stages the same number of rows and hash slots");
     alignas(128) unsigned char x[32 * CAP];   // rows (TMA destination); later ts | tout | vout
     uint32_t ht[HT];                          // claim: low16 = rep row + 1, high16 = count; later (count << 16) | series idx
     uint16_t soff[HT];                        // first point of the slot's series inside the bucket
@@ -684,9 +692,6 @@ struct GroupSmem {
     uint32_t total;
     uint32_t qcount, qbase;                   // fused EWMA: queued result rows, first output row of the CTA
 };
-// Five CTAs of the smallest class share an SM (228 KB, 1 KB reserved per CTA) with room for the fused instance's 256 B
-// segment table; the two queue words above sit in what was the struct's tail padding.
-static_assert(sizeof(GroupSmem<1024, 256>) == 45312, "the smallest capacity class must keep five CTAs per SM");
 
 // What the group kernel does with a bucket once its series are grouped, time-sorted and reduced.
 enum GroupMode : int {
@@ -704,6 +709,24 @@ __device__ __forceinline__ SegTable &seg_table()
 {
     __shared__ SegTable t;               // allocated only in the kernels that call this (the fused instances)
     return t;
+}
+
+// The fused instance of every capacity class keeps its planned CTAs per SM: each CTA holds its GroupSmem, the segment
+// table and the 1 KB the hardware reserves per CTA, out of 228 KB of shared memory per SM.
+template <int... C>
+constexpr bool group_classes_fit(std::integer_sequence<int, C...>)
+{
+    return ((group_class(C).ctas * (sizeof(GroupSmem<group_class(C).cap, group_class(C).threads>) + sizeof(SegTable) + 1024) <=
+             228 * 1024) && ...);
+}
+static_assert(group_classes_fit(std::make_integer_sequence<int, kGroupClasses>()), "a capacity class no longer fits its CTAs per SM");
+
+// the class of the capacity CAP (group_class)
+constexpr int group_class_of(int cap)
+{
+    int c = 0;
+    while (c + 1 < kGroupClasses && group_class(c).cap != cap) c++;
+    return c;
 }
 
 template <int NT>
@@ -771,11 +794,13 @@ __device__ __forceinline__ uint32_t count_lt_u64(const unsigned long long *a, ui
 }
 
 constexpr int kSlotHashBits = 13;      // hash-tag bits that pick the shared-memory slot (largest table: 2 * kGroupCap)
+static_assert(2 * kGroupCap <= (1 << kSlotHashBits), "every slot of the largest table must be reachable");
 
-// Fused instances: as many CTAs per SM as the shared memory allows (five of the smallest class: at most 48 registers),
-// which also lets ptxas keep the larger classes free of spills.  The other instances keep their plain bound.
+// Fused instances: as many CTAs per SM as the shared memory allows (group_class: five of the smallest class, at most 48
+// registers), which also keeps the registers of the larger classes within the occupancy their shared memory allows.  The
+// other instances keep their plain bound.
 template <int CAP, int NT, int MODE>
-__global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : CAP == kGroupCapSmall ? 5 : CAP == kGroupCapMid ? 2 : 1) group_kernel(const SegDesc seg, SeriesEntry *__restrict__ entries,
+__global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group_class_of(CAP)).ctas) group_kernel(const SegDesc seg, SeriesEntry *__restrict__ entries,
                                                    const uint32_t *__restrict__ offsets, const uint32_t *__restrict__ bucket_list,
                                                    uint32_t lo_rows,
                                                    uint64_t *__restrict__ csr_v, uint32_t *__restrict__ csr_t,
@@ -851,7 +876,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : CAP == kGroupCapS
             const uint32_t proto = w.w;                 // protocol | hash tag << 8 (equal keys carry equal tags)
             myT[j] = w.z;
             myV[j] = pack64(w.x, w.y);
-            uint32_t slot = (proto >> (32 - kSlotHashBits)) & (HT - 1);
+            uint32_t slot = ((proto >> (32 - kSlotHashBits)) * (uint32_t)HT) >> kSlotHashBits;
             while (true) {
                 uint32_t cur = *reinterpret_cast<volatile uint32_t *>(&s.ht[slot]);
                 if ((cur & 0xffffu) == 0u) {
@@ -863,7 +888,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : CAP == kGroupCapS
                 const uint4 kk = x4[2 * rep];
                 const uint32_t pp = x4[2 * rep + 1].w;
                 if (kk.x == k.x && kk.y == k.y && kk.z == k.z && kk.w == k.w && pp == proto) break;
-                slot = (slot + 1) & (HT - 1);
+                slot = slot + 1 == (uint32_t)HT ? 0u : slot + 1;
             }
             const uint32_t pos = atomicAdd(&s.ht[slot], 0x10000u) >> 16;
             mySP[j] = slot | (pos << 16);
@@ -1682,12 +1707,14 @@ cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *
     return cudaGetLastError();
 }
 
-template <int CAP, int NT, int MODE>
+// Class C's instance over its bucket list, one CTA per listed bucket.
+template <int C, int MODE>
 static cudaError_t launch_group_class(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets,
-                                      const uint32_t *bucket_list, uint32_t n_buckets, uint32_t lo_rows,
-                                      uint64_t *csr_v, uint32_t *csr_t, uint32_t *csr_p, uint32_t *nsb, uint32_t *npb,
-                                      int reducer, const GroupScore &score)
+                                      const uint32_t *bucket_list, uint32_t n_buckets, uint64_t *csr_v, uint32_t *csr_t,
+                                      uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, const GroupScore &score)
 {
+    constexpr int CAP = group_class(C).cap, NT = group_class(C).threads;
+    const uint32_t lo_rows = C ? (uint32_t)group_class(C - 1).cap : 0u;
     using S = GroupSmem<CAP, NT>;
     static std::atomic<bool> configured{false};
     auto kern = group_kernel<CAP, NT, MODE>;
@@ -1702,38 +1729,30 @@ static cudaError_t launch_group_class(cudaStream_t st, const SegDesc &seg, Serie
     return cudaGetLastError();
 }
 
-// Three shared-memory capacity classes (1024 / 2048 / 4096 rows): most buckets fit the first and run at the
-// highest occupancy.  Each class is launched over ITS OWN bucket list (built by the bucket scan), one CTA per
-// listed bucket -- launching all B CTAs per class and exiting early costs ~0.5 ms per class at 180 KB of shared
-// memory per CTA.  Empty buckets keep the zeroes the caller memset into nsb / npb.
-template <int MODE>
+// The shared-memory capacity classes (group_class): most buckets fit the first and run at the highest occupancy.  Each
+// class is launched over ITS OWN bucket list (built by the bucket scan), one CTA per listed bucket -- launching all B
+// CTAs per class and exiting early costs ~0.5 ms per class at 180 KB of shared memory per CTA.  Classes C, C - 1, ..., 0
+// in this order (the largest first); *launches gains one per non-empty list.  Empty buckets keep the zeroes the caller
+// memset into nsb / npb.
+template <int MODE, int C = kGroupClasses - 1>
 static cudaError_t launch_group_all(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets,
-                                    uint32_t B, const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v,
+                                    uint32_t B, const uint32_t *cls_list, const uint32_t n_cls[kGroupClasses], uint64_t *csr_v,
                                     uint32_t *csr_t, uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer,
                                     const GroupScore &score, int *launches)
 {
-    *launches = 0;
-    cudaError_t e = cudaSuccess;
-    if (n_cls[2]) {
-        e = launch_group_class<kGroupCap, 512, MODE>(st, seg, entries, offsets, cls_list + 2 * (size_t)B, n_cls[2], kGroupCapMid,
-                                                     csr_v, csr_t, csr_p, nsb, npb, reducer, score);
-        ++*launches;
-    }
-    if (e == cudaSuccess && n_cls[1]) {
-        e = launch_group_class<kGroupCapMid, 256, MODE>(st, seg, entries, offsets, cls_list + B, n_cls[1], kGroupCapSmall,
-                                                        csr_v, csr_t, csr_p, nsb, npb, reducer, score);
-        ++*launches;
-    }
-    if (e == cudaSuccess) {
-        e = launch_group_class<kGroupCapSmall, 256, MODE>(st, seg, entries, offsets, cls_list, n_cls[0], 0, csr_v, csr_t,
-                                                          csr_p, nsb, npb, reducer, score);
-        *launches += n_cls[0] ? 1 : 0;
-    }
+    if (C == kGroupClasses - 1) *launches = 0;
+    cudaError_t e = launch_group_class<C, MODE>(st, seg, entries, offsets, cls_list + (size_t)C * B, n_cls[C], csr_v, csr_t,
+                                                csr_p, nsb, npb, reducer, score);
+    *launches += n_cls[C] ? 1 : 0;
+    if constexpr (C > 0)
+        if (e == cudaSuccess)
+            e = launch_group_all<MODE, C - 1>(st, seg, entries, offsets, B, cls_list, n_cls, csr_v, csr_t, csr_p, nsb, npb, reducer,
+                                              score, launches);
     return e;
 }
 
 cudaError_t launch_group(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets, uint32_t B,
-                         const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v, uint32_t *csr_t,
+                         const uint32_t *cls_list, const uint32_t n_cls[kGroupClasses], uint64_t *csr_v, uint32_t *csr_t,
                          uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, int *launches)
 {
     const GroupScore none{};
@@ -1760,7 +1779,7 @@ static void ensure_rcp_table(cudaStream_t st)
 }
 
 cudaError_t launch_group_ewma(cudaStream_t st, const SegDesc &seg, const uint32_t *offsets, uint32_t B, const uint32_t *cls_list,
-                              const uint32_t n_cls[3], int reducer, const GroupScore &score, int *launches)
+                              const uint32_t n_cls[kGroupClasses], int reducer, const GroupScore &score, int *launches)
 {
     ensure_rcp_table(st);
     return launch_group_all<kGroupEwma>(st, seg, nullptr, offsets, B, cls_list, n_cls, nullptr, nullptr, nullptr, nullptr,

@@ -39,7 +39,7 @@ cudaError_t launch_residue_pack(cudaStream_t st, const ColPtrs &c, uint64_t R, c
 // Stored rows in[0, n) -> out columns at rows [at, at + n); null key columns are skipped.  One launch.
 cudaError_t launch_store_unpack(cudaStream_t st, const Row32 *in, uint64_t n, const PassCols &out, uint64_t at);
 cudaError_t launch_bucket_scan(cudaStream_t st, const uint32_t *hist, uint32_t *offsets, uint32_t *cursor, uint32_t B,
-                               uint32_t cap, uint32_t *big_list, uint32_t *big_base, uint32_t *cls_list /* 3 x B or null */,
+                               uint32_t cap, uint32_t *big_list, uint32_t *big_base, uint32_t *cls_list /* kGroupClasses x B or null */,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);
 size_t scan_sync_bytes();   // zero-initialised once; epoch must be > 0 and differ between launches
 // csr_p != nullptr: also rank every series by value and write the permutation (value rank -> time
@@ -47,7 +47,7 @@ size_t scan_sync_bytes();   // zero-initialised once; epoch must be > 0 and diff
 // `offsets` are the (virtual, contiguous) bucket offsets used for entries / csr arrays; the rows
 // themselves are read through `seg`.
 cudaError_t launch_group(cudaStream_t st, const SegDesc &seg, SeriesEntry *entries, const uint32_t *offsets, uint32_t B,
-                         const uint32_t *cls_list, const uint32_t n_cls[3], uint64_t *csr_v, uint32_t *csr_t,
+                         const uint32_t *cls_list, const uint32_t n_cls[kGroupClasses], uint64_t *csr_v, uint32_t *csr_t,
                          uint32_t *csr_p, uint32_t *nsb, uint32_t *npb, int reducer, int *launches);
 // EWMA scored inside the group kernel: every bucket of the class lists is grouped, time-sorted, reduced and scored in
 // shared memory, and its flagged points (every point with emit_all) go straight to out[0, out_cap); rows past out_cap are
@@ -61,7 +61,7 @@ struct GroupScore {
     int emit_all;
 };
 cudaError_t launch_group_ewma(cudaStream_t st, const SegDesc &seg, const uint32_t *offsets, uint32_t B, const uint32_t *cls_list,
-                              const uint32_t n_cls[3], int reducer, const GroupScore &score, int *launches);
+                              const uint32_t n_cls[kGroupClasses], int reducer, const GroupScore &score, int *launches);
 cudaError_t launch_series_scan(cudaStream_t st, const uint32_t *nsb, const uint32_t *npb, uint32_t *sbase, uint32_t B,
                                uint32_t *stats, void *scan_sync, uint32_t epoch);
 cudaError_t launch_detect_ewma(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase, uint32_t B,
