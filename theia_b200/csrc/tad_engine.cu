@@ -349,11 +349,7 @@ void free_buf(tad_ctx *ctx, DevBuf &b)
 
 void free_workspace(tad_ctx *ctx)
 {
-    for (DevBuf *b : workspace_bufs(ctx)) {
-        if (b->p) CU(cudaFree(b->p));
-        ctx->held -= b->cap;
-        *b = DevBuf{};
-    }
+    for (DevBuf *b : workspace_bufs(ctx)) free_buf(ctx, *b);
     for (auto &t : ctx->tdict) t.cap = 0;
 }
 
@@ -439,25 +435,6 @@ char *store_take_page(tad_ctx *ctx, uint64_t budget)
     ctx->store_free.pop_back();
     return p;
 }
-
-// One job's rows in the store: per low-hash-bit residue, a list of pages filled in order.  The pages go back to the
-// context when the job ends, however it ends.
-struct RowStore {
-    tad_ctx *ctx;
-    std::vector<char *> pages[kMaxPasses];
-    uint64_t rows[kMaxPasses] = {};
-    explicit RowStore(tad_ctx *c) : ctx(c) {}
-    void clear()
-    {
-        cudaStreamSynchronize(ctx->d2h_stream);       // no copy into a page is still in flight
-        for (int j = 0; j < kMaxPasses; j++) {
-            ctx->store_free.insert(ctx->store_free.end(), pages[j].begin(), pages[j].end());
-            pages[j].clear();
-            rows[j] = 0;
-        }
-    }
-    ~RowStore() { clear(); }
-};
 
 void set_progress(tad_job *job, int state, int completed)
 {
@@ -593,6 +570,40 @@ void set_col(ColPtrs &c, int i, const void *p)
 
 // Whether a job's rows carry key/value column i: its first block's column, or a text slot encoded into it on the device.
 bool has_col(const tad_job *job, int i) { return col_ptr(job->cols, i) || (i < 2 && job->text[i]); }
+
+// A block's columns as kernel input.
+ColPtrs col_ptrs(const tad_columns &b)
+{
+    ColPtrs c{};
+    for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(b, i));
+    return c;
+}
+
+// The columns from row `lo` on.
+ColPtrs offset_cols(ColPtrs c, uint64_t lo)
+{
+    auto at = [lo](auto *&p) { if (p) p += lo; };
+    at(c.src_ip); at(c.dst_ip); at(c.src_port); at(c.dst_port); at(c.proto);
+    at(c.flow_start); at(c.flow_end); at(c.value); at(c.src_ns); at(c.dst_ns);
+    return c;
+}
+
+// The job's time window and ns_ignore list as the kernels' row filter.  `ns`: the rows carry a namespace column, so a
+// non-empty list is uploaded.
+RowFilter row_filter(tad_ctx *ctx, const tad_job *job, bool ns)
+{
+    RowFilter f{};
+    f.start_time = job->spec.start_time;
+    f.end_time = job->spec.end_time;
+    if (ns && !job->ns_ignore.empty()) {
+        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
+        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice,
+                           ctx->stream));
+        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
+        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
+    }
+    return f;
+}
 
 struct OutLayout {
     size_t off[11];
@@ -817,15 +828,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     c.flow_end = (const uint32_t *)dcol[6]; c.value = (const uint64_t *)dcol[7];
     c.src_ns = (const uint32_t *)dcol[8]; c.dst_ns = (const uint32_t *)dcol[9];
 
-    RowFilter f{};
-    f.start_time = filters ? sp.start_time : 0;
-    f.end_time = filters ? sp.end_time : 0;
-    if (filters && !job->ns_ignore.empty() && (c.src_ns || c.dst_ns)) {
-        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
-        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
-        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
-        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
-    }
+    const RowFilter f = filters ? row_filter(ctx, job, c.src_ns || c.dst_ns) : RowFilter{};
 
     // ---- partition -------------------------------------------------------------------------
     const int world = ctx->cfg.world_size, me = ctx->cfg.rank;
@@ -886,20 +889,6 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     bool partitioned = false;
     uint32_t n_ovf = 0;
     const Row32 *ovf_rows = nullptr;
-    auto offset_cols = [&](uint64_t lo) {
-        ColPtrs ck = c;
-        if (ck.src_ip) ck.src_ip += lo;
-        if (ck.dst_ip) ck.dst_ip += lo;
-        if (ck.src_port) ck.src_port += lo;
-        if (ck.dst_port) ck.dst_port += lo;
-        if (ck.proto) ck.proto += lo;
-        if (ck.flow_start) ck.flow_start += lo;
-        if (ck.flow_end) ck.flow_end += lo;
-        if (ck.value) ck.value += lo;
-        if (ck.src_ns) ck.src_ns += lo;
-        if (ck.dst_ns) ck.dst_ns += lo;
-        return ck;
-    };
     // ---- single GPU, optimistic partition: no histogram pass.  Bucket b owns a fixed slot of kGroupCap rows; a
     // row that finds its slot full goes to the overflow list, and such buckets take the spill path.  With host input
     // the scatter of H2D chunk i runs while chunk i+1 is on the bus.  Falls back to the exact two-pass partition
@@ -918,7 +907,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
                 chunk_range(k, lo, hi);
                 CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
                 if (hi <= lo) continue;
-                CU(launch_scatter(st, offset_cols(lo), hi - lo, f, logB, cursor, part, kSlot, ovf, (uint32_t)ovf_cap,
+                CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, cursor, part, kSlot, ovf, (uint32_t)ovf_cap,
                                   d_stats + ST_OVF)); launches++;
             }
             mark(TAD_PHASE_H2D);          // copy + overlapped scatter of all chunks
@@ -1019,7 +1008,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
                 chunk_range(k, lo, hi);
                 CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
                 if (hi <= lo) continue;
-                CU(launch_scatter(st, offset_cols(lo), hi - lo, f, logB, xcursor, xpart, slotM, nullptr, 0, d_stats + ST_OVF)); launches++;
+                CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, xcursor, xpart, slotM, nullptr, 0, d_stats + ST_OVF)); launches++;
             }
             mark(TAD_PHASE_H2D);          // copy + overlapped scatter of all chunks
         } else {
@@ -1070,7 +1059,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
                 chunk_range(k, lo, hi);
                 CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
                 if (hi <= lo) continue;
-                CU(launch_hist(st, offset_cols(lo), hi - lo, f, logB, hist)); launches++;
+                CU(launch_hist(st, offset_cols(c, lo), hi - lo, f, logB, hist)); launches++;
             }
             mark(TAD_PHASE_H2D);          // copy + overlapped histogram of all chunks
         } else {
@@ -1135,7 +1124,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         mark(TAD_PHASE_H2D);
         for (int cx = 0; cx < K; cx++) {
             const uint64_t lo = xlo(cx), hi = xlo(cx + 1);
-            if (hi > lo) { CU(launch_hist(st, offset_cols(lo), hi - lo, f, logB, hist + (size_t)cx * B)); launches++; }
+            if (hi > lo) { CU(launch_hist(st, offset_cols(c, lo), hi - lo, f, logB, hist + (size_t)cx * B)); launches++; }
         }
         mark(TAD_PHASE_HIST);
         for (int cx = 0; cx < K; cx++) {
@@ -1182,7 +1171,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         ensure(ctx, ctx->exch, recv_total ? recv_total : 32);
         for (int cx = 0; cx < K; cx++) {
             const uint64_t lo = xlo(cx), hi = xlo(cx + 1);
-            if (hi > lo) { CU(launch_scatter(st, offset_cols(lo), hi - lo, f, logB, cursor + (size_t)cx * B, part + lo)); launches++; }
+            if (hi > lo) { CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, cursor + (size_t)cx * B, part + lo)); launches++; }
             CU(cudaEventRecord(ctx->x_ev[cx], st));
             CU(cudaStreamWaitEvent(cs, ctx->x_ev[cx], 0));
             uint64_t so[kMaxRanks], sb[kMaxRanks], ro[kMaxRanks], rb[kMaxRanks];
@@ -1405,10 +1394,9 @@ void publish_rows(tad_job *job, PinnedBlock block, uint64_t rows)
     job->rows.anomaly = ho.anomaly;
 }
 
-// Workspace of one pass of `rows` rows: the pipeline over device columns, the pass's key/value columns (d_col[0..7],
-// `col_rows` rows each), the host chunk staging and the pass counters.  fresh: on an empty workspace.
-size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_rows, bool optimistic, size_t stage_bytes,
-                 bool fresh)
+// The single-GPU pipeline's shape for `rows` input rows, with upper bounds for the rows owned, series and points; the
+// optimistic partition where asked for and its slot buffer may be used.
+PipeShape one_gpu_shape(const tad_ctx *ctx, const tad_job *job, uint64_t rows, bool optimistic)
 {
     PipeShape s;
     s.rows = rows;
@@ -1417,7 +1405,15 @@ size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_r
     s.optimistic = optimistic && ctx->optimistic && rows > 0 && (uint64_t)s.B * kGroupCap * sizeof(Row32) <= kSlotBudget;
     s.owned = s.series = rows;
     s.out_cap = out_cap_guess(rows, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
-    PipeSizes z = pipe_sizes(s);
+    return s;
+}
+
+// Workspace of one pass of `rows` rows: the pipeline over device columns, the pass's key/value columns (d_col[0..7],
+// `col_rows` rows each), the host chunk staging and the pass counters.  fresh: on an empty workspace.
+size_t pass_need(tad_ctx *ctx, const tad_job *job, uint64_t rows, uint64_t col_rows, bool optimistic, size_t stage_bytes,
+                 bool fresh)
+{
+    PipeSizes z = pipe_sizes(one_gpu_shape(ctx, job, rows, optimistic));
     for (int i = 0; i < 8; i++) z.col[i] = has_col(job, i) ? col_bytes(i, col_rows) : 0;
     auto bufs = pipe_bufs(ctx, z);
     bufs.push_back({&ctx->stage, stage_bytes});
@@ -1530,140 +1526,97 @@ void grow_keep(tad_ctx *ctx, DevBuf &b, size_t bytes, size_t keep, cudaStream_t 
 
 constexpr uint64_t kMaxPassRows = (1ull << 32) - 2;   // the pipeline's offsets are u32: the row cap of one pass
 
-// A single-GPU job in hash-range passes (DESIGN.md sections 9 and 10).  Pass (v, M) holds the rows whose key hash has
-// (h & (M - 1)) == v.  The first sweep counts the rows of every residue mod 64, which sizes every pass of every M exactly;
-// a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).  A sweep reads
-// the job's columns (device-resident: one split launch; host: double-buffered chunks behind the copies) or, for a
-// streamed job, the blocks of one round.  Every later sweep must count what the first one counted.
-// Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
-uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_budget_set, PassOut &acc)
+// The largest n <= hi whose workspace need(n) fits `budget`; 0 when none does.
+template <class Need>
+uint64_t largest_fit(uint64_t hi, uint64_t budget, Need need)
 {
-    cudaStream_t st = ctx->stream;
-    const bool stream = job->stream;
-    // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
-    tad_columns pend{};
-    tad_text_column pend_txt[2]{};
-    bool have_pend = stream && next_block(job, pend, pend_txt);
-    const tad_columns &hc = job->cols;
-    const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
-    const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
-    const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
-    auto staged = [&](int i) { return has_col(job, i) && (i < 8 || ns); };
-    // host input: double-buffered chunk staging, at most 1/16 of the budget
-    size_t row_bytes = 0;
-    for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
-    // text key slots: per staged row, kTextRowBytes of text staging (any IPv6 text) and the encode scratch
-    const bool text = job->text[0] || job->text[1];
-    constexpr size_t kTextRowBytes = 48;
-    const size_t text_row = text ? kTextRowBytes + text_scratch_bytes(1u << 20) / (1u << 20) + 1 : 0;
-    uint64_t chunk = 0;
-    size_t half_bytes = 0, tmarks = 0, text_bytes = 0;
-    if (host_input && row_bytes) {
-        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes + text_row))) & ~uint64_t(2047);
-        for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
+    uint64_t lo = 0;
+    while (lo < hi) {
+        const uint64_t mid = lo + (hi - lo + 1) / 2;
+        if (need(mid) <= budget) lo = mid; else hi = mid - 1;
     }
-    if (text && chunk) {
-        tmarks = exact_bytes((chunk / 32 + 2) * 8);
-        text_bytes = alloc_bytes(tmarks + chunk * kTextRowBytes) + alloc_bytes(text_scratch_bytes(chunk));
+    return lo;
+}
+
+// The pass columns: one pass's rows on the device, the job's key/value columns in d_col[0..8), `cap` rows each.  The
+// split and unpack kernels write them through out(); the pipeline reads them through as_input().
+struct PassColumns {
+    tad_ctx *ctx;
+    const tad_job *job;
+    uint64_t cap = 0;
+    PassColumns(tad_ctx *c, const tad_job *j) : ctx(c), job(j) {}
+    PassCols out() const
+    {
+        const DevBuf *d = ctx->d_col;
+        return PassCols{(uint32_t *)d[0].p, (uint32_t *)d[1].p, (uint32_t *)d[5].p, (uint32_t *)d[6].p,
+                        (uint16_t *)d[2].p, (uint16_t *)d[3].p, (uint8_t *)d[4].p, (uint64_t *)d[7].p};
     }
-    const size_t stage_bytes = 2 * half_bytes;
-    const size_t plan_stage = stage_bytes + text_bytes;      // the text staging is planned as part of the staging
-    // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits `b`
-    auto pass_cap = [&](uint64_t b) {
-        uint64_t lo = 0, hi = stream ? kMaxPassRows : std::min(R, kMaxPassRows);
-        while (lo < hi) {
-            const uint64_t mid = lo + (hi - lo + 1) / 2;
-            if (pass_need(ctx, job, mid, mid, false, plan_stage, true) <= b) lo = mid; else hi = mid - 1;
-        }
-        return lo;
-    };
-    uint64_t cap = pass_cap(budget);
-    // host row store (streamed input with a host budget, read once per job by store_trim): out-stage of two halves of
-    // `chunk` packed rows.  The plan above does not depend on it; the store is used only where the out-stage fits next
-    // to the round's buffers at `cap`.
-    const size_t pack_scratch = stream && chunk && host_budget_set ? exact_bytes(residue_pack_scratch_bytes(chunk)) : 0;
-    const size_t ostage_bytes = pack_scratch ? 2 * chunk * sizeof(Row32) + pack_scratch + 256 : 0;
-    const uint64_t host_budget =
-        ostage_bytes && store_round_need(ctx, job, cap, plan_stage, ostage_bytes) <= budget ? host_budget_set : 0;
-    if (host_budget && ctx->store_page == 0) fail(TAD_ERR_INTERNAL, "host row store without a page size");
-    if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
-    uint32_t P = 1;
-    while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
-    // pass columns: a table's passes get `cap` rows; a streamed round's from the hint (or 1M rows without one), grown
-    // geometrically up to `cap` while the first round arrives
-    uint64_t colcap = stream ? std::min(cap, R ? R / P + R / P / 8 + 2048 : uint64_t(1) << 20) : cap;
-    free_workspace(ctx);
-    for (int i = 0; i < 8; i++)
-        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
-    if (stage_bytes && !stream) ensure(ctx, ctx->stage, stage_bytes);
-    if (text_bytes) {
-        ensure(ctx, ctx->tstage, tmarks + chunk * kTextRowBytes);
-        ensure(ctx, ctx->tscratch, text_scratch_bytes(chunk));
+    // room for `rows` rows; `carry`: the first `keep` rows are carried over (the new buffer is allocated before the old
+    // one is freed), else the rows held are not kept
+    void size(uint64_t rows, bool carry = false, uint64_t keep = 0)
+    {
+        for (int i = 0; i < 8; i++)
+            if (has_col(job, i) && carry) grow_keep(ctx, ctx->d_col[i], col_bytes(i, rows), col_bytes(i, keep), ctx->stream);
+            else if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, rows));
+        cap = rows;
     }
-    ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 8);
-    ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
-    PassCols pcols{};
-    auto set_pcols = [&]() {
-        pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
-        pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
-        pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
-        pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
-    };
-    set_pcols();
-    RowFilter f{};
-    f.start_time = job->spec.start_time;
-    f.end_time = job->spec.end_time;
-    if (ns) {
-        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
-        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
-        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
-        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
+    // the columns freed (cap 0): a split into them only counts
+    void drop()
+    {
+        CU(cudaStreamSynchronize(ctx->stream));
+        for (int i = 0; i < 8; i++) free_buf(ctx, ctx->d_col[i]);
+        cap = 0;
     }
-    unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);   // [0, 64): rows per residue, [64]: pass cursor
-    const unsigned long long *h_cnt = ctx->h_small;
-    uint64_t nchunk = 0;             // host chunks staged in the current sweep
-    bool any_host = false;
-    bool count_only = false;         // the host row store fell back mid-round: the rest of the round is only counted
-    uint32_t sweeps = 0;
-    bool store = false;              // the current round goes to the host row store
-    uint64_t ub = 0, have = 0;       // first streamed round: bound of the rows in the pass columns; rows they hold
-    // ---- text key slots (DESIGN.md section 10, "Text keys on the device") ---------------------------------------------
-    // A host chunk's text slot is copied (its marks, then the bytes of its 32-row segments) into the text staging and
-    // encoded into the chunk's staged u32 key column on the copy stream, ahead of the chunk's split or pack.  The
-    // dictionaries live for the whole job, so ids are the same in every round.
-    bool text_dropped = false;       // the dictionaries took the first round's pass columns' room: that round only counted
-    auto dict_bytes = [&]() {
+    // a column the job does not have was never allocated: its pointer is null
+    tad_columns as_input(uint64_t rows) const
+    {
+        const PassCols o = out();
+        return tad_columns{rows, rows, TAD_MEM_DEVICE, 0, o.src_ip, o.dst_ip, o.src_port, o.dst_port, o.proto,
+                           o.flow_start, o.flow_end, o.value, nullptr, nullptr};
+    }
+};
+
+// ---- text key slots (DESIGN.md section 10, "Text keys on the device") -------------------------------------------------
+// A host chunk's text slot is copied (its marks, then the bytes of its 32-row segments) into the text staging and
+// encoded into the chunk's staged u32 key column on the copy stream, ahead of the chunk's split or pack.  The
+// dictionaries (ctx->tdict) live for the whole job, so ids are the same in every round.
+struct TextKeys {
+    tad_ctx *ctx;
+    tad_job *job;
+    uint64_t budget;                 // the job's memory budget (messages)
+    size_t tmarks;                   // the text staging's marks part: a chunk's marks; its text bytes follow
+    int mark;                        // a filtered job: the slot (1 / 2) whose ids carry the drop bit; 0: none
+    uint64_t &launches;
+    bool frozen = false;             // later rounds look names up and add none
+    PassColumns *yield = nullptr;    // the first round's pass columns: under the budget they give way to the dictionaries
+
+    size_t dict_bytes() const
+    {
         size_t b = 0;
         for (auto &t : ctx->tdict)
             for (DevBuf *x : t.bufs()) b += x->cap;
         return b;
-    };
-    // the first round's pass columns are freed for the dictionaries: the round only counts (or goes on to the store)
-    auto drop_pass_cols = [&]() {
-        CU(cudaStreamSynchronize(st));
-        for (int i = 0; i < 8; i++) free_buf(ctx, ctx->d_col[i]);
-        colcap = ub = 0;
-        set_pcols();
-        text_dropped = true;
-        if (!store) count_only = true;
-    };
+    }
     // room for `extra` more dictionary bytes under the budget: in the first round the pass columns give way
-    auto dict_room = [&](size_t extra) {
+    void room(size_t extra)
+    {
         if (!ctx->limit || ctx->held + extra <= ctx->limit) return;
-        if (sweeps == 0 && !text_dropped) drop_pass_cols();
+        if (yield && yield->cap) yield->drop();
         if (ctx->held + extra > ctx->limit)
             fail(TAD_ERR_NOMEM, "the text key dictionaries need %zu bytes of device workspace (%zu held); with the job's "
                  "staging that passes the memory budget of %llu bytes", dict_bytes() + extra, dict_bytes(),
                  (unsigned long long)budget);
-    };
-    auto dict_of = [&](int t) {
+    }
+    TextDict dict(int t) const
+    {
         auto &d = ctx->tdict[t];
         return TextDict{(unsigned long long *)d.slots.p, (uint32_t *)d.minrow.p, (uint32_t *)d.slot_id.p, d.cap,
                         (uint8_t *)d.arena.p, (uint64_t *)d.off.p, (uint64_t *)d.hash.p, (unsigned long long *)d.state.p,
-                        sweeps > 0 ? 1u : 0u};
-    };
+                        frozen ? 1u : 0u};
+    }
     // the dictionaries' names and bytes (exact again), and their decode error flags
-    auto text_sync = [&]() {
+    void sync()
+    {
         for (int t = 0; t < 2; t++)
             if (ctx->tdict[t].state.p)
                 CU(cudaMemcpyAsync(ctx->h_small + 192 + 8 * t, ctx->tdict[t].state.p, 8 * 8, cudaMemcpyDeviceToHost,
@@ -1682,17 +1635,19 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             d.names_ub = w[0];
             d.bytes_ub = w[1];
         }
-    };
-    auto grow_dict_buf = [&](DevBuf &b, size_t bytes, size_t keep) {
+    }
+    void grow_buf(DevBuf &b, size_t bytes, size_t keep)
+    {
         if (bytes <= b.cap) return;
         // geometric growth where the budget allows it, else the exact size
         if (!ctx->limit || ctx->held + exact_bytes(2 * b.cap) <= ctx->limit) bytes = std::max(bytes, 2 * b.cap);
-        dict_room(exact_bytes(bytes));
+        room(exact_bytes(bytes));
         grow_keep(ctx, b, bytes, keep, ctx->copy_stream);
-    };
+    }
     // slot t's dictionary takes `n` more rows of `span` text bytes: its load stays at or below 1/2 counting every row as
     // a new name
-    auto text_grow = [&](int t, uint64_t n, uint64_t span) {
+    void grow(int t, uint64_t n, uint64_t span)
+    {
         auto &d = ctx->tdict[t];
         auto ok = [&]() {
             const uint64_t nn = d.names_ub + n;
@@ -1702,42 +1657,42 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         if (!ok()) {
             if (!d.state.p) {                     // the job's first text chunk of this slot
                 d.names_ub = d.bytes_ub = 0;
-                dict_room(exact_bytes(64));
+                room(exact_bytes(64));
                 ensure(ctx, d.state, 64);
                 CU(cudaMemsetAsync(d.state.p, 0, 64, ctx->copy_stream));
-                grow_dict_buf(d.off, 4096, 0);
+                grow_buf(d.off, 4096, 0);
                 CU(cudaMemsetAsync(d.off.p, 0, 8, ctx->copy_stream));
                 if (const size_t m = job->name_pat[t].size()) {     // the predicate's pattern, for the match kernel
-                    dict_room(exact_bytes(m));
+                    room(exact_bytes(m));
                     ensure(ctx, d.pat, m);
                     CU(cudaMemcpyAsync(d.pat.p, job->name_pat[t].data(), m, cudaMemcpyHostToDevice, ctx->copy_stream));
                 }
             } else {
-                text_sync();
+                sync();
             }
             const uint64_t names = d.names_ub, bytes = d.bytes_ub, nn = names + n;
             if (nn > (1ull << 30))
                 fail(TAD_ERR_INVALID_ARG, "invalid request: a text key slot may hold at most 2^30 distinct names");
-            grow_dict_buf(d.off, (nn + 1) * 8, (names + 1) * 8);
-            grow_dict_buf(d.hash, std::max<uint64_t>(nn, 512) * 8, names * 8);
-            if (job->name_op[t]) grow_dict_buf(d.keep, std::max<uint64_t>(nn, 4096), names);
-            grow_dict_buf(d.arena, std::max<uint64_t>(bytes + span, 4096), bytes);
+            grow_buf(d.off, (nn + 1) * 8, (names + 1) * 8);
+            grow_buf(d.hash, std::max<uint64_t>(nn, 512) * 8, names * 8);
+            if (job->name_op[t]) grow_buf(d.keep, std::max<uint64_t>(nn, 4096), names);
+            grow_buf(d.arena, std::max<uint64_t>(bytes + span, 4096), bytes);
             if (!d.cap || 2 * nn > d.cap) {       // a larger table, the names re-inserted on the device
                 uint64_t c = 1024;                // nn <= 2^30: c <= 2^31
                 while (c < 2 * nn) c *= 2;
-                dict_room(exact_bytes((size_t)c * 8) + 2 * exact_bytes((size_t)c * 4));
+                room(exact_bytes((size_t)c * 8) + 2 * exact_bytes((size_t)c * 4));
                 DevBuf ns, nm, ni;
                 ensure(ctx, ns, (size_t)c * 8);
                 ensure(ctx, nm, (size_t)c * 4);
                 ensure(ctx, ni, (size_t)c * 4);
-                TextDict old = dict_of(t), nd = old;
+                TextDict old = dict(t), nd = old;
                 nd.slots = (unsigned long long *)ns.p;
                 nd.minrow = (uint32_t *)nm.p;
                 nd.slot_id = (uint32_t *)ni.p;
                 nd.cap = (uint32_t)c;
                 CU(launch_text_clear(ctx->copy_stream, nd));
                 CU(launch_text_rehash(ctx->copy_stream, old, nd, names));
-                acc.launches += names ? 1 : 0;
+                launches += names ? 1 : 0;
                 CU(cudaStreamSynchronize(ctx->copy_stream));
                 free_buf(ctx, d.slots);
                 free_buf(ctx, d.minrow);
@@ -1750,14 +1705,16 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         }
         d.names_ub += n;
         d.bytes_ub += span;
-    };
+    }
     // segment s's first byte in text slot t of a block of `rows` rows (the column's end for s = its segment count)
-    auto mark_at = [](const tad_text_column &tx, uint64_t rows, uint64_t s) {
+    static uint64_t mark_at(const tad_text_column &tx, uint64_t rows, uint64_t s)
+    {
         return s < (rows + 31) / 32 ? tx.marks[s] : tx.nbytes;
-    };
+    }
     // rows [lo, lo + n) of a block, cut at a mark where a slot's text does not fit the text staging; the staging grows
     // for a single segment larger than it
-    auto text_fit = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n) {
+    uint64_t fit(const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n)
+    {
         for (int t = 0; t < 2; t++) {
             if (!job->text[t]) continue;
             const uint64_t s0 = lo / 32;
@@ -1783,147 +1740,242 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             n = std::min(n, s1 * 32 - lo);
         }
         return n;
-    };
-    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids at dst[t] (device u32).  A filtered job then
-    // marks the rows its predicates drop (the first round also evaluates them on the names the chunk added); `proto` is
-    // the chunk's staged proto column.
-    const bool filt = job->filtered();
-    const int mark = filt ? (job->text[0] ? 1 : 2) : 0;          // the slot whose ids carry the drop bit
-    auto text_encode = [&](const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, char *const *dst,
-                           const char *proto) {
+    }
+    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids in the chunk's staged key columns `c`.  A
+    // filtered job then marks the rows its predicates drop (the first round also evaluates them on the names the chunk
+    // added) using the chunk's staged proto column.
+    void encode(const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, const ColPtrs &c)
+    {
+        uint32_t *dst[2] = {job->text[0] ? const_cast<uint32_t *>(c.src_ip) : nullptr,
+                            job->text[1] ? const_cast<uint32_t *>(c.dst_ip) : nullptr};
         for (int t = 0; t < 2; t++) {
             if (!job->text[t]) continue;
             const uint64_t s0 = lo / 32, s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
             const uint64_t a = mark_at(tx[t], rows, s0), span = mark_at(tx[t], rows, s1) - a;
             // the first round builds the dictionary; later rounds look names up in it and add none (a frozen table
             // needs no room: a missing name fails the round)
-            if (sweeps == 0 || !ctx->tdict[t].state.p) text_grow(t, n, span);
+            if (!frozen || !ctx->tdict[t].state.p) grow(t, n, span);
             char *m = static_cast<char *>(ctx->tstage.p);
             CU(cudaMemcpyAsync(m, tx[t].marks + s0, (s1 - s0) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
             if (span) CU(cudaMemcpyAsync(m + tmarks, tx[t].bytes + a, span, cudaMemcpyHostToDevice, ctx->copy_stream));
-            CU(launch_text_encode(ctx->copy_stream, dict_of(t), reinterpret_cast<const uint8_t *>(m + tmarks), span,
+            CU(launch_text_encode(ctx->copy_stream, dict(t), reinterpret_cast<const uint8_t *>(m + tmarks), span,
                                   reinterpret_cast<const uint64_t *>(m), (uint32_t)(s1 - s0), s0 * 32, rows, lo, n,
-                                  ctx->tscratch.p, ctx->tscratch.cap, reinterpret_cast<uint32_t *>(dst[t])));
-            acc.launches += kTextLaunches;
-            if (job->name_op[t] && sweeps == 0) {     // an open dictionary: its new names get their predicate byte
+                                  ctx->tscratch.p, ctx->tscratch.cap, dst[t]));
+            launches += kTextLaunches;
+            if (job->name_op[t] && !frozen) {     // an open dictionary: its new names get their predicate byte
                 auto &d = ctx->tdict[t];
-                CU(launch_text_match(ctx->copy_stream, dict_of(t), (uint8_t *)d.keep.p, job->name_op[t],
+                CU(launch_text_match(ctx->copy_stream, dict(t), (uint8_t *)d.keep.p, job->name_op[t],
                                      (const uint8_t *)d.pat.p, (uint32_t)job->name_pat[t].size(), n));
-                acc.launches++;
+                launches++;
             }
         }
-        if (filt) {
+        if (mark) {
             TextMark m{};
             for (int t = 0; t < 2; t++) {
-                m.ids[t] = reinterpret_cast<const uint32_t *>(dst[t]);
+                m.ids[t] = dst[t];
                 m.keep[t] = job->name_op[t] ? (const uint8_t *)ctx->tdict[t].keep.p : nullptr;
             }
-            m.proto = reinterpret_cast<const uint8_t *>(proto);
+            m.proto = c.proto;
             m.proto_eq = job->proto_eq;
-            m.mark = reinterpret_cast<uint32_t *>(dst[mark - 1]);
+            m.mark = dst[mark - 1];
             CU(launch_text_mark(ctx->copy_stream, m, n));
-            acc.launches++;
+            launches++;
         }
-    };
-    // enqueue the split of one block (a table, or one block of a streamed round) for pass (v, M).  Text slots: `tx`, of
-    // which the block's rows are rows [origin, origin + b.rows).
-    auto feed = [&](const tad_columns &b, uint32_t v, uint32_t M, const tad_text_column *tx, uint64_t origin) {
-        const uint64_t n_all = b.rows;
-        if (n_all == 0) return;
+    }
+    // each text slot's dictionary to host memory the job owns (tad_job_names); the device copy goes with the workspace
+    void export_names()
+    {
+        sync();
+        for (int t = 0; t < 2; t++) {
+            if (!job->text[t]) continue;
+            auto &d = ctx->tdict[t];
+            const uint64_t names = d.state.p ? d.names_ub : 0, bytes = d.state.p ? d.bytes_ub : 0;
+            job->names[t].resize(bytes);
+            job->names_off[t].assign(names + 1, 0);
+            if (bytes) CU(cudaMemcpy(job->names[t].data(), d.arena.p, bytes, cudaMemcpyDeviceToHost));
+            if (names) CU(cudaMemcpy(job->names_off[t].data(), d.off.p, (names + 1) * 8, cudaMemcpyDeviceToHost));
+        }
+        CU(release(ctx));
+    }
+    // A dictionary lives for one job.  Every buffer is freed, also on a context with a sticky error (a failed job's
+    // cleanup); returns the first error.
+    static cudaError_t release(tad_ctx *ctx)
+    {
+        cudaError_t e = cudaSuccess;
+        for (auto &t : ctx->tdict) {
+            for (DevBuf *b : t.bufs()) {
+                const cudaError_t f = b->p ? cudaFree(b->p) : cudaSuccess;
+                e = e == cudaSuccess ? f : e;
+                ctx->held -= b->cap;
+                *b = DevBuf{};
+            }
+            t.cap = 0;
+        }
+        return e;
+    }
+};
+
+// One sweep over a job's input for pass (v, M): the rows that pass the job's filters are counted per residue (per owner
+// rank and residue on several GPUs) and the pass's rows are split into the pass columns.  Host blocks go through two
+// staging halves of `chunk` rows each, the split of every chunk behind its copy on the copy stream.
+struct Sweep {
+    tad_ctx *ctx;
+    const tad_job *job;
+    PassOut &acc;
+    const bool ns;                   // the ns_ignore list filters rows: the namespace columns are staged too
+    uint64_t chunk = 0;              // rows per staging half; 0: no host input
+    size_t half_bytes = 0;
+    RowFilter f{};
+    unsigned long long *cnt = nullptr, *cursor = nullptr;   // the split's counters and the pass columns' cursor
+    int log_world = 0;               // as launch_pass_split takes it
+    const int mark;                  // a filtered job: the slot (1 / 2) whose ids carry the drop bit (host chunks only)
+    TextKeys *text = nullptr;        // the job's text key slots, encoded into the staged key columns
+    uint64_t nchunk = 0;             // host chunks staged in this sweep
+    bool any_host = false;
+
+    // `text_row`: text staging and encode scratch bytes per staged row, planned into the staging's 1/16 of the budget
+    Sweep(tad_ctx *c, const tad_job *j, PassOut &a, bool host_input, uint64_t budget, size_t text_row)
+        : ctx(c), job(j), acc(a), ns(!j->ns_ignore.empty() && (j->cols.src_ns || j->cols.dst_ns)),
+          mark(j->filtered() ? (j->text[0] ? 1 : 2) : 0)
+    {
+        size_t row_bytes = 0;
+        for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
+        if (host_input && row_bytes) {
+            chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes + text_row))) &
+                    ~uint64_t(2047);
+            for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
+        }
+    }
+    bool staged(int i) const { return has_col(job, i) && (i < 8 || ns); }
+    size_t stage_bytes() const { return 2 * half_bytes; }
+
+    // staging half h from row `at` as kernel input, with rows [lo, lo + n) of block `b` copied there on the copy stream
+    // (a null `b`: none); text slots are left to the encoder
+    ColPtrs stage(const tad_columns *b, uint64_t lo, uint64_t n, int h, uint64_t at) const
+    {
+        ColPtrs c{};
+        char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
+        for (int i = 0; i < 10; i++) {
+            if (!staged(i)) continue;
+            char *d = dst + col_bytes(i, at);
+            if (b && !(i < 2 && job->text[i]))
+                CU(cudaMemcpyAsync(d, static_cast<const char *>(col_ptr(*b, i)) + col_bytes(i, lo), col_bytes(i, n),
+                                   b->mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                                   ctx->copy_stream));
+            set_col(c, i, d);
+            dst += exact_bytes(col_bytes(i, chunk));
+        }
+        return c;
+    }
+    // the sweep's start (its counters are reset by the caller): the pass columns' previous readers are done before the
+    // copy stream writes again
+    void begin(bool host_input)
+    {
+        CU(cudaEventRecord(ctx->ev[0], ctx->stream));
+        nchunk = 0;
+        any_host = false;
+        if (host_input) {
+            CU(cudaEventRecord(ctx->start_ev, ctx->stream));
+            CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
+        }
+    }
+    // enqueue the split of rows [from, b.rows) of block `b` (a table, or one block of a streamed round; text slots: `tx`)
+    // for pass (v, M) into `pc`; `count_only`: the rows are only counted
+    void feed(const tad_columns &b, uint64_t from, uint32_t v, uint32_t M, const PassColumns &pc, bool count_only,
+              const tad_text_column *tx)
+    {
+        cudaStream_t st = ctx->stream;
+        if (from >= b.rows) return;
         if (b.mem == TAD_MEM_DEVICE) {
-            ColPtrs c{};
-            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(b, i));
-            CU(launch_pass_split(st, c, n_all, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
-                                 d_cnt));
+            CU(launch_pass_split(st, offset_cols(col_ptrs(b), from), b.rows - from, f, M - 1, v, pc.out(),
+                                 count_only ? 0u : (uint32_t)pc.cap, cursor, cnt, 0, log_world));
             acc.launches++;
             return;
         }
         any_host = true;
-        ensure(ctx, ctx->stage, stage_bytes);
-        for (uint64_t lo_r = 0, n; lo_r < n_all; lo_r += n, nchunk++) {
-            n = std::min<uint64_t>(chunk, n_all - lo_r);
-            if (text) n = text_fit(tx, origin + n_all, origin + lo_r, n);
+        ensure(ctx, ctx->stage, stage_bytes());
+        for (uint64_t lo = from, n; lo < b.rows; lo += n, nchunk++) {
+            n = std::min<uint64_t>(chunk, b.rows - lo);
+            if (text) n = text->fit(tx, b.rows, lo, n);
             const int h = (int)(nchunk & 1);
             if (nchunk >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
-            ColPtrs c{};
-            char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-            char *ids[2] = {nullptr, nullptr}, *proto = nullptr;
-            for (int i = 0; i < 10; i++) {
-                if (!staged(i)) continue;
-                const size_t w = col_bytes(i, 1);
-                if (i < 2 && job->text[i])
-                    ids[i] = dst;
-                else
-                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(b, i)) + lo_r * w, n * w,
-                                       cudaMemcpyHostToDevice, ctx->copy_stream));
-                if (i == 4) proto = dst;
-                set_col(c, i, dst);
-                dst += exact_bytes(col_bytes(i, chunk));
-            }
-            if (text) text_encode(tx, origin + n_all, origin + lo_r, n, ids, proto);
+            const ColPtrs c = stage(&b, lo, n, h, 0);
+            if (text) text->encode(tx, b.rows, lo, n, c);
             CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
             CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-            CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, count_only ? 0u : (uint32_t)colcap, d_cnt + kMaxPasses,
-                                 d_cnt, mark));
+            CU(launch_pass_split(st, c, n, f, M - 1, v, pc.out(), count_only ? 0u : (uint32_t)pc.cap, cursor, cnt, mark,
+                                 log_world));
             acc.launches++;
             CU(cudaEventRecord(ctx->stage_ev[h], st));
         }
-    };
-    // first streamed round: make room in the pass columns for every row the next `n` input rows can add (`ub` bounds the
-    // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
-    // With a host budget, rows that would pass `cap` go to the host row store instead: false, `have` = the rows the
-    // pass columns hold.
-    auto room = [&](uint64_t n) {
-        if ((colcap >= cap && !host_budget) || ub + n <= colcap) { ub += n; return true; }
-        CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        have = std::min<uint64_t>(ctx->h_small[128], colcap);
-        if (host_budget && have + n > cap) return false;
-        if (have + n > colcap) {
-            const uint64_t want = std::min(cap, std::max(2 * colcap, have + n));
-            if (text && ctx->limit) {        // beside the dictionaries the columns may not grow: the round only counts
-                size_t grow = 0;
-                for (int i = 0; i < 8; i++) grow += has_col(job, i) ? exact_bytes(col_bytes(i, want)) : 0;
-                if (ctx->held + grow > ctx->limit) {
-                    drop_pass_cols();
-                    return true;
-                }
-            }
-            for (int i = 0; i < 8; i++)
-                if (has_col(job, i)) grow_keep(ctx, ctx->d_col[i], col_bytes(i, want), col_bytes(i, have), st);
-            colcap = want;
-            set_pcols();
-        }
-        ub = have + n;
-        return true;
-    };
-    // ---- host row store (DESIGN.md section 11) ------------------------------------------------------------------------
-    // The first round's blocks are packed into the staging halves; every full half (and the last, partial one) is
-    // counted, scanned and scattered per residue into an out-stage half, whose residue segments are then copied to the
-    // residue's pages on the D2H stream.  The passes load their residues from the pages.
-    RowStore rs(ctx);
-    bool stored = false;             // the store holds the whole first round: the passes load from it
-    bool dropped = false;            // the store fell back in the first round: it only counted
+    }
+    // the sweep's end: its time goes to the h2d phase where it staged host rows (the split runs behind the copies);
+    // `counts`: the counters and the cursor are copied to h_small
+    void end(bool counts)
+    {
+        CU(cudaEventRecord(ctx->ev[1], ctx->stream));
+        if (counts) CU(cudaMemcpyAsync(ctx->h_small, cnt, (kMaxPasses + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        acc.phase_ms[any_host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;
+        acc.device_ms += ms;
+    }
+};
+
+// ---- host row store (DESIGN.md section 11) ----------------------------------------------------------------------------
+// One job's rows in the store: per low-hash-bit residue, a list of pages filled in order.  The pages go back to the
+// context when the job ends, however it ends.  The first round's blocks are packed into the staging halves; every full
+// half (and the last, partial one) is counted, scanned and scattered per residue into an out-stage half, whose residue
+// segments are then copied to the residue's pages on the D2H stream.  The passes load their residues from the pages.
+struct RowStore {
+    tad_ctx *ctx;
+    std::vector<char *> pages[kMaxPasses];
+    uint64_t rows[kMaxPasses] = {};
+    bool active = false;             // the current round goes to the store
+    Sweep *sw;                       // the round's staging, filter and counters
+    uint64_t budget;                 // the job's host budget
+    size_t scratch_bytes;
     uint64_t fill = 0, nhalf = 0, npack = 0;   // rows in the staging half being filled; halves filled; out-stage halves used
     int opend = -1;                  // out-stage half whose copies to the store are not issued yet
     Row32 *ost[2] = {nullptr, nullptr};
     void *pscratch = nullptr;
     uint32_t *d_chunk = nullptr;
-    auto pass_cols_of = [&](uint64_t lo) {        // the pass columns from row `lo`, as kernel input
-        ColPtrs c{};
-        for (int i = 0; i < 8; i++)
-            if (has_col(job, i)) set_col(c, i, static_cast<const char *>(ctx->d_col[i].p) + col_bytes(i, lo));
-        return c;
-    };
-    auto store_drop = [&]() {        // fallback: pages back to the context, the rest of the round is only counted
-        CU(cudaStreamSynchronize(st));          // no pack reads the staging halves any more
-        rs.clear();
-        store = false;
-        count_only = true;
+    RowStore(tad_ctx *c, Sweep &s, uint64_t host_budget, size_t pack_scratch)
+        : ctx(c), sw(&s), budget(host_budget), scratch_bytes(pack_scratch) {}
+    void clear()
+    {
+        cudaStreamSynchronize(ctx->d2h_stream);       // no copy into a page is still in flight
+        for (int j = 0; j < kMaxPasses; j++) {
+            ctx->store_free.insert(ctx->store_free.end(), pages[j].begin(), pages[j].end());
+            pages[j].clear();
+            rows[j] = 0;
+        }
+    }
+    ~RowStore() { clear(); }
+    // the out-stage: two halves of `chunk` packed rows, the pack scratch and the chunk counts
+    void start(size_t ostage_bytes)
+    {
+        ensure(ctx, ctx->stage, sw->stage_bytes());
+        ensure(ctx, ctx->ostage, ostage_bytes);
+        char *p = static_cast<char *>(ctx->ostage.p);
+        ost[0] = reinterpret_cast<Row32 *>(p);
+        ost[1] = reinterpret_cast<Row32 *>(p + sw->chunk * sizeof(Row32));
+        pscratch = p + 2 * sw->chunk * sizeof(Row32);
+        d_chunk = reinterpret_cast<uint32_t *>(p + 2 * sw->chunk * sizeof(Row32) + scratch_bytes);
+        active = true;
+    }
+    // fallback: the pages go back to the context
+    void drop()
+    {
+        CU(cudaStreamSynchronize(ctx->stream));      // no pack reads the staging halves any more
+        clear();
+        active = false;
         opend = -1;
-    };
+    }
     // copies of out-stage half `o`'s residue segments to the pages; false when the store would pass its budget
-    auto store_out = [&](int o) {
+    bool out(int o)
+    {
         const uint64_t page_rows = ctx->store_page / sizeof(Row32);
         CU(cudaEventSynchronize(ctx->cnt_ev[o]));
         CU(cudaStreamWaitEvent(ctx->d2h_stream, ctx->cnt_ev[o], 0));
@@ -1931,62 +1983,261 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         uint64_t at = 0;
         for (int j = 0; j < kMaxPasses; j++) {
             for (uint64_t left = n[j]; left;) {
-                const uint64_t used = rs.rows[j] % page_rows;
+                const uint64_t used = rows[j] % page_rows;
                 if (used == 0) {
-                    char *p = store_take_page(ctx, host_budget);
+                    char *p = store_take_page(ctx, budget);
                     if (!p) return false;
-                    rs.pages[j].push_back(p);
+                    pages[j].push_back(p);
                 }
                 const uint64_t k = std::min(left, page_rows - used);
-                CU(cudaMemcpyAsync(rs.pages[j].back() + used * sizeof(Row32), ost[o] + at, k * sizeof(Row32),
+                CU(cudaMemcpyAsync(pages[j].back() + used * sizeof(Row32), ost[o] + at, k * sizeof(Row32),
                                    cudaMemcpyDeviceToHost, ctx->d2h_stream));
-                rs.rows[j] += k;
+                rows[j] += k;
                 at += k;
                 left -= k;
             }
         }
         CU(cudaEventRecord(ctx->ost_ev[o], ctx->d2h_stream));
         return true;
-    };
+    }
     // count / scan / scatter `n` <= chunk device rows into the next out-stage half, then issue the copies of the previous
     // one (its counts are back by now; this chunk's copies are on the bus meanwhile).  `totals`: count them for the job.
     // `totals` also tells staged rows (marked rows of a filtered job among them) from the pass columns' clean ones.
-    auto pack = [&](const ColPtrs &c, uint64_t n, bool totals) {
+    void pack(const ColPtrs &c, uint64_t n, bool totals)
+    {
         const int o = (int)(npack++ & 1);
+        cudaStream_t st = ctx->stream;
         CU(cudaStreamWaitEvent(st, ctx->ost_ev[o], 0));      // the copies that last read out-stage half o are done
-        CU(launch_residue_pack(st, c, n, f, pscratch, pack_scratch, d_chunk, totals ? d_cnt : nullptr, ost[o],
-                               totals ? mark : 0));
-        acc.launches += 3;
+        CU(launch_residue_pack(st, c, n, sw->f, pscratch, scratch_bytes, d_chunk, totals ? sw->cnt : nullptr, ost[o],
+                               totals ? sw->mark : 0));
+        sw->acc.launches += 3;
         CU(cudaMemcpyAsync(ctx->h_chunk + kMaxPasses * o, d_chunk, kMaxPasses * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaEventRecord(ctx->cnt_ev[o], st));
-        if (opend >= 0 && !store_out(opend)) { store_drop(); return; }
+        if (opend >= 0 && !out(opend)) { drop(); return; }
         opend = o;
-    };
-    auto pack_half = [&]() {         // the staging half being filled
+    }
+    void pack_half()                 // the staging half being filled
+    {
         const int h = (int)(nhalf++ & 1);
-        ColPtrs c{};
-        char *src = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-        for (int i = 0; i < 10; i++) {
-            if (!staged(i)) continue;
-            set_col(c, i, src);
-            src += exact_bytes(col_bytes(i, chunk));
-        }
         CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
-        CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-        pack(c, fill, true);
-        CU(cudaEventRecord(ctx->stage_ev[h], st));
+        CU(cudaStreamWaitEvent(ctx->stream, ctx->chunk_ev[h], 0));
+        pack(sw->stage(nullptr, 0, 0, h, 0), fill, true);
+        CU(cudaEventRecord(ctx->stage_ev[h], ctx->stream));
         fill = 0;
+    }
+    // one block into the staging halves (a D2D copy for a device block); a full half is packed.  Returns the rows it
+    // took: the store may fall back inside the block.
+    uint64_t put(const tad_columns &b, const tad_text_column *tx)
+    {
+        uint64_t lo = 0;
+        sw->any_host = true;         // the round's time is the copies' (h2d phase), as for a sweep of host blocks
+        while (lo < b.rows && active) {
+            if (sw->job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+            const int h = (int)(nhalf & 1);
+            if (fill == 0) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // its last pack is done
+            uint64_t n = std::min(sw->chunk - fill, b.rows - lo);
+            if (sw->text) n = sw->text->fit(tx, b.rows, lo, n);
+            const ColPtrs c = sw->stage(&b, lo, n, h, fill);
+            if (sw->text) sw->text->encode(tx, b.rows, lo, n, c);
+            fill += n;
+            lo += n;
+            if (fill == sw->chunk) pack_half();
+        }
+        return lo;
+    }
+    // end of the round: the last half, the last copies; the out-stage is not needed any more.  True when the store
+    // holds the whole round.
+    bool end()
+    {
+        if (active && fill) pack_half();
+        if (active && opend >= 0 && !out(opend)) drop();
+        const bool stored = active;
+        if (active && opend >= 0) CU(cudaStreamWaitEvent(ctx->stream, ctx->ost_ev[opend], 0));
+        active = false;
+        CU(cudaStreamSynchronize(ctx->stream));
+        free_buf(ctx, ctx->ostage);
+        return stored;
+    }
+    // pass (v, M) from the store into the pass columns, through the staging halves
+    void load(uint32_t v, uint32_t M, const PassCols &to)
+    {
+        const uint64_t page_rows = ctx->store_page / sizeof(Row32), piece = sw->half_bytes / sizeof(Row32);
+        sw->begin(true);
+        sw->any_host = true;
+        uint64_t at = 0, k = 0;
+        for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M)
+            for (size_t pg = 0; pg < pages[j].size(); pg++) {
+                const uint64_t in_pg = std::min(page_rows, rows[j] - pg * page_rows);
+                for (uint64_t r0 = 0; r0 < in_pg; r0 += piece, k++) {
+                    const uint64_t n = std::min(piece, in_pg - r0);
+                    const int h = (int)(k & 1);
+                    Row32 *dst = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->stage.p) + h * sw->half_bytes);
+                    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));    // its last unpack is done
+                    CU(cudaMemcpyAsync(dst, pages[j][pg] + r0 * sizeof(Row32), n * sizeof(Row32),
+                                       cudaMemcpyHostToDevice, ctx->copy_stream));
+                    CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
+                    CU(cudaStreamWaitEvent(ctx->stream, ctx->chunk_ev[h], 0));
+                    CU(launch_store_unpack(ctx->stream, dst, n, to, at));
+                    sw->acc.launches++;
+                    CU(cudaEventRecord(ctx->stage_ev[h], ctx->stream));
+                    at += n;
+                }
+            }
+        sw->end(false);
+    }
+};
+
+// The buffers earlier passes grew are freed, except what every pass reads: the pass columns, the staging, the counters,
+// the ns_ignore list, the text key dictionaries and their staging, and `small` (run_pipeline ensures it first anyway).
+void free_pass_buffers(tad_ctx *ctx)
+{
+    for (DevBuf *b : workspace_bufs(ctx)) {
+        if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore || b == &ctx->small ||
+            (b >= ctx->d_col && b < ctx->d_col + 8) || b == &ctx->tstage || b == &ctx->tscratch ||
+            ((void *)b >= (void *)ctx->tdict && (void *)b < (void *)(ctx->tdict + 2)))
+            continue;
+        free_buf(ctx, *b);
+    }
+}
+
+using PassList = std::deque<std::pair<uint32_t, uint32_t>>;
+
+// The passes of a job in hash-range passes: (v, P) for v < P, in order, each run by run(v, M, rest, out) with `rest` the
+// passes queued behind it; an empty pass leaves `out` as it is.  A pass for which run returns true (split) is replaced by
+// (v, 2M) and (v + M, 2M) and gives its fits back.  Fills `acc` (sums over the passes, acc.block = all result rows) and
+// returns the number of passes.
+template <class Run>
+uint32_t run_pass_queue(tad_ctx *ctx, tad_job *job, uint32_t P, PassOut &acc, Run run)
+{
+    PassList todo;
+    for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
+    std::vector<PassOut> outs;
+    uint32_t passes = 0, planned = P;
+    set_passes(job, 0, planned);
+    try {
+        while (!todo.empty()) {
+            const tad_progress before = progress_of(job);
+            const uint32_t v = todo.front().first, M = todo.front().second;
+            todo.pop_front();
+            PassOut o;
+            if (run(v, M, (const PassList &)todo, o)) {
+                todo.push_front({v + M, 2 * M});
+                todo.push_front({v, 2 * M});
+                set_passes(job, passes, ++planned, &before);
+                continue;
+            }
+            add_pass(acc, o);
+            if (o.block.p) outs.push_back(o);
+            set_passes(job, ++passes, planned);
+        }
+        join_passes(ctx, outs, acc);
+    } catch (...) {
+        for (PassOut &o : outs) give_pinned(ctx, o.block);
+        throw;
+    }
+    return passes;
+}
+
+// A single-GPU job in hash-range passes (DESIGN.md sections 9 and 10).  Pass (v, M) holds the rows whose key hash has
+// (h & (M - 1)) == v.  The first sweep counts the rows of every residue mod 64, which sizes every pass of every M exactly;
+// a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).  A sweep reads
+// the job's columns (device-resident: one split launch; host: double-buffered chunks behind the copies) or, for a
+// streamed job, the blocks of one round.  Every later sweep must count what the first one counted.
+// Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
+uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_budget_set, PassOut &acc)
+{
+    cudaStream_t st = ctx->stream;
+    const bool stream = job->stream;
+    // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
+    tad_columns pend{};
+    tad_text_column pend_txt[2]{};
+    bool have_pend = stream && next_block(job, pend, pend_txt);
+    const tad_columns &hc = job->cols;
+    const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
+    const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
+    // host input: double-buffered chunk staging, at most 1/16 of the budget; text key slots: per staged row,
+    // kTextRowBytes of text staging (any IPv6 text) and the encode scratch
+    const bool text = job->text[0] || job->text[1];
+    constexpr size_t kTextRowBytes = 48;
+    Sweep sw(ctx, job, acc, host_input, budget,
+             text ? kTextRowBytes + text_scratch_bytes(1u << 20) / (1u << 20) + 1 : 0);
+    const uint64_t chunk = sw.chunk;
+    size_t tmarks = 0, text_bytes = 0;
+    if (text && chunk) {
+        tmarks = exact_bytes((chunk / 32 + 2) * 8);
+        text_bytes = alloc_bytes(tmarks + chunk * kTextRowBytes) + alloc_bytes(text_scratch_bytes(chunk));
+    }
+    const size_t stage_bytes = sw.stage_bytes();
+    const size_t plan_stage = stage_bytes + text_bytes;      // the text staging is planned as part of the staging
+    // rows one pass may hold: the largest count whose workspace (exact partition, empty workspace) fits `b`
+    auto pass_cap = [&](uint64_t b) {
+        return largest_fit(stream ? kMaxPassRows : std::min(R, kMaxPassRows), b,
+                           [&](uint64_t n) { return pass_need(ctx, job, n, n, false, plan_stage, true); });
     };
-    auto start_store = [&]() {
-        ensure(ctx, ctx->stage, stage_bytes);
-        ensure(ctx, ctx->ostage, ostage_bytes);
-        char *p = static_cast<char *>(ctx->ostage.p);
-        ost[0] = reinterpret_cast<Row32 *>(p);
-        ost[1] = reinterpret_cast<Row32 *>(p + chunk * sizeof(Row32));
-        pscratch = p + 2 * chunk * sizeof(Row32);
-        d_chunk = reinterpret_cast<uint32_t *>(p + 2 * chunk * sizeof(Row32) + pack_scratch);
-        store = true;
+    uint64_t cap = pass_cap(budget);
+    // host row store (streamed input with a host budget, read once per job by store_trim): out-stage of two halves of
+    // `chunk` packed rows.  The plan above does not depend on it; the store is used only where the out-stage fits next
+    // to the round's buffers at `cap`.
+    const size_t pack_scratch = stream && chunk && host_budget_set ? exact_bytes(residue_pack_scratch_bytes(chunk)) : 0;
+    const size_t ostage_bytes = pack_scratch ? 2 * chunk * sizeof(Row32) + pack_scratch + 256 : 0;
+    const uint64_t host_budget =
+        ostage_bytes && store_round_need(ctx, job, cap, plan_stage, ostage_bytes) <= budget ? host_budget_set : 0;
+    if (host_budget && ctx->store_page == 0) fail(TAD_ERR_INTERNAL, "host row store without a page size");
+    if (cap == 0) fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes does not hold one row of a pass", (unsigned long long)budget);
+    uint32_t P = 1;
+    while (P < (uint32_t)kMaxPasses && R / P > cap / 8 * 7) P *= 2;     // 1/8 head-room for hash imbalance
+    // pass columns: a table's passes get `cap` rows; a streamed round's from the hint (or 1M rows without one), grown
+    // geometrically up to `cap` while the first round arrives
+    free_workspace(ctx);
+    PassColumns pc(ctx, job);
+    pc.size(stream ? std::min(cap, R ? R / P + R / P / 8 + 2048 : uint64_t(1) << 20) : cap);
+    if (stage_bytes && !stream) ensure(ctx, ctx->stage, stage_bytes);
+    if (text_bytes) {
+        ensure(ctx, ctx->tstage, tmarks + chunk * kTextRowBytes);
+        ensure(ctx, ctx->tscratch, text_scratch_bytes(chunk));
+    }
+    ensure(ctx, ctx->pcnt, (kMaxPasses + 1) * 8);
+    ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
+    unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);   // [0, 64): rows per residue, [64]: pass cursor
+    const unsigned long long *h_cnt = ctx->h_small;
+    sw.f = row_filter(ctx, job, sw.ns);
+    sw.cnt = d_cnt;
+    sw.cursor = d_cnt + kMaxPasses;
+    TextKeys tk{ctx, job, budget, tmarks, sw.mark, acc.launches, false, &pc};
+    if (text) sw.text = &tk;
+    bool count_only = false;         // the first round's rows are only counted (the store fell back, or the pass columns
+                                     // gave way to the text key dictionaries)
+    uint32_t sweeps = 0;
+    uint64_t ub = 0, have = 0;       // first streamed round: bound of the rows in the pass columns; rows they hold
+    // first streamed round: make room in the pass columns for every row the next `n` input rows can add (`ub` bounds the
+    // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
+    // With a host budget, rows that would pass `cap` go to the host row store instead: false, `have` = the rows the
+    // pass columns hold.
+    auto room = [&](uint64_t n) {
+        if ((pc.cap >= cap && !host_budget) || ub + n <= pc.cap) { ub += n; return true; }
+        CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        have = std::min<uint64_t>(ctx->h_small[128], pc.cap);
+        if (host_budget && have + n > cap) return false;
+        if (have + n > pc.cap) {
+            const uint64_t want = std::min(cap, std::max(2 * pc.cap, have + n));
+            if (text && ctx->limit) {        // beside the dictionaries the columns may not grow: the round only counts
+                size_t grow = 0;
+                for (int i = 0; i < 8; i++) grow += has_col(job, i) ? exact_bytes(col_bytes(i, want)) : 0;
+                if (ctx->held + grow > ctx->limit) {
+                    pc.drop();
+                    count_only = true;
+                    return true;
+                }
+            }
+            pc.size(want, true, have);
+        }
+        ub = have + n;
+        return true;
     };
+    RowStore rs(ctx, sw, host_budget, pack_scratch);
+    bool stored = false;             // the store holds the whole first round: the passes load from it
+    bool dropped = false;            // the store fell back in the first round: it only counted
     // the pass columns overflow in the first round: their `have` rows go to the store first (counted already)
     auto switch_to_store = [&]() {
         // the out-stage was planned without the dictionaries: where it does not fit beside them, the round only counts
@@ -1995,110 +2246,19 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             count_only = true;
             return;
         }
-        start_store();
-        for (uint64_t lo = 0; lo < have && store; lo += chunk) pack(pass_cols_of(lo), std::min(chunk, have - lo), false);
-    };
-    // one block into the staging halves (a D2D copy for a device block); a full half is packed.  The rest of a block
-    // the store fell back in is counted.
-    auto put = [&](const tad_columns &b, const tad_text_column *tx) {
-        uint64_t lo = 0;
-        any_host = true;             // the round's time is the copies' (h2d phase), as for a sweep of host blocks
-        while (lo < b.rows && store) {
-            if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
-            const int h = (int)(nhalf & 1);
-            if (fill == 0) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // its last pack is done
-            uint64_t n = std::min(chunk - fill, b.rows - lo);
-            if (text) n = text_fit(tx, b.rows, lo, n);
-            char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-            char *ids[2] = {nullptr, nullptr}, *proto = nullptr;
-            for (int i = 0; i < 10; i++) {
-                if (!staged(i)) continue;
-                const size_t w = col_bytes(i, 1);
-                if (i < 2 && job->text[i])
-                    ids[i] = dst + fill * w;
-                else
-                    CU(cudaMemcpyAsync(dst + fill * w, static_cast<const char *>(col_ptr(b, i)) + lo * w, n * w,
-                                       b.mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
-                                       ctx->copy_stream));
-                if (i == 4) proto = dst + fill * w;
-                dst += exact_bytes(col_bytes(i, chunk));
-            }
-            if (text) text_encode(tx, b.rows, lo, n, ids, proto);
-            fill += n;
-            lo += n;
-            if (fill == chunk) pack_half();
-        }
-        if (lo < b.rows) {
-            tad_columns rest = b;
-            rest.rows -= lo;
-            void **cols[10] = {(void **)&rest.src_ip, (void **)&rest.dst_ip, (void **)&rest.src_port, (void **)&rest.dst_port,
-                               (void **)&rest.proto, (void **)&rest.flow_start, (void **)&rest.flow_end, (void **)&rest.value,
-                               (void **)&rest.src_ns, (void **)&rest.dst_ns};
-            for (int i = 0; i < 10; i++)
-                if (*cols[i]) *cols[i] = static_cast<char *>(*cols[i]) + col_bytes(i, lo);
-            feed(rest, 0, P, tx, lo);
-        }
-    };
-    // end of the store's round: the last half, the last copies; the out-stage is not needed any more
-    auto end_store = [&]() {
-        if (store && fill) pack_half();
-        if (store && opend >= 0 && !store_out(opend)) store_drop();
-        if (store) {
-            if (opend >= 0) CU(cudaStreamWaitEvent(st, ctx->ost_ev[opend], 0));
-            stored = true;
-            store = false;
-        }
-        CU(cudaStreamSynchronize(st));
-        free_buf(ctx, ctx->ostage);
-        dropped = count_only;
-        count_only = false;          // later rounds split their pass into the pass columns
-    };
-    // pass (v, M) from the store into the pass columns, through the staging halves
-    auto load = [&](uint32_t v, uint32_t M) {
-        const uint64_t page_rows = ctx->store_page / sizeof(Row32), piece = half_bytes / sizeof(Row32);
-        CU(cudaEventRecord(ctx->ev[0], st));
-        CU(cudaEventRecord(ctx->start_ev, st));
-        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
-        uint64_t at = 0, k = 0;
-        for (uint32_t j = v; j < (uint32_t)kMaxPasses; j += M)
-            for (size_t pg = 0; pg < rs.pages[j].size(); pg++) {
-                const uint64_t in_pg = std::min(page_rows, rs.rows[j] - pg * page_rows);
-                for (uint64_t r0 = 0; r0 < in_pg; r0 += piece, k++) {
-                    const uint64_t n = std::min(piece, in_pg - r0);
-                    const int h = (int)(k & 1);
-                    Row32 *dst = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->stage.p) + h * half_bytes);
-                    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));    // its last unpack is done
-                    CU(cudaMemcpyAsync(dst, rs.pages[j][pg] + r0 * sizeof(Row32), n * sizeof(Row32),
-                                       cudaMemcpyHostToDevice, ctx->copy_stream));
-                    CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
-                    CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-                    CU(launch_store_unpack(st, dst, n, pcols, at));
-                    acc.launches++;
-                    CU(cudaEventRecord(ctx->stage_ev[h], st));
-                    at += n;
-                }
-            }
-        CU(cudaEventRecord(ctx->ev[1], st));
-        CU(cudaStreamSynchronize(st));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        acc.phase_ms[TAD_PHASE_H2D] += ms;
-        acc.device_ms += ms;
+        rs.start(ostage_bytes);
+        const ColPtrs held = col_ptrs(pc.as_input(have));
+        for (uint64_t lo = 0; lo < have && rs.active; lo += chunk) rs.pack(offset_cols(held, lo), std::min(chunk, have - lo), false);
+        if (!rs.active) count_only = true;   // the store fell back: the rest of the round is only counted
     };
     uint64_t counts[kMaxPasses];
     bool open = false;               // a streamed round is swept and its caller waits in tad_stream_end
     // one sweep over the input: the rows of pass (v, M) -> the pass columns; returns the rows of the pass
     auto sweep = [&](uint32_t v, uint32_t M) -> uint64_t {
         CU(cudaMemsetAsync(d_cnt, 0, (kMaxPasses + 1) * 8, st));
-        CU(cudaEventRecord(ctx->ev[0], st));
-        nchunk = 0;
-        any_host = false;
-        if (host_input) {
-            CU(cudaEventRecord(ctx->start_ev, st));
-            CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
-        }
+        sw.begin(host_input);
         if (!stream) {
-            feed(hc, v, M, nullptr, 0);
+            sw.feed(hc, 0, v, M, pc, count_only, nullptr);
         } else {
             // the round's blocks; block k is released (its push returns) once block k+1 is enqueued and k's copy is done
             uint64_t rows = 0, k = 0;
@@ -2107,13 +2267,18 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             tad_text_column tx[2]{};
             bool got = have_pend ? (b = pend, tx[0] = pend_txt[0], tx[1] = pend_txt[1], true) : next_block(job, b, tx);
             have_pend = false;
-            if (sweeps == 0 && host_budget && P > 1) start_store();     // the hint plans passes: the round goes to the store
+            if (sweeps == 0 && host_budget && P > 1)         // the hint plans passes: the round goes to the store
+                rs.start(ostage_bytes);
             while (got) {
-                if (sweeps == 0 && host_budget && !store && !count_only && !room(b.rows)) switch_to_store();
+                // TextKeys::room drops the first round's pass columns (cap 0) for the dictionaries: the rest is only counted
+                if (sweeps == 0 && pc.cap == 0 && !rs.active) count_only = true;
+                if (sweeps == 0 && host_budget && !rs.active && !count_only && !room(b.rows)) switch_to_store();
                 else if (sweeps == 0 && !host_budget && !count_only) room(b.rows);
-                const bool to_store = store;
-                if (store) put(b, tx); else feed(b, v, M, tx, 0);
-                if (to_store && !store) {            // the store fell back inside this block: its rest was split on st
+                const bool to_store = rs.active;
+                const uint64_t took = to_store ? rs.put(b, tx) : 0;
+                count_only = count_only || (to_store && !rs.active);   // the store fell back: the rest is only counted
+                if (!rs.active) sw.feed(b, took, v, M, pc, count_only, tx);      // (v, M) = (0, P) while it stores
+                if (to_store && !rs.active) {
                     CU(cudaEventRecord(ctx->start_ev, st));
                     CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
                 }
@@ -2132,17 +2297,15 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                 got = next_block(job, b, tx);
             }
             if (sweeps == 0) job->round_rows = rows;
-            if (sweeps == 0 && ctx->ostage.p) end_store();
+            if (sweeps == 0 && ctx->ostage.p) {
+                stored = rs.end();
+                dropped = !stored;
+                count_only = false;          // later rounds split their pass into the pass columns
+            }
             open = true;
         }
-        CU(cudaEventRecord(ctx->ev[1], st));
-        CU(cudaMemcpyAsync(ctx->h_small, d_cnt, (kMaxPasses + 1) * 8, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        acc.phase_ms[any_host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;      // the split runs behind the copies
-        acc.device_ms += ms;
-        if (text) text_sync();
+        sw.end(true);
+        if (text) tk.sync();
         if (sweeps > 0)
             for (int j = 0; j < kMaxPasses; j++)
                 if (h_cnt[j] != counts[j])
@@ -2150,6 +2313,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                          "delivered %llu: the source changed between reads", sweeps + 1, (unsigned long long)h_cnt[j], j,
                          (unsigned long long)counts[j]);
         sweeps++;
+        tk.frozen = true;
+        tk.yield = nullptr;
         return h_cnt[kMaxPasses];
     };
     const uint64_t got0 = sweep(0, P);
@@ -2157,7 +2322,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     if (text) {
         count_only = false;
         // the passes run beside the dictionaries
-        const size_t held_dict = dict_bytes();
+        const size_t held_dict = tk.dict_bytes();
         cap = pass_cap(budget > held_dict ? budget - held_dict : 0);
         if (cap == 0)
             fail(TAD_ERR_NOMEM, "the text key dictionaries hold %zu bytes: beside them the memory budget of %llu bytes does "
@@ -2188,106 +2353,45 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
              pass_need(ctx, job, rows, rows, false, plan_stage, true), (unsigned long long)budget);
     };
     if (largest(P) > cap) too_big(largest(kMaxPasses));
-    bool loaded = !stored && !dropped && P == P0 && got0 <= colcap;     // pass (0, P) is in the pass columns already
-    std::deque<std::pair<uint32_t, uint32_t>> todo;
-    for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
-    // a streamed round stays open until the engine knows whether another sweep (round) follows
-    auto finish_round = [&]() {
+    bool loaded = !stored && !dropped && P == P0 && got0 <= pc.cap;     // pass (0, P) is in the pass columns already
+    // a streamed round stays open until the engine knows whether another sweep (round) follows: one does while a queued
+    // pass has rows that are not in the store
+    auto finish_round = [&](bool more) {
         if (!open) return;
-        bool more = false;
-        for (const auto &e : todo) more = more || (!stored && pass_rows(e.first, e.second) > 0);
-        close_round(job, more);
+        close_round(job, !stored && more);
         open = false;
     };
     if (stored)
         for (int j = 0; j < kMaxPasses; j++) job->stored_rows += rs.rows[j];
-    if (!loaded) finish_round();
-    std::vector<PassOut> outs;
-    uint32_t passes = 0, planned = P;
-    set_passes(job, 0, planned);
-    try {
-        while (!todo.empty()) {
-            if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
-            const tad_progress before = progress_of(job);
-            const uint32_t v = todo.front().first, M = todo.front().second;
-            todo.pop_front();
-            const uint64_t rows = pass_rows(v, M);
-            if (!loaded && rows) {
-                if (stream && rows > colcap) {          // later rounds: the counts size the pass columns exactly
-                    for (int i = 0; i < 8; i++)
-                        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, rows));
-                    colcap = rows;
-                    set_pcols();
-                }
-                if (stored) load(v, M); else sweep(v, M);
-            }
-            loaded = false;
-            bool split_pass = false;
-            if (rows) {
-                tad_columns pc{};
-                pc.rows = pc.capacity = rows;
-                pc.mem = TAD_MEM_DEVICE;
-                pc.src_ip = has_col(job, 0) ? pcols.src_ip : nullptr; pc.dst_ip = has_col(job, 1) ? pcols.dst_ip : nullptr;
-                pc.src_port = has_col(job, 2) ? pcols.src_port : nullptr; pc.dst_port = has_col(job, 3) ? pcols.dst_port : nullptr;
-                pc.proto = has_col(job, 4) ? pcols.proto : nullptr; pc.flow_start = has_col(job, 5) ? pcols.flow_start : nullptr;
-                pc.flow_end = pcols.flow_end; pc.value = pcols.value;
-                // optimistic partition where its slot buffer fits next to what the context holds; else the exact one, on
-                // a workspace cleared of earlier passes' buffers if need be (the planner sized `cap` for that)
-                const bool opt = pass_need(ctx, job, rows, cap, true, stage_bytes, false) <= budget;
-                if (!opt && pass_need(ctx, job, rows, cap, false, stage_bytes, false) > budget) {
-                    for (DevBuf *b : workspace_bufs(ctx)) {
-                        // kept: the pass columns, staging, counters and the ns_ignore list the sweeps read
-                        if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore ||
-                            (b >= ctx->d_col && b < ctx->d_col + 8) || b == &ctx->tstage || b == &ctx->tscratch ||
-                            (text && (void *)b >= (void *)ctx->tdict && (void *)b < (void *)(ctx->tdict + 2)))
-                            continue;
-                        if (b->p) CU(cudaFree(b->p));
-                        ctx->held -= b->cap;
-                        *b = DevBuf{};
-                    }
-                }
-                PassOut o;
-                try {
-                    run_pipeline(ctx, job, pc, false, !opt, o);
-                } catch (const PassSplit &) {
-                    CU(cudaStreamSynchronize(st));
-                    if (M >= (uint32_t)kMaxPasses) too_big(rows);
-                    todo.push_front({v + M, 2 * M});
-                    todo.push_front({v, 2 * M});
-                    split_pass = true;
-                }
-                if (!split_pass) {
-                    add_pass(acc, o);
-                    outs.push_back(o);
-                }
-            }
-            if (!split_pass) passes++;
-            else planned++;
-            set_passes(job, passes, planned, split_pass ? &before : nullptr);
-            finish_round();
+    if (!loaded) finish_round(largest(P) > 0);
+    auto run_one = [&](uint32_t v, uint32_t M, const PassList &rest, PassOut &o) {
+        const uint64_t rows = pass_rows(v, M);
+        bool more = rows > 0;        // the round the previous pass was swept in closes once that pass has run
+        for (const auto &e : rest) more = more || pass_rows(e.first, e.second) > 0;
+        if (!loaded) finish_round(more);
+        if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+        if (!loaded && rows) {
+            if (stream && rows > pc.cap) pc.size(rows);     // later rounds: the counts size the pass columns exactly
+            if (stored) rs.load(v, M, pc.out()); else sweep(v, M);
         }
-        join_passes(ctx, outs, acc);
-    } catch (...) {
-        for (PassOut &o : outs) give_pinned(ctx, o.block);
-        throw;
-    }
-    // each text slot's dictionary to host memory the job owns (tad_job_names); the device copy goes with the workspace
-    for (int t = 0; t < 2; t++) {
-        if (!job->text[t]) continue;
-        auto &d = ctx->tdict[t];
-        uint64_t names = 0, bytes = 0;
-        if (d.state.p) {
-            text_sync();
-            names = d.names_ub;
-            bytes = d.bytes_ub;
+        loaded = false;
+        if (!rows) return false;
+        // optimistic partition where its slot buffer fits next to what the context holds; else the exact one, on a
+        // workspace cleared of earlier passes' buffers if need be (the planner sized `cap` for that)
+        const bool opt = pass_need(ctx, job, rows, cap, true, stage_bytes, false) <= budget;
+        if (!opt && pass_need(ctx, job, rows, cap, false, stage_bytes, false) > budget) free_pass_buffers(ctx);
+        try {
+            run_pipeline(ctx, job, pc.as_input(rows), false, !opt, o);
+        } catch (const PassSplit &) {
+            CU(cudaStreamSynchronize(st));
+            if (M >= (uint32_t)kMaxPasses) too_big(rows);
+            return true;
         }
-        job->names[t].resize(bytes);
-        job->names_off[t].assign(names + 1, 0);
-        if (bytes) CU(cudaMemcpy(job->names[t].data(), d.arena.p, bytes, cudaMemcpyDeviceToHost));
-        if (names) CU(cudaMemcpy(job->names_off[t].data(), d.off.p, (names + 1) * 8, cudaMemcpyDeviceToHost));
-        for (DevBuf *x : d.bufs()) free_buf(ctx, *x);
-        d.cap = 0;
-    }
+        return false;
+    };
+    const uint32_t passes = run_pass_queue(ctx, job, P, acc, run_one);
+    finish_round(false);
+    if (text) tk.export_names();
     return passes;
 }
 
@@ -2384,16 +2488,8 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     const tad_columns &hc = job->cols;
     const uint64_t R = hc.rows;
     const bool host = hc.mem != TAD_MEM_DEVICE && R > 0;
-    const bool ns = !job->ns_ignore.empty() && (hc.src_ns || hc.dst_ns);
-    auto staged = [&](int i) { return col_ptr(hc, i) && (i < 8 || ns); };
-    size_t row_bytes = 0, half_bytes = 0;
-    for (int i = 0; i < 10; i++) row_bytes += staged(i) ? col_bytes(i, 1) : 0;
-    uint64_t chunk = 0;
-    if (host) {         // double-buffered chunk staging, at most 1/16 of the budget
-        chunk = std::min<uint64_t>(8u << 20, std::max<uint64_t>(2048, budget / 16 / (2 * row_bytes))) & ~uint64_t(2047);
-        for (int i = 0; i < 10; i++) half_bytes += staged(i) ? exact_bytes(col_bytes(i, chunk)) : 0;
-    }
-    const size_t stage_bytes = 2 * half_bytes;
+    Sweep sw(ctx, job, acc, host, budget, 0);
+    const size_t stage_bytes = sw.stage_bytes();
     const size_t NC = (size_t)W * kMaxPasses;               // one rank's (owner, residue) counters
     const size_t pcnt_bytes = (NC * (W + 1) + 1) * 8;        // mine, every rank's (all-gathered), the pass cursor
     set_progress(job, TAD_STATE_RUNNING, 0);
@@ -2402,22 +2498,17 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     // what every pass keeps: pass columns of `n` rows, staging, counters, the ns_ignore list (and kFixedBytes)
     auto kept_bytes = [&](uint64_t n) {
         std::vector<std::pair<DevBuf *, size_t>> b = {{&ctx->stage, stage_bytes}, {&ctx->pcnt, pcnt_bytes},
-                                                      {&ctx->ns_ignore, ns ? job->ns_ignore.size() * 4 : 0}};
+                                                      {&ctx->ns_ignore, sw.ns ? job->ns_ignore.size() * 4 : 0}};
         for (int i = 0; i < 8; i++) b.push_back({&ctx->d_col[i], has_col(job, i) ? col_bytes(i, n) : 0});
         return workspace_after(ctx, b, true);
     };
     // rows one pass may hold on this rank: the largest n for which a pass whose input rows, owned rows and largest shard
     // are all n fits the budget (exact partition)
-    auto need_n = [&](uint64_t n) {
+    const uint64_t cap = largest_fit(kMaxPassRows, budget, [&](uint64_t n) {
         const uint64_t g = n * (uint64_t)W;
         return kept_bytes(std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) + alloc_bytes(mp_xbuf_bytes(ctx, g, n, false));
-    };
-    uint64_t lo = 0, hi = kMaxPassRows;
-    while (lo < hi) {
-        const uint64_t mid = lo + (hi - lo + 1) / 2;
-        if (need_n(mid) <= budget) lo = mid; else hi = mid - 1;
-    }
-    const uint64_t cap = lo, colcap = std::min(cap, R);
+    });
+    const uint64_t colcap = std::min(cap, R);
 
     // The budget applies from the plan on: until then the context may still hold the exported buffer of an earlier job,
     // larger than this budget, which only the plan all-gather lets it free.  No rank may fail on its own before it.
@@ -2480,69 +2571,24 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     while (P < (uint32_t)kMaxPasses && !guess_ok(P)) P *= 2;
 
     // ---- pass columns and the sweep --------------------------------------------------------------------------------------
-    for (int i = 0; i < 8; i++)
-        if (has_col(job, i)) ensure(ctx, ctx->d_col[i], col_bytes(i, colcap));
+    PassColumns pc(ctx, job);
+    pc.size(colcap);
     if (stage_bytes) ensure(ctx, ctx->stage, stage_bytes);
     ensure(ctx, ctx->pcnt, pcnt_bytes);
     ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
-    PassCols pcols{};
-    pcols.src_ip = (uint32_t *)ctx->d_col[0].p; pcols.dst_ip = (uint32_t *)ctx->d_col[1].p;
-    pcols.src_port = (uint16_t *)ctx->d_col[2].p; pcols.dst_port = (uint16_t *)ctx->d_col[3].p;
-    pcols.proto = (uint8_t *)ctx->d_col[4].p; pcols.flow_start = (uint32_t *)ctx->d_col[5].p;
-    pcols.flow_end = (uint32_t *)ctx->d_col[6].p; pcols.value = (uint64_t *)ctx->d_col[7].p;
-    RowFilter f{};
-    f.start_time = job->spec.start_time;
-    f.end_time = job->spec.end_time;
-    if (ns) {
-        ensure(ctx, ctx->ns_ignore, job->ns_ignore.size() * 4);
-        CU(cudaMemcpyAsync(ctx->ns_ignore.p, job->ns_ignore.data(), job->ns_ignore.size() * 4, cudaMemcpyHostToDevice, st));
-        f.n_ns_ignore = (uint32_t)job->ns_ignore.size();
-        f.ns_ignore = static_cast<const uint32_t *>(ctx->ns_ignore.p);
-    }
     unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);
     unsigned long long *d_cursor = d_cnt + NC * (W + 1);
-    // the rows of pass (v, M) -> the pass columns, counted under (owner, residue); host input through the staging halves,
-    // the split of each chunk behind its copy
+    sw.f = row_filter(ctx, job, sw.ns);
+    sw.cnt = d_cnt;
+    sw.cursor = d_cursor;
+    sw.log_world = logW;
+    // the rows of pass (v, M) -> the pass columns, counted under (owner, residue)
     auto sweep = [&](uint32_t v, uint32_t M) {
         CU(cudaMemsetAsync(d_cnt, 0, NC * 8, st));
         CU(cudaMemsetAsync(d_cursor, 0, 8, st));
-        CU(cudaEventRecord(ctx->ev[0], st));
-        if (!host) {
-            ColPtrs c{};
-            for (int i = 0; i < 10; i++) set_col(c, i, col_ptr(hc, i));
-            CU(launch_pass_split(st, c, R, f, M - 1, v, pcols, (uint32_t)colcap, d_cursor, d_cnt, 0, logW));
-            acc.launches += R ? 1 : 0;
-        } else {
-            CU(cudaEventRecord(ctx->start_ev, st));
-            CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // the pass columns' previous readers are done
-            uint64_t k = 0;
-            for (uint64_t at = 0, n; at < R; at += n, k++) {
-                n = std::min<uint64_t>(chunk, R - at);
-                const int h = (int)(k & 1);
-                if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_ev[h], 0));   // split of chunk k-2 is done
-                ColPtrs c{};
-                char *dst = static_cast<char *>(ctx->stage.p) + h * half_bytes;
-                for (int i = 0; i < 10; i++) {
-                    if (!staged(i)) continue;
-                    const size_t w = col_bytes(i, 1);
-                    CU(cudaMemcpyAsync(dst, static_cast<const char *>(col_ptr(hc, i)) + at * w, n * w, cudaMemcpyHostToDevice,
-                                       ctx->copy_stream));
-                    set_col(c, i, dst);
-                    dst += exact_bytes(col_bytes(i, chunk));
-                }
-                CU(cudaEventRecord(ctx->chunk_ev[h], ctx->copy_stream));
-                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[h], 0));
-                CU(launch_pass_split(st, c, n, f, M - 1, v, pcols, (uint32_t)colcap, d_cursor, d_cnt, 0, logW));
-                acc.launches++;
-                CU(cudaEventRecord(ctx->stage_ev[h], st));
-            }
-        }
-        CU(cudaEventRecord(ctx->ev[1], st));
-        CU(cudaStreamSynchronize(st));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        acc.phase_ms[host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;     // the split runs behind the copies
-        acc.device_ms += ms;
+        sw.begin(host);
+        sw.feed(hc, 0, v, M, pc, false, nullptr);
+        sw.end(false);
     };
 
     // ---- counts ----------------------------------------------------------------------------------------------------------
@@ -2624,78 +2670,44 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     bool loaded = P == P0;           // pass (0, P) is in the pass columns already
 
     // ---- passes ----------------------------------------------------------------------------------------------------------
-    std::deque<std::pair<uint32_t, uint32_t>> todo;
-    for (uint32_t v = 0; v < P; v++) todo.push_back({v, P});
-    std::vector<PassOut> outs;
-    uint32_t passes = 0, planned = P;
-    set_passes(job, 0, planned);
-    try {
-        while (!todo.empty()) {
-            const uint32_t v = todo.front().first, M = todo.front().second;
-            todo.pop_front();
-            const PassDims d = dims(v, M);
-            if (!d.global) {              // the same on every rank: no collective
-                loaded = false;
-                set_passes(job, ++passes, planned);
-                continue;
-            }
-            if (!loaded) sweep(v, M);
+    auto run_one = [&](uint32_t v, uint32_t M, const PassList &, PassOut &o) {
+        const PassDims d = dims(v, M);
+        if (!d.global) {              // the same on every rank: no collective
             loaded = false;
-            // the buffers of earlier passes go where this pass's growth would pass the budget
-            const size_t xgrow = alloc_bytes(xplan) > ctx->xbuf.cap ? alloc_bytes(xplan) - ctx->xbuf.cap : 0;
-            if (workspace_after(ctx, mp_pipe_bufs(ctx, job, d.global, d.rows[me], d.owned[me], slots), false) + xgrow > budget)
-                for (DevBuf *b : workspace_bufs(ctx)) {
-                    if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore || b == &ctx->small ||
-                        (b >= ctx->d_col && b < ctx->d_col + 8))
-                        continue;
-                    free_buf(ctx, *b);
-                }
-            tad_columns pc{};
-            pc.rows = pc.capacity = d.rows[me];
-            pc.mem = TAD_MEM_DEVICE;
-            pc.src_ip = has_col(job, 0) ? pcols.src_ip : nullptr; pc.dst_ip = has_col(job, 1) ? pcols.dst_ip : nullptr;
-            pc.src_port = has_col(job, 2) ? pcols.src_port : nullptr; pc.dst_port = has_col(job, 3) ? pcols.dst_port : nullptr;
-            pc.proto = has_col(job, 4) ? pcols.proto : nullptr; pc.flow_start = has_col(job, 5) ? pcols.flow_start : nullptr;
-            pc.flow_end = pcols.flow_end; pc.value = pcols.value;
-            const tad_progress before = progress_of(job);
-            PassOut o;
-            bool split_here = false;
-            try {
-                const AgreedPass ap{d.global, d.max_rows};
-                run_pipeline(ctx, job, pc, false, !slots, o, &ap);
-            } catch (const PassSplit &) {
-                CU(cudaStreamSynchronize(st));
-                split_here = true;
-            }
-            // ---- the agreed end of the pass: {split, cancelled} of every rank ----
-            ctx->h_small[0] = (split_here ? 1u : 0u) | (job->cancel.load() ? 2u : 0u);
-            gather(1);
-            int split_r = -1, cancel_r = -1;
-            for (int r = W - 1; r >= 0; r--) {
-                if (ctx->h_small[1 + r] & 1) split_r = r;
-                if (ctx->h_small[1 + r] & 2) cancel_r = r;
-            }
-            if (cancel_r >= 0 || split_r >= 0) {
-                give_pinned(ctx, o.block);
-                if (cancel_r >= 0) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", cancel_r);
-                if (M >= (uint32_t)kMaxPasses)
-                    fail(TAD_ERR_NOMEM, "rank %d: the oversized-bucket scratch or result buffer of a 1/%d hash range of the "
-                         "table (%llu rows owned) does not fit its memory budget of %llu bytes", split_r, kMaxPasses,
-                         (unsigned long long)d.owned[split_r], (unsigned long long)rk[split_r].budget);
-                todo.push_front({v + M, 2 * M});
-                todo.push_front({v, 2 * M});
-                set_passes(job, passes, ++planned, &before);
-                continue;
-            }
-            add_pass(acc, o);
-            outs.push_back(o);
-            set_passes(job, ++passes, planned);
+            return false;
         }
-        join_passes(ctx, outs, acc);
-    } catch (...) {
-        for (PassOut &o : outs) give_pinned(ctx, o.block);
-        throw;
-    }
+        if (!loaded) sweep(v, M);
+        loaded = false;
+        // the buffers of earlier passes go where this pass's growth would pass the budget
+        const size_t xgrow = alloc_bytes(xplan) > ctx->xbuf.cap ? alloc_bytes(xplan) - ctx->xbuf.cap : 0;
+        if (workspace_after(ctx, mp_pipe_bufs(ctx, job, d.global, d.rows[me], d.owned[me], slots), false) + xgrow > budget)
+            free_pass_buffers(ctx);
+        bool split_here = false;
+        try {
+            const AgreedPass ap{d.global, d.max_rows};
+            run_pipeline(ctx, job, pc.as_input(d.rows[me]), false, !slots, o, &ap);
+        } catch (const PassSplit &) {
+            CU(cudaStreamSynchronize(st));
+            split_here = true;
+        }
+        // ---- the agreed end of the pass: {split, cancelled} of every rank ----
+        ctx->h_small[0] = (split_here ? 1u : 0u) | (job->cancel.load() ? 2u : 0u);
+        gather(1);
+        int split_r = -1, cancel_r = -1;
+        for (int r = W - 1; r >= 0; r--) {
+            if (ctx->h_small[1 + r] & 1) split_r = r;
+            if (ctx->h_small[1 + r] & 2) cancel_r = r;
+        }
+        if (cancel_r < 0 && split_r < 0) return false;
+        give_pinned(ctx, o.block);
+        if (cancel_r >= 0) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", cancel_r);
+        if (M >= (uint32_t)kMaxPasses)
+            fail(TAD_ERR_NOMEM, "rank %d: the oversized-bucket scratch or result buffer of a 1/%d hash range of the "
+                 "table (%llu rows owned) does not fit its memory budget of %llu bytes", split_r, kMaxPasses,
+                 (unsigned long long)d.owned[split_r], (unsigned long long)rk[split_r].budget);
+        return true;
+    };
+    const uint32_t passes = run_pass_queue(ctx, job, P, acc, run_one);
     acc.phase_ms[TAD_PHASE_SYNC] += gather_ms;
     acc.device_ms += gather_ms;
     return passes;
@@ -2733,14 +2745,8 @@ void run_job(tad_ctx *ctx, tad_job *job)
     } else if (ctx->cfg.world_size == 1 && R > 0) {
         const uint64_t set = ctx->budget.load();
         budget = context_budget();
-        PipeShape s;
-        s.rows = R;
+        PipeShape s = one_gpu_shape(ctx, job, R, true);
         s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
-        s.algo = job->spec.algo;
-        s.B = s.Bl = 1u << pick_logb(ctx, R);
-        s.optimistic = ctx->optimistic && (uint64_t)s.B * kGroupCap * sizeof(Row32) <= kSlotBudget;
-        s.owned = s.series = R;
-        s.out_cap = out_cap_guess(R, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
         if (workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), true) > budget) {
             s.optimistic = false;
             force_exact = true;
@@ -2816,14 +2822,7 @@ void worker_main(tad_ctx *ctx)
             cudaStreamSynchronize(ctx->stream);
             cudaStreamSynchronize(ctx->d2h_stream);
             cudaGetLastError();
-            for (auto &t : ctx->tdict) {       // a dictionary lives for one job
-                for (DevBuf *b : t.bufs()) {
-                    if (b->p) cudaFree(b->p);
-                    ctx->held -= b->cap;
-                    *b = DevBuf{};
-                }
-                t.cap = 0;
-            }
+            TextKeys::release(ctx);
             std::lock_guard<std::mutex> lk(job->mu);
             job->st.state = TAD_STATE_FAILED;
             job->st.error = f.code;
