@@ -203,7 +203,22 @@ struct tad_ctx {
     DevBuf d_col[10], hist, offsets, cursor, big_list, big_base, cls_list, csr_p, stats, part, csr_v, csr_t, nsb, npb, sbase, outb, ns_ignore, spill,
         dbx, dbi, exch, scan_sync, small, hist_all, seg_off, seg_total, entries, ar_y, ar_pred, ar_lam, ovf;
     int optimistic = 1;      // TAD_OPTIMISTIC=0: always the exact (histogram + scan + scatter) partition
-    unsigned long long *h_small = nullptr;   // pinned, 256 x u64
+    unsigned long long *h_small = nullptr;   // pinned, kSmallWords x u64
+    // Word offsets in h_small and in the device scratch `small` (d_small) that mirrors it.  From word 0: gather_small, the
+    // exact partition's rows per segment, the pass counts.  The regions one path uses together do not overlap.
+    static constexpr int kSmallWords = 256, kSmallDevWords = 512, kGatherMax = 16;   // kGatherMax: largest gather_small message
+    static constexpr int kWOvf = 32;          // multi-GPU slot path: every rank's overflow rows
+    static constexpr int kWPullSkip = 40;     // exact pull: rows in front of my bucket range in every rank's partition
+    static constexpr int kWBarrier = 48, kWBarrierIn = 56;   // peer barrier (d_small only): the word sent, the words received
+    static constexpr int kWSendLo = 64;       // NCCL exchange: send boundaries of every chunk, kMaxRanks + 1 per chunk
+    static constexpr int kWPassCursor = 128;  // hash-range passes: the pass cursor alone, read while the counts are held
+    static constexpr int kWTextState = 192;   // text keys: 8 state words per dictionary
+    static_assert(kGatherMax * (1 + kMaxRanks) <= kSmallWords && kSmallWords <= kSmallDevWords, "small scratch size");
+    static_assert(kMaxSeg <= kWOvf && kWOvf + kMaxRanks <= kWPullSkip && kWPullSkip + kMaxRanks <= kWBarrier &&
+                  kWBarrier < kWBarrierIn && kWBarrierIn + kMaxRanks <= kWSendLo &&
+                  kWSendLo + kMaxXChunks * (kMaxRanks + 1) <= kSmallWords, "partition scratch regions overlap");
+    static_assert(kMaxPasses + 1 <= kWPassCursor && kWPassCursor < kWTextState && kWTextState + 2 * 8 <= kSmallWords,
+                  "pass scratch regions overlap");
     uint32_t scan_epoch = 0;
     uint32_t *h_stats = nullptr;   // pinned readback of the device scalars
     // ARIMA fit launch (wait_arima_fit): pinned [0, 2): the fit counters while the kernel runs, [2, 4): once it has ended,
@@ -723,6 +738,97 @@ size_t workspace_after(tad_ctx *ctx, const std::vector<std::pair<DevBuf *, size_
     return total;
 }
 
+// ---- partition decisions of run_pipeline, which the planners share ----------------------------------------------------
+// On several GPUs they depend only on values every rank shares (the global rows, the job, the world size and the run-time
+// switches every rank must see alike), so every rank computes them for every other rank.
+int log_world(const tad_ctx *ctx)
+{
+    int l = 0;
+    while ((1 << l) < ctx->cfg.world_size) l++;
+    return l;
+}
+
+uint32_t buckets(const tad_ctx *ctx, uint64_t global)      // global buckets; a rank owns B >> log_world of them
+{
+    return 1u << std::max(pick_logb(ctx, global), log_world(ctx));
+}
+
+// Whether one GPU takes the optimistic partition: its slot buffer at most half of an 80 GB H100 (kSlotBudget).
+bool one_gpu_optimistic(const tad_ctx *ctx, uint64_t rows, uint64_t B)
+{
+    return ctx->optimistic && rows > 0 && B * kGroupCap * sizeof(Row32) <= kSlotBudget;
+}
+
+// Multi-GPU slot rows of a bucket: a source holds 1/world of a bucket on average.
+uint32_t slot(const tad_ctx *ctx) { return std::max<uint32_t>(256u, (uint32_t)kGroupCap / (uint32_t)ctx->cfg.world_size); }
+// The exported buffer's arrival counters of B buckets, padded; the rows follow them.
+size_t xbuf_cnt_bytes(uint64_t B) { return (B * 4 + 65535) & ~size_t(65535); }
+size_t slot_xbuf_bytes(const tad_ctx *ctx, uint64_t B) { return xbuf_cnt_bytes(B) + B * slot(ctx) * sizeof(Row32); }
+
+// Whether several GPUs may take the optimistic slot path for `global` rows.
+bool slots_allowed(const tad_ctx *ctx, uint64_t global)
+{
+    const uint64_t B = buckets(ctx, global);
+    return ctx->peer_pull && ctx->optimistic && global > 0 && B * slot(ctx) <= (1ull << 31) &&
+           slot_xbuf_bytes(ctx, B) <= ctx->x_budget;
+}
+
+// Exported-buffer bytes for `global` rows: the exact partition pulled by the peers (every rank's buffer holds the largest
+// shard, `max_rows`) and, with `slots`, the optimistic slots of all B buckets.
+size_t xbuf_bytes(const tad_ctx *ctx, uint64_t global, uint64_t max_rows, bool slots)
+{
+    const uint64_t B = buckets(ctx, global);
+    size_t x = ctx->peer_pull && ctx->exact_pull ? xbuf_cnt_bytes(B) + std::max<uint64_t>(max_rows, 1) * sizeof(Row32) : 0;
+    if (slots && slots_allowed(ctx, global)) x = std::max(x, slot_xbuf_bytes(ctx, B));
+    return x;
+}
+
+// The multi-GPU exact partition's buffers for K row chunks per rank, in the order run_pipeline grows them.
+std::vector<std::pair<DevBuf *, size_t>> exact_bufs(tad_ctx *ctx, size_t B, size_t Bl, size_t K)
+{
+    const size_t NS = (size_t)ctx->cfg.world_size * K;      // segments: (source rank, chunk)
+    return {{&ctx->hist, B * 4 * K}, {&ctx->offsets, (B + 1) * 4 * K}, {&ctx->cursor, B * 4 * K},
+            {&ctx->hist_all, B * 4 * NS}, {&ctx->seg_off, (Bl + 1) * 4 * NS}, {&ctx->seg_total, Bl * 4}};
+}
+
+// ---- collectives through the small scratch (tad_ctx::kSmallWords) ----------------------------------------------------
+// Blocking all-gather of h_small[0, n) of every rank into h_small[n, n + n * world) on ctx->stream.  `timed`: returns the
+// collective's time in ms (the ranks' arrival skew), measured with ctx->ev[0..1]; else 0.
+float gather_small(tad_ctx *ctx, int n, bool timed)
+{
+    cudaStream_t st = ctx->stream;
+    unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
+    CU(cudaMemcpyAsync(d_small, ctx->h_small, n * 8, cudaMemcpyHostToDevice, st));
+    if (timed) CU(cudaEventRecord(ctx->ev[0], st));
+    if (nccl_allgather(&ctx->nccl, d_small, d_small + n, n * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+    if (timed) CU(cudaEventRecord(ctx->ev[1], st));
+    CU(cudaMemcpyAsync(ctx->h_small + n, d_small + n, (size_t)n * 8 * ctx->cfg.world_size, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    float ms = 0;
+    if (timed) CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+    return ms;
+}
+
+// Barrier of the ranks on ctx->stream (an 8-byte all-gather); nccl_allgather's return code.
+int peer_barrier(tad_ctx *ctx)
+{
+    unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
+    return nccl_allgather(&ctx->nccl, d_small + tad_ctx::kWBarrier, d_small + tad_ctx::kWBarrierIn, 8, ctx->stream);
+}
+
+// Unmaps every peer's exported buffer; the first error.
+cudaError_t unmap_peers(tad_ctx *ctx)
+{
+    cudaError_t err = cudaSuccess;
+    for (void *&p : ctx->peer_x) {
+        const cudaError_t e = p ? cudaIpcCloseMemHandle(p) : cudaSuccess;
+        if (err == cudaSuccess) err = e;
+        p = nullptr;
+    }
+    ctx->peers_mapped = false;
+    return err;
+}
+
 // Result of one pipeline run: a one-pass job or one hash-range pass.
 struct PassOut {
     uint64_t kept = 0, owned = 0, points = 0, series = 0, out_rows = 0, spill_rows = 0, launches = 0;
@@ -767,6 +873,10 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
     uint32_t *d_stats = static_cast<uint32_t *>(ctx->stats.p);
     CU(cudaMemsetAsync(d_stats, 0, 64 * sizeof(uint32_t), st));
+    auto read_stats = [&]() {             // the device scalars -> h_stats, with everything enqueued before
+        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+    };
     if (!ctx->scan_sync.p) {
         ensure(ctx, ctx->scan_sync, scan_sync_bytes());
         CU(cudaMemsetAsync(ctx->scan_sync.p, 0, scan_sync_bytes(), st));
@@ -776,7 +886,6 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     // Host input is copied in chunks on a second stream; the bucket histogram is additive, so the
     // histogram of chunk i runs while chunk i+1 is still on the PCIe bus.
     ColPtrs c{};
-    const void *dcol[10];
     const bool host_input = hc.mem != TAD_MEM_DEVICE && R > 0;
     PipeShape shape;
     shape.rows = R;
@@ -785,14 +894,9 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     PipeSizes z = pipe_sizes(shape);
     for (int i = 0; i < 10; i++) {
         void *src = col_ptr(hc, i);
-        dcol[i] = nullptr;
         if (!src || R == 0) continue;
-        if (hc.mem == TAD_MEM_DEVICE) {
-            dcol[i] = src;
-        } else {
-            ensure(ctx, ctx->d_col[i], z.col[i]);
-            dcol[i] = ctx->d_col[i].p;
-        }
+        if (hc.mem != TAD_MEM_DEVICE) ensure(ctx, ctx->d_col[i], z.col[i]);
+        set_col(c, i, hc.mem == TAD_MEM_DEVICE ? src : ctx->d_col[i].p);
     }
     int nchunks = 1;
     if (host_input) {
@@ -800,18 +904,15 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         if (nchunks > kMaxChunks) nchunks = kMaxChunks;
         if (nchunks < 1) nchunks = 1;
     }
-    auto chunk_lo = [&](int k) { return ((R * (uint64_t)k / nchunks) + 15) & ~uint64_t(15); };   // keeps every column 16-byte aligned
-    auto chunk_range = [&](int k, uint64_t &lo, uint64_t &hi) {
-        lo = k == 0 ? 0 : (chunk_lo(k) < R ? chunk_lo(k) : R);
-        hi = k + 1 == nchunks ? R : (chunk_lo(k + 1) < R ? chunk_lo(k + 1) : R);
+    auto chunk_lo = [&](int k) -> uint64_t {      // host chunk k is [chunk_lo(k), chunk_lo(k + 1)): 16-byte aligned columns
+        return k == 0 ? 0 : k == nchunks ? R : std::min<uint64_t>(((R * (uint64_t)k / nchunks) + 15) & ~uint64_t(15), R);
     };
     mark(-1);
     if (host_input) {
         CU(cudaEventRecord(ctx->start_ev, st));
         CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));   // workspace of the previous job is free
         for (int k = 0; k < nchunks; k++) {
-            uint64_t lo, hi;
-            chunk_range(k, lo, hi);
+            const uint64_t lo = chunk_lo(k), hi = chunk_lo(k + 1);
             for (int i = 0; i < 10 && hi > lo; i++) {
                 const char *src = static_cast<const char *>(col_ptr(hc, i));
                 if (!src) continue;
@@ -822,18 +923,30 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             CU(cudaEventRecord(ctx->chunk_ev[k], ctx->copy_stream));
         }
     }
-    c.src_ip = (const uint32_t *)dcol[0]; c.dst_ip = (const uint32_t *)dcol[1];
-    c.src_port = (const uint16_t *)dcol[2]; c.dst_port = (const uint16_t *)dcol[3];
-    c.proto = (const uint8_t *)dcol[4]; c.flow_start = (const uint32_t *)dcol[5];
-    c.flow_end = (const uint32_t *)dcol[6]; c.value = (const uint64_t *)dcol[7];
-    c.src_ns = (const uint32_t *)dcol[8]; c.dst_ns = (const uint32_t *)dcol[9];
 
     const RowFilter f = filters ? row_filter(ctx, job, c.src_ns || c.dst_ns) : RowFilter{};
+    // launch(cols, rows) over the input: host input once per non-empty chunk, each behind its copy (the copies and the
+    // overlapped launches are the H2D phase); device input in one launch that closes `phase`
+    auto feed_chunks = [&](auto launch, int phase) {
+        mark(-1);
+        if (host_input) {
+            for (int k = 0; k < nchunks; k++) {
+                const uint64_t lo = chunk_lo(k), hi = chunk_lo(k + 1);
+                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
+                if (hi <= lo) continue;
+                CU(launch(offset_cols(c, lo), hi - lo)); launches++;
+            }
+            mark(TAD_PHASE_H2D);
+        } else {
+            CU(launch(c, R)); launches += R ? 1 : 0;
+            mark(phase);
+        }
+    };
 
     // ---- partition -------------------------------------------------------------------------
     const int world = ctx->cfg.world_size, me = ctx->cfg.rank;
     uint64_t R_total = R;
-    ensure(ctx, ctx->small, 4096);
+    ensure(ctx, ctx->small, tad_ctx::kSmallDevWords * 8);
     unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
     if (world > 1 && pass) {
         R_total = pass->global_rows;   // the pass's total from the all-gathered counts
@@ -842,27 +955,19 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     } else if (world > 1) {
         // global row count -> same bucket count on every rank
         ctx->h_small[0] = R;
-        CU(cudaMemcpyAsync(d_small, ctx->h_small, 8, cudaMemcpyHostToDevice, st));
-        if (nccl_allgather(&ctx->nccl, d_small, d_small + 8, 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-        CU(cudaMemcpyAsync(ctx->h_small, d_small + 8, 8 * world, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        gather_small(ctx, 1, false);
         mark(TAD_PHASE_SYNC);          // arrival skew of the ranks at job start (avoided when the host passes global_rows)
         R_total = 0;
-        for (int r = 0; r < world; r++) R_total += ctx->h_small[r];
+        for (int r = 0; r < world; r++) R_total += ctx->h_small[1 + r];
     }
-    int logB = pick_logb(ctx, R_total);
-    int logW = 0;
-    while ((1 << logW) < world) logW++;
-    if (logB < logW) logB = logW;
-    const uint32_t B = 1u << logB;                 // global buckets
-    const uint32_t Bl = B >> logW;                 // buckets owned by one rank
+    const uint32_t B = buckets(ctx, R_total);      // global buckets
+    const int logB = __builtin_ctz(B);
+    const uint32_t Bl = B >> log_world(ctx);       // buckets owned by one rank
     const uint32_t b_lo = Bl * (uint32_t)me;
-    // slot buffer at most half of an 80 GB H100: the inputs, series entries and per-series arrays need the rest
     constexpr uint32_t kSlot = kGroupCap;      // = the largest shared-memory class: overflow is as rare as a spill was
-    const uint64_t slot_rows = (uint64_t)B * kSlot;
     shape.B = B;
     shape.Bl = Bl;
-    shape.optimistic = world == 1 && ctx->optimistic && R > 0 && slot_rows * sizeof(Row32) <= kSlotBudget && !force_exact;
+    shape.optimistic = world == 1 && one_gpu_optimistic(ctx, R, B) && !force_exact;
     z = pipe_sizes(shape);
     ensure(ctx, ctx->hist, z.hist);
     ensure(ctx, ctx->offsets, z.offsets);
@@ -900,27 +1005,14 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         part = (Row32 *)ctx->part.p;
         Row32 *ovf = (Row32 *)ctx->ovf.p;
         CU(cudaMemsetAsync(cursor, 0, (size_t)B * 4, st));
-        mark(-1);
-        if (host_input) {
-            for (int k = 0; k < nchunks; k++) {
-                uint64_t lo, hi;
-                chunk_range(k, lo, hi);
-                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
-                if (hi <= lo) continue;
-                CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, cursor, part, kSlot, ovf, (uint32_t)ovf_cap,
-                                  d_stats + ST_OVF)); launches++;
-            }
-            mark(TAD_PHASE_H2D);          // copy + overlapped scatter of all chunks
-        } else {
-            CU(launch_scatter(st, c, R, f, logB, cursor, part, kSlot, ovf, (uint32_t)ovf_cap, d_stats + ST_OVF)); launches++;
-            mark(TAD_PHASE_SCATTER);
-        }
+        feed_chunks([&](const ColPtrs &cc, uint64_t n) {
+            return launch_scatter(st, cc, n, f, logB, cursor, part, kSlot, ovf, (uint32_t)ovf_cap, d_stats + ST_OVF);
+        }, TAD_PHASE_SCATTER);
         // arrival counts -> (virtual) bucket offsets, capacity-class lists, list of over-full buckets
         CU(launch_bucket_scan(st, cursor, offsets, hist /* unused cursor copy */, B, kSlot, big_list, big_base, cls_list,
                               d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
         mark(TAD_PHASE_SCAN);
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        read_stats();
         if (ctx->h_stats[ST_OVF] <= ovf_cap) {
             partitioned = true;
             n_ovf = ctx->h_stats[ST_OVF];
@@ -939,12 +1031,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     }
 
     // ---- exported buffer + peer mappings (multi-GPU peer pull) -----------------------------------------------------------
-    auto gather16 = [&]() {        // blocking 128-byte all-gather through pinned memory (rare: regrow, exact-path row counts)
-        CU(cudaMemcpyAsync(d_small, ctx->h_small, 16 * 8, cudaMemcpyHostToDevice, st));
-        if (nccl_allgather(&ctx->nccl, d_small, d_small + 16, 16 * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-        CU(cudaMemcpyAsync(ctx->h_small + 16, d_small + 16, 16 * 8 * world, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-    };
+    // blocking 128-byte all-gathers (rare: regrow, exact-path row counts): rank r's words land at h_small + G * (1 + r)
+    constexpr int G = tad_ctx::kGatherMax;
     // Every rank calls this with the SAME `need` in the same job (it depends only on values all ranks share), so all ranks
     // regrow together: unmap, barrier (nobody maps a buffer that is about to be freed), reallocate, exchange the IPC
     // handles, map.  First job or a larger table only.
@@ -953,23 +1041,21 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         // capacity (which may differ when one rank's allocation fell back to the exact size under memory pressure)
         if (need <= ctx->x_agreed && ctx->peers_mapped) return;
         static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-        for (int r = 0; r < world; r++)
-            if (ctx->peer_x[r]) { CU(cudaIpcCloseMemHandle(ctx->peer_x[r])); ctx->peer_x[r] = nullptr; }
-        ctx->peers_mapped = false;
-        memset(ctx->h_small, 0, 16 * 8);
-        gather16();
+        CU(unmap_peers(ctx));
+        memset(ctx->h_small, 0, G * 8);
+        gather_small(ctx, G, false);
         ensure(ctx, ctx->xbuf, need);
         cudaIpcMemHandle_t mine;
         CU(cudaIpcGetMemHandle(&mine, ctx->xbuf.p));
-        memset(ctx->h_small, 0, 16 * 8);
+        memset(ctx->h_small, 0, G * 8);
         ctx->h_small[0] = ctx->xbuf.cap;
         memcpy(ctx->h_small + 2, &mine, sizeof(mine));
-        gather16();
+        gather_small(ctx, G, false);
         for (int r = 0; r < world; r++) {
             if (r == me) continue;
             cudaIpcMemHandle_t h;
-            memcpy(&h, ctx->h_small + 16 + 16 * r + 2, sizeof(h));
-            if (ctx->h_small[16 + 16 * r] < need) fail(TAD_ERR_INTERNAL, "rank %d exports a smaller partition buffer", r);
+            memcpy(&h, ctx->h_small + G * (1 + r) + 2, sizeof(h));
+            if (ctx->h_small[G * (1 + r)] < need) fail(TAD_ERR_INTERNAL, "rank %d exports a smaller partition buffer", r);
             cudaError_t e = cudaIpcOpenMemHandle(&ctx->peer_x[r], h, cudaIpcMemLazyEnablePeerAccess);
             if (e != cudaSuccess) {
                 cudaGetLastError();
@@ -988,35 +1074,32 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     // any slot overflowed anywhere, all ranks take the exact path below (same decision everywhere: it is made on the
     // gathered data).  Otherwise each rank reads the arrival counters of its bucket range out of the peers' buffers and
     // its group kernel pulls the rows themselves, segment by segment, with the bulk copies it issues anyway.
-    const uint32_t slotM = std::max<uint32_t>(256u, (uint32_t)kGroupCap / (uint32_t)world);
-    const size_t x_cnt_bytes = (((size_t)B * 4) + 65535) & ~size_t(65535);
-    const size_t x_need = x_cnt_bytes + (size_t)B * slotM * sizeof(Row32);
+    const uint32_t slotM = slot(ctx);
+    const size_t x_cnt_bytes = xbuf_cnt_bytes(B);
+    // the peers' exported partitions as segments: rank r's rows from skip[r] (null: 0), its offsets at off + r * off_stride
+    auto peer_segments = [&](const uint32_t *off, size_t off_stride, const unsigned long long *skip) {
+        seg.nseg = world;
+        for (int r = 0; r < world; r++) {
+            const char *xb = r == me ? static_cast<const char *>(ctx->xbuf.p) : static_cast<const char *>(ctx->peer_x[r]);
+            seg.base[r] = reinterpret_cast<const Row32 *>(xb + x_cnt_bytes) + (skip ? skip[r] : 0);
+            seg.off[r] = off + r * off_stride;
+        }
+    };
     bool sync_at_end = false;
-    if (world > 1 && ctx->peer_pull && ctx->optimistic && R_total > 0 && (uint64_t)B * slotM <= (1ull << 31) &&
-        x_need <= ctx->x_budget && !force_exact) {
-        ensure_exported(x_need);
+    if (world > 1 && slots_allowed(ctx, R_total) && !force_exact) {
+        ensure_exported(slot_xbuf_bytes(ctx, B));
         uint32_t *xcursor = static_cast<uint32_t *>(ctx->xbuf.p);
         Row32 *xpart = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->xbuf.p) + x_cnt_bytes);
         ensure(ctx, ctx->xcnt, (size_t)Bl * 4 * world);
         ensure(ctx, ctx->xtotal, (size_t)Bl * 4);
         uint32_t *xcnt = (uint32_t *)ctx->xcnt.p, *xtotal = (uint32_t *)ctx->xtotal.p;
         CU(cudaMemsetAsync(xcursor, 0, (size_t)B * 4, st));
-        mark(-1);
-        if (host_input) {
-            for (int k = 0; k < nchunks; k++) {
-                uint64_t lo, hi;
-                chunk_range(k, lo, hi);
-                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
-                if (hi <= lo) continue;
-                CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, xcursor, xpart, slotM, nullptr, 0, d_stats + ST_OVF)); launches++;
-            }
-            mark(TAD_PHASE_H2D);          // copy + overlapped scatter of all chunks
-        } else {
-            CU(launch_scatter(st, c, R, f, logB, xcursor, xpart, slotM, nullptr, 0, d_stats + ST_OVF)); launches += R ? 1 : 0;
-            mark(TAD_PHASE_SCATTER);
-        }
+        feed_chunks([&](const ColPtrs &cc, uint64_t n) {
+            return launch_scatter(st, cc, n, f, logB, xcursor, xpart, slotM, nullptr, 0, d_stats + ST_OVF);
+        }, TAD_PHASE_SCATTER);
         // barrier + overflow agreement: {overflow rows, -} of every rank
-        if (nccl_allgather(&ctx->nccl, d_stats + ST_OVF, d_small + 32, 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+        if (nccl_allgather(&ctx->nccl, d_stats + ST_OVF, d_small + tad_ctx::kWOvf, 8, st))
+            fail(TAD_ERR_NCCL, "%s", nccl_last_error());
         mark(TAD_PHASE_SYNC);
         PeerCounters pc{};
         for (int r = 0; r < world; r++) pc.p[r] = r == me ? xcursor : static_cast<const uint32_t *>(ctx->peer_x[r]);
@@ -1025,25 +1108,19 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         CU(launch_bucket_scan(st, xtotal, offsets, cursor, Bl, kGroupCap, big_list, big_base, cls_list, d_stats,
                               ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
         mark(TAD_PHASE_SCAN);
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(ctx->h_small + 32, d_small + 32, 8 * world, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWOvf, d_small + tad_ctx::kWOvf, 8 * world, cudaMemcpyDeviceToHost, st));
+        read_stats();
         check_cancel();
         uint64_t any_ovf = 0;
-        for (int r = 0; r < world; r++) any_ovf += (uint32_t)ctx->h_small[32 + r];
+        for (int r = 0; r < world; r++) any_ovf += (uint32_t)ctx->h_small[tad_ctx::kWOvf + r];
         sync_at_end = true;       // peers may still read this rank's slots: no rank starts its next job before all are done
         if (any_ovf == 0) {
             partitioned = true;
             kept = ctx->h_stats[ST_LOCALKEPT];
             owned = ctx->h_stats[ST_KEPT];
-            seg.nseg = world;
             seg.stride = slotM;
             seg.b_lo = b_lo;
-            for (int r = 0; r < world; r++) {
-                const char *xb = r == me ? static_cast<const char *>(ctx->xbuf.p) : static_cast<const char *>(ctx->peer_x[r]);
-                seg.base[r] = reinterpret_cast<const Row32 *>(xb + x_cnt_bytes);
-                seg.off[r] = xcnt + (size_t)r * Bl;
-            }
+            peer_segments(xcnt, Bl, nullptr);
             ensure(ctx, ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
             entries = static_cast<SeriesEntry *>(ctx->entries.p);
         } else {
@@ -1052,28 +1129,14 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     }
     if (world == 1 && !partitioned) {
         CU(cudaMemsetAsync(hist, 0, (size_t)B * 4, st));
-        mark(-1);
-        if (host_input) {
-            for (int k = 0; k < nchunks; k++) {
-                uint64_t lo, hi;
-                chunk_range(k, lo, hi);
-                CU(cudaStreamWaitEvent(st, ctx->chunk_ev[k], 0));
-                if (hi <= lo) continue;
-                CU(launch_hist(st, offset_cols(c, lo), hi - lo, f, logB, hist)); launches++;
-            }
-            mark(TAD_PHASE_H2D);          // copy + overlapped histogram of all chunks
-        } else {
-            CU(launch_hist(st, c, R, f, logB, hist)); launches += R ? 1 : 0;
-            mark(TAD_PHASE_HIST);
-        }
+        feed_chunks([&](const ColPtrs &cc, uint64_t n) { return launch_hist(st, cc, n, f, logB, hist); }, TAD_PHASE_HIST);
         // single GPU: these are the final bucket offsets; multi GPU: offsets inside the local send buffer
         CU(launch_bucket_scan(st, hist, offsets, cursor, B, world > 1 ? 0xffffffffu : (uint32_t)kGroupCap, big_list, big_base,
                               world > 1 ? nullptr : cls_list, d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
         mark(TAD_PHASE_SCAN);
         CU(launch_scatter(st, c, R, f, logB, cursor, part)); launches += R ? 1 : 0;
         mark(TAD_PHASE_SCATTER);
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        read_stats();
         kept = owned = ctx->h_stats[ST_KEPT];
         seg.nseg = 1;
         seg.base[0] = part;
@@ -1098,23 +1161,18 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         if (pull) {
             // the exported buffer must hold the largest shard: the ranks agree on it (blocking 128-byte all-gather; this path
             // is the fallback for skewed or very large tables, where a host sync more does not matter)
-            memset(ctx->h_small, 0, 16 * 8);
+            memset(ctx->h_small, 0, G * 8);
             ctx->h_small[0] = R;
-            gather16();
-            uint64_t max_rows = 1;
-            for (int r = 0; r < world; r++) max_rows = std::max<uint64_t>(max_rows, ctx->h_small[16 + 16 * r]);
-            ensure_exported(x_cnt_bytes + max_rows * sizeof(Row32));
+            gather_small(ctx, G, false);
+            uint64_t max_rows = 0;
+            for (int r = 0; r < world; r++) max_rows = std::max<uint64_t>(max_rows, ctx->h_small[G * (1 + r)]);
+            ensure_exported(xbuf_bytes(ctx, R_total, max_rows, false));
             part = reinterpret_cast<Row32 *>(static_cast<char *>(ctx->xbuf.p) + x_cnt_bytes);
         } else {
             ensure(ctx, ctx->part, (R ? R : 1) * sizeof(Row32));
             part = (Row32 *)ctx->part.p;
         }
-        ensure(ctx, ctx->hist, (size_t)B * 4 * K);
-        ensure(ctx, ctx->offsets, ((size_t)B + 1) * 4 * K);
-        ensure(ctx, ctx->cursor, (size_t)B * 4 * K);
-        ensure(ctx, ctx->hist_all, (size_t)B * 4 * NS);
-        ensure(ctx, ctx->seg_off, ((size_t)Bl + 1) * 4 * NS);
-        ensure(ctx, ctx->seg_total, (size_t)Bl * 4);
+        for (const auto &b : exact_bufs(ctx, B, Bl, K)) ensure(ctx, *b.first, b.second);
         hist = (uint32_t *)ctx->hist.p; offsets = (uint32_t *)ctx->offsets.p; cursor = (uint32_t *)ctx->cursor.p;
         uint32_t *hist_all = (uint32_t *)ctx->hist_all.p, *seg_off = (uint32_t *)ctx->seg_off.p;
         uint32_t *seg_total = (uint32_t *)ctx->seg_total.p;
@@ -1134,12 +1192,14 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         mark(TAD_PHASE_SCAN);
         // every rank learns every (rank, chunk) histogram: segment offsets of the owned bucket range, receive sizes
         if (nccl_allgather(&ctx->nccl, hist, hist_all, (size_t)B * 4 * K, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-        CU(launch_segment_scan(st, hist_all, B, b_lo, Bl, NS, seg_off, seg_total, d_small, pull ? d_small + 40 : nullptr)); launches += 2;
+        unsigned long long *pull_skip = ctx->h_small + tad_ctx::kWPullSkip;
+        CU(launch_segment_scan(st, hist_all, B, b_lo, Bl, NS, seg_off, seg_total, d_small,
+                               pull ? d_small + tad_ctx::kWPullSkip : nullptr)); launches += 2;
         CU(cudaMemcpyAsync(ctx->h_small, d_small, 8 * NS, cudaMemcpyDeviceToHost, st));
-        if (pull) CU(cudaMemcpyAsync(ctx->h_small + 40, d_small + 40, 8 * NS, cudaMemcpyDeviceToHost, st));
+        if (pull) CU(cudaMemcpyAsync(pull_skip, d_small + tad_ctx::kWPullSkip, 8 * NS, cudaMemcpyDeviceToHost, st));
         for (int cx = 0; cx < K; cx++)        // send boundaries of chunk cx: offsets_cx[p * Bl], p = 0..world
-            CU(cudaMemcpy2DAsync(ctx->h_small + 64 + cx * (kMaxRanks + 1), 8, offsets + (size_t)cx * (B + 1), (size_t)Bl * 4, 4,
-                                 world + 1, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpy2DAsync(ctx->h_small + tad_ctx::kWSendLo + cx * (kMaxRanks + 1), 8, offsets + (size_t)cx * (B + 1),
+                                 (size_t)Bl * 4, 4, world + 1, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         check_cancel();
         uint64_t recv_off[kMaxSeg], recv_total = 0, send_lo[kMaxXChunks][kMaxRanks + 1];
@@ -1149,7 +1209,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             owned += ctx->h_small[sgi];
         }
         for (int cx = 0; cx < K; cx++) {
-            for (int p = 0; p <= world; p++) send_lo[cx][p] = (uint32_t)ctx->h_small[64 + cx * (kMaxRanks + 1) + p];
+            for (int p = 0; p <= world; p++)
+                send_lo[cx][p] = (uint32_t)ctx->h_small[tad_ctx::kWSendLo + cx * (kMaxRanks + 1) + p];
             kept += send_lo[cx][world];
         }
         if (owned >= (1ull << 32) - 1) fail(TAD_ERR_INVALID_ARG, "more than 2^32-2 rows owned by one GPU after the exchange");
@@ -1158,48 +1219,42 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             CU(launch_scatter(st, c, R, f, logB, cursor, part)); launches += R ? 1 : 0;
             mark(TAD_PHASE_SCATTER);
             // barrier: every rank's exact partition is complete
-            if (nccl_allgather(&ctx->nccl, d_small + 48, d_small + 56, 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+            if (peer_barrier(ctx)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
             mark(TAD_PHASE_SYNC);
-            seg.nseg = world;
-            for (int r = 0; r < world; r++) {
-                const char *xb = r == me ? static_cast<const char *>(ctx->xbuf.p) : static_cast<const char *>(ctx->peer_x[r]);
-                seg.base[r] = reinterpret_cast<const Row32 *>(xb + x_cnt_bytes) + ctx->h_small[40 + r];   // rows in front of my range
-                seg.off[r] = seg_off + (size_t)r * (Bl + 1);
-            }
+            peer_segments(seg_off, Bl + 1, pull_skip);      // rows in front of my range skipped
             sync_at_end = true;
         } else {
-        ensure(ctx, ctx->exch, recv_total ? recv_total : 32);
-        for (int cx = 0; cx < K; cx++) {
-            const uint64_t lo = xlo(cx), hi = xlo(cx + 1);
-            if (hi > lo) { CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, cursor + (size_t)cx * B, part + lo)); launches++; }
-            CU(cudaEventRecord(ctx->x_ev[cx], st));
-            CU(cudaStreamWaitEvent(cs, ctx->x_ev[cx], 0));
-            uint64_t so[kMaxRanks], sb[kMaxRanks], ro[kMaxRanks], rb[kMaxRanks];
-            for (int p = 0; p < world; p++) {
-                so[p] = (lo + send_lo[cx][p]) * 32;
-                sb[p] = (send_lo[cx][p + 1] - send_lo[cx][p]) * 32;
-                ro[p] = recv_off[p * K + cx];
-                rb[p] = ctx->h_small[p * K + cx] * 32;
+            ensure(ctx, ctx->exch, recv_total ? recv_total : 32);
+            for (int cx = 0; cx < K; cx++) {
+                const uint64_t lo = xlo(cx), hi = xlo(cx + 1);
+                if (hi > lo) { CU(launch_scatter(st, offset_cols(c, lo), hi - lo, f, logB, cursor + (size_t)cx * B, part + lo)); launches++; }
+                CU(cudaEventRecord(ctx->x_ev[cx], st));
+                CU(cudaStreamWaitEvent(cs, ctx->x_ev[cx], 0));
+                uint64_t so[kMaxRanks], sb[kMaxRanks], ro[kMaxRanks], rb[kMaxRanks];
+                for (int p = 0; p < world; p++) {
+                    so[p] = (lo + send_lo[cx][p]) * 32;
+                    sb[p] = (send_lo[cx][p + 1] - send_lo[cx][p]) * 32;
+                    ro[p] = recv_off[p * K + cx];
+                    rb[p] = ctx->h_small[p * K + cx] * 32;
+                }
+                if (nccl_alltoallv(&ctx->nccl, part, so, sb, ctx->exch.p, ro, rb, cs)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
             }
-            if (nccl_alltoallv(&ctx->nccl, part, so, sb, ctx->exch.p, ro, rb, cs)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-        }
-        mark(TAD_PHASE_SCATTER);
-        CU(cudaEventRecord(ctx->x_ev[K], cs));
-        CU(cudaStreamWaitEvent(st, ctx->x_ev[K], 0));
-        seg.nseg = NS;
-        for (int sgi = 0; sgi < NS; sgi++) {
-            const int r = sgi / K, cx = sgi % K;
-            seg.base[sgi] = r == me ? part + xlo(cx) + send_lo[cx][me]
-                                    : reinterpret_cast<const Row32 *>((const char *)ctx->exch.p + recv_off[sgi]);
-            seg.off[sgi] = seg_off + (size_t)sgi * (Bl + 1);
-        }
+            mark(TAD_PHASE_SCATTER);
+            CU(cudaEventRecord(ctx->x_ev[K], cs));
+            CU(cudaStreamWaitEvent(st, ctx->x_ev[K], 0));
+            seg.nseg = NS;
+            for (int sgi = 0; sgi < NS; sgi++) {
+                const int r = sgi / K, cx = sgi % K;
+                seg.base[sgi] = r == me ? part + xlo(cx) + send_lo[cx][me]
+                                        : reinterpret_cast<const Row32 *>((const char *)ctx->exch.p + recv_off[sgi]);
+                seg.off[sgi] = seg_off + (size_t)sgi * (Bl + 1);
+            }
         }
         // final (virtual) bucket offsets of the owned range, oversized-bucket list, capacity-class lists
         CU(launch_bucket_scan(st, seg_total, offsets, cursor, Bl, kGroupCap, big_list, big_base, cls_list, d_stats,
                               ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
         mark(TAD_PHASE_EXCHANGE);           // = the part of the exchange NOT hidden behind the scatter
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        read_stats();
         ensure(ctx, ctx->entries, (owned ? owned : 1) * sizeof(SeriesEntry));
         entries = static_cast<SeriesEntry *>(ctx->entries.p);
     }
@@ -1259,8 +1314,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     uint64_t points = 0;
     if (!fused || n_big) {
         CU(launch_series_scan(st, nsb, npb, sbase, Bl, d_stats, ctx->scan_sync.p, ++ctx->scan_epoch)); launches++;
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        read_stats();
         check_cancel();
         S = ctx->h_stats[ST_SERIES];
         points = ctx->h_stats[ST_POINTS];
@@ -1319,8 +1373,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             fail(TAD_ERR_UNSUPPORTED, "algorithm %d is not implemented by this build", sp.algo);
         }
         mark(TAD_PHASE_DETECT);
-        CU(cudaMemcpyAsync(ctx->h_stats, d_stats, ST_COUNT * 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        read_stats();
         out_rows = ctx->h_stats[ST_OUTCOUNT];
         if (out_rows <= out_cap) break;
         out_cap = out_rows;                 // capacity guess too small: rerun detect (idempotent)
@@ -1338,7 +1391,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         // end-of-job barrier of the peer-pull path: my slots and counters may be overwritten (next job) only after every
         // peer's group kernel has read them; its wait is the ranks' arrival skew, accounted as TAD_PHASE_SYNC
         mark(-1);
-        if (nccl_allgather(&ctx->nccl, d_small + 48, d_small + 56, 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+        if (peer_barrier(ctx)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
         mark(TAD_PHASE_SYNC);
     }
 
@@ -1401,8 +1454,8 @@ PipeShape one_gpu_shape(const tad_ctx *ctx, const tad_job *job, uint64_t rows, b
     PipeShape s;
     s.rows = rows;
     s.algo = job->spec.algo;
-    s.B = s.Bl = 1u << pick_logb(ctx, rows);
-    s.optimistic = optimistic && ctx->optimistic && rows > 0 && (uint64_t)s.B * kGroupCap * sizeof(Row32) <= kSlotBudget;
+    s.B = s.Bl = buckets(ctx, rows);
+    s.optimistic = optimistic && one_gpu_optimistic(ctx, rows, s.B);
     s.owned = s.series = rows;
     s.out_cap = out_cap_guess(rows, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
     return s;
@@ -1619,13 +1672,13 @@ struct TextKeys {
     {
         for (int t = 0; t < 2; t++)
             if (ctx->tdict[t].state.p)
-                CU(cudaMemcpyAsync(ctx->h_small + 192 + 8 * t, ctx->tdict[t].state.p, 8 * 8, cudaMemcpyDeviceToHost,
-                                   ctx->copy_stream));
+                CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWTextState + 8 * t, ctx->tdict[t].state.p, 8 * 8,
+                                   cudaMemcpyDeviceToHost, ctx->copy_stream));
         CU(cudaStreamSynchronize(ctx->copy_stream));
         for (int t = 0; t < 2; t++) {
             auto &d = ctx->tdict[t];
             if (!d.state.p) continue;
-            const unsigned long long *w = ctx->h_small + 192 + 8 * t;
+            const unsigned long long *w = ctx->h_small + tad_ctx::kWTextState + 8 * t;
             if (w[2])
                 fail(TAD_ERR_INVALID_ARG, "invalid request: the %s text column of a streamed block does not match its marks "
                      "(a VarUInt length runs past a mark or the column's end)", t ? "dst_ip" : "src_ip");
@@ -2215,9 +2268,9 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     // pass columns hold.
     auto room = [&](uint64_t n) {
         if ((pc.cap >= cap && !host_budget) || ub + n <= pc.cap) { ub += n; return true; }
-        CU(cudaMemcpyAsync(ctx->h_small + 128, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWPassCursor, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        have = std::min<uint64_t>(ctx->h_small[128], pc.cap);
+        have = std::min<uint64_t>(ctx->h_small[tad_ctx::kWPassCursor], pc.cap);
         if (host_budget && have + n > cap) return false;
         if (have + n > pc.cap) {
             const uint64_t want = std::min(cap, std::max(2 * pc.cap, have + n));
@@ -2396,41 +2449,6 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
 }
 
 // ---- several GPUs in hash-range passes (DESIGN.md section 9, "Several GPUs") ---------------------------------------------
-// The sizes below depend only on values every rank shares (the pass's counts, the job, the world size and the run-time
-// switches every rank must see alike), so every rank computes them for every other rank.
-int log_world(const tad_ctx *ctx)
-{
-    int l = 0;
-    while ((1 << l) < ctx->cfg.world_size) l++;
-    return l;
-}
-
-uint32_t mp_buckets(const tad_ctx *ctx, uint64_t global)      // global buckets, as run_pipeline picks them
-{
-    return 1u << std::max(pick_logb(ctx, global), log_world(ctx));
-}
-
-uint32_t mp_slot(const tad_ctx *ctx) { return std::max<uint32_t>(256u, (uint32_t)kGroupCap / (uint32_t)ctx->cfg.world_size); }
-
-// Whether run_pipeline may take the optimistic slot path for a pass of `global` rows.
-bool mp_slots_allowed(const tad_ctx *ctx, uint64_t global)
-{
-    const uint64_t B = mp_buckets(ctx, global);
-    const size_t x = ((B * 4 + 65535) & ~size_t(65535)) + B * mp_slot(ctx) * sizeof(Row32);
-    return ctx->peer_pull && ctx->optimistic && global > 0 && B * mp_slot(ctx) <= (1ull << 31) && x <= ctx->x_budget;
-}
-
-// Exported-buffer bytes of a pass: the exact partition pulled by the peers (every rank's buffer holds the pass's largest
-// shard, `max_rows`) and, with `slots`, the optimistic slots of all B buckets.
-size_t mp_xbuf_bytes(const tad_ctx *ctx, uint64_t global, uint64_t max_rows, bool slots)
-{
-    const uint64_t B = mp_buckets(ctx, global);
-    const size_t cnt = (B * 4 + 65535) & ~size_t(65535);
-    size_t x = ctx->peer_pull && ctx->exact_pull ? cnt + std::max<uint64_t>(max_rows, 1) * sizeof(Row32) : 0;
-    if (slots && mp_slots_allowed(ctx, global)) x = std::max(x, cnt + B * mp_slot(ctx) * sizeof(Row32));
-    return x;
-}
-
 // The pipeline buffers one multi-GPU pass grows (the exported buffer apart), with upper bounds as pass_need: `rows` input
 // rows of this rank, `owned` rows it owns, `global` rows over all ranks; both partitions when `slots` (an overflow falls
 // back to the exact one).
@@ -2441,21 +2459,18 @@ std::vector<std::pair<DevBuf *, size_t>> mp_pipe_bufs(tad_ctx *ctx, const tad_jo
     PipeShape s;
     s.rows = rows;
     s.algo = job->spec.algo;
-    s.B = mp_buckets(ctx, global);
+    s.B = buckets(ctx, global);
     s.Bl = s.B >> log_world(ctx);
     s.owned = s.series = owned;
     s.out_cap = out_cap_guess(owned, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
     PipeSizes z = pipe_sizes(s);
     const bool pull = ctx->peer_pull && ctx->exact_pull;
-    const size_t K = pull ? 1 : ctx->exchange_chunks, B = s.B, Bl = s.Bl;
+    const size_t Bl = s.Bl;
     z.part = pull ? 0 : std::max<uint64_t>(rows, 1) * sizeof(Row32);
     z.entries = std::max<uint64_t>(owned, 1) * sizeof(SeriesEntry);
-    z.hist = z.cursor = B * 4 * K;
-    z.offsets = (B + 1) * 4 * K;
+    z.hist = z.cursor = z.offsets = 0;      // in exact_bufs, with the most chunks the exchange may take
     auto v = pipe_bufs(ctx, z);
-    v.push_back({&ctx->hist_all, B * 4 * W * K});
-    v.push_back({&ctx->seg_off, (Bl + 1) * 4 * W * K});
-    v.push_back({&ctx->seg_total, Bl * 4});
+    for (const auto &b : exact_bufs(ctx, s.B, Bl, pull ? 1 : ctx->exchange_chunks)) v.push_back(b);
     v.push_back({&ctx->exch, pull ? 0 : std::max<uint64_t>(owned, 1) * sizeof(Row32)});
     v.push_back({&ctx->xcnt, slots ? Bl * 4 * W : 0});
     v.push_back({&ctx->xtotal, slots ? Bl * 4 : 0});
@@ -2506,49 +2521,33 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     // are all n fits the budget (exact partition)
     const uint64_t cap = largest_fit(kMaxPassRows, budget, [&](uint64_t n) {
         const uint64_t g = n * (uint64_t)W;
-        return kept_bytes(std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) + alloc_bytes(mp_xbuf_bytes(ctx, g, n, false));
+        return kept_bytes(std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) + alloc_bytes(xbuf_bytes(ctx, g, n, false));
     });
     const uint64_t colcap = std::min(cap, R);
 
     // The budget applies from the plan on: until then the context may still hold the exported buffer of an earlier job,
     // larger than this budget, which only the plan all-gather lets it free.  No rank may fail on its own before it.
     ctx->limit = 0;
-    ensure(ctx, ctx->small, 4096);
-    unsigned long long *d_small = static_cast<unsigned long long *>(ctx->small.p);
-    // all-gather of h_small[0, n) into h_small[n, n + n * W); its time is the ranks' skew (phase sync)
-    double gather_ms = 0;
-    auto gather = [&](int n) {
-        CU(cudaMemcpyAsync(d_small, ctx->h_small, n * 8, cudaMemcpyHostToDevice, st));
-        CU(cudaEventRecord(ctx->ev[0], st));
-        if (nccl_allgather(&ctx->nccl, d_small, d_small + n, n * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-        CU(cudaEventRecord(ctx->ev[1], st));
-        CU(cudaMemcpyAsync(ctx->h_small + n, d_small + n, (size_t)n * 8 * W, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        gather_ms += ms;
-    };
+    ensure(ctx, ctx->small, tad_ctx::kSmallDevWords * 8);
+    double gather_ms = 0;            // the small all-gathers' time: the ranks' skew (phase sync)
     // the exported buffer of an earlier job is freed for the plan: unmap the peers' buffers now, free ours once every rank
     // has (after the plan all-gather).  peers_mapped is the same on every rank.
-    const bool had_x = ctx->peers_mapped;
-    for (int r = 0; r < W && had_x; r++)
-        if (ctx->peer_x[r]) { CU(cudaIpcCloseMemHandle(ctx->peer_x[r])); ctx->peer_x[r] = nullptr; }
-    ctx->peers_mapped = false;
+    if (ctx->peers_mapped) CU(unmap_peers(ctx));
     ctx->x_agreed = 0;
     struct RankPlan {
         uint64_t rows, cap, budget, kept;
         bool cancel;
     } rk[kMaxRanks];
-    memset(ctx->h_small, 0, 16 * 8);
+    memset(ctx->h_small, 0, tad_ctx::kGatherMax * 8);
     ctx->h_small[0] = R;
     ctx->h_small[1] = cap;
     ctx->h_small[2] = budget;
     ctx->h_small[3] = kept_bytes(colcap);
     ctx->h_small[4] = job->cancel.load() ? 1 : 0;
-    gather(16);
+    gather_ms += gather_small(ctx, tad_ctx::kGatherMax, true);
     uint64_t total = 0;
     for (int r = 0; r < W; r++) {
-        const unsigned long long *w = ctx->h_small + 16 + 16 * r;
+        const unsigned long long *w = ctx->h_small + tad_ctx::kGatherMax * (1 + r);
         rk[r] = RankPlan{w[0], w[1], w[2], w[3], w[4] != 0};
         total += w[0];
     }
@@ -2630,7 +2629,7 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
         size_t x = 0;
         for (uint32_t v = 0; v < M; v++) {
             const PassDims d = dims(v, M);
-            if (d.global) x = std::max(x, mp_xbuf_bytes(ctx, d.global, d.max_rows, slots));
+            if (d.global) x = std::max(x, xbuf_bytes(ctx, d.global, d.max_rows, slots));
         }
         return x;
     };
@@ -2692,7 +2691,7 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
         }
         // ---- the agreed end of the pass: {split, cancelled} of every rank ----
         ctx->h_small[0] = (split_here ? 1u : 0u) | (job->cancel.load() ? 2u : 0u);
-        gather(1);
+        gather_ms += gather_small(ctx, 1, true);
         int split_r = -1, cancel_r = -1;
         for (int r = W - 1; r >= 0; r--) {
             if (ctx->h_small[1 + r] & 1) split_r = r;
@@ -2747,14 +2746,16 @@ void run_job(tad_ctx *ctx, tad_job *job)
         budget = context_budget();
         PipeShape s = one_gpu_shape(ctx, job, R, true);
         s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
-        if (workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), true) > budget) {
+        auto bufs = pipe_bufs(ctx, pipe_sizes(s));
+        if (workspace_after(ctx, bufs, true) > budget) {
             s.optimistic = false;
             force_exact = true;
-            split = workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), true) > budget;
+            bufs = pipe_bufs(ctx, pipe_sizes(s));
+            split = workspace_after(ctx, bufs, true) > budget;
         }
         if (set || force_exact) {
             ctx->limit = budget;
-            if (split || workspace_after(ctx, pipe_bufs(ctx, pipe_sizes(s)), false) > budget) free_workspace(ctx);
+            if (split || workspace_after(ctx, bufs, false) > budget) free_workspace(ctx);
         }
     }
     ctx->peak = ctx->held;
@@ -3080,7 +3081,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     if (const char *e = getenv("TAD_EXCHANGE_CHUNKS")) ctx->exchange_chunks = atoi(e) < 1 ? 1 : (atoi(e) > kMaxXChunks ? kMaxXChunks : atoi(e));
     for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void **)&ctx->h_small, 256 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
+    ok = ok && cudaHostAlloc((void **)&ctx->h_small, tad_ctx::kSmallWords * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 5 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     if (ok) ctx->h_fits[4] = 1;
@@ -3115,11 +3116,8 @@ void tad_shutdown(tad_ctx *ctx)
     cudaSetDevice(ctx->cfg.device);
     if (ctx->peers_mapped && ctx->nccl.comm && ctx->small.p && ctx->stream) {
         // an exported buffer must outlive every peer's mapping of it: unmap, meet the peers, only then free
-        for (int r = 0; r < kMaxRanks; r++)
-            if (ctx->peer_x[r]) { cudaIpcCloseMemHandle(ctx->peer_x[r]); ctx->peer_x[r] = nullptr; }
-        unsigned long long *d = static_cast<unsigned long long *>(ctx->small.p);
-        if (nccl_allgather(&ctx->nccl, d + 48, d + 56, 8, ctx->stream) == 0) cudaStreamSynchronize(ctx->stream);
-        ctx->peers_mapped = false;
+        unmap_peers(ctx);
+        if (peer_barrier(ctx) == 0) cudaStreamSynchronize(ctx->stream);
     }
     nccl_comm_destroy(&ctx->nccl);
     if (ctx->xbuf.p) cudaFree(ctx->xbuf.p);
