@@ -97,15 +97,18 @@ __host__ __device__ __forceinline__ uint64_t key_hash(uint64_t a, uint64_t b, ui
 }
 
 // Shared-memory capacity classes of the group kernel, smallest first: a bucket of 0 < n <= kGroupCap rows goes to the
-// first class whose capacity holds it.  Every class runs four rows per thread.  `ctas` is the CTAs per SM the fused
-// (EWMA) instance is built for (its __launch_bounds__); a static_assert on each class's shared-memory footprint keeps it
-// reachable.  The bucket scan, the class lists, the ST_NCLS* counters and the group launchers all derive from this table.
+// first class whose capacity holds it.  Every class runs four rows per thread except the 768-row class, which runs six:
+// seven CTAs of 192 threads would leave the fused instance 40 registers (it spills), seven of 128 leave it 72.  `ctas` is
+// the CTAs per SM the fused (EWMA) instance is built for (its __launch_bounds__); a static_assert on each class's
+// shared-memory footprint keeps it reachable.  The bucket scan, the class lists, the ST_NCLS* counters and the group
+// launchers all derive from this table.
 struct GroupClass { int cap, threads, ctas; };
-constexpr int kGroupClasses = 4;
+constexpr int kGroupClasses = 7;
 __host__ __device__ constexpr GroupClass group_class(int c)
 {
-    return c == 0 ? GroupClass{1024, 256, 5} : c == 1 ? GroupClass{1536, 384, 3} : c == 2 ? GroupClass{2048, 512, 2}
-                                                                                        : GroupClass{4096, 1024, 1};
+    constexpr GroupClass t[kGroupClasses] = {{512, 128, 10}, {768, 128, 7}, {1024, 256, 5}, {1280, 320, 4},
+                                             {1536, 384, 3}, {2048, 512, 2}, {4096, 1024, 1}};
+    return t[c];
 }
 
 // device scalars the host reads back between phases

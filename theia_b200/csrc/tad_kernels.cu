@@ -22,6 +22,7 @@
 #include "tad_kernels.h"
 
 #include <atomic>
+#include <cstddef>
 #include <cstdio>
 #include <mutex>
 #include <type_traits>
@@ -682,11 +683,13 @@ __device__ __forceinline__ double ewma_series(const unsigned long long *__restri
 // ----------------------------------------------------------------------------------------
 template <int CAP, int NT>
 struct GroupSmem {
-    static constexpr int HT = 2 * CAP;        // need not be a power of two: slots are picked by multiply-shift
+    // at most CAP keys in 1.5 CAP slots (a load of 2/3 at worst); HT need not be a power of two: slots are picked by
+    // multiply-shift.  40 bytes of shared memory per row of capacity.
+    static constexpr int HT = 3 * CAP / 2;
     static_assert(CAP % NT == 0 && HT % NT == 0, "every thread stages the same number of rows and hash slots");
     alignas(128) unsigned char x[32 * CAP];   // rows (TMA destination); later ts | tout | vout
     uint32_t ht[HT];                          // claim: low16 = rep row + 1, high16 = count; later (count << 16) | series idx
-    uint16_t soff[HT];                        // first point of the slot's series inside the bucket
+    uint16_t soff[CAP];                       // per series index: its first point inside the bucket
     alignas(8) unsigned long long mbar;
     uint32_t warp_sums[32];
     uint32_t total;
@@ -793,10 +796,11 @@ __device__ __forceinline__ uint32_t count_lt_u64(const unsigned long long *a, ui
     return c;
 }
 
-constexpr int kSlotHashBits = 13;      // hash-tag bits that pick the shared-memory slot (largest table: 2 * kGroupCap)
-static_assert(2 * kGroupCap <= (1 << kSlotHashBits), "every slot of the largest table must be reachable");
+constexpr int kSlotHashBits = 13;      // hash-tag bits that pick the shared-memory slot
+static_assert(GroupSmem<kGroupCap, group_class(kGroupClasses - 1).threads>::HT <= (1 << kSlotHashBits),
+              "every slot of the largest table must be reachable");
 
-// Fused instances: as many CTAs per SM as the shared memory allows (group_class: five of the smallest class, at most 48
+// Fused instances: as many CTAs per SM as the shared memory allows (group_class: ten of the smallest class, at most 48
 // registers), which also keeps the registers of the larger classes within the occupancy their shared memory allows.  The
 // other instances keep their plain bound.
 template <int CAP, int NT, int MODE>
@@ -918,7 +922,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
                 uint4 kk{};
                 uint32_t pp = 0;
                 if constexpr (!FUSED) { kk = x4[2 * rep]; pp = x4[2 * rep + 1].w; }
-                s.soff[base + i] = (uint16_t)so;
+                s.soff[k] = (uint16_t)so;
                 s.ht[base + i] = (cnt << 16) | k;
                 if constexpr (!FUSED) {
                     // series entry, in place over the (already staged) bucket rows
@@ -967,9 +971,8 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
         const uint32_t r = tid + j * NT;
         myB[j] = 0;
         if (r < n) {
-            const uint32_t slot = mySP[j] & 0xffffu;
-            const uint32_t w = s.ht[slot], so = s.soff[slot];
-            const uint32_t cnt = w >> 16, k = w & 0xffffu;
+            const uint32_t w = s.ht[mySP[j] & 0xffffu];
+            const uint32_t cnt = w >> 16, k = w & 0xffffu, so = s.soff[k];
             const uint32_t lo = tmin[k], range = tmax[k] - lo;
             uint32_t bin = 0;
             if (range) {
@@ -1019,9 +1022,10 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
             }
             tout[pos] = t;
             vout[pos] = myV[j];
+            const uint32_t k = s.ht[slot] & 0xffffu;
             if (VRANK) pslot[pos] = (uint16_t)slot;
-            if (FUSED) pser[pos] = (uint16_t)s.ht[slot];
-            mySP[j] = pos | ((pos > s.soff[slot] ? 1u : 0u) << 31);
+            if (FUSED) pser[pos] = (uint16_t)k;
+            mySP[j] = pos | ((pos > s.soff[k] ? 1u : 0u) << 31);
         }
     }
     __syncthreads();
@@ -1043,7 +1047,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
             const uint32_t w = s.ht[sl];
             const uint32_t cnt = w >> 16;
             if (cnt < 2) continue;
-            const uint32_t so = s.soff[sl];
+            const uint32_t so = s.soff[w & 0xffffu];
             uint32_t wr = 0;
             for (uint32_t q = 1; q < cnt; q++) {
                 if (tout[so + q] == tout[so + wr]) {
@@ -1075,6 +1079,8 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
         // memory from here on: ts [0, 4 CAP), binc [20 CAP, 24 CAP), tmin / tmax [24 CAP, 32 CAP), and ht / soff once
         // sinfo is built.
         static_assert(CAP <= (int)kRcpTable, "every count of the Welford chain must have its reciprocal in the table");
+        static_assert(offsetof(S, soff) == offsetof(S, ht) + sizeof(s.ht) && sizeof(s.ht) + sizeof(s.soff) >= 8 * CAP,
+                      "sdv (a double per series) spans ht and soff");
         uint32_t *queue = ts;                                                 // point | series << 16 | flag << 31
         uint32_t *sinfo = binc;                                               // per series: first point | points << 16
         double *ewma = reinterpret_cast<double *>(s.x + 24 * CAP);            // EWMA value at every point
@@ -1082,7 +1088,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
 #pragma unroll
         for (int i = 0; i < SPT; i++) {
             const uint32_t w = s.ht[tid * SPT + i];
-            if (w >> 16) sinfo[w & 0xffffu] = s.soff[tid * SPT + i] | (w & 0xffff0000u);
+            if (w >> 16) sinfo[w & 0xffffu] = s.soff[w & 0xffffu] | (w & 0xffff0000u);
         }
         __syncthreads();
         for (uint32_t k = tid; k < ns; k += NT) {
@@ -1140,7 +1146,7 @@ __global__ void __launch_bounds__(NT, MODE != kGroupEwma ? 0 : group_class(group
         __syncthreads();
         for (uint32_t p = tid; p < n; p += NT) {
             const uint32_t slot = pslot[p];
-            const uint32_t so = s.soff[slot], cnt = s.ht[slot] >> 16, me = p - so;
+            const uint32_t w = s.ht[slot], so = s.soff[w & 0xffffu], cnt = w >> 16, me = p - so;
             if (me >= cnt) continue;                    // hole left by the duplicate reduce
             const unsigned long long v = vout[p];
             uint32_t rank = (v == ~0ull) ? me : count_lt_u64(vout, so, so + me, v + 1ull);
