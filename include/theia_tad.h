@@ -201,8 +201,10 @@ int tad_result(tad_job *job, tad_rows *rows);
  * TAD_ERR_CANCELLED at its next check.  An ARIMA job on one GPU checks inside its fit kernel: every warp stops at its
  * next evaluation round and drops the fits in flight, so the job stops within one likelihood evaluation of the longest
  * prefix being fitted, whatever the series' length (within one phase of the pipeline otherwise, and at the end of the job
- * when world_size > 1, or of the current pass under a memory budget).  tad_release of a job that
- * has not finished cancels it and waits until it has failed; the context then runs the next queued job. */
+ * when world_size > 1, or of the current pass under a memory budget).  An ARIMA job whose fit is parked while other jobs
+ * run (tad_set_fit_sharing) fails once the job running in its place has ended; its parked buffers are then freed.
+ * tad_release of a job that has not finished cancels it and waits until it has failed (for a parked ARIMA job, at most
+ * the run time of the job running in its place); the context then runs the next queued job. */
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
 
@@ -224,7 +226,9 @@ int tad_job_progress(tad_job *job, tad_progress *p);
  * whole pipeline; the result rows are the same rows a one-pass run gives.  Host-resident input is read over PCIe once
  * per pass.  A job fails with TAD_ERR_NOMEM only when a 1/64 hash range of it does not fit.  Caller-owned columns and
  * pinned host memory are not counted.  If the budget drops below what the context holds, the workspace is freed before
- * the next job.  Applies to jobs that start after the call; TAD_ERR_INVALID_ARG below the floor of 64 MiB.
+ * the next job.  Applies to jobs that start after the call; TAD_ERR_INVALID_ARG below the floor of 64 MiB.  With fit
+ * sharing on (tad_set_fit_sharing), an ARIMA tad_submit job plans in this budget less the reserve (TAD_ERR_NOMEM when
+ * that is below 64 MiB), and the jobs run beside its fit plan in the reserve.
  *
  * Several GPUs (world_size > 1): 0 means "no planning", not free memory: a job without a budget runs exactly as it does
  * without this call (no planning collective, launch or sync).  With one, the ranks run the same passes over their shards
@@ -240,6 +244,28 @@ int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
 /* For a COMPLETED job: the passes it ran in (the same count on every rank of a multi-GPU job) and the largest device
  * workspace the context held while it ran (TAD_ERR_STATE otherwise). */
 int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_bytes);
+
+/* Fit sharing (single GPU).  A context runs its jobs one at a time, and an ARIMA job's fit phase can take minutes: without
+ * sharing, every job submitted meanwhile waits for it.  reserve_bytes = 0 (default): off, jobs run strictly in submit order.
+ * Nonzero: an ARIMA tad_submit job plans its passes in the memory budget less `reserve_bytes`, and while its fit runs, an
+ * EWMA or DBSCAN tad_submit job in the queue makes the fit yield within one evaluation round.  The fit's device buffers
+ * are then parked (kept, the rest of its workspace freed), the EWMA and DBSCAN tad_submit jobs queued at that moment run
+ * in submit order with the reserve as their memory budget (in hash-range passes if need be), and the fit resumes where
+ * it stopped.  Its forecasts, rows and fit counts are those of an uninterrupted run.  A queued job whose 1/64 hash range
+ * does not fit the reserve is not failed: that is found out by running it in the reserve (its first sweep reads its
+ * input; it shows RUNNING, then SCHEDULED again with its stages and progress back at 0), and it then waits for its
+ * turn, as without sharing.  A yield drops the fits in flight, which the resume fits again; the fit does not yield again
+ * until all of them have finished and it has run at least as long as the jobs run in its place took, so no fit is
+ * dropped twice and a steady stream of short jobs at most about doubles its fit phase.  The ARIMA job's device_ms and
+ * detect phase leave out the time it was parked (tad_job_yields); its tad_job_memory peak leaves out the workspace of the
+ * jobs run in its place, theirs leaves out its parked buffers and stays within the reserve, so the two stay inside the
+ * budget.  Streamed jobs neither yield nor run in a yield.  Applies to jobs that start after the call.
+ * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit left
+ * early would strand its peers, as for the cancel). */
+int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);
+/* For a COMPLETED ARIMA job: how many times its fit phase yielded and the time it spent parked (ms).  TAD_ERR_STATE for
+ * any other job or state. */
+int tad_job_yields(tad_job *job, uint32_t *yields, double *parked_ms);
 
 /* Pinned host memory this context may hold for its host row store (bytes).  0 (default) = no store.  With a store, a
  * streamed job (tad_submit_stream) that needs more than one hash-range pass keeps its first round's filtered rows in

@@ -22,7 +22,8 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_release", "tad_get_unique_id", "tad_alloc_ns_columns", "tad_ch_string_index", "tad_ch_parse_ipv4",
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
            "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
-           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered", "tad_job_progress")
+           "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered", "tad_job_progress",
+           "tad_set_fit_sharing", "tad_job_yields")
 TAD_NAME_OPS = {"any": 0, "eq": 1, "nonempty": 2, "icontains": 3}
 
 
@@ -110,6 +111,8 @@ def load():
     L.tad_job_progress.argtypes = [C.c_void_p, C.POINTER(TadProgress)]
     L.tad_set_memory_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+    L.tad_set_fit_sharing.argtypes = [C.c_void_p, C.c_uint64]
+    L.tad_job_yields.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
     L.tad_set_host_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_host_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.tad_ch_string_index.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]

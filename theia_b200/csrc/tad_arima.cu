@@ -556,11 +556,18 @@ __host__ __device__ void arima_fit(const ArimaObj &o, double x[3])
 // ------------------------------------------------------------------------------------------
 // kernels
 // ------------------------------------------------------------------------------------------
-// one series: validity, Box-Cox lambda, transformed series into yb[]; returns its prefix fits (n - 3 with a lambda, else 0)
+// pred[t] of a prefix fit not written yet (a fit that can yield): a quiet NaN whose payload no computation makes.  The fit
+// reads finite data only, so every NaN it can produce descends from the device's canonical NaN (0x7fffffffffffffff) or
+// from NAN (0x7ff8000000000000), never from this payload.  A sentinel rather than a bitmap of written prefixes: it needs
+// no buffer beyond pred[] and no atomics, and the resume launch reads the word it would overwrite anyway.
+constexpr unsigned long long kPredUnset = 0x7ff80000000a7f17ull;
+
+// one series: validity, Box-Cox lambda, transformed series into yb[]; returns its prefix fits (n - 3 with a lambda, else 0).
+// unset (a fit that can yield): pred[], whose prefix forecasts [3, n) are marked kPredUnset.
 __device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                         const uint32_t *__restrict__ sbase, uint32_t B, uint32_t i,
                                                         const uint64_t *__restrict__ csr_v, double *__restrict__ yb,
-                                                        double *__restrict__ lam)
+                                                        double *__restrict__ lam, double *__restrict__ unset)
 {
     const SeriesEntry e = load_entry(entries, offsets, sbase, B, i);
     const uint64_t *v = csr_v + e.off;
@@ -584,6 +591,8 @@ __device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__res
         finite = isfinite(y[q]);
     }
     lam[i] = finite ? l : NAN;                             // overflowing transform -> the series yields no rows
+    if (finite && unset)
+        for (uint32_t q = 3; q < n; q++) unset[e.off + q] = __longlong_as_double((long long)kPredUnset);
     return finite ? n - 3 : 0u;
 }
 
@@ -591,10 +600,11 @@ __device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__res
 __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                            const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
                                                            const uint64_t *__restrict__ csr_v, double *__restrict__ yb,
-                                                           double *__restrict__ lam, uint32_t *__restrict__ fits_total)
+                                                           double *__restrict__ lam, uint32_t *__restrict__ fits_total,
+                                                           double *__restrict__ unset)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t fits = i < S ? arima_boxcox_series(entries, offsets, sbase, B, i, csr_v, yb, lam) : 0u;
+    uint32_t fits = i < S ? arima_boxcox_series(entries, offsets, sbase, B, i, csr_v, yb, lam, unset) : 0u;
     fits = __reduce_add_sync(0xffffffffu, fits);          // the grid covers whole warps
     if ((threadIdx.x & 31) == 0 && fits) atomicAdd(fits_total, fits);
 }
@@ -609,22 +619,42 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
 // starts with it; once it is nonzero the warp leaves at once, dropping the fits in flight unfinished -- a cancelled job
 // fails without reading pred[].  So the wait is bounded by one round (one evaluation of the longest prefix in flight),
 // not by one fit (tens of rounds) or one series.  *fits_done gains the fits finished, one atomic per warp and round.
+// Yield (resume != null): a cancel word of 2 ends the launch the same way; each warp then writes its series' resume point
+// resume[2i], the longest prefix it has not finished (0 once all are done): every prefix above it has its forecast, and
+// below it only those fitted while longer ones were in flight; resume[2i + 1] = the fits it dropped in flight, also added
+// to resume[2S].  The kResume launch starts each series at its resume point and hands out only the prefixes whose pred[t]
+// still holds kPredUnset, so the fits dropped in flight are fitted again from their start values and each fit finishes,
+// and is counted, once.  The dropped fits are the unset prefixes above the point where the hand-out had got to, so they
+// are the warp's first resume[2i + 1] hand-outs; resume[2S + 1] counts those that have finished again, which lets the host
+// hold the next yield until all have (so no fit is dropped twice).  kMode: 0 a fit that cannot yield (resume is null),
+// 1 one that can, 2 its resume launch; mode 0 is the fit kernel as it is without fit sharing.
+template <int kMode>
 __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                              const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
                                                              const double *__restrict__ yb, const double *__restrict__ lam,
                                                              double *__restrict__ pred, const volatile uint32_t *cancel,
-                                                             uint32_t *__restrict__ fits_done)
+                                                             uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume)
 {
     const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     if (i >= S) return;                                    // warp-uniform
     if (isnan(lam[i])) return;
+    constexpr bool kResume = kMode == 2;
+    int next;                                              // next job to hand out (warp-uniform), down to 3
+    uint32_t redo = 0;                                     // kResume: hand-outs left that redo a dropped fit (warp-uniform)
+    if (kResume) {
+        next = (int)resume[2 * i];
+        redo = resume[2 * i + 1];
+        if (next < 3) return;                              // every prefix of the series has its forecast
+    }
     const SeriesEntry e = load_entry(entries, offsets, sbase, B, i);
     const double *y = yb + e.off;
     double *p = pred + e.off;
-    for (uint32_t t = lane; t < min(e.n, 3u); t += 32) p[t] = y[t];      // train = first three points (:241,255)
-    int next = (int)e.n - 1;                               // next job to hand out (warp-uniform), down to 3
-    bool busy = false;
+    if (!kResume) {
+        for (uint32_t t = lane; t < min(e.n, 3u); t += 32) p[t] = y[t];      // train = first three points (:241,255)
+        next = (int)e.n - 1;
+    }
+    bool busy = false, redoing = false;
     ArimaObj o{y, 0};
     double u[3] = {0.0, 0.0, 0.0};
     Lbfgs st;
@@ -634,8 +664,25 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
     for (;;) {
         if (__shfl_sync(0xffffffffu, stop, 0)) break;      // cancelled: the fits in flight are dropped
         // ---- hand the next jobs to the idle lanes --------------------------------------------
-        const uint32_t idle = __ballot_sync(0xffffffffu, !busy);
-        if (idle && next >= 3) {
+        uint32_t idle = __ballot_sync(0xffffffffu, !busy);
+        if (kResume) {
+            // a prefix whose forecast is written is passed over; its idle lane takes the next one
+            while (idle && next >= 3) {
+                const int t = next - __popc(idle & ((1u << lane) - 1u));
+                const bool take = !busy && t >= 3 && __double_as_longlong(p[t]) == (long long)kPredUnset;
+                const uint32_t took = __ballot_sync(0xffffffffu, take);
+                if (take) {
+                    o.n = (uint32_t)t;
+                    arima_start(o, u);
+                    lbfgs_init(st);
+                    busy = true;
+                    redoing = __popc(took & ((1u << lane) - 1u)) < redo;      // longest first: in lane order
+                }
+                redo -= min(redo, (uint32_t)__popc(took));
+                next -= __popc(idle);
+                idle = __ballot_sync(0xffffffffu, !busy);
+            }
+        } else if (idle && next >= 3) {
             const int rank = __popc(idle & ((1u << lane) - 1u));
             if (!busy && next - rank >= 3) {
                 o.n = (uint32_t)(next - rank);
@@ -664,6 +711,20 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
         }
         const uint32_t fin = __ballot_sync(0xffffffffu, ended);
         if (lane == 0 && fin) atomicAdd(fits_done, (uint32_t)__popc(fin));
+        if (kResume) {
+            const uint32_t again = __ballot_sync(0xffffffffu, ended && redoing);
+            if (lane == 0 && again) atomicAdd(resume + 2 * S + 1, (uint32_t)__popc(again));
+            if (ended) redoing = false;
+        }
+    }
+    if (kMode != 0) {
+        const int held = (int)__reduce_max_sync(0xffffffffu, busy ? o.n : 0u);    // the longest fit dropped in flight
+        const uint32_t dropped = (uint32_t)__popc(__ballot_sync(0xffffffffu, busy));
+        if (lane == 0) {
+            resume[2 * i] = (uint32_t)max(max(next, held), 0);
+            resume[2 * i + 1] = dropped;
+            if (dropped) atomicAdd(resume + 2 * S, dropped);
+        }
     }
 }
 
@@ -765,13 +826,32 @@ __global__ void __launch_bounds__(NT) detect_arima_kernel(const SeriesEntry *__r
 
 cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                              uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits)
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume)
 {
     if (S == 0) return cudaSuccess;
-    arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam, fits);
+    arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam, fits,
+                                                         resume ? scratch_pred : nullptr);
     const uint64_t threads = (uint64_t)S * 32;
-    arima_fit_sync_kernel<<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                            scratch_lam, scratch_pred, cancel, fits + 1);
+    if (resume)
+        arima_fit_sync_kernel<1><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
+                                                                                    scratch_lam, scratch_pred, cancel, fits + 1,
+                                                                                    resume);
+    else
+        arima_fit_sync_kernel<0><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
+                                                                                    scratch_lam, scratch_pred, cancel, fits + 1,
+                                                                                    nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
+                                uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
+                                const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume)
+{
+    if (S == 0) return cudaSuccess;
+    const uint64_t threads = (uint64_t)S * 32;
+    arima_fit_sync_kernel<2><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
+                                                                                  scratch_lam, scratch_pred, cancel, fits + 1,
+                                                                                  resume);
     return cudaGetLastError();
 }
 

@@ -149,6 +149,12 @@ struct tad_job {
     uint32_t passes = 0;             // hash-range passes the job ran in (tad_job_memory)
     tad_progress prog{};             // passes and ARIMA fits so far (tad_job_progress), under `mu`
     uint64_t peak_workspace = 0;     // largest device workspace the context held while the job ran
+    // fit sharing (tad_set_fit_sharing)
+    uint64_t share = 0;              // an ARIMA tad_submit job: the reserve read when it started (0: its fit does not yield)
+    bool no_interleave = false;      // did not fit a reserve: waits for its turn in the queue
+    uint32_t yields = 0;             // times the fit phase yielded (tad_job_yields), under `mu`
+    double parked_ms = 0;            // time the job was parked, under `mu`
+    double quiet_until = 0;          // now_ms() before which the fit does not yield again
     // streamed input (tad_submit_stream): the caller hands the worker one column block at a time, under `mu`.  `cols`
     // then holds the first block: its non-NULL columns are the set every block must carry.
     bool stream = false;
@@ -184,6 +190,7 @@ struct tad_ctx {
     tad_config cfg{};
     cudaStream_t stream = nullptr, copy_stream = nullptr;
     cudaEvent_t ev[kMaxEvents]{};
+    cudaEvent_t ev_alt[kMaxEvents]{};     // ev of the jobs run while an ARIMA pass is parked (its own ev keep its times)
     cudaEvent_t chunk_ev[kMaxChunks]{};
     cudaEvent_t start_ev = nullptr;
     cudaEvent_t x_ev[kMaxXChunks + 1]{};
@@ -201,7 +208,7 @@ struct tad_ctx {
     int num_sms = 132;
     // device workspace (grow-only, reused across jobs; jobs are serialized by the worker)
     DevBuf d_col[10], hist, offsets, cursor, big_list, big_base, cls_list, csr_p, stats, part, csr_v, csr_t, nsb, npb, sbase, outb, ns_ignore, spill,
-        dbx, dbi, exch, scan_sync, small, hist_all, seg_off, seg_total, entries, ar_y, ar_pred, ar_lam, ovf;
+        dbx, dbi, exch, scan_sync, small, hist_all, seg_off, seg_total, entries, ar_y, ar_pred, ar_lam, ar_res, ovf;
     int optimistic = 1;      // TAD_OPTIMISTIC=0: always the exact (histogram + scan + scatter) partition
     unsigned long long *h_small = nullptr;   // pinned, kSmallWords x u64
     // Word offsets in h_small and in the device scratch `small` (d_small) that mirrors it.  From word 0: gather_small, the
@@ -222,8 +229,10 @@ struct tad_ctx {
     uint32_t scan_epoch = 0;
     uint32_t *h_stats = nullptr;   // pinned readback of the device scalars
     // ARIMA fit launch (wait_arima_fit): pinned [0, 2): the fit counters while the kernel runs, [2, 4): once it has ended,
-    // [4]: 1, the value a cancel copies into the kernel's cancel word
+    // [4]: 1, the value a cancel copies into the kernel's cancel word; [5]: 2, the value a yield copies there; [6], [7]:
+    // the fits the last yield dropped, and those of them finished again
     uint32_t *h_fits = nullptr;
+    std::atomic<uint64_t> fit_share{0};             // tad_set_fit_sharing: the reserve of the jobs run beside a fit (0: off)
     cudaEvent_t fit_ev[2]{};        // [0]: the fit counters are reset; [1]: the fit kernel has ended
     cudaEvent_t fits_ev = nullptr;  // a copy of the fit counters has reached h_fits
     std::mutex pool_mu;
@@ -347,7 +356,7 @@ std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
                                &ctx->csr_p, &ctx->stats, &ctx->part, &ctx->csr_v, &ctx->csr_t, &ctx->nsb, &ctx->npb,
                                &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx, &ctx->dbi, &ctx->exch,
                                &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total, &ctx->entries,
-                               &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
+                               &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ar_res, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
                                &ctx->stage, &ctx->pcnt, &ctx->ostage, &ctx->tstage, &ctx->tscratch};
     for (auto &t : ctx->tdict)
         for (DevBuf *b : t.bufs()) v.push_back(b);
@@ -482,8 +491,20 @@ void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progres
 // kernel, copies tad_cancel into the kernel's cancel word (single GPU only: on several GPUs a rank that left early would
 // strand its peers at the end-of-job all-gather) and about every 50 ms copies the pass's fit counters back; both copies
 // run on the copy stream, beside the kernel.  The counters are published added to the job's counts before the pass.
-// Returns once the kernel has ended, its final counts published.
-void wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits)
+// Fit sharing (tad_set_fit_sharing): when a fit that can yield (job->share) sees a job waiting that interleave() would run,
+// it copies 2 into the cancel word instead; once the kernel has left, the pass is parked, the waiting jobs run, and
+// `resume` launches the rest of the fit (launch_arima_resume), waited for the same way.  d_redo (the resume array's words
+// [2S, 2S + 2), zeroed before the fit launch): the fits a yield dropped, and those of them the resume has finished again.
+// Fairness: after a resume the fit does not yield again until every fit the last yield dropped has finished again and it
+// has run at least as long as that interleave took (job->quiet_until).  So no fit is dropped twice: the work yields throw
+// away is at most one fitting of each prefix, and under a steady stream of short jobs the fit phase (parked time left
+// out) takes at most about twice as long.  Each resume launch is added to `launches`.
+// Returns once the kernel has ended, its final counts published: the time the pass was parked (ms).
+bool interleave_waiting(tad_ctx *ctx);
+void interleave(tad_ctx *ctx, tad_job *job);
+bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve);
+template <class Resume>
+double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_redo, uint64_t &launches, Resume resume)
 {
     uint64_t done0, total0;
     {
@@ -497,39 +518,200 @@ void wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits)
         job->prog.fits_done = done0 + h[1];
     };
     const bool cancellable = ctx->cfg.world_size == 1;
-    CU(cudaEventRecord(ctx->fit_ev[1], ctx->stream));
+    double parked = 0;
+    uint32_t dropped = 0, redone = 0;    // the fits the last yield dropped; of those, finished again (as last copied back)
+    double t_word = 0;
     CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));     // no copy touches the words before their reset
-    bool copying = false, cancelled = false;
-    double next_copy = now_ms();
     for (;;) {
-        if (cancellable && !cancelled && job->cancel.load()) {
-            CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 4, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-            cancelled = true;
-        }
-        const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
-        if (e != cudaErrorNotReady) {
-            CU(e);
-            break;
-        }
-        if (copying) {
-            const cudaError_t c = cudaEventQuery(ctx->fits_ev);
-            if (c != cudaErrorNotReady) {
-                CU(c);
-                publish(ctx->h_fits);
-                copying = false;
+        CU(cudaEventRecord(ctx->fit_ev[1], ctx->stream));
+        bool copying = false, cancelled = false, yielded = false;
+        double next_copy = now_ms();
+        for (;;) {
+            if (cancellable && !cancelled && job->cancel.load()) {
+                CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 4, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+                cancelled = true;
             }
+            if (job->share && !cancelled && !yielded && redone >= dropped && now_ms() >= job->quiet_until &&
+                interleave_waiting(ctx)) {
+                CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 5, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+                yielded = true;
+                t_word = now_ms();
+            }
+            const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
+            if (e != cudaErrorNotReady) {
+                CU(e);
+                break;
+            }
+            if (copying) {
+                const cudaError_t c = cudaEventQuery(ctx->fits_ev);
+                if (c != cudaErrorNotReady) {
+                    CU(c);
+                    publish(ctx->h_fits);
+                    if (redone < dropped) redone = ctx->h_fits[7];
+                    copying = false;
+                }
+            }
+            // every 50 ms; every poll while the next yield waits for the dropped fits only
+            if (!copying && (now_ms() >= next_copy || redone < dropped)) {
+                CU(cudaMemcpyAsync(ctx->h_fits, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                if (redone < dropped) CU(cudaMemcpyAsync(ctx->h_fits + 7, d_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
+                copying = true;
+                next_copy = now_ms() + 50.0;
+            }
+            std::this_thread::sleep_for(std::chrono::milliseconds(1));
         }
-        if (!copying && now_ms() >= next_copy) {
-            CU(cudaMemcpyAsync(ctx->h_fits, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
-            CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
-            copying = true;
-            next_copy = now_ms() + 50.0;
+        CU(cudaMemcpyAsync(ctx->h_fits + 2, d_fits, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        publish(ctx->h_fits + 2);
+        // not yielded, cancelled (the caller fails the job), or every fit finished before the kernel saw the word
+        if (!yielded || cancelled || ctx->h_fits[3] == ctx->h_fits[2]) return parked;
+        const double t0 = now_ms();
+        CU(cudaStreamSynchronize(ctx->copy_stream));           // the yield has reached the word before it is reset
+        CU(cudaMemcpyAsync(ctx->h_fits + 6, d_redo, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        dropped = ctx->h_fits[6];
+        redone = 0;
+        if (getenv("TAD_DEBUG_YIELD")) fprintf(stderr, "yield: kernel left %.2f ms after the word, %u fits dropped\n", t0 - t_word, dropped);
+        interleave(ctx, job);
+        CU(cudaMemsetAsync(d_fits + 2, 0, 4, ctx->stream));
+        CU(cudaMemsetAsync(d_redo, 0, 8, ctx->stream));
+        CU(cudaEventRecord(ctx->fit_ev[0], ctx->stream));
+        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
+        const double t1 = now_ms();
+        parked += t1 - t0;
+        job->quiet_until = t1 + (t1 - t0);
+        {
+            std::lock_guard<std::mutex> lk(job->mu);
+            job->yields++;
+            job->parked_ms += t1 - t0;
         }
-        std::this_thread::sleep_for(std::chrono::milliseconds(1));
+        resume();
+        launches++;
     }
-    CU(cudaMemcpyAsync(ctx->h_fits + 2, d_fits, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    publish(ctx->h_fits + 2);
+}
+
+// Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN tad_submit job that has not been
+// found too large for the reserve.
+bool interleavable(const tad_job *j)
+{
+    return !j->stream && !j->no_interleave && (j->spec.algo == TAD_ALGO_EWMA || j->spec.algo == TAD_ALGO_DBSCAN);
+}
+
+// Whether a yield would run a job now: a cancelled one is not worth a yield (it fails at once in its turn).
+bool interleave_waiting(tad_ctx *ctx)
+{
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    for (const tad_job *j : ctx->queue)
+        if (interleavable(j) && !j->cancel.load()) return true;
+    return false;
+}
+
+// A parked ARIMA pass: the buffers the rest of its fit, its detect_arima and its pass driver read are moved out of the
+// context into `bufs` (ctx->held leaves them out).  Everything else stays for the jobs run meanwhile to reuse: each plans
+// under the reserve and frees the workspace first when it does not fit there (run_job), so the parked bytes plus theirs
+// stay inside the budget the ARIMA job planned in plus the reserve.  Nothing is freed before they run, which would sit
+// in their wait (cudaFree); their workspace is freed at the restore, after they have completed.  The list:
+//   the fit and detect_arima: the series entries (`entries` after the optimistic partition, in place in `part` after the
+//     exact one), offsets, sbase, csr_v, csr_t, ar_y, ar_pred, ar_lam, the resume points ar_res, the stats words (fit
+//     counters, cancel word, result count) and outb, into which the pass's result layout points;
+//   the pass driver (run_passes), which took pointers to them at its start: the pass columns d_col[0..8), the staging,
+//     the pass counters and the ns_ignore list.
+// What the interleaved jobs may overwrite is rebuilt before the ARIMA job reads it again:
+//   hist, cursor, big_list, big_base, cls_list, nsb, npb, csr_p, ovf, spill, sortb, dbx, dbi, small: the partition and
+//     group scratch, which the next pass's pipeline ensures and writes before reading (scan_sync: freed at the restore, so
+//     that pipeline allocates and zeroes it again for the scan's epochs);
+//   d_col[8..10): a one-pass job's host namespace columns, read before the fit only;
+//   h_stats and h_small: read back again after the fit (read_stats) and after every sweep (the counts);
+//   h_fits: the fit counters are published before the park;
+//   ev: the interleaved jobs record ev_alt, so the pass's phase events survive;
+//   limit, peak and store_peak: restored.
+// The text key buffers are empty here: a streamed job never yields.
+struct Parked {
+    tad_ctx *ctx;
+    std::vector<std::pair<DevBuf *, DevBuf>> bufs;
+    size_t limit, peak, store_peak;
+    bool out = false;
+
+    Parked(tad_ctx *c) : ctx(c), limit(c->limit), peak(c->peak), store_peak(c->store_peak)
+    {
+        std::vector<DevBuf *> keep = {&ctx->part, &ctx->entries, &ctx->offsets, &ctx->sbase, &ctx->csr_v, &ctx->csr_t,
+                                      &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ar_res, &ctx->stats, &ctx->outb,
+                                      &ctx->stage, &ctx->pcnt, &ctx->ns_ignore};
+        for (int i = 0; i < 8; i++) keep.push_back(&ctx->d_col[i]);
+        CU(cudaStreamSynchronize(ctx->stream));
+        for (DevBuf *b : keep) {
+            if (!b->p) continue;
+            bufs.push_back({b, *b});
+            ctx->held -= b->cap;
+            *b = DevBuf{};
+        }
+        out = true;
+        std::swap(ctx->ev, ctx->ev_alt);
+    }
+    // the interleaved jobs' workspace is freed and the parked buffers return; drop: they are freed too (a cancel)
+    void restore(bool drop = false)
+    {
+        if (!out) return;
+        out = false;
+        std::swap(ctx->ev, ctx->ev_alt);
+        cudaStreamSynchronize(ctx->stream);
+        for (DevBuf *b : workspace_bufs(ctx))
+            if (b->p) cudaFree(b->p);
+        for (DevBuf *b : workspace_bufs(ctx)) *b = DevBuf{};
+        for (auto &t : ctx->tdict) t.cap = 0;
+        ctx->held = 0;
+        for (auto &b : bufs) {
+            if (drop) {
+                cudaFree(b.second.p);
+                continue;
+            }
+            *b.first = b.second;
+            ctx->held += b.second.cap;
+        }
+        bufs.clear();
+        ctx->limit = limit;
+        ctx->peak = std::max(peak, ctx->held);
+        ctx->store_peak = store_peak;
+    }
+    ~Parked() { restore(); }
+};
+
+// Runs the eligible jobs queued now, in FIFO order, while the ARIMA pass of `job` is parked: each inside the reserve
+// (run_one), so one whose 1/64 hash range does not fit it is put back where it was and runs in its turn.  A cancel of
+// `job` takes effect once the job in progress has ended: the parked buffers are freed and the job fails.
+void interleave(tad_ctx *ctx, tad_job *job)
+{
+    std::vector<tad_job *> batch;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        for (tad_job *j : ctx->queue)
+            if (interleavable(j)) batch.push_back(j);
+    }
+    const double t0 = now_ms();
+    Parked park(ctx);
+    const double t1 = now_ms();
+    for (tad_job *j : batch) {
+        if (job->cancel.load()) break;
+        size_t at;
+        {
+            std::lock_guard<std::mutex> lk(ctx->mu);       // only this thread takes jobs out of the queue
+            at = (size_t)(std::find(ctx->queue.begin(), ctx->queue.end(), j) - ctx->queue.begin());
+            if (at == ctx->queue.size()) continue;
+            ctx->queue.erase(ctx->queue.begin() + at);
+        }
+        if (!run_one(ctx, j, job->share)) {
+            std::lock_guard<std::mutex> lk(ctx->mu);       // jobs submitted meanwhile went behind it
+            ctx->queue.insert(ctx->queue.begin() + at, j);
+        }
+    }
+    CU(cudaSetDevice(ctx->cfg.device));
+    const double t2 = now_ms();
+    const bool cancelled = job->cancel.load() != 0;
+    park.restore(cancelled);
+    if (getenv("TAD_DEBUG_YIELD"))
+        fprintf(stderr, "yield: park %.2f ms, %zu jobs %.2f ms, restore %.2f ms\n", t1 - t0, batch.size(), t2 - t1, now_ms() - t2);
+    if (cancelled) fail(TAD_ERR_CANCELLED, "job cancelled");
 }
 
 int pick_logb(const tad_ctx *ctx, uint64_t rows)
@@ -677,11 +859,12 @@ struct PipeShape {
     int algo = TAD_ALGO_EWMA;
     uint32_t B = 1, Bl = 1;          // buckets; buckets this GPU owns
     bool optimistic = false;         // fixed-capacity bucket slots instead of the exact partition
+    bool resume = false;             // an ARIMA fit that can yield: its resume points (tad_set_fit_sharing)
     uint64_t owned = 0, series = 0, out_cap = 1;
 };
 struct PipeSizes {
     size_t col[10], part, slots, ovf, entries, hist, offsets, cursor, big_list, big_base, cls_list, nsb, npb, csr_v, csr_t,
-        csr_p, sbase, outb, dbx, dbi, ar_y, ar_pred, ar_lam;
+        csr_p, sbase, outb, dbx, dbi, ar_y, ar_pred, ar_lam, ar_res;
 };
 constexpr size_t kOutWidth[11] = {8, 8, 8, 4, 4, 4, 4, 2, 2, 1, 1};   // bytes per result row of each out_layout column
 constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad_set_memory_budget accepts
@@ -710,6 +893,7 @@ PipeSizes pipe_sizes(const PipeShape &s)
     z.outb = out_layout(s.out_cap).total;
     z.ar_y = z.ar_pred = s.algo == TAD_ALGO_ARIMA ? cap_rows * 8 : 0;
     z.ar_lam = s.algo == TAD_ALGO_ARIMA ? ((size_t)s.series + 1) * 8 : 0;
+    z.ar_res = s.algo == TAD_ALGO_ARIMA && s.resume ? ((size_t)s.series + 1) * 8 : 0;
     return z;
 }
 
@@ -721,7 +905,7 @@ std::vector<std::pair<DevBuf *, size_t>> pipe_bufs(tad_ctx *ctx, const PipeSizes
         {&ctx->offsets, z.offsets}, {&ctx->cursor, z.cursor}, {&ctx->big_list, z.big_list}, {&ctx->big_base, z.big_base},
         {&ctx->cls_list, z.cls_list}, {&ctx->nsb, z.nsb}, {&ctx->npb, z.npb}, {&ctx->csr_v, z.csr_v}, {&ctx->csr_t, z.csr_t},
         {&ctx->csr_p, z.csr_p}, {&ctx->sbase, z.sbase}, {&ctx->outb, z.outb}, {&ctx->dbx, z.dbx}, {&ctx->dbi, z.dbi},
-        {&ctx->ar_y, z.ar_y}, {&ctx->ar_pred, z.ar_pred}, {&ctx->ar_lam, z.ar_lam}};
+        {&ctx->ar_y, z.ar_y}, {&ctx->ar_pred, z.ar_pred}, {&ctx->ar_lam, z.ar_lam}, {&ctx->ar_res, z.ar_res}};
     for (int i = 0; i < 10; i++) v.push_back({&ctx->d_col[i], z.col[i]});
     return v;
 }
@@ -891,6 +1075,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     shape.rows = R;
     shape.host = host_input ? &hc : nullptr;
     shape.algo = sp.algo;
+    shape.resume = job->share != 0;
     PipeSizes z = pipe_sizes(shape);
     for (int i = 0; i < 10; i++) {
         void *src = col_ptr(hc, i);
@@ -1329,6 +1514,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     OutLayout L{};
     OutCols oc{};
     shape.series = S;
+    double parked_ms = 0;                 // the ARIMA fit's time parked while other jobs ran: not this job's device time
     for (int attempt = 0; attempt < 3; attempt++) {
         shape.out_cap = out_cap;
         z = pipe_sizes(shape);
@@ -1358,12 +1544,19 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             ensure(ctx, ctx->ar_y, z.ar_y);
             ensure(ctx, ctx->ar_pred, z.ar_pred);
             ensure(ctx, ctx->ar_lam, z.ar_lam);
+            ensure(ctx, ctx->ar_res, z.ar_res);
             if (attempt == 0 && S) {
+                double *y = (double *)ctx->ar_y.p, *pred = (double *)ctx->ar_pred.p, *lam = (double *)ctx->ar_lam.p;
+                uint32_t *res = job->share ? (uint32_t *)ctx->ar_res.p : nullptr;
                 CU(cudaMemsetAsync(d_stats + ST_FITS, 0, 12, st));      // fit counters and cancel word
+                if (res) CU(cudaMemsetAsync(res + 2 * (size_t)S, 0, 8, st));
                 CU(cudaEventRecord(ctx->fit_ev[0], st));
-                CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, (double *)ctx->ar_y.p, (double *)ctx->ar_pred.p,
-                                    (double *)ctx->ar_lam.p, d_stats + ST_FITS + 2, d_stats + ST_FITS));
-                wait_arima_fit(ctx, job, d_stats + ST_FITS);
+                CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, y, pred, lam, d_stats + ST_FITS + 2,
+                                    d_stats + ST_FITS, res));
+                parked_ms = wait_arima_fit(ctx, job, d_stats + ST_FITS, res ? res + 2 * (size_t)S : nullptr, launches, [&] {
+                    CU(launch_arima_resume(st, entries, offsets, sbase, Bl, S, y, pred, lam, d_stats + ST_FITS + 2,
+                                           d_stats + ST_FITS, res));
+                });
                 if (ctx->cfg.world_size == 1) check_cancel();      // pred[] is incomplete: no detect
             }
             CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
@@ -1425,6 +1618,10 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         if (ev_phase[i] == TAD_PHASE_DETECT || (ev_phase[i] == TAD_PHASE_SYNC && last_k >= 0)) last_k = i;
     }
     if (first_k >= 0 && last_k > first_k) CU(cudaEventElapsedTime(&total, ctx->ev[first_k], ctx->ev[last_k]));
+    if (parked_ms > 0) {
+        phase_ms[TAD_PHASE_DETECT] = std::max(0.0, phase_ms[TAD_PHASE_DETECT] - parked_ms);
+        total = (float)std::max(0.0, (double)total - parked_ms);
+    }
     out.kept = kept;
     out.owned = owned;
     out.points = points_all;
@@ -1456,6 +1653,7 @@ PipeShape one_gpu_shape(const tad_ctx *ctx, const tad_job *job, uint64_t rows, b
     s.algo = job->spec.algo;
     s.B = s.Bl = buckets(ctx, rows);
     s.optimistic = optimistic && one_gpu_optimistic(ctx, rows, s.B);
+    s.resume = job->share != 0;
     s.owned = s.series = rows;
     s.out_cap = out_cap_guess(rows, (job->spec.flags & TAD_FLAG_EMIT_ALL) != 0);
     return s;
@@ -2712,7 +2910,8 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     return passes;
 }
 
-void run_job(tad_ctx *ctx, tad_job *job)
+// `reserve`: a job run while an ARIMA fit is parked (interleave), with the fit-sharing reserve as its budget.
+void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
 {
     CU(cudaSetDevice(ctx->cfg.device));
     // several GPUs under a budget: every rank joins the plan all-gather, a job cancelled before it started too
@@ -2722,11 +2921,14 @@ void run_job(tad_ctx *ctx, tad_job *job)
     const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
     const uint64_t host_budget = store_trim(ctx);      // the job's one read of the host budget
+    // fit sharing: a single-GPU ARIMA tad_submit job plans in the budget less the reserve, and its fit yields
+    job->share = !reserve && !job->stream && ctx->cfg.world_size == 1 && job->spec.algo == TAD_ALGO_ARIMA ? ctx->fit_share.load() : 0;
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
+    const uint64_t set = reserve ? reserve : ctx->budget.load();
     auto context_budget = [&]() -> uint64_t {
-        if (const uint64_t set = ctx->budget.load()) return set;
+        if (set) return set;
         size_t free_b = 0, total_b = 0;
         CU(cudaMemGetInfo(&free_b, &total_b));
         return free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
@@ -2742,8 +2944,13 @@ void run_job(tad_ctx *ctx, tad_job *job)
         budget = multi_budget;          // run_passes_multi applies it once the plan has freed the exported buffer
         free_workspace(ctx);
     } else if (ctx->cfg.world_size == 1 && R > 0) {
-        const uint64_t set = ctx->budget.load();
         budget = context_budget();
+        if (job->share) {
+            if (budget < job->share + kBudgetFloor)
+                fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes less the fit-sharing reserve of %llu bytes is below the "
+                     "64 MiB floor", (unsigned long long)budget, (unsigned long long)job->share);
+            budget -= job->share;
+        }
         PipeShape s = one_gpu_shape(ctx, job, R, true);
         s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
         auto bufs = pipe_bufs(ctx, pipe_sizes(s));
@@ -2753,7 +2960,7 @@ void run_job(tad_ctx *ctx, tad_job *job)
             bufs = pipe_bufs(ctx, pipe_sizes(s));
             split = workspace_after(ctx, bufs, true) > budget;
         }
-        if (set || force_exact) {
+        if (set || force_exact || job->share) {
             ctx->limit = budget;
             if (split || workspace_after(ctx, bufs, false) > budget) free_workspace(ctx);
         }
@@ -2802,6 +3009,36 @@ void run_job(tad_ctx *ctx, tad_job *job)
     }
 }
 
+// Runs `job` and reports a failure on it.  `reserve` (interleave): false when the job failed with TAD_ERR_NOMEM inside
+// the reserve; it is then SCHEDULED again with no progress, is not run beside a fit again, and waits for its turn.
+bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve)
+{
+    try {
+        run_job(ctx, job, reserve);
+    } catch (const JobFail &f) {
+        // nothing of this job may still be reading the caller's columns once it is reported FAILED
+        cudaStreamSynchronize(ctx->copy_stream);
+        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->d2h_stream);
+        cudaGetLastError();
+        TextKeys::release(ctx);
+        std::lock_guard<std::mutex> lk(job->mu);
+        if (reserve && f.code == TAD_ERR_NOMEM && !job->cancel.load()) {
+            job->no_interleave = true;
+            job->st.state = TAD_STATE_SCHEDULED;
+            job->st.completed_stages = 0;
+            job->prog = tad_progress{};
+            return false;
+        }
+        job->st.state = TAD_STATE_FAILED;
+        job->st.error = f.code;
+        snprintf(job->st.err_msg, sizeof(job->st.err_msg), "%s", f.msg);
+        job->st.total_ms = now_ms() - job->t_submit;
+        job->cv.notify_all();
+    }
+    return true;
+}
+
 void worker_main(tad_ctx *ctx)
 {
     if (ctx->numa.ok) sched_setaffinity(0, sizeof(ctx->numa.cpus), &ctx->numa.cpus);      // this thread only
@@ -2815,22 +3052,7 @@ void worker_main(tad_ctx *ctx)
             job = ctx->queue.front();
             ctx->queue.pop_front();
         }
-        try {
-            run_job(ctx, job);
-        } catch (const JobFail &f) {
-            // nothing of this job may still be reading the caller's columns once it is reported FAILED
-            cudaStreamSynchronize(ctx->copy_stream);
-            cudaStreamSynchronize(ctx->stream);
-            cudaStreamSynchronize(ctx->d2h_stream);
-            cudaGetLastError();
-            TextKeys::release(ctx);
-            std::lock_guard<std::mutex> lk(job->mu);
-            job->st.state = TAD_STATE_FAILED;
-            job->st.error = f.code;
-            snprintf(job->st.err_msg, sizeof(job->st.err_msg), "%s", f.msg);
-            job->st.total_ms = now_ms() - job->t_submit;
-            job->cv.notify_all();
-        }
+        run_one(ctx, job, 0);
     }
 }
 
@@ -3080,11 +3302,15 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     if (getenv("TAD_EXCHANGE_CHUNKS")) ctx->exchange_chunks_forced = true;
     if (const char *e = getenv("TAD_EXCHANGE_CHUNKS")) ctx->exchange_chunks = atoi(e) < 1 ? 1 : (atoi(e) > kMaxXChunks ? kMaxXChunks : atoi(e));
     for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
+    for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev_alt[i]) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_small, tad_ctx::kSmallWords * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 5 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    if (ok) ctx->h_fits[4] = 1;
+    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 8 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
+    if (ok) {
+        ctx->h_fits[4] = 1;
+        ctx->h_fits[5] = 2;
+    }
     for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->fit_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->fits_ev, cudaEventDisableTiming) == cudaSuccess;
     if (!ok) {
@@ -3132,8 +3358,10 @@ void tad_shutdown(tad_ctx *ctx)
     for (int i = 0; i < 2; i++)
         if (ctx->fit_ev[i]) cudaEventDestroy(ctx->fit_ev[i]);
     if (ctx->fits_ev) cudaEventDestroy(ctx->fits_ev);
-    for (int i = 0; i < kMaxEvents; i++)
+    for (int i = 0; i < kMaxEvents; i++) {
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+        if (ctx->ev_alt[i]) cudaEventDestroy(ctx->ev_alt[i]);
+    }
     for (int i = 0; i < kMaxChunks; i++)
         if (ctx->chunk_ev[i]) cudaEventDestroy(ctx->chunk_ev[i]);
     if (ctx->start_ev) cudaEventDestroy(ctx->start_ev);
@@ -3365,6 +3593,25 @@ int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes)
     if (!ctx) return TAD_ERR_INVALID_ARG;
     if (bytes && bytes < kBudgetFloor) return TAD_ERR_INVALID_ARG;
     ctx->budget.store(bytes);
+    return TAD_OK;
+}
+
+int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes)
+{
+    if (!ctx) return TAD_ERR_INVALID_ARG;
+    if (ctx->cfg.world_size > 1) return TAD_ERR_UNSUPPORTED;
+    if (reserve_bytes && reserve_bytes < kBudgetFloor) return TAD_ERR_INVALID_ARG;
+    ctx->fit_share.store(reserve_bytes);
+    return TAD_OK;
+}
+
+int tad_job_yields(tad_job *job, uint32_t *yields, double *parked_ms)
+{
+    if (!job) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->st.state != TAD_STATE_COMPLETED || job->spec.algo != TAD_ALGO_ARIMA) return TAD_ERR_STATE;
+    if (yields) *yields = job->yields;
+    if (parked_ms) *parked_ms = job->parked_ms;
     return TAD_OK;
 }
 

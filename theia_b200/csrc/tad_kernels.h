@@ -78,9 +78,17 @@ cudaError_t launch_detect_dbscan(cudaStream_t st, const SeriesEntry *entries, co
 // cancel: a device word the fit kernel reads in every round; nonzero = every warp leaves at its next round and drops the
 // fits in flight, so pred[] is then incomplete.  fits[0] gains the prefix fits of the series, fits[1] the fits finished
 // (u32: one fit per point, fewer than 2^32 points per pass).
+// resume (2 S + 2 u32, or null): the fit can yield.  A cancel word of 2 makes every warp leave like a cancel, after it has
+// written its series' resume point and the fits it dropped there ([2i], [2i + 1]); [2S] gains the fits dropped, [2S + 1]
+// the dropped fits a resume launch has finished again (both zeroed by the caller).  launch_arima_resume fits what is left
+// (the fits dropped in flight and those never started) into the same pred[] and counters, so the forecasts and counts are
+// those of one launch.
 cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                              uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits);
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
+cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
+                                uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
+                                const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
 cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                                 uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, const double *scratch_pred,
                                 const double *scratch_lam, const OutCols &out, uint32_t out_cap, uint32_t *stats, int emit_all);

@@ -164,6 +164,15 @@ class Job:
             raise TadError(rc, "tad_job_progress")
         return {"passes_done": p.passes_done, "passes": p.passes, "fits_done": p.fits_done, "fits_total": p.fits_total}
 
+    def yields(self) -> dict:
+        """Of a COMPLETED ARIMA job (tad_job_yields): how many times its fit phase yielded to queued jobs and the time
+        it was parked meanwhile (see TadEngine.set_fit_sharing)."""
+        n, ms = C.c_uint32(), C.c_double()
+        rc = self.eng.lib.tad_job_yields(self.h, C.byref(n), C.byref(ms))
+        if rc != 0:
+            raise TadError(rc, "tad_job_yields")
+        return {"yields": n.value, "parked_ms": ms.value}
+
     def cancel(self):
         """tad_cancel: returns at once; an ARIMA job on one GPU stops within one evaluation round of its fit kernel."""
         self.eng.lib.tad_cancel(self.h)
@@ -289,6 +298,14 @@ class TadEngine:
         rc = self.lib.tad_set_memory_budget(self.ctx, int(nbytes))
         if rc != 0:
             raise TadError(rc, "tad_set_memory_budget(%d)" % nbytes)
+
+    def set_fit_sharing(self, reserve: int):
+        """Single GPU (tad_set_fit_sharing): with a nonzero reserve (at least 64 MiB) an ARIMA job's fit phase yields to
+        queued EWMA and DBSCAN jobs, which run in the reserve while it is parked; the ARIMA job plans in the memory
+        budget less the reserve.  0 (default) = off: jobs run in submit order."""
+        rc = self.lib.tad_set_fit_sharing(self.ctx, int(reserve))
+        if rc != 0:
+            raise TadError(rc, "tad_set_fit_sharing(%d)" % reserve)
 
     @staticmethod
     def get_unique_id() -> bytes:
