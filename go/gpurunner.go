@@ -19,6 +19,7 @@ import "C"
 import (
 	"fmt"
 	"sync"
+	"sync/atomic"
 	"unsafe"
 )
 
@@ -66,8 +67,9 @@ type gpuJob struct {
 }
 
 type gpuJobRunner struct {
-	ctx  *C.tad_ctx
-	jobs sync.Map // id -> *gpuJob
+	ctx   *C.tad_ctx
+	jobs  sync.Map    // id -> *gpuJob
+	share atomic.Bool // SetFitSharing turned fit sharing on: StartStream flags its jobs
 }
 
 func newGPUJobRunner(device int) (*gpuJobRunner, error) {
@@ -97,6 +99,19 @@ func (r *gpuJobRunner) SetHostBudget(bytes uint64) error {
 	if rc := C.tad_set_host_budget(r.ctx, C.uint64_t(bytes)); rc != C.TAD_OK {
 		return fmt.Errorf("tad_set_host_budget: %s", C.GoString(C.tad_strerror(rc)))
 	}
+	return nil
+}
+
+// SetFitSharing turns fit sharing on with a reserve of `reserve` device bytes (0 = off, the default; nonzero values below
+// 64 MiB are refused).  While an ARIMA job fits, a queued EWMA or DBSCAN job then runs in the reserve instead of waiting
+// for the whole fit phase, and the ARIMA job plans in the memory budget less the reserve.  Jobs from Start take part as
+// they are; StartStream flags its jobs (TAD_FLAG_SHARE) while sharing is on.  It takes effect for jobs that start after
+// the call.  The controller calls it next to SetMemoryBudget.
+func (r *gpuJobRunner) SetFitSharing(reserve uint64) error {
+	if rc := C.tad_set_fit_sharing(r.ctx, C.uint64_t(reserve)); rc != C.TAD_OK {
+		return fmt.Errorf("tad_set_fit_sharing: %s", C.GoString(C.tad_strerror(rc)))
+	}
+	r.share.Store(reserve != 0)
 	return nil
 }
 
@@ -231,6 +246,10 @@ func (r *gpuJobRunner) StartStream(spec JobSpec, rowsHint uint64, blockRows int,
 	js := C.tad_job_spec{algo: algoCode(spec.Algo), start_time: C.uint32_t(spec.StartTime), end_time: C.uint32_t(spec.EndTime)}
 	if spec.SumReducer {
 		js.reducer = C.TAD_REDUCE_SUM
+	}
+	if r.share.Load() {
+		// an ARIMA job's fit yields; an EWMA or DBSCAN job may run, its SELECT read, while a fit is parked
+		js.flags |= C.TAD_FLAG_SHARE
 	}
 	if len(spec.NSIgnore) > 0 {
 		js.n_ns_ignore = C.uint32_t(len(spec.NSIgnore))

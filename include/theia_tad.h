@@ -60,6 +60,7 @@ typedef enum { TAD_MEM_HOST = 0, TAD_MEM_DEVICE = 1 } tad_mem;
 /* tad_job_spec.flags */
 #define TAD_FLAG_EMIT_ALL 1u   /* emit every point with its flag (parity/debug), not only anomalies */
 #define TAD_FLAG_PROFILE  2u   /* record per-phase CUDA-event times into tad_status.phase_ms         */
+#define TAD_FLAG_SHARE    4u   /* a streamed job takes part in fit sharing (tad_set_fit_sharing)     */
 
 typedef struct tad_ctx tad_ctx;
 typedef struct tad_job tad_job;
@@ -227,8 +228,8 @@ int tad_job_progress(tad_job *job, tad_progress *p);
  * per pass.  A job fails with TAD_ERR_NOMEM only when a 1/64 hash range of it does not fit.  Caller-owned columns and
  * pinned host memory are not counted.  If the budget drops below what the context holds, the workspace is freed before
  * the next job.  Applies to jobs that start after the call; TAD_ERR_INVALID_ARG below the floor of 64 MiB.  With fit
- * sharing on (tad_set_fit_sharing), an ARIMA tad_submit job plans in this budget less the reserve (TAD_ERR_NOMEM when
- * that is below 64 MiB), and the jobs run beside its fit plan in the reserve.
+ * sharing on (tad_set_fit_sharing), an ARIMA tad_submit job, or a streamed one with TAD_FLAG_SHARE, plans in this budget
+ * less the reserve (TAD_ERR_NOMEM when that is below 64 MiB), and the jobs run beside its fit plan in the reserve.
  *
  * Several GPUs (world_size > 1): 0 means "no planning", not free memory: a job without a budget runs exactly as it does
  * without this call (no planning collective, launch or sync).  With one, the ranks run the same passes over their shards
@@ -259,7 +260,22 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * dropped twice and a steady stream of short jobs at most about doubles its fit phase.  The ARIMA job's device_ms and
  * detect phase leave out the time it was parked (tad_job_yields); its tad_job_memory peak leaves out the workspace of the
  * jobs run in its place, theirs leaves out its parked buffers and stays within the reserve, so the two stay inside the
- * budget.  Streamed jobs neither yield nor run in a yield.  Applies to jobs that start after the call.
+ * budget.  Applies to jobs that start after the call.
+ *
+ * Streamed jobs (tad_submit_stream, tad_submit_stream_filtered) take part only with TAD_FLAG_SHARE in their spec's flags;
+ * without it a streamed job neither yields nor runs in a yield, as with sharing off.  The flag is ignored on tad_submit
+ * jobs, which take part anyway, and on a context whose sharing is off.  A streamed ARIMA job with the flag plans in the
+ * budget less the reserve and its fit yields as above: its text key dictionaries, its round in progress and its host
+ * row store pages are kept while it is parked, and its feeder's pending push or end call goes on with the same round.  A
+ * streamed EWMA or DBSCAN job with the flag runs in a yield only once its feeder has pushed its first block (or ended
+ * its round): a job whose caller has not started delivering never parks a fit.  It then runs in the reserve as the
+ * others do, with its own dictionaries and as many rounds as it needs, and its caller's blocks are taken meanwhile; the
+ * fit stays parked until its input has ended and its result is published.  Its host row store use stays within the host
+ * budget less the pages the parked job holds; without room it asks for rounds, as a job without a store does.  If it
+ * does not fit the reserve, the round it was running in is read to its end without being used and its tad_stream_end
+ * returns *again = 1; the job is SCHEDULED again with its stages and progress at 0, is not run in a yield again, and
+ * its next round's blocks are taken once the context reaches the job in its turn, which starts it again from its first
+ * round.
  * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit left
  * early would strand its peers, as for the cancel). */
 int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);
@@ -295,7 +311,9 @@ int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host
  * Submit: rows_hint is the caller's estimate of one round's rows (its SELECT count()), 0 = unknown.  It only chooses the
  * pass count and sizes the pass columns before the first round: a wrong hint may cost one round more, never a different
  * result.  TAD_ERR_UNSUPPORTED when world_size > 1.  A context still runs one job at a time: a streamed job holds the
- * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.
+ * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.  The
+ * one exception is fit sharing (tad_set_fit_sharing): with TAD_FLAG_SHARE in its spec, a streamed EWMA or DBSCAN job
+ * whose caller has pushed its first block may run while an ARIMA fit is parked, and a streamed ARIMA job's fit yields.
  *
  * Blocks: mem is TAD_MEM_HOST (any host memory; pinned buffers from tad_alloc_columns copy at the full PCIe rate) or
  * TAD_MEM_DEVICE (read in place); fewer than 2^32 rows; flow_end and value are required; every block carries the same

@@ -150,7 +150,7 @@ struct tad_job {
     tad_progress prog{};             // passes and ARIMA fits so far (tad_job_progress), under `mu`
     uint64_t peak_workspace = 0;     // largest device workspace the context held while the job ran
     // fit sharing (tad_set_fit_sharing)
-    uint64_t share = 0;              // an ARIMA tad_submit job: the reserve read when it started (0: its fit does not yield)
+    uint64_t share = 0;              // an ARIMA job whose fit yields: the reserve read when it started (0: it does not)
     bool no_interleave = false;      // did not fit a reserve: waits for its turn in the queue
     uint32_t yields = 0;             // times the fit phase yielded (tad_job_yields), under `mu`
     double parked_ms = 0;            // time the job was parked, under `mu`
@@ -171,6 +171,7 @@ struct tad_job {
         bool input_done = false;     // tad_stream_end returned again = 0
         tad_text_column txt[2]{};    // the handed-over block's text slots (tad_stream_push_text)
         uint64_t pushed = 0, taken = 0, released = 0;   // blocks handed over / taken / no longer read by the engine
+        uint64_t round_start = 0;    // `taken` when the last round was closed
         int err = 0;                 // a bad block: the worker fails the job with this code and message
         char msg[200] = {0};
     } in;
@@ -435,6 +436,19 @@ uint64_t store_trim(tad_ctx *ctx)
     return budget;
 }
 
+// store_trim for a job run while an ARIMA pass is parked (interleave): the parked job's pages stay where they are, so no
+// slab is freed and the free list is kept.  The job takes free pages and new slabs within the host budget less every slab
+// held, the parked job's included.  Returns the budget it read, or 0 (no store) when its page size is not the context's.
+uint64_t store_share(tad_ctx *ctx)
+{
+    const uint64_t budget = ctx->host_budget.load();
+    const size_t page = budget ? store_page_bytes(budget) : 0;
+    if (!page || (ctx->store_page && page != ctx->store_page)) return 0;
+    ctx->store_page = page;          // was 0: the context holds no slab
+    ctx->store_peak = ctx->store_held;
+    return budget;
+}
+
 // A free page; a new slab when none is left.  Null when the slab would pass the budget or cannot be pinned.
 char *store_take_page(tad_ctx *ctx, uint64_t budget)
 {
@@ -591,18 +605,23 @@ double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_
     }
 }
 
-// Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN tad_submit job that has not been
-// found too large for the reserve.
-bool interleavable(const tad_job *j)
+// Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
+// large for the reserve.  A streamed one only with TAD_FLAG_SHARE and once its feeder has handed over its first block or
+// closed its round: a job whose caller has not started delivering would hold the fit parked while it waits.
+bool interleavable(tad_job *j)
 {
-    return !j->stream && !j->no_interleave && (j->spec.algo == TAD_ALGO_EWMA || j->spec.algo == TAD_ALGO_DBSCAN);
+    if (j->no_interleave || (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN)) return false;
+    if (!j->stream) return true;
+    if (!(j->spec.flags & TAD_FLAG_SHARE)) return false;
+    std::lock_guard<std::mutex> lk(j->mu);
+    return j->in.pushed > 0 || j->in.end_req;
 }
 
 // Whether a yield would run a job now: a cancelled one is not worth a yield (it fails at once in its turn).
 bool interleave_waiting(tad_ctx *ctx)
 {
     std::lock_guard<std::mutex> lk(ctx->mu);
-    for (const tad_job *j : ctx->queue)
+    for (tad_job *j : ctx->queue)
         if (interleavable(j) && !j->cancel.load()) return true;
     return false;
 }
@@ -616,7 +635,14 @@ bool interleave_waiting(tad_ctx *ctx)
 //     exact one), offsets, sbase, csr_v, csr_t, ar_y, ar_pred, ar_lam, the resume points ar_res, the stats words (fit
 //     counters, cancel word, result count) and outb, into which the pass's result layout points;
 //   the pass driver (run_passes), which took pointers to them at its start: the pass columns d_col[0..8), the staging,
-//     the pass counters and the ns_ignore list.
+//     the pass counters and the ns_ignore list;
+//   a streamed job's text key slots: both dictionaries (table, arena, offsets, hashes, keep bytes, pattern, state words,
+//     with their sizes), which its later rounds look names up in and its end copies out, so its ids stay the same, and
+//     the text staging and encode scratch its sweeps take as sized.  They were planned in the budget less the reserve.
+// What else a parked streamed pass needs is not in the workspace and no interleaved job touches it: the job's stream
+// input state (tad_job::in: its feeder, blocked in a push or end call, goes on with the same round) and the host row
+// store pages of its passes (its RowStore's lists).  An interleaved job takes store pages only from the free list and
+// new slabs within the host budget less the slabs held (store_share), and frees no slab.
 // What the interleaved jobs may overwrite is rebuilt before the ARIMA job reads it again:
 //   hist, cursor, big_list, big_base, cls_list, nsb, npb, csr_p, ovf, spill, sortb, dbx, dbi, small: the partition and
 //     group scratch, which the next pass's pipeline ensures and writes before reading (scan_sync: freed at the restore, so
@@ -624,12 +650,13 @@ bool interleave_waiting(tad_ctx *ctx)
 //   d_col[8..10): a one-pass job's host namespace columns, read before the fit only;
 //   h_stats and h_small: read back again after the fit (read_stats) and after every sweep (the counts);
 //   h_fits: the fit counters are published before the park;
-//   ev: the interleaved jobs record ev_alt, so the pass's phase events survive;
+//   ev: the interleaved jobs record ev_alt, so the pass's phase events survive; the other events of a sweep are
+//     recorded in that sweep before they are waited for;
 //   limit, peak and store_peak: restored.
-// The text key buffers are empty here: a streamed job never yields.
 struct Parked {
     tad_ctx *ctx;
     std::vector<std::pair<DevBuf *, DevBuf>> bufs;
+    tad_ctx::TextSlot dict[2];       // the dictionaries' sizes (their buffers are in `bufs`)
     size_t limit, peak, store_peak;
     bool out = false;
 
@@ -637,9 +664,17 @@ struct Parked {
     {
         std::vector<DevBuf *> keep = {&ctx->part, &ctx->entries, &ctx->offsets, &ctx->sbase, &ctx->csr_v, &ctx->csr_t,
                                       &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ar_res, &ctx->stats, &ctx->outb,
-                                      &ctx->stage, &ctx->pcnt, &ctx->ns_ignore};
+                                      &ctx->stage, &ctx->pcnt, &ctx->ns_ignore, &ctx->tstage, &ctx->tscratch};
         for (int i = 0; i < 8; i++) keep.push_back(&ctx->d_col[i]);
+        for (auto &t : ctx->tdict)
+            for (DevBuf *b : t.bufs()) keep.push_back(b);
         CU(cudaStreamSynchronize(ctx->stream));
+        CU(cudaStreamSynchronize(ctx->copy_stream));
+        for (int t = 0; t < 2; t++) {
+            dict[t] = ctx->tdict[t];
+            ctx->tdict[t].cap = 0;
+            ctx->tdict[t].names_ub = ctx->tdict[t].bytes_ub = 0;
+        }
         for (DevBuf *b : keep) {
             if (!b->p) continue;
             bufs.push_back({b, *b});
@@ -656,6 +691,7 @@ struct Parked {
         out = false;
         std::swap(ctx->ev, ctx->ev_alt);
         cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->copy_stream);
         for (DevBuf *b : workspace_bufs(ctx))
             if (b->p) cudaFree(b->p);
         for (DevBuf *b : workspace_bufs(ctx)) *b = DevBuf{};
@@ -670,6 +706,11 @@ struct Parked {
             ctx->held += b.second.cap;
         }
         bufs.clear();
+        for (int t = 0; t < 2 && !drop; t++) {
+            ctx->tdict[t].cap = dict[t].cap;
+            ctx->tdict[t].names_ub = dict[t].names_ub;
+            ctx->tdict[t].bytes_ub = dict[t].bytes_ub;
+        }
         ctx->limit = limit;
         ctx->peak = std::max(peak, ctx->held);
         ctx->store_peak = store_peak;
@@ -1749,10 +1790,30 @@ void close_round(tad_job *job, bool again)
 {
     std::lock_guard<std::mutex> lk(job->mu);
     job->in.released = job->in.taken;
+    job->in.round_start = job->in.taken;
     job->in.end_req = false;
     job->in.again = again;
     job->in.round_done = true;
     job->cv.notify_all();
+}
+
+// A streamed job put back in the queue (run_one): the round in progress, if one is, is taken to its end unread and
+// closed with again = 1, so that its caller delivers the rows again once the job's turn comes.  A round not yet begun
+// is left to that turn: its first block waits there.
+void discard_round(tad_job *job)
+{
+    {
+        std::lock_guard<std::mutex> lk(job->mu);
+        if (!job->in.end_req && job->in.taken == job->in.round_start) return;
+    }
+    tad_columns b{};
+    tad_text_column tx[2]{};
+    while (next_block(job, b, tx)) {
+        std::lock_guard<std::mutex> lk(job->mu);
+        job->in.released = job->in.taken;
+        job->cv.notify_all();
+    }
+    close_round(job, true);
 }
 
 // Device buffer grown to `bytes` with its first `keep` bytes carried over (ensure() frees before it allocates).
@@ -2394,8 +2455,9 @@ uint32_t run_pass_queue(tad_ctx *ctx, tad_job *job, uint32_t P, PassOut &acc, Ru
 // a pass whose spill scratch or result buffer turns out not to fit is split into (v, 2M) and (v + M, 2M).  A sweep reads
 // the job's columns (device-resident: one split launch; host: double-buffered chunks behind the copies) or, for a
 // streamed job, the blocks of one round.  Every later sweep must count what the first one counted.
-// Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.
-uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_budget_set, PassOut &acc)
+// Fills `acc` (sums over passes, acc.block = all result rows) and returns the number of passes.  `shared`: a job run while
+// an ARIMA pass is parked (interleave), whose last round stays open until its passes are done.
+uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_budget_set, bool shared, PassOut &acc)
 {
     cudaStream_t st = ctx->stream;
     const bool stream = job->stream;
@@ -2606,10 +2668,12 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     if (largest(P) > cap) too_big(largest(kMaxPasses));
     bool loaded = !stored && !dropped && P == P0 && got0 <= pc.cap;     // pass (0, P) is in the pass columns already
     // a streamed round stays open until the engine knows whether another sweep (round) follows: one does while a queued
-    // pass has rows that are not in the store
-    auto finish_round = [&](bool more) {
-        if (!open) return;
-        close_round(job, !stored && more);
+    // pass has rows that are not in the store.  A shared job's last round stays open until `done`: should a pass not fit
+    // the reserve, the caller has not been told its input is complete and delivers the rows again in the job's turn.
+    auto finish_round = [&](bool more, bool done = false) {
+        const bool again = !stored && more;
+        if (!open || (shared && !again && !done)) return;
+        close_round(job, again);
         open = false;
     };
     if (stored)
@@ -2641,7 +2705,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         return false;
     };
     const uint32_t passes = run_pass_queue(ctx, job, P, acc, run_one);
-    finish_round(false);
+    finish_round(false, true);
     if (text) tk.export_names();
     return passes;
 }
@@ -2920,9 +2984,11 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
     const tad_columns &hc = job->cols;     // a streamed job's first push writes it: not read here for streams
     const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
-    const uint64_t host_budget = store_trim(ctx);      // the job's one read of the host budget
-    // fit sharing: a single-GPU ARIMA tad_submit job plans in the budget less the reserve, and its fit yields
-    job->share = !reserve && !job->stream && ctx->cfg.world_size == 1 && job->spec.algo == TAD_ALGO_ARIMA ? ctx->fit_share.load() : 0;
+    const uint64_t host_budget = reserve ? store_share(ctx) : store_trim(ctx);      // the job's one read of the host budget
+    // fit sharing: a single-GPU ARIMA job, submitted or streamed with TAD_FLAG_SHARE, plans in the budget less the reserve,
+    // and its fit yields
+    const bool may_share = !job->stream || (job->spec.flags & TAD_FLAG_SHARE);
+    job->share = !reserve && may_share && ctx->cfg.world_size == 1 && job->spec.algo == TAD_ALGO_ARIMA ? ctx->fit_share.load() : 0;
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
@@ -2933,10 +2999,17 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
         CU(cudaMemGetInfo(&free_b, &total_b));
         return free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
     };
+    auto less_reserve = [&](uint64_t b) {
+        if (!job->share) return b;
+        if (b < job->share + kBudgetFloor)
+            fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes less the fit-sharing reserve of %llu bytes is below the "
+                 "64 MiB floor", (unsigned long long)b, (unsigned long long)job->share);
+        return b - job->share;
+    };
     if (job->stream) {
         // streamed input always runs through the pass columns (one pass when it fits), under the budget
         set_progress(job, TAD_STATE_RUNNING, 0);
-        budget = context_budget();
+        budget = less_reserve(context_budget());
         ctx->limit = budget;
         free_workspace(ctx);
         split = true;
@@ -2944,13 +3017,7 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
         budget = multi_budget;          // run_passes_multi applies it once the plan has freed the exported buffer
         free_workspace(ctx);
     } else if (ctx->cfg.world_size == 1 && R > 0) {
-        budget = context_budget();
-        if (job->share) {
-            if (budget < job->share + kBudgetFloor)
-                fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes less the fit-sharing reserve of %llu bytes is below the "
-                     "64 MiB floor", (unsigned long long)budget, (unsigned long long)job->share);
-            budget -= job->share;
-        }
+        budget = less_reserve(context_budget());
         PipeShape s = one_gpu_shape(ctx, job, R, true);
         s.host = hc.mem != TAD_MEM_DEVICE ? &hc : nullptr;
         auto bufs = pipe_bufs(ctx, pipe_sizes(s));
@@ -2983,7 +3050,7 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
             split = true;
         }
     }
-    if (split) passes = run_passes(ctx, job, budget, host_budget, acc);
+    if (split) passes = run_passes(ctx, job, budget, host_budget, reserve != 0, acc);
     publish_rows(job, acc.block, acc.out_rows);
     ctx->limit = 0;
     {
@@ -3010,32 +3077,44 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
 }
 
 // Runs `job` and reports a failure on it.  `reserve` (interleave): false when the job failed with TAD_ERR_NOMEM inside
-// the reserve; it is then SCHEDULED again with no progress, is not run beside a fit again, and waits for its turn.
+// the reserve; it is then SCHEDULED again with no progress, is not run beside a fit again, and waits for its turn.  A
+// streamed one first has its round in progress closed with again = 1 (discard_round) and starts again from its first
+// round, with empty dictionaries.
 bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve)
 {
+    JobFail f;
     try {
         run_job(ctx, job, reserve);
-    } catch (const JobFail &f) {
-        // nothing of this job may still be reading the caller's columns once it is reported FAILED
-        cudaStreamSynchronize(ctx->copy_stream);
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->d2h_stream);
-        cudaGetLastError();
-        TextKeys::release(ctx);
-        std::lock_guard<std::mutex> lk(job->mu);
-        if (reserve && f.code == TAD_ERR_NOMEM && !job->cancel.load()) {
+        return true;
+    } catch (const JobFail &e) {
+        f = e;
+    }
+    // nothing of this job may still be reading the caller's columns once it is reported FAILED
+    cudaStreamSynchronize(ctx->copy_stream);
+    cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(ctx->d2h_stream);
+    cudaGetLastError();
+    TextKeys::release(ctx);
+    if (reserve && f.code == TAD_ERR_NOMEM && !job->cancel.load()) {
+        try {
+            if (job->stream) discard_round(job);
+            std::lock_guard<std::mutex> lk(job->mu);
             job->no_interleave = true;
             job->st.state = TAD_STATE_SCHEDULED;
             job->st.completed_stages = 0;
             job->prog = tad_progress{};
+            job->round_rows = job->stored_rows = 0;
             return false;
+        } catch (const JobFail &e) {       // cancelled, or a bad block, while the round was taken to its end
+            f = e;
         }
-        job->st.state = TAD_STATE_FAILED;
-        job->st.error = f.code;
-        snprintf(job->st.err_msg, sizeof(job->st.err_msg), "%s", f.msg);
-        job->st.total_ms = now_ms() - job->t_submit;
-        job->cv.notify_all();
     }
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->st.state = TAD_STATE_FAILED;
+    job->st.error = f.code;
+    snprintf(job->st.err_msg, sizeof(job->st.err_msg), "%s", f.msg);
+    job->st.total_ms = now_ms() - job->t_submit;
+    job->cv.notify_all();
     return true;
 }
 

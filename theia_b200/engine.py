@@ -302,7 +302,8 @@ class TadEngine:
     def set_fit_sharing(self, reserve: int):
         """Single GPU (tad_set_fit_sharing): with a nonzero reserve (at least 64 MiB) an ARIMA job's fit phase yields to
         queued EWMA and DBSCAN jobs, which run in the reserve while it is parked; the ARIMA job plans in the memory
-        budget less the reserve.  0 (default) = off: jobs run in submit order."""
+        budget less the reserve.  Streamed jobs take part when submitted with ``share=True``.  0 (default) = off: jobs
+        run in submit order."""
         rc = self.lib.tad_set_fit_sharing(self.ctx, int(reserve))
         if rc != 0:
             raise TadError(rc, "tad_set_fit_sharing(%d)" % reserve)
@@ -322,12 +323,12 @@ class TadEngine:
         return self.alloc_columns(max(1, len(table["flow_end"]))).fill(table)
 
     @staticmethod
-    def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep):
+    def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep, share=False):
         spec = L.TadJobSpec()
         spec.algo = L.ALGOS[algo] if isinstance(algo, str) else int(algo)
         spec.reducer = reducer
         spec.start_time, spec.end_time = int(start_time), int(end_time)
-        spec.flags = L.TAD_FLAG_EMIT_ALL if emit_all else 0
+        spec.flags = (L.TAD_FLAG_EMIT_ALL if emit_all else 0) | (L.TAD_FLAG_SHARE if share else 0)
         spec.id = tad_id.encode()[:39]
         spec.global_rows = int(global_rows)
         if len(ns_ignore):
@@ -354,13 +355,14 @@ class TadEngine:
 
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
-                      check: bool = True, text_filter=None) -> StreamJob:
+                      check: bool = True, text_filter=None, share: bool = False) -> StreamJob:
         """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
         ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
         (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
-        for every row."""
+        for every row.  ``share``: TAD_FLAG_SHARE, the job takes part in fit sharing (set_fit_sharing): an ARIMA job's
+        fit yields, an EWMA or DBSCAN job may run while a fit is parked."""
         keep = []
-        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep)
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share)
         h = C.c_void_p()
         if text_filter is None:
             rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
