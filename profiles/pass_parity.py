@@ -9,13 +9,17 @@ text slots' dictionaries, and a SHA-256 of the result rows sorted by every colum
 The matrix: every input kind (device-resident, pinned host, streamed 65,536-row blocks hinted / unhinted / over-hinted,
 streamed with a host row store that holds the round and one that falls back, streamed text keys with one IPv6 address in
 five, streamed with string predicates) at no budget, a two-pass budget and the 64 MiB floor; then EWMA, DBSCAN and a small
-ARIMA table in passes, oversized-bucket spills under the floor, and a job cancelled while it waits behind another.
+ARIMA table in passes, oversized-bucket spills under the floor, and a job cancelled while it waits behind another; then
+fit sharing: an ARIMA fit that parks for a submitted EWMA job and a streamed DBSCAN job, a queued job too large for the
+reserve, and a cancel of the parked ARIMA job.
 Run it with each build in the same GPU session; --compare prints every difference and exits 1 if there is one."""
 import argparse
 import hashlib
 import json
 import os
 import sys
+import threading
+import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
@@ -24,6 +28,8 @@ if ROOT not in sys.path:
 MB = 1 << 20
 TWO_PASSES = 150 * MB          # the 2M-row table runs in two passes under it
 DBSCAN_TWO_PASSES = 100 * MB   # DBSCAN's one pass is smaller: it needs a lower budget for two passes or more
+SHARE_BUDGET = 1024 * MB       # fit sharing: the ARIMA job plans in it less the reserve
+SHARE_RESERVE = 256 * MB
 BLOCK = 65536
 STATUS = ("state", "error", "err_msg", "completed_stages", "total_stages", "rows_in", "rows_kept", "rows_owned", "points",
           "series", "result_rows", "spill_rows", "gpu_launches")
@@ -71,8 +77,9 @@ def text_column(values):
     return b"".join(enc[i] for i in inv), starts[::32].copy()
 
 
-def job_record(job, st):
-    rec = {k: st[k] for k in STATUS}
+def job_record(job, st, timed=()):
+    """`timed`: status fields left out because they depend on timing (a yielding fit's resume launches)."""
+    rec = {k: st[k] for k in STATUS if k not in timed}
     rec["progress"] = job.progress()
     if st["state"] == "COMPLETED":
         rec["memory"] = job.memory()
@@ -89,32 +96,42 @@ def run_table(eng, cols, budget, **kw):
         job.release()
 
 
-def run_stream(eng, table, budget, hint, host=0, text=False, **kw):
-    """One streamed job: 65,536-row numpy blocks; with `text` the address columns go as text slots."""
-    eng.set_memory_budget(budget)
-    eng.set_host_budget(host)
-    n = len(table["flow_end"])
+def stream_blocks(table, text=False):
+    """The table in 65,536-row numpy blocks; with `text` the address columns go as text slots."""
     blocks = []
-    for lo in range(0, n, BLOCK):
+    for lo in range(0, len(table["flow_end"]), BLOCK):
         b = {k: v[lo:lo + BLOCK] for k, v in table.items()}
         txt = None
         if text:
             txt = {s: text_column(b[s]) for s in ("src_ip", "dst_ip")}
             b["src_ip"] = b["dst_ip"] = None
         blocks.append((b, txt))
+    return blocks
+
+
+def feed(job, blocks, again_seq):
+    """Every round of a streamed job until its input is complete; what each tad_stream_end returned goes to again_seq."""
+    again = True
+    while again and len(again_seq) < 200:
+        try:
+            for b, txt in blocks:
+                job.push(b, text=txt)
+            again = job.end()
+        except Exception as e:           # a failed job: its status tells why
+            again_seq.append("error: %s" % e)
+            break
+        again_seq.append(again)
+
+
+def run_stream(eng, table, budget, hint, host=0, text=False, **kw):
+    """One streamed job: 65,536-row numpy blocks; with `text` the address columns go as text slots."""
+    eng.set_memory_budget(budget)
+    eng.set_host_budget(host)
+    blocks = stream_blocks(table, text)
     job = eng.submit_stream(rows_hint=hint, **kw)
     again_seq = []
     try:
-        again = True
-        while again and len(again_seq) < 200:
-            try:
-                for b, txt in blocks:
-                    job.push(b, text=txt)
-                again = job.end()
-            except Exception as e:           # a failed job: its status tells why
-                again_seq.append("error: %s" % e)
-                break
-            again_seq.append(again)
+        feed(job, blocks, again_seq)
         rec = job_record(job, job.wait(check=False))
         rec["again"] = again_seq
         if text and rec["state"] == "COMPLETED":
@@ -124,6 +141,72 @@ def run_stream(eng, table, budget, hint, host=0, text=False, **kw):
     finally:
         job.release()
         eng.set_host_budget(0)
+
+
+def wait_fitting(job, timeout=120.0):
+    """Until the ARIMA job's fit phase has started (or it has ended)."""
+    t0 = time.time()
+    while job.progress()["fits_done"] == 0 and job.poll()["state"] in ("SCHEDULED", "RUNNING"):
+        if time.time() - t0 > timeout:
+            raise RuntimeError("the fit phase did not start")
+        time.sleep(0.002)
+
+
+def run_sharing(eng, arima, cols, table, big):
+    """Fit sharing: the ARIMA job on `arima` parks its pass for queued jobs, which run in the reserve (`cols`: `table` in
+    host columns; `big`: a table whose 1/64 hash range does not fit 64 MiB).  Only what does not depend on when the
+    yields come is recorded: not the ARIMA job's launches, its yield count or its progress after a cancel."""
+    out = {}
+    blocks = stream_blocks(table)
+    eng.set_memory_budget(SHARE_BUDGET)
+    eng.set_fit_sharing(SHARE_RESERVE)
+    try:
+        # an EWMA job and a flagged streamed DBSCAN job, queued together once the fit has started, run in its yield
+        job = eng.submit(arima, algo="ARIMA", emit_all=True)
+        wait_fitting(job)
+        ewma = eng.submit(cols, emit_all=True)
+        dbscan = eng.submit_stream(algo="DBSCAN", rows_hint=len(table["flow_end"]), share=True)
+        again_seq = []
+        fd = threading.Thread(target=feed, args=(dbscan, blocks, again_seq))
+        fd.start()
+        out["share/arima"] = job_record(job, job.wait(check=False), timed=("gpu_launches",))
+        out["share/arima"]["yielded"] = job.yields()["yields"] >= 1
+        out["share/ewma"] = job_record(ewma, ewma.wait(check=False))
+        fd.join()
+        out["share/dbscan-stream"] = job_record(dbscan, dbscan.wait(check=False))
+        out["share/dbscan-stream"]["again"] = again_seq
+        for j in (job, ewma, dbscan):
+            j.release()
+
+        # a job too large for a 64 MiB reserve: it goes back to its place in the queue and runs after the fit
+        eng.set_fit_sharing(64 * MB)
+        job = eng.submit(arima, algo="ARIMA", emit_all=True)
+        wait_fitting(job)
+        q = eng.submit(big)
+        out["share-too-large/arima"] = job_record(job, job.wait(check=False), timed=("gpu_launches",))
+        out["share-too-large/arima"]["yielded"] = job.yields()["yields"] >= 1
+        out["share-too-large/queued"] = job_record(q, q.wait(check=False))
+        job.release()
+        q.release()
+
+        # a cancel of the parked ARIMA job: it fails once the job run in its place has ended
+        eng.set_fit_sharing(SHARE_RESERVE)
+        job = eng.submit(arima, algo="ARIMA", emit_all=True)
+        wait_fitting(job)
+        q = eng.submit(cols, emit_all=True)
+        t0 = time.time()
+        while q.poll()["state"] == "SCHEDULED" and time.time() - t0 < 5.0:
+            time.sleep(0.001)
+        job.cancel()
+        st = job.wait(check=False)
+        out["share-cancel/arima"] = {k: st[k] for k in ("state", "error", "err_msg")}
+        out["share-cancel/in-its-place"] = job_record(q, q.wait(check=False))
+        job.release()
+        q.release()
+    finally:
+        eng.set_fit_sharing(0)
+        eng.set_memory_budget(0)
+    return out
 
 
 def run_matrix():
@@ -196,6 +279,20 @@ def run_matrix():
         first.release()
         second.release()
         cols.free()
+
+        # ---- fit sharing ----
+        # a fit phase of about 1.4 s, long enough to be parked
+        a = synth.torch_cols_to_numpy(synth.make_flows_torch(20000, 100, seed=67, device=torch.device("cuda", 0),
+                                                             noisy=True))
+        arima, cols = eng.columns_from_numpy(a), eng.columns_from_numpy(t)
+        big_t = synth.make_flows_torch(500_000, 100, seed=31, device=torch.device("cuda", 0))    # 5e7 rows
+        torch.cuda.synchronize()
+        big = DeviceColumns(int(big_t["value"].numel()), {k: v.data_ptr() for k, v in big_t.items()})
+        big.keepalive = big_t
+        out.update(run_sharing(eng, arima, cols, t, big))
+        arima.free()
+        cols.free()
+        big.free()
     return out
 
 

@@ -279,6 +279,12 @@ struct tad_ctx {
         uint32_t cap = 0;                           // table slots (0: no dictionary yet)
         uint64_t names_ub = 0, bytes_ub = 0;        // upper bounds of its names / arena bytes, exact after each readback
         std::vector<DevBuf *> bufs() { return {&slots, &minrow, &slot_id, &arena, &off, &hash, &state, &keep, &pat}; }
+        void swap_sizes(TextSlot &o)                // a parked slot's sizes are parked with its buffers
+        {
+            std::swap(cap, o.cap);
+            std::swap(names_ub, o.names_ub);
+            std::swap(bytes_ub, o.bytes_ub);
+        }
     } tdict[2];
     DevBuf tstage, tscratch;                        // a chunk's marks and text bytes; the encode scratch
 };
@@ -315,68 +321,135 @@ struct JobFail {
 size_t alloc_bytes(size_t bytes) { return (bytes + bytes / 16 + 256 + 255) & ~size_t(255); }   // what ensure() asks for
 size_t exact_bytes(size_t bytes) { return (bytes + 255) & ~size_t(255); }
 
-// Grow-only workspace buffer.  Under a budget (ctx->limit != 0) the 1/16 slack is dropped where it would not fit, and
-// growth past the budget is a planning error: the planner sized every buffer it can know in advance.
-void ensure(tad_ctx *ctx, DevBuf &b, size_t bytes)
+// Whether the workspace may grow by `extra` bytes inside the budget (always, without one).
+bool can_grow(const tad_ctx *ctx, size_t extra) { return !ctx->limit || ctx->held + extra <= ctx->limit; }
+
+// Whether ensure(b, bytes) stays inside the budget.
+bool fits(const tad_ctx *ctx, const DevBuf &b, size_t bytes)
 {
-    if (bytes <= b.cap) return;
-    const size_t rest = ctx->held - b.cap;
-    if (b.p) CU(cudaFree(b.p));
-    b.p = nullptr;
-    b.cap = 0;
-    ctx->held = rest;
+    return bytes <= b.cap || can_grow(ctx, exact_bytes(bytes) - b.cap);
+}
+
+// The allocate step: a new block of at least `bytes`, counted in `held` and `peak`.  Under a budget (ctx->limit != 0) the
+// 1/16 slack is dropped where it would not fit, and growth past the budget is a planning error: the planner sized every
+// buffer it can know in advance.  A failed cudaMalloc is retried once at the exact size.
+DevBuf alloc_buf(tad_ctx *ctx, size_t bytes)
+{
     size_t want = alloc_bytes(bytes);
-    if (ctx->limit && rest + want > ctx->limit) want = exact_bytes(bytes);
-    if (ctx->limit && rest + want > ctx->limit)
-        fail(TAD_ERR_INTERNAL, "workspace would grow to %zu bytes, past the memory budget of %zu bytes", rest + want, ctx->limit);
-    cudaError_t e = cudaMalloc(&b.p, want);
-    if (e != cudaSuccess) {
+    if (!can_grow(ctx, want)) want = exact_bytes(bytes);
+    if (!can_grow(ctx, want))
+        fail(TAD_ERR_INTERNAL, "workspace would grow to %zu bytes, past the memory budget of %zu bytes", ctx->held + want, ctx->limit);
+    DevBuf b;
+    if (cudaMalloc(&b.p, want) != cudaSuccess) {
         cudaGetLastError();
         want = exact_bytes(bytes);
         CU(cudaMalloc(&b.p, want));
     }
     b.cap = want;
-    ctx->held = rest + want;
+    ctx->held += want;
     ctx->peak = std::max(ctx->peak, ctx->held);
+    return b;
 }
 
-// Whether ensure(b, bytes) stays inside the budget (always, without one).
-bool fits(const tad_ctx *ctx, const DevBuf &b, size_t bytes)
+// The free step: `b` is freed and empty, and `held` leaves it out.  Returns the cudaFree's error, for the callers that
+// free on a context with a sticky error (a failed job's cleanup) and go on.
+cudaError_t drop_buf(tad_ctx *ctx, DevBuf &b)
 {
-    return !ctx->limit || bytes <= b.cap || ctx->held - b.cap + exact_bytes(bytes) <= ctx->limit;
+    const cudaError_t e = b.p ? cudaFree(b.p) : cudaSuccess;
+    ctx->held -= b.cap;
+    b = DevBuf{};
+    return e;
+}
+
+void free_buf(tad_ctx *ctx, DevBuf &b) { CU(drop_buf(ctx, b)); }
+
+// Grow-only workspace buffer (freed before it is allocated again).
+void ensure(tad_ctx *ctx, DevBuf &b, size_t bytes)
+{
+    if (bytes <= b.cap) return;
+    free_buf(ctx, b);
+    b = alloc_buf(ctx, bytes);
 }
 
 // A pass whose oversized-bucket spill scratch or result buffer (sizes known only while it runs) would not fit the budget:
 // the job driver splits it by the next hash bit.
 struct PassSplit {};
 
-// Every workspace buffer of a single-GPU job except the exported multi-GPU buffer and its mappings.
-std::vector<DevBuf *> workspace_bufs(tad_ctx *ctx)
+// Lifetimes of the workspace buffers (workspace_bufs).  kJobs and kPasses name the events a buffer is kept across (the
+// others free it); kParked, what a parked ARIMA pass takes out of the context.
+constexpr int kJobs = 1;     // kept when a job ends: all but the text key dictionaries, which live for one job
+constexpr int kPasses = 2;   // kept across the passes of a job: what every pass reads (free_pass_buffers frees the rest)
+constexpr int kParked = 4;   // moved out of the context while an ARIMA pass is parked (Parked), the rest left for reuse
+
+// Every workspace buffer with its lifetime, the exported multi-GPU buffer `xbuf` apart (ranks agree on its size).
+//
+// Kept across passes: the pass columns d_col[0..8), the staging, the pass counters, the stats words, the ns_ignore list,
+// the text key dictionaries and their staging, and `small` (run_pipeline ensures it first anyway).
+//
+// Parked: a parked ARIMA pass moves out the buffers the rest of its fit, its detect_arima and its pass driver read
+// (ctx->held leaves them out).  Everything else stays for the jobs run meanwhile to reuse: each plans under the reserve
+// and frees the workspace first when it does not fit there (run_job), so the parked bytes plus theirs stay inside the
+// budget the ARIMA job planned in plus the reserve.  Nothing is freed before they run, which would sit in their wait
+// (cudaFree); their workspace is freed at the restore, after they have completed.  The parked buffers:
+//   the fit and detect_arima: the series entries (`entries` after the optimistic partition, in place in `part` after the
+//     exact one), offsets, sbase, csr_v, csr_t, ar_y, ar_pred, ar_lam, the resume points ar_res, the stats words (fit
+//     counters, cancel word, result count) and outb, into which the pass's result layout points;
+//   the pass driver (run_passes), which took pointers to them at its start: the pass columns d_col[0..8), the staging,
+//     the pass counters and the ns_ignore list;
+//   a streamed job's text key slots: both dictionaries (table, arena, offsets, hashes, keep bytes, pattern, state words,
+//     with their sizes), which its later rounds look names up in and its end copies out, so its ids stay the same, and
+//     the text staging and encode scratch its sweeps take as sized.  They were planned in the budget less the reserve.
+// What else a parked streamed pass needs is not in the workspace and no interleaved job touches it: the job's stream
+// input state (tad_job::in: its feeder, blocked in a push or end call, goes on with the same round) and the host row
+// store pages of its passes (its RowStore's lists).  An interleaved job takes store pages only from the free list and
+// new slabs within the host budget less the slabs held (store_share), and frees no slab.
+// What the interleaved jobs may overwrite is rebuilt before the ARIMA job reads it again:
+//   hist, cursor, big_list, big_base, cls_list, nsb, npb, csr_p, ovf, spill, sortb, dbx, dbi, small: the partition and
+//     group scratch, which the next pass's pipeline ensures and writes before reading (scan_sync: freed at the restore, so
+//     that pipeline allocates and zeroes it again for the scan's epochs);
+//   d_col[8..10): a one-pass job's host namespace columns, read before the fit only;
+//   h_stats and h_small: read back again after the fit (read_stats) and after every sweep (the counts);
+//   h_fits: the fit counters are published before the park;
+//   ev: the interleaved jobs record ev_alt, so the pass's phase events survive; the other events of a sweep are
+//     recorded in that sweep before they are waited for;
+//   limit, peak and store_peak: restored.
+std::vector<std::pair<DevBuf *, int>> workspace_bufs(tad_ctx *ctx)
 {
-    std::vector<DevBuf *> v = {&ctx->hist, &ctx->offsets, &ctx->cursor, &ctx->big_list, &ctx->big_base, &ctx->cls_list,
-                               &ctx->csr_p, &ctx->stats, &ctx->part, &ctx->csr_v, &ctx->csr_t, &ctx->nsb, &ctx->npb,
-                               &ctx->sbase, &ctx->outb, &ctx->ns_ignore, &ctx->spill, &ctx->dbx, &ctx->dbi, &ctx->exch,
-                               &ctx->scan_sync, &ctx->small, &ctx->hist_all, &ctx->seg_off, &ctx->seg_total, &ctx->entries,
-                               &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ar_res, &ctx->ovf, &ctx->sortb, &ctx->xcnt, &ctx->xtotal,
-                               &ctx->stage, &ctx->pcnt, &ctx->ostage, &ctx->tstage, &ctx->tscratch};
-    for (auto &t : ctx->tdict)
-        for (DevBuf *b : t.bufs()) v.push_back(b);
-    for (int i = 0; i < 10; i++) v.push_back(&ctx->d_col[i]);
+    tad_ctx &c = *ctx;
+    std::vector<std::pair<DevBuf *, int>> v;
+    auto add = [&](int life, const std::vector<DevBuf *> &bufs) {
+        for (DevBuf *b : bufs) v.push_back({b, life});
+    };
+    add(kJobs, {&c.hist, &c.cursor, &c.big_list, &c.big_base, &c.cls_list, &c.csr_p, &c.nsb, &c.npb, &c.ovf, &c.spill,
+                &c.sortb, &c.dbx, &c.dbi, &c.scan_sync, &c.exch, &c.hist_all, &c.seg_off, &c.seg_total, &c.xcnt,
+                &c.xtotal, &c.ostage, &c.d_col[8], &c.d_col[9]});
+    add(kJobs | kPasses, {&c.small});
+    add(kJobs | kParked, {&c.part, &c.entries, &c.offsets, &c.sbase, &c.csr_v, &c.csr_t, &c.ar_y, &c.ar_pred, &c.ar_lam,
+                          &c.ar_res, &c.outb});
+    add(kJobs | kPasses | kParked, {&c.stats, &c.stage, &c.pcnt, &c.ns_ignore, &c.tstage, &c.tscratch});
+    for (int i = 0; i < 8; i++) add(kJobs | kPasses | kParked, {&c.d_col[i]});
+    for (auto &t : c.tdict) add(kPasses | kParked, t.bufs());
     return v;
 }
 
-void free_buf(tad_ctx *ctx, DevBuf &b)
+// The free step over the list: every workspace buffer whose lifetime has no flag of `keep` is freed, also on a context
+// with a sticky error; returns the first error.  A text key slot without buffers has no dictionary: its sizes go too.
+cudaError_t free_bufs(tad_ctx *ctx, int keep = 0)
 {
-    if (b.p) CU(cudaFree(b.p));
-    ctx->held -= b.cap;
-    b = DevBuf{};
+    cudaError_t e = cudaSuccess;
+    for (auto [b, life] : workspace_bufs(ctx)) {
+        const cudaError_t f = (life & keep) ? cudaSuccess : drop_buf(ctx, *b);
+        if (e == cudaSuccess) e = f;
+    }
+    for (auto &t : ctx->tdict)
+        if (!t.state.p) {
+            t.cap = 0;
+            t.names_ub = t.bytes_ub = 0;
+        }
+    return e;
 }
 
-void free_workspace(tad_ctx *ctx)
-{
-    for (DevBuf *b : workspace_bufs(ctx)) free_buf(ctx, *b);
-    for (auto &t : ctx->tdict) t.cap = 0;
-}
+void free_workspace(tad_ctx *ctx) { CU(free_bufs(ctx)); }
 
 PinnedBlock take_pinned(tad_ctx *ctx, size_t bytes)
 {
@@ -626,33 +699,8 @@ bool interleave_waiting(tad_ctx *ctx)
     return false;
 }
 
-// A parked ARIMA pass: the buffers the rest of its fit, its detect_arima and its pass driver read are moved out of the
-// context into `bufs` (ctx->held leaves them out).  Everything else stays for the jobs run meanwhile to reuse: each plans
-// under the reserve and frees the workspace first when it does not fit there (run_job), so the parked bytes plus theirs
-// stay inside the budget the ARIMA job planned in plus the reserve.  Nothing is freed before they run, which would sit
-// in their wait (cudaFree); their workspace is freed at the restore, after they have completed.  The list:
-//   the fit and detect_arima: the series entries (`entries` after the optimistic partition, in place in `part` after the
-//     exact one), offsets, sbase, csr_v, csr_t, ar_y, ar_pred, ar_lam, the resume points ar_res, the stats words (fit
-//     counters, cancel word, result count) and outb, into which the pass's result layout points;
-//   the pass driver (run_passes), which took pointers to them at its start: the pass columns d_col[0..8), the staging,
-//     the pass counters and the ns_ignore list;
-//   a streamed job's text key slots: both dictionaries (table, arena, offsets, hashes, keep bytes, pattern, state words,
-//     with their sizes), which its later rounds look names up in and its end copies out, so its ids stay the same, and
-//     the text staging and encode scratch its sweeps take as sized.  They were planned in the budget less the reserve.
-// What else a parked streamed pass needs is not in the workspace and no interleaved job touches it: the job's stream
-// input state (tad_job::in: its feeder, blocked in a push or end call, goes on with the same round) and the host row
-// store pages of its passes (its RowStore's lists).  An interleaved job takes store pages only from the free list and
-// new slabs within the host budget less the slabs held (store_share), and frees no slab.
-// What the interleaved jobs may overwrite is rebuilt before the ARIMA job reads it again:
-//   hist, cursor, big_list, big_base, cls_list, nsb, npb, csr_p, ovf, spill, sortb, dbx, dbi, small: the partition and
-//     group scratch, which the next pass's pipeline ensures and writes before reading (scan_sync: freed at the restore, so
-//     that pipeline allocates and zeroes it again for the scan's epochs);
-//   d_col[8..10): a one-pass job's host namespace columns, read before the fit only;
-//   h_stats and h_small: read back again after the fit (read_stats) and after every sweep (the counts);
-//   h_fits: the fit counters are published before the park;
-//   ev: the interleaved jobs record ev_alt, so the pass's phase events survive; the other events of a sweep are
-//     recorded in that sweep before they are waited for;
-//   limit, peak and store_peak: restored.
+// A parked ARIMA pass: the buffers workspace_bufs() marks kParked, with the dictionaries' sizes, are moved out of the
+// context into `bufs` and `dict`, and ctx->held leaves them out.
 struct Parked {
     tad_ctx *ctx;
     std::vector<std::pair<DevBuf *, DevBuf>> bufs;
@@ -662,25 +710,15 @@ struct Parked {
 
     Parked(tad_ctx *c) : ctx(c), limit(c->limit), peak(c->peak), store_peak(c->store_peak)
     {
-        std::vector<DevBuf *> keep = {&ctx->part, &ctx->entries, &ctx->offsets, &ctx->sbase, &ctx->csr_v, &ctx->csr_t,
-                                      &ctx->ar_y, &ctx->ar_pred, &ctx->ar_lam, &ctx->ar_res, &ctx->stats, &ctx->outb,
-                                      &ctx->stage, &ctx->pcnt, &ctx->ns_ignore, &ctx->tstage, &ctx->tscratch};
-        for (int i = 0; i < 8; i++) keep.push_back(&ctx->d_col[i]);
-        for (auto &t : ctx->tdict)
-            for (DevBuf *b : t.bufs()) keep.push_back(b);
         CU(cudaStreamSynchronize(ctx->stream));
         CU(cudaStreamSynchronize(ctx->copy_stream));
-        for (int t = 0; t < 2; t++) {
-            dict[t] = ctx->tdict[t];
-            ctx->tdict[t].cap = 0;
-            ctx->tdict[t].names_ub = ctx->tdict[t].bytes_ub = 0;
-        }
-        for (DevBuf *b : keep) {
-            if (!b->p) continue;
+        for (auto [b, life] : workspace_bufs(ctx)) {
+            if (!(life & kParked) || !b->p) continue;
             bufs.push_back({b, *b});
             ctx->held -= b->cap;
             *b = DevBuf{};
         }
+        for (int t = 0; t < 2; t++) ctx->tdict[t].swap_sizes(dict[t]);
         out = true;
         std::swap(ctx->ev, ctx->ev_alt);
     }
@@ -692,25 +730,14 @@ struct Parked {
         std::swap(ctx->ev, ctx->ev_alt);
         cudaStreamSynchronize(ctx->stream);
         cudaStreamSynchronize(ctx->copy_stream);
-        for (DevBuf *b : workspace_bufs(ctx))
-            if (b->p) cudaFree(b->p);
-        for (DevBuf *b : workspace_bufs(ctx)) *b = DevBuf{};
-        for (auto &t : ctx->tdict) t.cap = 0;
-        ctx->held = 0;
-        for (auto &b : bufs) {
-            if (drop) {
-                cudaFree(b.second.p);
-                continue;
-            }
-            *b.first = b.second;
-            ctx->held += b.second.cap;
+        free_bufs(ctx);
+        for (auto [b, parked] : bufs) {
+            *b = parked;
+            ctx->held += parked.cap;
         }
         bufs.clear();
-        for (int t = 0; t < 2 && !drop; t++) {
-            ctx->tdict[t].cap = dict[t].cap;
-            ctx->tdict[t].names_ub = dict[t].names_ub;
-            ctx->tdict[t].bytes_ub = dict[t].bytes_ub;
-        }
+        for (int t = 0; t < 2; t++) ctx->tdict[t].swap_sizes(dict[t]);
+        if (drop) free_bufs(ctx);
         ctx->limit = limit;
         ctx->peak = std::max(peak, ctx->held);
         ctx->store_peak = store_peak;
@@ -1820,20 +1847,11 @@ void discard_round(tad_job *job)
 void grow_keep(tad_ctx *ctx, DevBuf &b, size_t bytes, size_t keep, cudaStream_t st)
 {
     if (bytes <= b.cap) return;
-    size_t want = alloc_bytes(bytes);
-    if (ctx->limit && ctx->held + want > ctx->limit) want = exact_bytes(bytes);
-    if (ctx->limit && ctx->held + want > ctx->limit)
-        fail(TAD_ERR_INTERNAL, "workspace would grow to %zu bytes, past the memory budget of %zu bytes", ctx->held + want, ctx->limit);
-    void *p = nullptr;
-    CU(cudaMalloc(&p, want));
-    ctx->held += want;
-    ctx->peak = std::max(ctx->peak, ctx->held);
-    if (keep) CU(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, st));
+    const DevBuf n = alloc_buf(ctx, bytes);
+    if (keep) CU(cudaMemcpyAsync(n.p, b.p, keep, cudaMemcpyDeviceToDevice, st));
     CU(cudaStreamSynchronize(st));
-    if (b.p) CU(cudaFree(b.p));
-    ctx->held -= b.cap;
-    b.p = p;
-    b.cap = want;
+    free_buf(ctx, b);
+    b = n;
 }
 
 constexpr uint64_t kMaxPassRows = (1ull << 32) - 2;   // the pipeline's offsets are u32: the row cap of one pass
@@ -1912,9 +1930,9 @@ struct TextKeys {
     // room for `extra` more dictionary bytes under the budget: in the first round the pass columns give way
     void room(size_t extra)
     {
-        if (!ctx->limit || ctx->held + extra <= ctx->limit) return;
+        if (can_grow(ctx, extra)) return;
         if (yield && yield->cap) yield->drop();
-        if (ctx->held + extra > ctx->limit)
+        if (!can_grow(ctx, extra))
             fail(TAD_ERR_NOMEM, "the text key dictionaries need %zu bytes of device workspace (%zu held); with the job's "
                  "staging that passes the memory budget of %llu bytes", dict_bytes() + extra, dict_bytes(),
                  (unsigned long long)budget);
@@ -1952,7 +1970,7 @@ struct TextKeys {
     {
         if (bytes <= b.cap) return;
         // geometric growth where the budget allows it, else the exact size
-        if (!ctx->limit || ctx->held + exact_bytes(2 * b.cap) <= ctx->limit) bytes = std::max(bytes, 2 * b.cap);
+        if (can_grow(ctx, exact_bytes(2 * b.cap))) bytes = std::max(bytes, 2 * b.cap);
         room(exact_bytes(bytes));
         grow_keep(ctx, b, bytes, keep, ctx->copy_stream);
     }
@@ -2111,20 +2129,7 @@ struct TextKeys {
     }
     // A dictionary lives for one job.  Every buffer is freed, also on a context with a sticky error (a failed job's
     // cleanup); returns the first error.
-    static cudaError_t release(tad_ctx *ctx)
-    {
-        cudaError_t e = cudaSuccess;
-        for (auto &t : ctx->tdict) {
-            for (DevBuf *b : t.bufs()) {
-                const cudaError_t f = b->p ? cudaFree(b->p) : cudaSuccess;
-                e = e == cudaSuccess ? f : e;
-                ctx->held -= b->cap;
-                *b = DevBuf{};
-            }
-            t.cap = 0;
-        }
-        return e;
-    }
+    static cudaError_t release(tad_ctx *ctx) { return free_bufs(ctx, kJobs); }
 };
 
 // One sweep over a job's input for pass (v, M): the rows that pass the job's filters are counted per residue (per owner
@@ -2399,18 +2404,8 @@ struct RowStore {
     }
 };
 
-// The buffers earlier passes grew are freed, except what every pass reads: the pass columns, the staging, the counters,
-// the ns_ignore list, the text key dictionaries and their staging, and `small` (run_pipeline ensures it first anyway).
-void free_pass_buffers(tad_ctx *ctx)
-{
-    for (DevBuf *b : workspace_bufs(ctx)) {
-        if (b == &ctx->stage || b == &ctx->pcnt || b == &ctx->stats || b == &ctx->ns_ignore || b == &ctx->small ||
-            (b >= ctx->d_col && b < ctx->d_col + 8) || b == &ctx->tstage || b == &ctx->tscratch ||
-            ((void *)b >= (void *)ctx->tdict && (void *)b < (void *)(ctx->tdict + 2)))
-            continue;
-        free_buf(ctx, *b);
-    }
-}
+// The buffers earlier passes grew are freed, except what every pass reads (kPasses).
+void free_pass_buffers(tad_ctx *ctx) { CU(free_bufs(ctx, kPasses)); }
 
 using PassList = std::deque<std::pair<uint32_t, uint32_t>>;
 
@@ -2534,10 +2529,10 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         if (host_budget && have + n > cap) return false;
         if (have + n > pc.cap) {
             const uint64_t want = std::min(cap, std::max(2 * pc.cap, have + n));
-            if (text && ctx->limit) {        // beside the dictionaries the columns may not grow: the round only counts
+            if (text) {                      // beside the dictionaries the columns may not grow: the round only counts
                 size_t grow = 0;
                 for (int i = 0; i < 8; i++) grow += has_col(job, i) ? exact_bytes(col_bytes(i, want)) : 0;
-                if (ctx->held + grow > ctx->limit) {
+                if (!can_grow(ctx, grow)) {
                     pc.drop();
                     count_only = true;
                     return true;
@@ -2554,8 +2549,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     // the pass columns overflow in the first round: their `have` rows go to the store first (counted already)
     auto switch_to_store = [&]() {
         // the out-stage was planned without the dictionaries: where it does not fit beside them, the round only counts
-        if (text && ctx->limit &&
-            ctx->held + exact_bytes(ostage_bytes) + (stage_bytes > ctx->stage.cap ? exact_bytes(stage_bytes) : 0) > ctx->limit) {
+        if (text && !can_grow(ctx, exact_bytes(ostage_bytes) + (stage_bytes > ctx->stage.cap ? exact_bytes(stage_bytes) : 0))) {
             count_only = true;
             return;
         }
@@ -3425,9 +3419,8 @@ void tad_shutdown(tad_ctx *ctx)
         if (peer_barrier(ctx) == 0) cudaStreamSynchronize(ctx->stream);
     }
     nccl_comm_destroy(&ctx->nccl);
-    if (ctx->xbuf.p) cudaFree(ctx->xbuf.p);
-    for (DevBuf *b : workspace_bufs(ctx))
-        if (b->p) cudaFree(b->p);
+    drop_buf(ctx, ctx->xbuf);
+    free_bufs(ctx);
     for (auto &b : ctx->pinned_pool) cudaFreeHost(b.p);
     for (auto &b : ctx->store_slabs) cudaFreeHost(b.p);
     if (ctx->h_chunk) cudaFreeHost(ctx->h_chunk);
