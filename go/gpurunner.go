@@ -67,9 +67,10 @@ type gpuJob struct {
 }
 
 type gpuJobRunner struct {
-	ctx   *C.tad_ctx
-	jobs  sync.Map    // id -> *gpuJob
-	share atomic.Bool // SetFitSharing turned fit sharing on: StartStream flags its jobs
+	ctx    *C.tad_ctx
+	jobs   sync.Map    // id -> *gpuJob
+	share  atomic.Bool // SetFitSharing turned fit sharing on: StartStream flags its jobs
+	beside atomic.Bool // SetFitBeside: Start flags its ARIMA jobs to fit beside a running fit
 }
 
 func newGPUJobRunner(device int) (*gpuJobRunner, error) {
@@ -113,6 +114,15 @@ func (r *gpuJobRunner) SetFitSharing(reserve uint64) error {
 	}
 	r.share.Store(reserve != 0)
 	return nil
+}
+
+// SetFitBeside lets an ARIMA job from Start fit beside another ARIMA job's fit while fit sharing is on (off by default):
+// Start flags its ARIMA jobs (TAD_FLAG_FIT_BESIDE), and a flagged job queued behind a running fit then runs in that
+// fit's reserve, its fit in one launch with the rest of the running one, instead of waiting for the whole fit phase.
+// The running fit keeps about half the GPU meanwhile.  Streamed jobs do not take part.  It takes effect for jobs that
+// start after the call.
+func (r *gpuJobRunner) SetFitBeside(on bool) {
+	r.beside.Store(on)
 }
 
 func algoCode(a string) C.int32_t {
@@ -192,6 +202,9 @@ func (r *gpuJobRunner) Start(spec JobSpec, in *FlowColumns) error {
 		// tad_submit copies the list: the Go slice need not outlive the call (cgo pins it for its duration)
 		js.n_ns_ignore = C.uint32_t(len(spec.NSIgnore))
 		js.ns_ignore = (*C.uint32_t)(unsafe.Pointer(&spec.NSIgnore[0]))
+	}
+	if r.beside.Load() && js.algo == C.TAD_ALGO_ARIMA {
+		js.flags |= C.TAD_FLAG_FIT_BESIDE
 	}
 	cid := C.CString(spec.ID)
 	C.strncpy(&js.id[0], cid, 39)

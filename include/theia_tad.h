@@ -61,6 +61,9 @@ typedef enum { TAD_MEM_HOST = 0, TAD_MEM_DEVICE = 1 } tad_mem;
 #define TAD_FLAG_EMIT_ALL 1u   /* emit every point with its flag (parity/debug), not only anomalies */
 #define TAD_FLAG_PROFILE  2u   /* record per-phase CUDA-event times into tad_status.phase_ms         */
 #define TAD_FLAG_SHARE    4u   /* a streamed job takes part in fit sharing (tad_set_fit_sharing)     */
+#define TAD_FLAG_FIT_BESIDE 8u /* an ARIMA tad_submit job may fit beside another job's fit while fit  */
+                               /* sharing is on (tad_set_fit_sharing); ignored on EWMA and DBSCAN     */
+                               /* jobs, on streamed jobs and while sharing is off                     */
 
 typedef struct tad_ctx tad_ctx;
 typedef struct tad_job tad_job;
@@ -276,6 +279,19 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * returns *again = 1; the job is SCHEDULED again with its stages and progress at 0, is not run in a yield again, and
  * its next round's blocks are taken once the context reaches the job in its turn, which starts it again from its first
  * round.
+ *
+ * An ARIMA tad_submit job with TAD_FLAG_FIT_BESIDE may run in a yield too, and fits beside the yielded fit instead of
+ * waiting for it: one such job per yield, the first queued, while the yielded job's reserve is at least 128 MiB.  It
+ * plans in half the reserve and keeps the other half as its own reserve, so its fit yields in turn to the EWMA and DBSCAN
+ * jobs queued meanwhile, which run in that half.  Its fit runs in one launch with the rest of the yielded fit, each with
+ * about half the GPU; once all its fits are done the launch ends within one evaluation round (after the yielded fit has
+ * finished again the fits its yield dropped), its rows are scored and it completes, and the yielded fit resumes as after
+ * any yield.  Every job's forecasts, rows and fit counts are those of a solo run.  A job whose 1/64 hash range does not
+ * fit half the reserve waits for its turn as above.  A cancel of the flagged job ends the joint launch; a cancel of the
+ * yielded job stops its part at once and takes effect once the flagged job has ended.  The yielded job's detect phase and
+ * device_ms count its time in the joint launch as fit time; its tad_job_memory peak leaves out the flagged job's
+ * workspace, whose own peak stays within half the reserve.  Streamed ARIMA jobs do not run in a yield; the flag is
+ * ignored on them.
  * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit left
  * early would strand its peers, as for the cancel). */
 int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);

@@ -14,7 +14,7 @@ PHASE_NAMES = ("h2d", "hist", "scan", "scatter", "exchange", "group", "spill", "
 ALGOS = {"EWMA": 0, "ARIMA": 1, "DBSCAN": 2}
 STATE_NAMES = ("NEW", "SCHEDULED", "RUNNING", "COMPLETED", "FAILED")
 TAD_MEM_HOST, TAD_MEM_DEVICE = 0, 1
-TAD_FLAG_EMIT_ALL, TAD_FLAG_PROFILE, TAD_FLAG_SHARE = 1, 2, 4
+TAD_FLAG_EMIT_ALL, TAD_FLAG_PROFILE, TAD_FLAG_SHARE, TAD_FLAG_FIT_BESIDE = 1, 2, 4, 8
 TAD_REDUCE_MAX, TAD_REDUCE_SUM = 0, 1
 
 EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_alloc_columns",

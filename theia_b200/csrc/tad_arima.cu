@@ -628,15 +628,15 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
 // are the warp's first resume[2i + 1] hand-outs; resume[2S + 1] counts those that have finished again, which lets the host
 // hold the next yield until all have (so no fit is dropped twice).  kMode: 0 a fit that cannot yield (resume is null),
 // 1 one that can, 2 its resume launch; mode 0 is the fit kernel as it is without fit sharing.
+// arima_fit_series is the work of the warp that fits series i (lane = its lane): the one body of both fit kernels.
 template <int kMode>
-__global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
-                                                             const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
-                                                             const double *__restrict__ yb, const double *__restrict__ lam,
-                                                             double *__restrict__ pred, const volatile uint32_t *cancel,
-                                                             uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume)
+__device__ __forceinline__ void arima_fit_series(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
+                                                 const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
+                                                 const double *__restrict__ yb, const double *__restrict__ lam,
+                                                 double *__restrict__ pred, const volatile uint32_t *cancel,
+                                                 uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume,
+                                                 const uint32_t i, const uint32_t lane)
 {
-    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
     if (i >= S) return;                                    // warp-uniform
     if (isnan(lam[i])) return;
     constexpr bool kResume = kMode == 2;
@@ -725,6 +725,56 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
             resume[2 * i + 1] = dropped;
             if (dropped) atomicAdd(resume + 2 * S, dropped);
         }
+    }
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
+                                                             const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
+                                                             const double *__restrict__ yb, const double *__restrict__ lam,
+                                                             double *__restrict__ pred, const volatile uint32_t *cancel,
+                                                             uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume)
+{
+    arima_fit_series<kMode>(entries, offsets, sbase, B, S, yb, lam, pred, cancel, fits_done, resume,
+                            (blockIdx.x * blockDim.x + threadIdx.x) >> 5, threadIdx.x & 31);
+}
+
+// The lowest series of `a` a resume launch still has fits for (resume point >= 3), into *from (set to ~0 by the caller).
+__global__ void __launch_bounds__(128) arima_unfinished_from_kernel(FitPart a, uint32_t *__restrict__ from)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool left = i < a.S && !isnan(a.lam[i]) && a.resume[2 * i] >= 3;
+    const uint32_t lo = __reduce_min_sync(0xffffffffu, left ? i : ~0u);    // the grid covers whole warps
+    if ((threadIdx.x & 31) == 0 && lo != ~0u) atomicMin(from, lo);
+}
+
+// Joint fit (fit sharing, TAD_FLAG_FIT_BESIDE): the fits of part b and the unfinished ones of a yielded fit, part a, in one
+// launch, so that both share the SMs (a second launch beside a resume would not: the earlier grid's blocks are dispatched
+// first and a block of a long series lives for minutes).  Part a runs as its resume launch (mode 2) over its series
+// a_from ..< a_from + n_a, the series from its lowest unfinished one on; part b runs mode kModeB (1 its first launch, 2 its
+// resume after a yield of its own).  The split: warps alternate between the two parts, a on the even warps and b on the odd,
+// until the smaller part has all its series; the warps after that take the rest of the larger part.  So each part holds
+// about half the warps while both have series left, and a yielded fit's finished series take no warp.  Each part reads
+// its own cancel word and writes its own counters and resume points, so each leaves as a launch of its own would; the
+// per-series work is arima_fit_series, so every forecast is the one its job computes alone.
+template <int kModeB>
+__global__ void __launch_bounds__(128) arima_fit_pair_kernel(FitPart a, uint32_t a_from, uint32_t n_a, FitPart b)
+{
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    const uint32_t m = min(n_a, b.S);
+    const bool on_b = w < 2 * m ? (w & 1) != 0 : b.S > n_a;
+    const uint32_t at = w < 2 * m ? w >> 1 : w - m;
+    if (kModeB == 2) {              // both parts resume: one call site
+        arima_fit_series<2>(on_b ? b.entries : a.entries, on_b ? b.offsets : a.offsets, on_b ? b.sbase : a.sbase,
+                            on_b ? b.B : a.B, on_b ? b.S : a.S, on_b ? b.y : a.y, on_b ? b.lam : a.lam, on_b ? b.pred : a.pred,
+                            on_b ? b.cancel : a.cancel, on_b ? b.fits_done : a.fits_done, on_b ? b.resume : a.resume,
+                            on_b ? at : a_from + at, lane);
+    } else if (on_b) {
+        arima_fit_series<kModeB>(b.entries, b.offsets, b.sbase, b.B, b.S, b.y, b.lam, b.pred, b.cancel, b.fits_done, b.resume,
+                                 at, lane);
+    } else {
+        arima_fit_series<2>(a.entries, a.offsets, a.sbase, a.B, a.S, a.y, a.lam, a.pred, a.cancel, a.fits_done, a.resume,
+                            a_from + at, lane);
     }
 }
 
@@ -852,6 +902,31 @@ cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, con
     arima_fit_sync_kernel<2><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
                                                                                   scratch_lam, scratch_pred, cancel, fits + 1,
                                                                                   resume);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_arima_unfinished(cudaStream_t st, const FitPart &a, uint32_t *from)
+{
+    cudaError_t e = cudaMemsetAsync(from, 0xff, 4, st);
+    if (e != cudaSuccess || a.S == 0) return e;
+    arima_unfinished_from_kernel<<<(a.S + 127) / 128, 128, 0, st>>>(a, from);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &b, const uint64_t *csr_v, uint32_t *fits_total)
+{
+    if (b.S == 0) return cudaSuccess;
+    arima_boxcox_kernel<<<(b.S + 127) / 128, 128, 0, st>>>(b.entries, b.offsets, b.sbase, b.B, b.S, csr_v, b.y, b.lam,
+                                                           fits_total, b.pred);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_arima_pair(cudaStream_t st, const FitPart &a, uint32_t a_from, uint32_t n_a, const FitPart &b, bool b_first)
+{
+    const uint64_t threads = ((uint64_t)n_a + b.S) * 32;
+    if (threads == 0) return cudaSuccess;
+    if (b_first) arima_fit_pair_kernel<1><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(a, a_from, n_a, b);
+    else arima_fit_pair_kernel<2><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(a, a_from, n_a, b);
     return cudaGetLastError();
 }
 

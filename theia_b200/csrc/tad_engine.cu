@@ -134,6 +134,18 @@ double now_ms()
 
 }  // namespace
 
+// A fit that has yielded (fit sharing), as a flagged ARIMA job run in its yield fits beside it (wait_pair_fit): its
+// buffers stay parked in device memory, so its part of the joint launch needs only its launch arguments.
+struct YieldedFit {
+    tad_job *job;
+    FitPart part;                    // its series, buffers, cancel word, fits finished and resume points
+    uint32_t *d_fits;                // its fit counters [0, 2) and cancel word [2]
+    uint64_t done0 = 0, total0 = 0;  // its fit counts before the pass (tad_job_progress adds the pass's counters to them)
+    uint32_t dropped = 0;            // fits its last leave dropped: the next launch it takes part in redoes them
+    bool joint = false;              // a joint launch ran since the yield: `dropped` is that launch's
+    double fit_ms = 0;               // time its part spent in joint launches since the yield: fit time, not parked time
+};
+
 struct tad_job {
     tad_ctx *ctx = nullptr;
     tad_job_spec spec{};
@@ -191,7 +203,10 @@ struct tad_ctx {
     tad_config cfg{};
     cudaStream_t stream = nullptr, copy_stream = nullptr;
     cudaEvent_t ev[kMaxEvents]{};
-    cudaEvent_t ev_alt[kMaxEvents]{};     // ev of the jobs run while an ARIMA pass is parked (its own ev keep its times)
+    cudaEvent_t ev_alt[2][kMaxEvents]{};  // ev of the jobs run while an ARIMA pass is parked, one set per level of parking
+                                          // (a fit beside a parked one can yield too): each parked pass keeps its times
+    int park_depth = 0;                   // ARIMA passes parked now (Parked)
+    YieldedFit *beside = nullptr;         // while a fit's yield runs jobs: the fit a flagged ARIMA job may fit beside
     cudaEvent_t chunk_ev[kMaxChunks]{};
     cudaEvent_t start_ev = nullptr;
     cudaEvent_t x_ev[kMaxXChunks + 1]{};
@@ -232,6 +247,7 @@ struct tad_ctx {
     // ARIMA fit launch (wait_arima_fit): pinned [0, 2): the fit counters while the kernel runs, [2, 4): once it has ended,
     // [4]: 1, the value a cancel copies into the kernel's cancel word; [5]: 2, the value a yield copies there; [6], [7]:
     // the fits the last yield dropped, and those of them finished again
+    // [8, 16): the same words for the yielded part of a joint fit (wait_pair_fit)
     uint32_t *h_fits = nullptr;
     std::atomic<uint64_t> fit_share{0};             // tad_set_fit_sharing: the reserve of the jobs run beside a fit (0: off)
     cudaEvent_t fit_ev[2]{};        // [0]: the fit counters are reset; [1]: the fit kernel has ended
@@ -380,6 +396,7 @@ struct PassSplit {};
 constexpr int kJobs = 1;     // kept when a job ends: all but the text key dictionaries, which live for one job
 constexpr int kPasses = 2;   // kept across the passes of a job: what every pass reads (free_pass_buffers frees the rest)
 constexpr int kParked = 4;   // moved out of the context while an ARIMA pass is parked (Parked), the rest left for reuse
+constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad_set_memory_budget accepts
 
 // Every workspace buffer with its lifetime, the exported multi-GPU buffer `xbuf` apart (ranks agree on its size).
 //
@@ -586,12 +603,15 @@ void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progres
 // has run at least as long as that interleave took (job->quiet_until).  So no fit is dropped twice: the work yields throw
 // away is at most one fitting of each prefix, and under a steady stream of short jobs the fit phase (parked time left
 // out) takes at most about twice as long.  Each resume launch is added to `launches`.
+// yf (a fit that can yield, null otherwise): its launch arguments, which a flagged ARIMA job run in the yield fits beside
+// (wait_pair_fit); the time its part of such joint launches took is fit time, not parked time.
 // Returns once the kernel has ended, its final counts published: the time the pass was parked (ms).
-bool interleave_waiting(tad_ctx *ctx);
-void interleave(tad_ctx *ctx, tad_job *job);
+bool interleave_waiting(tad_ctx *ctx, const tad_job *job);
+void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf);
 bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve);
 template <class Resume>
-double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_redo, uint64_t &launches, Resume resume)
+double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_redo, uint64_t &launches, YieldedFit *yf,
+                      Resume resume)
 {
     uint64_t done0, total0;
     {
@@ -619,7 +639,7 @@ double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_
                 cancelled = true;
             }
             if (job->share && !cancelled && !yielded && redone >= dropped && now_ms() >= job->quiet_until &&
-                interleave_waiting(ctx)) {
+                interleave_waiting(ctx, job)) {
                 CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 5, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
                 yielded = true;
                 t_word = now_ms();
@@ -660,18 +680,30 @@ double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_
         dropped = ctx->h_fits[6];
         redone = 0;
         if (getenv("TAD_DEBUG_YIELD")) fprintf(stderr, "yield: kernel left %.2f ms after the word, %u fits dropped\n", t0 - t_word, dropped);
-        interleave(ctx, job);
+        if (yf) {
+            yf->done0 = done0;
+            yf->total0 = total0;
+            yf->dropped = dropped;
+            yf->joint = false;
+            yf->fit_ms = 0;
+        }
+        interleave(ctx, job, yf);
+        double away = now_ms() - t0;
+        if (yf && yf->joint) {           // its part fitted beside another job: those fits are the ones to finish again
+            dropped = yf->dropped;
+            away = std::max(0.0, away - yf->fit_ms);
+        }
         CU(cudaMemsetAsync(d_fits + 2, 0, 4, ctx->stream));
         CU(cudaMemsetAsync(d_redo, 0, 8, ctx->stream));
         CU(cudaEventRecord(ctx->fit_ev[0], ctx->stream));
         CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
         const double t1 = now_ms();
-        parked += t1 - t0;
-        job->quiet_until = t1 + (t1 - t0);
+        parked += away;
+        job->quiet_until = t1 + away;
         {
             std::lock_guard<std::mutex> lk(job->mu);
             job->yields++;
-            job->parked_ms += t1 - t0;
+            job->parked_ms += away;
         }
         resume();
         launches++;
@@ -681,21 +713,33 @@ double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_
 // Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
 // large for the reserve.  A streamed one only with TAD_FLAG_SHARE and once its feeder has handed over its first block or
 // closed its round: a job whose caller has not started delivering would hold the fit parked while it waits.
-bool interleavable(tad_job *j)
+// `beside`: the yield is that of a fit parked at the outer level whose reserve halves to the 64 MiB floor or more; then a
+// tad_submit ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (wait_pair_fit).
+bool interleavable(tad_job *j, bool beside)
 {
-    if (j->no_interleave || (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN)) return false;
+    if (j->no_interleave) return false;
+    if (j->spec.algo == TAD_ALGO_ARIMA) return beside && !j->stream && (j->spec.flags & TAD_FLAG_FIT_BESIDE);
+    if (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN) return false;
     if (!j->stream) return true;
     if (!(j->spec.flags & TAD_FLAG_SHARE)) return false;
     std::lock_guard<std::mutex> lk(j->mu);
     return j->in.pushed > 0 || j->in.end_req;
 }
 
-// Whether a yield would run a job now: a cancelled one is not worth a yield (it fails at once in its turn).
-bool interleave_waiting(tad_ctx *ctx)
+// Whether a yield of `job`'s fit may run an ARIMA job beside it: the job parks at the outer level (a job fitting beside a
+// parked fit takes no ARIMA partner) and half its reserve, the partner's budget, is at least the 64 MiB floor.
+bool beside_ok(const tad_ctx *ctx, const tad_job *job)
 {
+    return ctx->park_depth == 0 && job->share / 2 >= kBudgetFloor;
+}
+
+// Whether a yield would run a job now: a cancelled one is not worth a yield (it fails at once in its turn).
+bool interleave_waiting(tad_ctx *ctx, const tad_job *job)
+{
+    const bool beside = beside_ok(ctx, job);
     std::lock_guard<std::mutex> lk(ctx->mu);
     for (tad_job *j : ctx->queue)
-        if (interleavable(j) && !j->cancel.load()) return true;
+        if (interleavable(j, beside) && !j->cancel.load()) return true;
     return false;
 }
 
@@ -720,14 +764,14 @@ struct Parked {
         }
         for (int t = 0; t < 2; t++) ctx->tdict[t].swap_sizes(dict[t]);
         out = true;
-        std::swap(ctx->ev, ctx->ev_alt);
+        std::swap(ctx->ev, ctx->ev_alt[ctx->park_depth++]);
     }
     // the interleaved jobs' workspace is freed and the parked buffers return; drop: they are freed too (a cancel)
     void restore(bool drop = false)
     {
         if (!out) return;
         out = false;
-        std::swap(ctx->ev, ctx->ev_alt);
+        std::swap(ctx->ev, ctx->ev_alt[--ctx->park_depth]);
         cudaStreamSynchronize(ctx->stream);
         cudaStreamSynchronize(ctx->copy_stream);
         free_bufs(ctx);
@@ -748,16 +792,23 @@ struct Parked {
 // Runs the eligible jobs queued now, in FIFO order, while the ARIMA pass of `job` is parked: each inside the reserve
 // (run_one), so one whose 1/64 hash range does not fit it is put back where it was and runs in its turn.  A cancel of
 // `job` takes effect once the job in progress has ended: the parked buffers are freed and the job fails.
-void interleave(tad_ctx *ctx, tad_job *job)
+// At most one ARIMA job (TAD_FLAG_FIT_BESIDE) runs per yield, the first queued: its fit runs beside the rest of `job`'s,
+// described by `yf` (ctx->beside while the batch runs).
+void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
 {
     std::vector<tad_job *> batch;
+    bool beside = yf && beside_ok(ctx, job);
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         for (tad_job *j : ctx->queue)
-            if (interleavable(j)) batch.push_back(j);
+            if (interleavable(j, beside)) {
+                batch.push_back(j);
+                if (j->spec.algo == TAD_ALGO_ARIMA) beside = false;
+            }
     }
     const double t0 = now_ms();
     Parked park(ctx);
+    if (yf && ctx->park_depth == 1) ctx->beside = yf;
     const double t1 = now_ms();
     for (tad_job *j : batch) {
         if (job->cancel.load()) break;
@@ -773,6 +824,7 @@ void interleave(tad_ctx *ctx, tad_job *job)
             ctx->queue.insert(ctx->queue.begin() + at, j);
         }
     }
+    if (ctx->beside == yf) ctx->beside = nullptr;
     CU(cudaSetDevice(ctx->cfg.device));
     const double t2 = now_ms();
     const bool cancelled = job->cancel.load() != 0;
@@ -780,6 +832,141 @@ void interleave(tad_ctx *ctx, tad_job *job)
     if (getenv("TAD_DEBUG_YIELD"))
         fprintf(stderr, "yield: park %.2f ms, %zu jobs %.2f ms, restore %.2f ms\n", t1 - t0, batch.size(), t2 - t1, now_ms() - t2);
     if (cancelled) fail(TAD_ERR_CANCELLED, "job cancelled");
+}
+
+// The fit of `job`, an ARIMA job run in the yield of the fit `a` (TAD_FLAG_FIT_BESIDE): Box-Cox, then joint launches of
+// its series beside the ones `a` has left (launch_arima_pair), waited for as wait_arima_fit waits for one fit.  `b`: its
+// part, with its counters d_fits[0, 2) and cancel word d_fits[2] (zeroed by the caller, as are b's resume words [2S, 2S + 2));
+// d_fits[3] is scratch.  The worker watches both jobs, polling every millisecond:
+//   end: once every fit of `job` is done and `a` has finished again all fits its last leave dropped (so none of them is
+//     dropped twice), 2 goes into a's word: its part leaves within one evaluation round, its resume points written;
+//   a cancel of `job` ends the launch (1 in its word, 2 in a's); one of `a` puts 1 in a's word only: its part leaves and
+//     job's goes on (`a` fails once `job` has ended, like any parked job);
+//   yield: an EWMA or DBSCAN job waiting makes both parts leave (2 in both words), once both have finished again the fits
+//     their last leave dropped and the quiet time of job's last yield has passed; job's pass is parked in turn
+//     (interleave, one level deeper, which runs EWMA and DBSCAN jobs only, in job's reserve), and both parts then resume
+//     in one joint launch;
+//   both jobs' fit counts (tad_job_progress) are published as they are copied back.
+// a->dropped, a->joint and a->fit_ms tell a's wait_arima_fit what its part did.  Returns the time job's pass was parked (ms).
+double wait_pair_fit(tad_ctx *ctx, tad_job *job, YieldedFit *a, const FitPart &b, const uint64_t *csr_v, uint32_t *d_fits,
+                     uint64_t &launches)
+{
+    cudaStream_t st = ctx->stream;
+    uint32_t *hb = ctx->h_fits, *ha = ctx->h_fits + 8;      // [0, 2) counters while running, [2, 4) at the end, [6] [7] redo
+    uint32_t *b_redo = b.resume + 2 * (size_t)b.S, *a_redo = a->part.resume + 2 * (size_t)a->part.S;
+    uint64_t done0, total0;
+    {
+        std::lock_guard<std::mutex> lk(job->mu);
+        done0 = job->prog.fits_done;
+        total0 = job->prog.fits_total;
+    }
+    auto publish = [&](const uint32_t *h_b, const uint32_t *h_a) {
+        {
+            std::lock_guard<std::mutex> lk(job->mu);
+            job->prog.fits_total = total0 + h_b[0];
+            job->prog.fits_done = done0 + h_b[1];
+        }
+        std::lock_guard<std::mutex> lk(a->job->mu);
+        a->job->prog.fits_total = a->total0 + h_a[0];
+        a->job->prog.fits_done = a->done0 + h_a[1];
+    };
+    auto word = [&](uint32_t *d_word, int value) {          // value 1 (cancel) or 2 (leave), beside the kernel
+        CU(cudaMemcpyAsync(d_word, ctx->h_fits + 3 + value, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+    };
+    CU(launch_arima_boxcox(st, b, csr_v, d_fits));          // job's fit count is final before the joint launch
+    double parked = 0;
+    uint32_t b_dropped = 0;
+    for (bool first = true;; first = false) {
+        // a's part: its series from the lowest one with fits left on
+        CU(cudaMemsetAsync(a->d_fits + 2, 0, 4, st));
+        CU(cudaMemsetAsync(a_redo, 0, 8, st));
+        CU(launch_arima_unfinished(st, a->part, d_fits + 3));
+        CU(cudaMemcpyAsync(ha + 6, d_fits + 3, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        const uint32_t from = ha[6] == ~0u ? 0 : ha[6], n_a = ha[6] == ~0u ? 0 : a->part.S - ha[6];
+        if (!first) {
+            CU(cudaMemsetAsync(d_fits + 2, 0, 4, st));
+            CU(cudaMemsetAsync(b_redo, 0, 8, st));
+        }
+        CU(cudaEventRecord(ctx->fit_ev[0], st));
+        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
+        const double t_launch = now_ms();
+        CU(launch_arima_pair(st, a->part, from, n_a, b, first));
+        launches += first ? 1 : 2;          // the caller counts the Box-Cox and the first joint launch
+        CU(cudaEventRecord(ctx->fit_ev[1], st));
+        bool copying = false, counted = false, a_cancelled = false, a_left = false, b_cancelled = false, yielded = false;
+        uint32_t a_redone = 0, b_redone = 0;
+        for (;;) {
+            if (!a_cancelled && !a_left && a->job->cancel.load()) {
+                word(a->d_fits + 2, 1);
+                a_cancelled = true;
+            }
+            if (!b_cancelled && job->cancel.load()) {
+                word(d_fits + 2, 1);
+                if (!a_cancelled && !a_left) word(a->d_fits + 2, 2);
+                b_cancelled = a_left = true;
+            }
+            const bool a_clear = a_cancelled || a_redone >= a->dropped;
+            if (counted && !a_left && !a_cancelled && hb[1] == hb[0] && a_clear) {      // every fit of job is done
+                word(a->d_fits + 2, 2);
+                a_left = true;
+            }
+            if (job->share && !b_cancelled && !a_left && !yielded && a_clear && b_redone >= b_dropped &&
+                now_ms() >= job->quiet_until && interleave_waiting(ctx, job)) {
+                word(d_fits + 2, 2);
+                if (!a_cancelled) word(a->d_fits + 2, 2);
+                yielded = true;
+            }
+            const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
+            if (e != cudaErrorNotReady) {
+                CU(e);
+                break;
+            }
+            if (copying) {
+                const cudaError_t c = cudaEventQuery(ctx->fits_ev);
+                if (c != cudaErrorNotReady) {
+                    CU(c);
+                    publish(hb, ha);
+                    b_redone = hb[7];
+                    a_redone = ha[7];
+                    counted = true;
+                    copying = false;
+                }
+            }
+            if (!copying) {
+                CU(cudaMemcpyAsync(hb, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                CU(cudaMemcpyAsync(ha, a->d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                CU(cudaMemcpyAsync(hb + 7, b_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                CU(cudaMemcpyAsync(ha + 7, a_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
+                copying = true;
+            }
+            std::this_thread::sleep_for(std::chrono::milliseconds(1));
+        }
+        CU(cudaStreamSynchronize(ctx->copy_stream));            // no copy or word write is left behind the kernel
+        CU(cudaMemcpyAsync(hb + 2, d_fits, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ha + 2, a->d_fits, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(hb + 6, b_redo, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ha + 6, a_redo, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        publish(hb + 2, ha + 2);
+        a->dropped = ha[6];
+        a->joint = true;
+        const double t0 = now_ms();
+        a->fit_ms += t0 - t_launch;
+        b_dropped = hb[6];
+        // done, cancelled (the caller fails the job), or every fit finished before the kernel saw the yield
+        if (!yielded || b_cancelled || hb[3] == hb[2]) return parked;
+        if (getenv("TAD_DEBUG_YIELD")) fprintf(stderr, "joint yield: %u + %u fits dropped\n", b_dropped, a->dropped);
+        interleave(ctx, job, nullptr);
+        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
+        const double t1 = now_ms();
+        parked += t1 - t0;
+        job->quiet_until = t1 + (t1 - t0);
+        std::lock_guard<std::mutex> lk(job->mu);
+        job->yields++;
+        job->parked_ms += t1 - t0;
+    }
 }
 
 int pick_logb(const tad_ctx *ctx, uint64_t rows)
@@ -935,7 +1122,6 @@ struct PipeSizes {
         csr_p, sbase, outb, dbx, dbi, ar_y, ar_pred, ar_lam, ar_res;
 };
 constexpr size_t kOutWidth[11] = {8, 8, 8, 4, 4, 4, 4, 2, 2, 1, 1};   // bytes per result row of each out_layout column
-constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad_set_memory_budget accepts
 constexpr uint64_t kBudgetHeadroom = 512ull << 20; // default budget: device memory left free for the CUDA context and others
 constexpr size_t kFixedBytes = 1u << 20;        // stats, scan flags, ns_ignore list, small staging
 constexpr uint64_t kSlotBudget = 40ull << 30;   // optimistic slot buffer at most half of an 80 GB H100
@@ -1618,13 +1804,21 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
                 uint32_t *res = job->share ? (uint32_t *)ctx->ar_res.p : nullptr;
                 CU(cudaMemsetAsync(d_stats + ST_FITS, 0, 12, st));      // fit counters and cancel word
                 if (res) CU(cudaMemsetAsync(res + 2 * (size_t)S, 0, 8, st));
-                CU(cudaEventRecord(ctx->fit_ev[0], st));
-                CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, y, pred, lam, d_stats + ST_FITS + 2,
-                                    d_stats + ST_FITS, res));
-                parked_ms = wait_arima_fit(ctx, job, d_stats + ST_FITS, res ? res + 2 * (size_t)S : nullptr, launches, [&] {
-                    CU(launch_arima_resume(st, entries, offsets, sbase, Bl, S, y, pred, lam, d_stats + ST_FITS + 2,
-                                           d_stats + ST_FITS, res));
-                });
+                // this pass's fit as the part a job run in its yield may fit beside (its buffers stay parked meanwhile)
+                YieldedFit yf{job, FitPart{entries, offsets, sbase, Bl, S, y, lam, pred, d_stats + ST_FITS + 2,
+                                           d_stats + ST_FITS + 1, res}, d_stats + ST_FITS};
+                if (ctx->beside && ctx->beside->job != job) {      // this job runs in that yield: it fits beside it
+                    parked_ms = wait_pair_fit(ctx, job, ctx->beside, yf.part, csr_v, d_stats + ST_FITS, launches);
+                } else {
+                    CU(cudaEventRecord(ctx->fit_ev[0], st));
+                    CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, y, pred, lam, d_stats + ST_FITS + 2,
+                                        d_stats + ST_FITS, res));
+                    parked_ms = wait_arima_fit(ctx, job, d_stats + ST_FITS, res ? res + 2 * (size_t)S : nullptr, launches,
+                                               res ? &yf : nullptr, [&] {
+                        CU(launch_arima_resume(st, entries, offsets, sbase, Bl, S, y, pred, lam, d_stats + ST_FITS + 2,
+                                               d_stats + ST_FITS, res));
+                    });
+                }
                 if (ctx->cfg.world_size == 1) check_cancel();      // pred[] is incomplete: no detect
             }
             CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
@@ -2983,6 +3177,9 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
     // and its fit yields
     const bool may_share = !job->stream || (job->spec.flags & TAD_FLAG_SHARE);
     job->share = !reserve && may_share && ctx->cfg.world_size == 1 && job->spec.algo == TAD_ALGO_ARIMA ? ctx->fit_share.load() : 0;
+    // an ARIMA job run in a yield fits beside the parked fit (TAD_FLAG_FIT_BESIDE): it is a sharing job whose budget is
+    // the reserve and whose own reserve, where the jobs run in its yields go, is half of it
+    if (reserve && job->spec.algo == TAD_ALGO_ARIMA) job->share = reserve / 2;
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
@@ -3375,11 +3572,11 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     if (getenv("TAD_EXCHANGE_CHUNKS")) ctx->exchange_chunks_forced = true;
     if (const char *e = getenv("TAD_EXCHANGE_CHUNKS")) ctx->exchange_chunks = atoi(e) < 1 ? 1 : (atoi(e) > kMaxXChunks ? kMaxXChunks : atoi(e));
     for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
-    for (int i = 0; ok && i < kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev_alt[i]) == cudaSuccess;
+    for (int i = 0; ok && i < 2 * kMaxEvents; i++) ok = cudaEventCreate(&ctx->ev_alt[i / kMaxEvents][i % kMaxEvents]) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_small, tad_ctx::kSmallWords * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 8 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
+    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 16 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     if (ok) {
         ctx->h_fits[4] = 1;
         ctx->h_fits[5] = 2;
@@ -3432,7 +3629,8 @@ void tad_shutdown(tad_ctx *ctx)
     if (ctx->fits_ev) cudaEventDestroy(ctx->fits_ev);
     for (int i = 0; i < kMaxEvents; i++) {
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
-        if (ctx->ev_alt[i]) cudaEventDestroy(ctx->ev_alt[i]);
+        for (auto &alt : ctx->ev_alt)
+            if (alt[i]) cudaEventDestroy(alt[i]);
     }
     for (int i = 0; i < kMaxChunks; i++)
         if (ctx->chunk_ev[i]) cudaEventDestroy(ctx->chunk_ev[i]);

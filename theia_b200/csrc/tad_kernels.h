@@ -89,6 +89,24 @@ cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const 
 cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                                 uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
                                 const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
+// Fitting beside a yielded fit (TAD_FLAG_FIT_BESIDE): one job's fit as a part of a joint launch -- its series, the
+// buffers launch_arima_fit takes, its cancel word, fits finished (fits[1]) and resume array (2 S + 2 words, not null).
+struct FitPart {
+    const SeriesEntry *entries;
+    const uint32_t *offsets, *sbase;
+    uint32_t B, S;
+    double *y, *lam, *pred;
+    const volatile uint32_t *cancel;
+    uint32_t *fits_done, *resume;
+};
+// launch_arima_boxcox: launch_arima_fit's Box-Cox kernel for part b (its pred[] marked for a fit that can yield).
+// launch_arima_unfinished: *from = the lowest series of the yielded part a that has fits left (~0u: none).
+// launch_arima_pair: one launch fits part b beside the fits a has left, a's series a_from ..< a_from + n_a, each part as
+// its own launch would (a as its resume launch, b as launch_arima_fit's fit kernel when b_first, else as its resume
+// launch), about half the warps each.
+cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &b, const uint64_t *csr_v, uint32_t *fits_total);
+cudaError_t launch_arima_unfinished(cudaStream_t st, const FitPart &a, uint32_t *from);
+cudaError_t launch_arima_pair(cudaStream_t st, const FitPart &a, uint32_t a_from, uint32_t n_a, const FitPart &b, bool b_first);
 cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                                 uint32_t B, uint32_t S, const uint64_t *csr_v, const uint32_t *csr_t, const double *scratch_pred,
                                 const double *scratch_lam, const OutCols &out, uint32_t out_cap, uint32_t *stats, int emit_all);

@@ -323,12 +323,14 @@ class TadEngine:
         return self.alloc_columns(max(1, len(table["flow_end"]))).fill(table)
 
     @staticmethod
-    def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep, share=False):
+    def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep, share=False,
+              fit_beside=False):
         spec = L.TadJobSpec()
         spec.algo = L.ALGOS[algo] if isinstance(algo, str) else int(algo)
         spec.reducer = reducer
         spec.start_time, spec.end_time = int(start_time), int(end_time)
-        spec.flags = (L.TAD_FLAG_EMIT_ALL if emit_all else 0) | (L.TAD_FLAG_SHARE if share else 0)
+        spec.flags = (L.TAD_FLAG_EMIT_ALL if emit_all else 0) | (L.TAD_FLAG_SHARE if share else 0) | \
+            (L.TAD_FLAG_FIT_BESIDE if fit_beside else 0)
         spec.id = tad_id.encode()[:39]
         spec.global_rows = int(global_rows)
         if len(ns_ignore):
@@ -346,9 +348,13 @@ class TadEngine:
         return job
 
     def submit(self, cols, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
-               tad_id: str = "", emit_all: bool = False, ns_ignore=(), check: bool = True, global_rows: int = 0) -> Job:
+               tad_id: str = "", emit_all: bool = False, ns_ignore=(), check: bool = True, global_rows: int = 0,
+               fit_beside: bool = False) -> Job:
+        """``fit_beside``: TAD_FLAG_FIT_BESIDE, an ARIMA job queued behind another ARIMA job's fit may fit beside it
+        while fit sharing is on (set_fit_sharing), instead of waiting for the whole fit phase."""
         keep = [cols]
-        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep)
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep,
+                          fit_beside=fit_beside)
         h = C.c_void_p()
         rc = self.lib.tad_submit(self.ctx, C.byref(spec), C.byref(cols.c), C.byref(h))
         return self._checked(Job(self, h, keep), rc, check)
