@@ -10,7 +10,9 @@
 //   * Hannan-Rissanen start values.
 // Compute-bound FP64 (about n^2/2 Kalman steps x ~100 likelihood evaluations per series), so the
 // mapping is one WARP per series with one lane per prefix fit; the series lives in L1.
+#include <algorithm>
 #include <cfloat>
+#include <vector>
 
 #include "tad_kernels.h"
 
@@ -562,6 +564,50 @@ __host__ __device__ void arima_fit(const ArimaObj &o, double x[3])
 // no buffer beyond pred[] and no atomics, and the resume launch reads the word it would overwrite anyway.
 constexpr unsigned long long kPredUnset = 0x7ff80000000a7f17ull;
 
+// The per-series steps of the detector, shared by the kernels and the host reference (tad_debug_arima_series), so that the
+// reference runs the kernels' own arithmetic.
+__host__ __device__ __forceinline__ double u64_to_double(uint64_t v)
+{
+#ifdef __CUDA_ARCH__
+    return __ull2double_rn(v);
+#else
+    return (double)v;                                      // round to nearest, as __ull2double_rn
+#endif
+}
+
+// log of the values into y[] and their sum; false if the series yields no rows: n <= 3, a zero value or constant values
+__host__ __device__ __forceinline__ bool arima_log_series(const uint64_t *__restrict__ v, uint32_t n, double *__restrict__ y,
+                                                          double &sumlog)
+{
+    bool valid = n > 3;                                   // anomaly_detection.py:232-234
+    bool constant = true;
+    sumlog = 0.0;
+    for (uint32_t q = 0; q < n && valid; q++) {
+        if (v[q] == 0) valid = false;                     // Box-Cox needs positive data (:260-264 -> None)
+        if (v[q] != v[0]) constant = false;
+        const double lx = log(u64_to_double(v[q]));
+        y[q] = lx;
+        sumlog += lx;
+    }
+    return valid && !constant;
+}
+
+// y[] = log x -> the Box-Cox transform at lambda l, in place; false if it is not finite (the series yields no rows)
+__host__ __device__ __forceinline__ bool arima_boxcox_transform(double *__restrict__ y, uint32_t n, double l)
+{
+    bool finite = isfinite(l);
+    for (uint32_t q = 0; q < n && finite; q++) {
+        y[q] = l == 0.0 ? y[q] : expm1(l * y[q]) / l;     // scipy.special.boxcox
+        finite = isfinite(y[q]);
+    }
+    return finite;
+}
+
+__host__ __device__ __forceinline__ double inv_boxcox_d(double y, double l)
+{
+    return l == 0.0 ? exp(y) : exp(log1p(l * y) / l);     // scipy.special.inv_boxcox
+}
+
 // one series: validity, Box-Cox lambda, transformed series into yb[]; returns its prefix fits (n - 3 with a lambda, else 0).
 // unset (a fit that can yield): pred[], whose prefix forecasts [3, n) are marked kPredUnset.
 __device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
@@ -573,23 +619,10 @@ __device__ __forceinline__ uint32_t arima_boxcox_series(const SeriesEntry *__res
     const uint64_t *v = csr_v + e.off;
     double *y = yb + e.off;
     const uint32_t n = e.n;
-    bool valid = n > 3;                                   // anomaly_detection.py:232-234
-    bool constant = true;
-    double sumlog = 0.0;
-    for (uint32_t q = 0; q < n && valid; q++) {
-        if (v[q] == 0) valid = false;                     // Box-Cox needs positive data (:260-264 -> None)
-        if (v[q] != v[0]) constant = false;
-        const double lx = log(__ull2double_rn(v[q]));
-        y[q] = lx;
-        sumlog += lx;
-    }
-    if (!valid || constant) { lam[i] = NAN; return 0; }
+    double sumlog;
+    if (!arima_log_series(v, n, y, sumlog)) { lam[i] = NAN; return 0; }
     const double l = boxcox_mle_lambda(y, n, sumlog);
-    bool finite = isfinite(l);
-    for (uint32_t q = 0; q < n && finite; q++) {
-        y[q] = l == 0.0 ? y[q] : expm1(l * y[q]) / l;     // scipy.special.boxcox
-        finite = isfinite(y[q]);
-    }
+    const bool finite = arima_boxcox_transform(y, n, l);
     lam[i] = finite ? l : NAN;                             // overflowing transform -> the series yields no rows
     if (finite && unset)
         for (uint32_t q = 3; q < n; q++) unset[e.off + q] = __longlong_as_double((long long)kPredUnset);
@@ -794,11 +827,6 @@ __device__ __forceinline__ double arima_stddev(const uint64_t *__restrict__ v, u
     return has_sd ? __dsqrt_rn(__ddiv_rn(m2, __dsub_rn(cnt, 1.0))) : __longlong_as_double(0x7ff8000000000000LL);
 }
 
-__device__ __forceinline__ double inv_boxcox_d(double y, double l)
-{
-    return l == 0.0 ? exp(y) : exp(log1p(l * y) / l);     // scipy.special.inv_boxcox
-}
-
 template <int NT>
 __global__ void __launch_bounds__(NT) detect_arima_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                           const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
@@ -964,4 +992,262 @@ extern "C" int tad_debug_arima_fit(const double *y, uint32_t n, double *u_out, d
     if (u_out) { u_out[0] = u[0]; u_out[1] = u[1]; u_out[2] = u[2]; u_out[6] = -ll / n; }
     if (forecast) *forecast = fc;
     return 0;
+}
+
+namespace tad {
+
+// The steps of the per-series reference (tad_debug_arima_series and tad_debug_arima_series_device), the same on the host and
+// the device: the kernels' functions in the kernels' order.
+// Transform: arima_log_series, the Box-Cox MLE lambda (or lambda_in if it is not NaN) and arima_boxcox_transform into y[];
+// returns the lambda, or NaN if the series yields no rows; *tried = the lambda tried (NaN if none).
+__host__ __device__ double arima_ref_transform(const uint64_t *v, uint32_t n, double lambda_in, double *y, double *tried)
+{
+    double sumlog;
+    *tried = NAN;
+    if (!arima_log_series(v, n, y, sumlog)) return NAN;
+    const double l = isnan(lambda_in) ? boxcox_mle_lambda(y, n, sumlog) : lambda_in;
+    *tried = l;
+    return arima_boxcox_transform(y, n, l) ? l : NAN;
+}
+
+// every point one ulp up (nudge 1), down (-1), or in a random direction seeded by any other nonzero nudge
+__host__ __device__ void arima_ref_nudge(double *y, uint32_t n, int nudge)
+{
+    uint64_t state = 0x9e3779b97f4a7c15ull * (uint64_t)(int64_t)nudge;
+    for (uint32_t q = 0; q < n && nudge != 0; q++) {
+        bool up = nudge == 1;
+        if (nudge != 1 && nudge != -1) {
+            state = state * 6364136223846793005ull + 1442695040888963407ull;
+            up = (state >> 63) != 0;
+        }
+        y[q] = nextafter(y[q], up ? (double)INFINITY : -(double)INFINITY);
+    }
+}
+
+// pred[t]: the train point for t < 3, else the forecast of the prefix fit on y[0 .. t) (start values, L-BFGS, forecast)
+__host__ __device__ double arima_ref_prefix(const double *y, uint32_t t)
+{
+    if (t < 3) return y[t];
+    const ArimaObj o{y, t};
+    double u[3], phi, theta, s2, fc = 0.0;
+    arima_start(o, u);
+    arima_fit(o, u);
+    arima_transform(u, phi, theta, s2);
+    arima_loglike(o, phi, theta, s2, &fc);
+    return fc;
+}
+
+// calc[] = the inverse transform of pred[]; false if any is not finite (the series yields no rows)
+__host__ __device__ bool arima_ref_inverse(const double *p, uint32_t n, double l, double *calc)
+{
+    bool finite = true;
+    for (uint32_t q = 0; q < n; q++) {
+        calc[q] = inv_boxcox_d(p[q], l);
+        finite = finite && isfinite(calc[q]);
+    }
+    return finite;
+}
+
+__global__ void __launch_bounds__(64) arima_ref_transform_kernel(const uint64_t *v, const uint32_t *off, const uint32_t *len,
+                                                                 const double *lam_in, bool y_given, double *y, double *lam,
+                                                                 uint32_t cases)
+{
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cases) return;
+    double tried;
+    lam[c] = y_given ? lam_in[c] : arima_ref_transform(v + off[c], len[c], lam_in[c], y + off[c], &tried);
+}
+
+__global__ void __launch_bounds__(64) arima_ref_prefix_kernel(const uint32_t *job_case, const uint32_t *job_t, uint32_t jobs,
+                                                              const uint32_t *off, const double *lam, const double *y, double *p)
+{
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= jobs) return;
+    const uint32_t c = job_case[j], t = job_t[j];
+    if (!isnan(lam[c])) p[off[c] + t] = arima_ref_prefix(y + off[c], t);
+}
+
+__global__ void __launch_bounds__(64) arima_ref_inverse_kernel(const uint32_t *off, const uint32_t *len, const double *lam,
+                                                               const double *p, double *calc, int32_t *ok, uint32_t cases)
+{
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < cases) ok[c] = !isnan(lam[c]) && arima_ref_inverse(p + off[c], len[c], lam[c], calc + off[c]);
+}
+
+}  // namespace tad
+
+// Hooks of the per-prefix tests (not part of the C ABI in theia_tad.h): a series through the detector's whole path with the
+// kernels' functions in the kernels' order, one prefix fit at a time (arima_fit, as a lane of the fit kernel runs it but
+// without the warp's scheduling).  lambda_in: the lambda to transform with, or NaN for the Brent MLE.
+// Host: nudge perturbs every transformed point by one ulp before the fits (arima_ref_nudge; 0 none) -- a fit whose forecast
+// moves under such a nudge is path dependent, and the spread of the nudged runs measures by how much.  y_io (may be null)
+// receives the transformed series before the nudge, or with y_given holds it on entry (then lambda_in is the lambda).
+// Returns 1 if the series yields rows (calc[n] = the forecasts after the inverse transform; a null calc stops after the
+// transform), else 0; *lambda_out = the lambda tried (NaN if there is none).
+extern "C" int tad_debug_arima_series(const uint64_t *v, uint32_t n, double lambda_in, int nudge, double *calc,
+                                      double *lambda_out, double *y_io, int y_given)
+{
+    std::vector<double> y(n), p(n);
+    double l;
+    if (y_given) {
+        std::copy(y_io, y_io + n, y.begin());
+        l = *lambda_out = lambda_in;
+    } else {
+        l = tad::arima_ref_transform(v, n, lambda_in, y.data(), lambda_out);
+        if (y_io) std::copy(y.begin(), y.end(), y_io);
+    }
+    if (isnan(l)) return 0;
+    if (!calc) return 1;                                   // the transform only
+    tad::arima_ref_nudge(y.data(), n, nudge);
+    for (uint32_t t = 0; t < n; t++) p[t] = tad::arima_ref_prefix(y.data(), t);
+    return tad::arima_ref_inverse(p.data(), n, l, calc) ? 1 : 0;
+}
+
+// Device: `cases` series, series c on v[off[c] .. off[c] + len[c]) with lambda lam[c]; one thread per series for the transform
+// and the inverse and one per prefix fit (longest first).  y_in (may be null): the transformed series, in v's layout, to fit
+// instead (then lam[c] is the lambda).  calc and y_out (may be null) in v's layout; ok[c] = 1 if series c yields rows.
+// Allocates and frees its own memory on the current device; returns once the results are copied back (0, or the CUDA error).
+extern "C" int tad_debug_arima_series_device(const uint64_t *v, const uint32_t *off, const uint32_t *len, const double *lam,
+                                             const double *y_in, uint32_t cases, double *calc, double *y_out, int32_t *ok)
+{
+    if (cases == 0) return 0;
+    size_t words = 1;
+    std::vector<std::pair<uint32_t, uint32_t>> jobs;                     // (t, case)
+    for (uint32_t c = 0; c < cases; c++) {
+        words = std::max(words, (size_t)off[c] + len[c]);
+        for (uint32_t t = 0; t < len[c]; t++) jobs.emplace_back(t, c);
+    }
+    std::sort(jobs.begin(), jobs.end(), [](const auto &a, const auto &b) { return a.first > b.first; });
+    std::vector<uint32_t> jc(jobs.size() + 1), jt(jobs.size() + 1);
+    for (size_t j = 0; j < jobs.size(); j++) { jt[j] = jobs[j].first; jc[j] = jobs[j].second; }
+    const uint32_t njobs = (uint32_t)jobs.size();
+    uint64_t *dv = nullptr;
+    uint32_t *doff = nullptr, *dlen = nullptr, *djc = nullptr, *djt = nullptr;
+    double *dlam_in = nullptr, *dlam = nullptr, *dy = nullptr, *dp = nullptr, *dcalc = nullptr;
+    int32_t *dok = nullptr;
+    cudaError_t e = cudaMalloc(&dv, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dy, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dp, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dcalc, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&doff, cases * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dlen, cases * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dok, cases * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dlam_in, cases * 8ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dlam, cases * 8ull);
+    if (e == cudaSuccess) e = cudaMalloc(&djc, jc.size() * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&djt, jt.size() * 4);
+    if (e == cudaSuccess) e = cudaMemcpy(dv, v, words * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && y_in) e = cudaMemcpy(dy, y_in, words * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(doff, off, cases * 4ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dlen, len, cases * 4ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dlam_in, lam, cases * 8ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(djc, jc.data(), jc.size() * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(djt, jt.data(), jt.size() * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        const uint32_t cb = (cases + 63) / 64, jb = (njobs + 63) / 64;
+        tad::arima_ref_transform_kernel<<<cb, 64>>>(dv, doff, dlen, dlam_in, y_in != nullptr, dy, dlam, cases);
+        if (jb) tad::arima_ref_prefix_kernel<<<jb, 64>>>(djc, djt, njobs, doff, dlam, dy, dp);
+        tad::arima_ref_inverse_kernel<<<cb, 64>>>(doff, dlen, dlam, dp, dcalc, dok, cases);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(calc, dcalc, words * 8, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && y_out) e = cudaMemcpy(y_out, dy, words * 8, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(ok, dok, cases * 4ull, cudaMemcpyDeviceToHost);
+    for (void *q : {(void *)dv, (void *)dy, (void *)dp, (void *)dcalc, (void *)doff, (void *)dlen, (void *)dok, (void *)dlam_in,
+                    (void *)dlam, (void *)djc, (void *)djt})
+        cudaFree(q);
+    return (int)e;
+}
+
+namespace tad {
+
+// One case of tad_debug_arima_host / tad_debug_arima_device: the same core function on either side.  x: the case's n
+// inputs (u64 values for op 0, doubles otherwise), par: 4 parameters, out: 8 results, tmp: n doubles of scratch.
+//   op 0  x = values: out = {Box-Cox MLE lambda of log(x) as the kernel takes it, sum of the logs}
+//   op 1  x = log values, par[0] = lambda: out[0] = boxcox_neg_llf
+//   op 2  x = series, par = {phi, theta, s2}: out = {arima_loglike, forecast}
+//   op 3  x = series, par = u: out[0..3] = arima_fg's f and g, out[4..7] = arima_objective at u, u + 1e-8 e_0, e_1, e_2
+//   op 4  x = series: out[0..2] = arima_start
+__host__ __device__ void arima_debug_case(int op, const void *x, uint32_t n, const double *par, double *out, double *tmp)
+{
+    const double *y = static_cast<const double *>(x);
+    const ArimaObj o{y, n};
+    for (int c = 0; c < 8; c++) out[c] = 0.0;
+    if (op == 0) {
+        double sumlog = 0.0;
+        const uint64_t *v = static_cast<const uint64_t *>(x);
+        for (uint32_t q = 0; q < n; q++) { tmp[q] = log(u64_to_double(v[q])); sumlog += tmp[q]; }
+        out[0] = boxcox_mle_lambda(tmp, n, sumlog);
+        out[1] = sumlog;
+    } else if (op == 1) {
+        double sumlog = 0.0;
+        for (uint32_t q = 0; q < n; q++) sumlog += y[q];
+        out[0] = boxcox_neg_llf(par[0], y, n, sumlog);
+    } else if (op == 2) {
+        out[0] = arima_loglike(o, par[0], par[1], par[2], &out[1]);
+    } else if (op == 3) {
+        double u[3] = {par[0], par[1], par[2]};
+        arima_fg(o, u, out[0], out + 1);
+        out[4] = arima_objective(o, u);
+        for (int c = 0; c < 3; c++) {
+            double uc[3] = {u[0], u[1], u[2]};
+            uc[c] = u[c] + 1e-8;
+            out[5 + c] = arima_objective(o, uc);
+        }
+    } else if (op == 4) {
+        arima_start(o, out);
+    }
+}
+
+__global__ void __launch_bounds__(64) arima_debug_kernel(int op, const uint8_t *x, const uint32_t *off, const uint32_t *len,
+                                                         const double *par, double *out, double *tmp, uint32_t cases)
+{
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < cases) arima_debug_case(op, x + 8ull * off[c], len[c], par + 4ull * c, out + 8ull * c, tmp + off[c]);
+}
+
+}  // namespace tad
+
+// Hooks for the precision tests of the numerical core (not part of the C ABI in theia_tad.h): `cases` cases of one op of
+// tad::arima_debug_case, case c on the 8-byte words x[off[c] .. off[c] + len[c]) with par[4c ..] into out[8c ..].  The
+// host hook runs them in turn; the device hook runs one thread per case on the current device, allocating and freeing its
+// own memory, and returns once the results are copied back (0, or the CUDA error).
+extern "C" int tad_debug_arima_host(int op, const void *x, const uint32_t *off, const uint32_t *len, const double *par,
+                                    uint32_t cases, double *out)
+{
+    for (uint32_t c = 0; c < cases; c++) {
+        std::vector<double> tmp(len[c] ? len[c] : 1);
+        tad::arima_debug_case(op, static_cast<const uint64_t *>(x) + off[c], len[c], par + 4ull * c, out + 8ull * c, tmp.data());
+    }
+    return 0;
+}
+
+extern "C" int tad_debug_arima_device(int op, const void *x, const uint32_t *off, const uint32_t *len, const double *par,
+                                      uint32_t cases, double *out)
+{
+    if (cases == 0) return 0;
+    size_t words = 1;
+    for (uint32_t c = 0; c < cases; c++) words = std::max(words, (size_t)off[c] + len[c]);
+    uint8_t *dx = nullptr;
+    uint32_t *doff = nullptr, *dlen = nullptr;
+    double *dpar = nullptr, *dout = nullptr, *dtmp = nullptr;
+    cudaError_t e = cudaMalloc(&dx, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dtmp, words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&doff, cases * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dlen, cases * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dpar, cases * 32ull);
+    if (e == cudaSuccess) e = cudaMalloc(&dout, cases * 64ull);
+    if (e == cudaSuccess) e = cudaMemcpy(dx, x, words * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(doff, off, cases * 4ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dlen, len, cases * 4ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dpar, par, cases * 32ull, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        tad::arima_debug_kernel<<<(cases + 63) / 64, 64>>>(op, dx, doff, dlen, dpar, dout, dtmp, cases);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(out, dout, cases * 64ull, cudaMemcpyDeviceToHost);
+    for (void *p : {(void *)dx, (void *)dtmp, (void *)doff, (void *)dlen, (void *)dpar, (void *)dout}) cudaFree(p);
+    return (int)e;
 }
