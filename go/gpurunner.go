@@ -70,7 +70,7 @@ type gpuJobRunner struct {
 	ctx    *C.tad_ctx
 	jobs   sync.Map    // id -> *gpuJob
 	share  atomic.Bool // SetFitSharing turned fit sharing on: StartStream flags its jobs
-	beside atomic.Bool // SetFitBeside: Start flags its ARIMA jobs to fit beside a running fit
+	beside atomic.Bool // SetFitBeside: Start (StartStream while share is on) flags its ARIMA jobs to fit beside a running fit
 }
 
 func newGPUJobRunner(device int) (*gpuJobRunner, error) {
@@ -119,8 +119,10 @@ func (r *gpuJobRunner) SetFitSharing(reserve uint64) error {
 // SetFitBeside lets an ARIMA job from Start fit beside another ARIMA job's fit while fit sharing is on (off by default):
 // Start flags its ARIMA jobs (TAD_FLAG_FIT_BESIDE), and a flagged job queued behind a running fit then runs in that
 // fit's reserve, its fit in one launch with the rest of the running one, instead of waiting for the whole fit phase.
-// The running fit keeps about half the GPU meanwhile.  Streamed jobs do not take part.  It takes effect for jobs that
-// start after the call.
+// The running fit keeps about half the GPU meanwhile.  StartStream flags its ARIMA jobs too while fit sharing is on
+// (SetFitSharing): a streamed job then fits beside a running fit once its SELECT has delivered its first block, and the
+// running fit stays parked while further rounds of the SELECT are read.  It takes effect for jobs that start after the
+// call.
 func (r *gpuJobRunner) SetFitBeside(on bool) {
 	r.beside.Store(on)
 }
@@ -263,6 +265,9 @@ func (r *gpuJobRunner) StartStream(spec JobSpec, rowsHint uint64, blockRows int,
 	if r.share.Load() {
 		// an ARIMA job's fit yields; an EWMA or DBSCAN job may run, its SELECT read, while a fit is parked
 		js.flags |= C.TAD_FLAG_SHARE
+		if r.beside.Load() && js.algo == C.TAD_ALGO_ARIMA {
+			js.flags |= C.TAD_FLAG_FIT_BESIDE
+		}
 	}
 	if len(spec.NSIgnore) > 0 {
 		js.n_ns_ignore = C.uint32_t(len(spec.NSIgnore))

@@ -61,9 +61,10 @@ typedef enum { TAD_MEM_HOST = 0, TAD_MEM_DEVICE = 1 } tad_mem;
 #define TAD_FLAG_EMIT_ALL 1u   /* emit every point with its flag (parity/debug), not only anomalies */
 #define TAD_FLAG_PROFILE  2u   /* record per-phase CUDA-event times into tad_status.phase_ms         */
 #define TAD_FLAG_SHARE    4u   /* a streamed job takes part in fit sharing (tad_set_fit_sharing)     */
-#define TAD_FLAG_FIT_BESIDE 8u /* an ARIMA tad_submit job may fit beside another job's fit while fit  */
-                               /* sharing is on (tad_set_fit_sharing); ignored on EWMA and DBSCAN     */
-                               /* jobs, on streamed jobs and while sharing is off                     */
+#define TAD_FLAG_FIT_BESIDE 8u /* an ARIMA job may fit beside another job's fit while fit sharing is  */
+                               /* on (tad_set_fit_sharing): a tad_submit job, or a streamed one that  */
+                               /* has TAD_FLAG_SHARE too; ignored on EWMA and DBSCAN jobs, on         */
+                               /* streamed jobs without TAD_FLAG_SHARE and while sharing is off       */
 
 typedef struct tad_ctx tad_ctx;
 typedef struct tad_job tad_job;
@@ -208,7 +209,8 @@ int tad_result(tad_job *job, tad_rows *rows);
  * when world_size > 1, or of the current pass under a memory budget).  An ARIMA job whose fit is parked while other jobs
  * run (tad_set_fit_sharing) fails once the job running in its place has ended; its parked buffers are then freed.
  * tad_release of a job that has not finished cancels it and waits until it has failed (for a parked ARIMA job, at most
- * the run time of the job running in its place); the context then runs the next queued job. */
+ * the run time of the job running in its place; when that is a streamed ARIMA job fitting beside it, until that job's
+ * input has ended and its result is published); the context then runs the next queued job. */
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
 
@@ -290,8 +292,17 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * fit half the reserve waits for its turn as above.  A cancel of the flagged job ends the joint launch; a cancel of the
  * yielded job stops its part at once and takes effect once the flagged job has ended.  The yielded job's detect phase and
  * device_ms count its time in the joint launch as fit time; its tad_job_memory peak leaves out the flagged job's
- * workspace, whose own peak stays within half the reserve.  Streamed ARIMA jobs do not run in a yield; the flag is
- * ignored on them.
+ * workspace, whose own peak stays within half the reserve.
+ *
+ * A streamed ARIMA job fits beside a yielded fit under the same rules when its spec carries both TAD_FLAG_SHARE and
+ * TAD_FLAG_FIT_BESIDE (either flag alone leaves it waiting for its turn), and, like a streamed EWMA or DBSCAN job, only
+ * once its feeder has pushed its first block or ended its round.  Its passes each fit in one launch with the rest of the
+ * yielded fit; between them the yielded fit stays parked while its caller delivers further rounds (without a host row
+ * store), and its store pages come from the host budget less every page held, as above.  If it does not fit half the
+ * reserve (a 1/64 hash range, or its text key dictionaries), its round ends with *again = 1 and it waits for its turn as
+ * above.  A cancel of it ends the joint launch, and its feeder's pending push or end call returns TAD_ERR_CANCELLED.  A
+ * cancel of the yielded job takes effect once the streamed job's input has ended and its result is published; a
+ * tad_release of the yielded job waits that long too.
  * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit left
  * early would strand its peers, as for the cancel). */
 int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);
@@ -329,7 +340,8 @@ int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host
  * result.  TAD_ERR_UNSUPPORTED when world_size > 1.  A context still runs one job at a time: a streamed job holds the
  * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.  The
  * one exception is fit sharing (tad_set_fit_sharing): with TAD_FLAG_SHARE in its spec, a streamed EWMA or DBSCAN job
- * whose caller has pushed its first block may run while an ARIMA fit is parked, and a streamed ARIMA job's fit yields.
+ * whose caller has pushed its first block may run while an ARIMA fit is parked, and a streamed ARIMA job's fit yields;
+ * with TAD_FLAG_FIT_BESIDE as well, a streamed ARIMA job so fed may fit beside a parked fit.
  *
  * Blocks: mem is TAD_MEM_HOST (any host memory; pinned buffers from tad_alloc_columns copy at the full PCIe rate) or
  * TAD_MEM_DEVICE (read in place); fewer than 2^32 rows; flow_end and value are required; every block carries the same

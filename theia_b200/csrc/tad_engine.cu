@@ -713,13 +713,17 @@ double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_
 // Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
 // large for the reserve.  A streamed one only with TAD_FLAG_SHARE and once its feeder has handed over its first block or
 // closed its round: a job whose caller has not started delivering would hold the fit parked while it waits.
-// `beside`: the yield is that of a fit parked at the outer level whose reserve halves to the 64 MiB floor or more; then a
-// tad_submit ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (wait_pair_fit).
+// `beside`: the yield is that of a fit parked at the outer level whose reserve halves to the 64 MiB floor or more; then an
+// ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (wait_pair_fit): a tad_submit one, or a streamed one
+// with TAD_FLAG_SHARE as well, fed as above.
 bool interleavable(tad_job *j, bool beside)
 {
     if (j->no_interleave) return false;
-    if (j->spec.algo == TAD_ALGO_ARIMA) return beside && !j->stream && (j->spec.flags & TAD_FLAG_FIT_BESIDE);
-    if (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN) return false;
+    if (j->spec.algo == TAD_ALGO_ARIMA) {
+        if (!beside || !(j->spec.flags & TAD_FLAG_FIT_BESIDE)) return false;
+    } else if (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN) {
+        return false;
+    }
     if (!j->stream) return true;
     if (!(j->spec.flags & TAD_FLAG_SHARE)) return false;
     std::lock_guard<std::mutex> lk(j->mu);

@@ -361,14 +361,16 @@ class TadEngine:
 
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
-                      check: bool = True, text_filter=None, share: bool = False) -> StreamJob:
+                      check: bool = True, text_filter=None, share: bool = False,
+                      fit_beside: bool = False) -> StreamJob:
         """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
         ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
         (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
         for every row.  ``share``: TAD_FLAG_SHARE, the job takes part in fit sharing (set_fit_sharing): an ARIMA job's
-        fit yields, an EWMA or DBSCAN job may run while a fit is parked."""
+        fit yields, an EWMA or DBSCAN job may run while a fit is parked.  ``fit_beside``: TAD_FLAG_FIT_BESIDE, with
+        ``share`` an ARIMA job queued behind another ARIMA job's fit may fit beside it once its first block is pushed."""
         keep = []
-        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share)
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share, fit_beside)
         h = C.c_void_p()
         if text_filter is None:
             rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
