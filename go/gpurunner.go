@@ -269,6 +269,12 @@ func (r *gpuJobRunner) StartStream(spec JobSpec, rowsHint uint64, blockRows int,
 			js.flags |= C.TAD_FLAG_FIT_BESIDE
 		}
 	}
+	// The ignore list goes as ids, and every block carries the SrcNS / DstNS ids the BlockReader's dictionary gave the
+	// namespaces.  A reader that hands over the two namespace String columns as clickhouse-go received them (their
+	// bytes and the offset of every 32nd row) would instead pass the list as names, in a tad_stream_filter_ns to
+	// tad_submit_stream_filtered_ns with n_ns_ignore = 0 here, and each block's namespace text to
+	// tad_stream_push_text_ns with src_ns / dst_ns NULL: the GPU then tests every row against the names and the host
+	// builds no namespace dictionary (DESIGN.md section 10, "The namespace ignore list on the device").
 	if len(spec.NSIgnore) > 0 {
 		js.n_ns_ignore = C.uint32_t(len(spec.NSIgnore))
 		js.ns_ignore = (*C.uint32_t)(unsafe.Pointer(&spec.NSIgnore[0]))

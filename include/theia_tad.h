@@ -436,6 +436,46 @@ typedef struct {
 int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, const tad_stream_filter *filter,
                                tad_job **out);
 
+/* ---- Namespace ignore list on namespace text ---------------------------------------------------------------------
+ * Replaces: sourcePodNamespace NOT IN (...) AND destinationPodNamespace NOT IN (...) (anomaly_detection.py:576-580) for a
+ * streamed job whose blocks hand their namespace columns over as Native String text (tad_stream_push_text_ns), so that
+ * no namespace column is dictionary-encoded on the host.  The list is given as names; the engine tests every row's
+ * namespace against it on the GPU, in every round and pass:
+ *   - a name is listed when its bytes equal a listed name's bytes exactly (no case folding, no trimming, no Unicode
+ *     normalisation: the reference's NOT IN compares String bytes);
+ *   - the empty namespace is a name like any other: it is dropped only when "" is in the list;
+ *   - a row is dropped when its source or its destination namespace is listed (a slot the block does not carry is
+ *     never listed);
+ *   - a dropped row counts as filtered everywhere a time-window or ns_ignore filter does: rows_kept, the per-residue
+ *     round-consistency counts and the host row store see only kept rows.
+ * An empty list drops nothing, and the namespace text is then not read.  At most 1024 names of at most 32 KiB in all.
+ * A job that pushes namespace text gives its list here and spec->n_ns_ignore = 0; a job that pushes u32 namespace ids
+ * keeps spec->ns_ignore as before and gives no names here. */
+typedef struct {
+    tad_stream_filter rows;        /* the text slots' row predicates, as for tad_submit_stream_filtered                */
+    uint32_t n_ns_ignore;          /* --ns-ignore-list as names                                                        */
+    const uint8_t *ns_ignore_bytes;    /* the names back to back; copied by the call                                  */
+    const uint64_t *ns_ignore_offsets; /* n_ns_ignore + 1 offsets from 0: name k is bytes[offsets[k] .. offsets[k + 1])*/
+} tad_stream_filter_ns;
+/* tad_submit_stream_filtered with the ignore list as names.  TAD_ERR_INVALID_ARG at submit (the job is returned FAILED)
+ * for what tad_submit_stream_filtered rejects, offsets that do not start at 0 or decrease, NULL bytes or offsets with a
+ * nonzero count, a list over the limits above, or names given together with spec->n_ns_ignore != 0.  A NULL filter is
+ * tad_submit_stream. */
+int tad_submit_stream_filtered_ns(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint,
+                                  const tad_stream_filter_ns *filter, tad_job **out);
+/* tad_stream_push_text with src_ns / dst_ns given as text too (tad_text_column: the column's bytes and the offset of
+ * every 32nd row), any of the four pointers NULL.  A namespace slot given as text must have its u32 column NULL in
+ * `block`, and a block gives its namespace columns either all as text or all as u32 ids.  Which slots are text is part
+ * of the job's column set: every block must make its first block's choice.  A job whose first block gives namespace
+ * text must have no spec->ns_ignore ids; a job with ignore-list names must not give its namespace columns as ids.  Host
+ * blocks only.  The namespace text is staged, cut at marks and counted in the memory budget with the address text; it
+ * needs no dictionary.  A block that breaks one of these, marks that decrease or pass nbytes, or (found on the GPU,
+ * reported by this call or a later push / end call) VarUInt lengths that do not end exactly at the next mark fail the
+ * job with TAD_ERR_INVALID_ARG; the context stays usable.  Otherwise as tad_stream_push_text, which is this call with
+ * src_ns = dst_ns = NULL. */
+int tad_stream_push_text_ns(tad_job *job, const tad_columns *block, const tad_text_column *src_ip,
+                            const tad_text_column *dst_ip, const tad_text_column *src_ns, const tad_text_column *dst_ns);
+
 const char *tad_strerror(int err);
 int tad_abi_version(void);
 

@@ -23,7 +23,7 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
            "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
            "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered", "tad_job_progress",
-           "tad_set_fit_sharing", "tad_job_yields")
+           "tad_set_fit_sharing", "tad_job_yields", "tad_submit_stream_filtered_ns", "tad_stream_push_text_ns")
 TAD_NAME_OPS = {"any": 0, "eq": 1, "nonempty": 2, "icontains": 3}
 
 
@@ -45,6 +45,11 @@ class TadTextColumn(C.Structure):
 
 class TadStreamFilter(C.Structure):
     _fields_ = [("op", C.c_int32 * 2), ("pattern", C.c_void_p * 2), ("pattern_len", C.c_uint32 * 2), ("proto_eq", C.c_int32)]
+
+
+class TadStreamFilterNs(C.Structure):
+    _fields_ = [("rows", TadStreamFilter), ("n_ns_ignore", C.c_uint32), ("ns_ignore_bytes", C.c_void_p),
+                ("ns_ignore_offsets", C.c_void_p)]
 
 
 class TadJobSpec(C.Structure):
@@ -97,10 +102,14 @@ def load():
     L.tad_submit_stream.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(C.c_void_p)]
     L.tad_submit_stream_filtered.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(TadStreamFilter),
                                              C.POINTER(C.c_void_p)]
+    L.tad_submit_stream_filtered_ns.argtypes = [C.c_void_p, C.POINTER(TadJobSpec), C.c_uint64, C.POINTER(TadStreamFilterNs),
+                                                C.POINTER(C.c_void_p)]
     L.tad_debug_name_match.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+    L.tad_debug_ns_match.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64]
     L.tad_stream_push.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_stream_end.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
     L.tad_stream_push_text.argtypes = [C.c_void_p, C.POINTER(TadColumns), C.POINTER(TadTextColumn), C.POINTER(TadTextColumn)]
+    L.tad_stream_push_text_ns.argtypes = [C.c_void_p, C.POINTER(TadColumns)] + [C.POINTER(TadTextColumn)] * 4
     L.tad_job_names.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
     L.tad_poll.argtypes = [C.c_void_p, C.POINTER(TadStatus)]
     L.tad_wait.argtypes = [C.c_void_p, C.c_int64, C.POINTER(TadStatus)]

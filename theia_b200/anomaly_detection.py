@@ -328,7 +328,7 @@ def _dictionary_ids(col, idx, dictionary: Dictionary) -> np.ndarray:
 def _branch_columns(flows: dict, plan: QueryPlan, br: Branch, masks: tuple, dicts: dict, ns_dict: Dictionary,
                     ipv4_as_u32: bool, text_slots=(), keep_all: bool = False) -> dict:
     """One branch's engine columns from a flows table or one block of it: the host predicates, then key slots,
-    ``flow_end`` / ``value`` and, with an ignore list, the namespace ids.  ``ipv4_as_u32``: an address column of IPv4 text
+    ``flow_end`` / ``value`` and, with an ignore list and ``ns_dict``, the namespace ids.  ``ipv4_as_u32``: an address column of IPv4 text
     becomes its u32 value (a whole table); otherwise text addresses go through the dictionary like every other String
     key, which keeps a name's id the same in every block of a stream.  ``text_slots``: key slots the engine encodes from
     the block's text itself (left None here).  ``keep_all``: every row, the host predicates left to the engine."""
@@ -355,7 +355,7 @@ def _branch_columns(flows: dict, plan: QueryPlan, br: Branch, masks: tuple, dict
                 cols[slot] = dicts[slot].encode(raw)
     cols["flow_end"] = np.asarray(flows["flowEndSeconds"])[idx]
     cols["value"] = np.asarray(flows["throughput"])[idx]
-    if plan.ns_ignore:
+    if plan.ns_ignore and ns_dict is not None:
         cols["src_ns"] = _dictionary_ids(flows["sourcePodNamespace"], idx, ns_dict)
         cols["dst_ns"] = _dictionary_ids(flows["destinationPodNamespace"], idx, ns_dict)
     return cols
@@ -414,7 +414,8 @@ def _block_table(block: dict) -> dict:
 
 def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_time: str = "", tad_id: str = "",
                       ns_ignore_list=(), agg_flow=None, pod_label=None, external_ip=None, svc_port_name=None,
-                      pod_name=None, pod_namespace=None, rows_hint: int = 0, on_job=None, device_text: bool = False):
+                      pod_name=None, pod_namespace=None, rows_hint: int = 0, on_job=None, device_text: bool = False,
+                      device_ns: bool = False):
     """:func:`run_engine` over streamed input: ``blocks()`` yields one round of decoded Native blocks
     (``{column: numpy array or clickhouse_native.StringColumn}``, as ``read_blocks`` / ``read_blocks_stream`` yield them)
     and is called again for every round the engine asks for.  Each block's branches are pushed as they are built (two
@@ -428,17 +429,20 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
     as ``clickhouse_native.Names`` (tad_job_names).  Connection mode is the one mode whose host mask keeps every row and
     reads no key text; with ``device_text=True`` the pod / svc / external modes keep their host encoding.
     ``device_text="all"``: those modes push their String keys as text too, every row of a block, and the engine
-    evaluates their string predicates on the GPU (tad_submit_stream_filtered; :func:`_device_text_branches`)."""
+    evaluates their string predicates on the GPU (tad_submit_stream_filtered; :func:`_device_text_branches`).
+
+    ``device_ns``: a job with an ignore list pushes the two namespace columns as text (``src_ns`` / ``dst_ns``,
+    tad_stream_push_text_ns) and gives the list as names (tad_submit_stream_filtered_ns): the GPU tests every row's
+    namespaces against it, and no namespace column is decoded or dictionary-encoded here.  That needs every row of a
+    block pushed (connection mode, and the modes ``device_text="all"`` takes as text) and a list of names the GPU
+    compares as the host path does (:func:`_ns_names_on_device`); otherwise the namespaces keep their host encoding."""
     from .clickhouse_native import Names
     if algo_type not in VALID_ALGOS:
         raise ValueError("Algorithm should be in {}".format(" or ".join(VALID_ALGOS)))
     plan = plan_query(start_time, end_time, ns_ignore_list, agg_flow, pod_label, external_ip, svc_port_name, pod_name,
                       pod_namespace)
     dicts = {slot: Dictionary() for slot in KEY_SLOTS}
-    ns_dict = Dictionary()
     ignore = [str(x) for x in plan.ns_ignore]
-    ns_dict.encode(np.asarray(ignore, dtype=object))
-    ignore_ids = sorted({ns_dict.ids[x] for x in ignore})
     masks = (pod_label, pod_name, pod_namespace, external_ip, svc_port_name)
     # as in run_engine: the window's lower bound reaches the engine only through a flow_start key column
     start = _epoch(plan.start_time) if all("flow_start" in br.key for br in plan.branches) else 0
@@ -451,7 +455,18 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
         branch_text, text_filter = _device_text_branches(plan, head[0], *masks)
     elif device_text and not plan.agg_flow:
         branch_text = [{"src_ip": "sourceIP", "dst_ip": "destinationIP"}]
-    text_cols = {c for bt in branch_text for c in bt.values()}
+    # every row of a block is pushed in connection mode (its host mask keeps them all) and where the engine takes the
+    # mode's predicates: only then can a block's namespace text stand for the rows pushed
+    ns_text = bool(device_ns and ignore and (not plan.agg_flow or text_filter is not None) and _ns_names_on_device(ignore))
+    ns_cols = {"src_ns": "sourcePodNamespace", "dst_ns": "destinationPodNamespace"} if ns_text else {}
+    text_cols = {c for bt in branch_text for c in bt.values()} | set(ns_cols.values())
+    if ns_text:
+        ns_dict, ignore_ids, ns_kw = None, [], {"ns_ignore_names": [x.encode() for x in ignore]}
+    else:
+        # the namespace dictionary starts with the ignore list, whose ids the job spec needs at submit
+        ns_dict, ns_kw = Dictionary(), {}
+        ns_dict.encode(np.asarray(ignore, dtype=object))
+        ignore_ids = sorted({ns_dict.ids[x] for x in ignore})
 
     def round0():
         while head:
@@ -460,12 +475,12 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
                 yield b
         yield from (blocks() if rest is None else rest)
 
-    # the namespace columns of an ignore list stay host-encoded, also where they are a text key
-    host_cols = {"sourcePodNamespace", "destinationPodNamespace"} if plan.ns_ignore else set()
+    # without namespace text, the namespace columns of an ignore list stay host-encoded, also where they are a text key
+    host_cols = {"sourcePodNamespace", "destinationPodNamespace"} if plan.ns_ignore and not ns_text else set()
     pushed_text = False
     kw = {} if text_filter is None else {"text_filter": text_filter}
     job = engine.submit_stream(algo=algo_type, reducer=plan.reducer, start_time=start, end_time=_epoch(plan.end_time),
-                               tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint), **kw)
+                               tad_id=tad_id, ns_ignore=ignore_ids, rows_hint=int(rows_hint), **kw, **ns_kw)
     if on_job is not None:
         on_job(job)
     try:
@@ -480,9 +495,9 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
                     cols = _branch_columns(flows, plan, br, masks, dicts, ns_dict, ipv4_as_u32=False, text_slots=slots,
                                            keep_all=text_filter is not None)
                     if len(cols["flow_end"]):
-                        if slots:
-                            job.push(cols, text={slot: col.text() for slot, col in slots.items()})
-                            pushed_text = True
+                        if slots or ns_cols:
+                            job.push(cols, text={slot: raw[c].text() for slot, c in {**bt, **ns_cols}.items()})
+                            pushed_text = pushed_text or bool(slots)
                         else:
                             job.push(cols)
                     del cols
@@ -503,6 +518,21 @@ def run_engine_stream(engine, algo_type: str, blocks, start_time: str = "", end_
             on_job(None)
         job.release()
     return got, st, plan, dicts
+
+
+def _ns_names_on_device(names) -> bool:
+    """Whether the GPU's byte equality lists the same rows as the host path for these ignore-list names.  The host path
+    compares the names with namespaces decoded as UTF-8 with errors replaced, so a name holding U+FFFD would also list
+    the namespaces whose bytes are not UTF-8; a name that is not valid Unicode (a lone surrogate from the JSON list)
+    has no bytes.  Both keep the host encoding; Kubernetes namespace names are ASCII."""
+    for x in names:
+        if "\ufffd" in x:
+            return False
+        try:
+            x.encode("utf-8")
+        except UnicodeEncodeError:
+            return False
+    return True
 
 
 def _device_text_branches(plan: QueryPlan, first, pod_label, pod_name, pod_namespace, external_ip, svc_port_name):
@@ -808,9 +838,11 @@ def _select_blocks(transport, sql: str):
     return blocks
 
 
-def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str, device_text: bool = False):
+def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, tad_id: str, device_text: bool = False,
+                  device_ns: bool = False):
     """main()'s job on streamed input (TAD_STREAM_INPUT=1): (result SoA, plan, dictionaries).  ``device_text``
-    (TAD_DEVICE_TEXT=1: True, text addresses only; TAD_DEVICE_TEXT=all: "all"): run_engine_stream's ``device_text``."""
+    (TAD_DEVICE_TEXT=1: True, text addresses only; TAD_DEVICE_TEXT=all: "all"): run_engine_stream's ``device_text``.
+    ``device_ns`` (TAD_DEVICE_NS=1): run_engine_stream's ``device_ns``, with and without push-down."""
     hint = 0
     if hasattr(transport, "count"):
         hint = int(transport.count(count_sql(plan))) * len(plan.branches)    # pod: every row feeds both branches
@@ -822,7 +854,7 @@ def _run_streamed(engine, transport, a: dict, plan: QueryPlan, pushdown: bool, t
         return run_engine_stream(engine, a["algo"], _select_blocks(transport, sql), a["start_time"], a["end_time"], tad_id,
                                  a["ns_ignore_list"], a["agg_flow"] or None, a["pod_label"] or None, a["external_ip"] or None,
                                  a["svc_port_name"] or None, a["pod_name"] or None, a["pod_namespace"] or None, rows_hint=hint,
-                                 device_text=False if ipv4_pushdown else device_text)
+                                 device_text=False if ipv4_pushdown else device_text, device_ns=device_ns)
     try:
         got, _st, plan, dicts = run(pushdown)
     except Exception as e:
@@ -861,7 +893,9 @@ def main(argv=None, engine=None, transport=None) -> int:
             # TAD_DEVICE_TEXT=1: the address text of a connection-mode job is dictionary-encoded on the GPU (no push-down);
             # TAD_DEVICE_TEXT=all: every mode's String keys, its string predicates evaluated on the GPU
             device_text = {"1": True, "all": "all"}.get(os.getenv("TAD_DEVICE_TEXT", "0"), False) if not pushdown else False
-            got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id, device_text)
+            # TAD_DEVICE_NS=1: the namespace ignore list is tested on the GPU from the namespace text columns
+            device_ns = os.getenv("TAD_DEVICE_NS", "0") == "1"
+            got, plan, dicts = _run_streamed(engine, transport, a, plan, pushdown, tad_id, device_text, device_ns)
         else:
             sql = raw_select_sql(plan, a["pod_label"], a["pod_name"], a["pod_namespace"], ipv4_pushdown=pushdown)
             def read(q):          # block-by-block while the response arrives when the transport can stream, else the whole body

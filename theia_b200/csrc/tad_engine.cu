@@ -181,21 +181,26 @@ struct tad_job {
         bool round_done = false;     // the worker finished with the round; `again` is valid
         bool again = false;
         bool input_done = false;     // tad_stream_end returned again = 0
-        tad_text_column txt[2]{};    // the handed-over block's text slots (tad_stream_push_text)
+        tad_text_column txt[4]{};    // the handed-over block's text slots (tad_stream_push_text_ns)
         uint64_t pushed = 0, taken = 0, released = 0;   // blocks handed over / taken / no longer read by the engine
         uint64_t round_start = 0;    // `taken` when the last round was closed
         int err = 0;                 // a bad block: the worker fails the job with this code and message
         char msg[200] = {0};
     } in;
-    // text key slots (tad_stream_push_text): src_ip / dst_ip arrive as Native String bytes and are dictionary-encoded
-    // on the device; set by the first block.  On completion each slot's dictionary is copied here (tad_job_names).
-    bool text[2] = {false, false};
+    // text slots (tad_stream_push_text_ns), set by the first block: src_ip / dst_ip arrive as Native String bytes and
+    // are dictionary-encoded on the device; src_ns / dst_ns (slots 2, 3) are only tested against the ignore list's
+    // names.  On completion each key slot's dictionary is copied here (tad_job_names).
+    bool text[4] = {false, false, false, false};
     std::vector<uint8_t> names[2];
     std::vector<uint64_t> names_off[2];
     // row predicates (tad_submit_stream_filtered): per text slot a TAD_NAME_* op and its pattern, and proto_eq (-1: none)
     int32_t name_op[2] = {TAD_NAME_ANY, TAD_NAME_ANY};
     std::vector<uint8_t> name_pat[2];
     int32_t proto_eq = -1;
+    // the ignore list as names (tad_submit_stream_filtered_ns): its device image (ns_list_image) and name count; the
+    // row filter's list `ns_ignore` is then {kNsListed}, the verdict the namespace slots stage per row
+    std::vector<uint8_t> ns_image;
+    uint32_t ns_names = 0;
     bool filtered() const { return name_op[0] != TAD_NAME_ANY || name_op[1] != TAD_NAME_ANY || proto_eq >= 0; }
 };
 
@@ -235,12 +240,12 @@ struct tad_ctx {
     static constexpr int kWBarrier = 48, kWBarrierIn = 56;   // peer barrier (d_small only): the word sent, the words received
     static constexpr int kWSendLo = 64;       // NCCL exchange: send boundaries of every chunk, kMaxRanks + 1 per chunk
     static constexpr int kWPassCursor = 128;  // hash-range passes: the pass cursor alone, read while the counts are held
-    static constexpr int kWTextState = 192;   // text keys: 8 state words per dictionary
+    static constexpr int kWTextState = 192;   // text slots: 8 state words per dictionary, then the ignore list's 16
     static_assert(kGatherMax * (1 + kMaxRanks) <= kSmallWords && kSmallWords <= kSmallDevWords, "small scratch size");
     static_assert(kMaxSeg <= kWOvf && kWOvf + kMaxRanks <= kWPullSkip && kWPullSkip + kMaxRanks <= kWBarrier &&
                   kWBarrier < kWBarrierIn && kWBarrierIn + kMaxRanks <= kWSendLo &&
                   kWSendLo + kMaxXChunks * (kMaxRanks + 1) <= kSmallWords, "partition scratch regions overlap");
-    static_assert(kMaxPasses + 1 <= kWPassCursor && kWPassCursor < kWTextState && kWTextState + 2 * 8 <= kSmallWords,
+    static_assert(kMaxPasses + 1 <= kWPassCursor && kWPassCursor < kWTextState && kWTextState + 4 * 8 <= kSmallWords,
                   "pass scratch regions overlap");
     uint32_t scan_epoch = 0;
     uint32_t *h_stats = nullptr;   // pinned readback of the device scalars
@@ -303,6 +308,7 @@ struct tad_ctx {
         }
     } tdict[2];
     DevBuf tstage, tscratch;                        // a chunk's marks and text bytes; the encode scratch
+    DevBuf nsl;                                     // the ignore list of namespace text slots (ns_list_image)
 };
 
 namespace {
@@ -400,8 +406,9 @@ constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad
 
 // Every workspace buffer with its lifetime, the exported multi-GPU buffer `xbuf` apart (ranks agree on its size).
 //
-// Kept across passes: the pass columns d_col[0..8), the staging, the pass counters, the stats words, the ns_ignore list,
-// the text key dictionaries and their staging, and `small` (run_pipeline ensures it first anyway).
+// Kept across passes: the pass columns d_col[0..8), the staging, the pass counters, the stats words, the ns_ignore list
+// (ids, and the names of namespace text slots), the text key dictionaries and their staging, and `small` (run_pipeline
+// ensures it first anyway).
 //
 // Parked: a parked ARIMA pass moves out the buffers the rest of its fit, its detect_arima and its pass driver read
 // (ctx->held leaves them out).  Everything else stays for the jobs run meanwhile to reuse: each plans under the reserve
@@ -415,7 +422,8 @@ constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad
 //     the pass counters and the ns_ignore list;
 //   a streamed job's text key slots: both dictionaries (table, arena, offsets, hashes, keep bytes, pattern, state words,
 //     with their sizes), which its later rounds look names up in and its end copies out, so its ids stay the same, and
-//     the text staging and encode scratch its sweeps take as sized.  They were planned in the budget less the reserve.
+//     the text staging and encode scratch its sweeps take as sized, and the ignore list its namespace text slots are
+//     tested against in every later round.  They were planned in the budget less the reserve.
 // What else a parked streamed pass needs is not in the workspace and no interleaved job touches it: the job's stream
 // input state (tad_job::in: its feeder, blocked in a push or end call, goes on with the same round) and the host row
 // store pages of its passes (its RowStore's lists).  An interleaved job takes store pages only from the free list and
@@ -443,7 +451,7 @@ std::vector<std::pair<DevBuf *, int>> workspace_bufs(tad_ctx *ctx)
     add(kJobs | kPasses, {&c.small});
     add(kJobs | kParked, {&c.part, &c.entries, &c.offsets, &c.sbase, &c.csr_v, &c.csr_t, &c.ar_y, &c.ar_pred, &c.ar_lam,
                           &c.ar_res, &c.outb});
-    add(kJobs | kPasses | kParked, {&c.stats, &c.stage, &c.pcnt, &c.ns_ignore, &c.tstage, &c.tscratch});
+    add(kJobs | kPasses | kParked, {&c.stats, &c.stage, &c.pcnt, &c.ns_ignore, &c.tstage, &c.tscratch, &c.nsl});
     for (int i = 0; i < 8; i++) add(kJobs | kPasses | kParked, {&c.d_col[i]});
     for (auto &t : c.tdict) add(kPasses | kParked, t.bufs());
     return v;
@@ -1024,8 +1032,11 @@ void set_col(ColPtrs &c, int i, const void *p)
     }
 }
 
-// Whether a job's rows carry key/value column i: its first block's column, or a text slot encoded into it on the device.
-bool has_col(const tad_job *job, int i) { return col_ptr(job->cols, i) || (i < 2 && job->text[i]); }
+// Whether column i of a job's blocks arrives as text: a key slot (src_ip, dst_ip) or a namespace slot (src_ns, dst_ns).
+bool is_text(const tad_job *job, int i) { return i < 2 ? job->text[i] : i >= 8 && job->text[i - 6]; }
+
+// Whether a job's rows carry column i: its first block's column, or a text slot encoded (or tested) into it on the device.
+bool has_col(const tad_job *job, int i) { return col_ptr(job->cols, i) || is_text(job, i); }
 
 // A block's columns as kernel input.
 ColPtrs col_ptrs(const tad_columns &b)
@@ -1990,8 +2001,7 @@ bool next_block(tad_job *job, tad_columns &b, tad_text_column *txt)
         if (job->in.err) fail(job->in.err, "%s", job->in.msg);
         if (job->in.has_blk) {
             b = job->in.blk;
-            txt[0] = job->in.txt[0];
-            txt[1] = job->in.txt[1];
+            for (int t = 0; t < 4; t++) txt[t] = job->in.txt[t];
             job->in.has_blk = false;
             job->in.taken++;
             job->cv.notify_all();
@@ -2032,7 +2042,7 @@ void discard_round(tad_job *job)
         if (!job->in.end_req && job->in.taken == job->in.round_start) return;
     }
     tad_columns b{};
-    tad_text_column tx[2]{};
+    tad_text_column tx[4]{};
     while (next_block(job, b, tx)) {
         std::lock_guard<std::mutex> lk(job->mu);
         job->in.released = job->in.taken;
@@ -2107,13 +2117,15 @@ struct PassColumns {
 // ---- text key slots (DESIGN.md section 10, "Text keys on the device") -------------------------------------------------
 // A host chunk's text slot is copied (its marks, then the bytes of its 32-row segments) into the text staging and
 // encoded into the chunk's staged u32 key column on the copy stream, ahead of the chunk's split or pack.  The
-// dictionaries (ctx->tdict) live for the whole job, so ids are the same in every round.
+// dictionaries (ctx->tdict) live for the whole job, so ids are the same in every round.  A namespace text slot is staged
+// the same way and tested against the ignore list (ctx->nsl) into the chunk's staged namespace column, in every round.
 struct TextKeys {
     tad_ctx *ctx;
     tad_job *job;
     uint64_t budget;                 // the job's memory budget (messages)
     size_t tmarks;                   // the text staging's marks part: a chunk's marks; its text bytes follow
     int mark;                        // a filtered job: the slot (1 / 2) whose ids carry the drop bit; 0: none
+    bool ns;                         // the ignore list filters rows: the namespace text slots are tested
     uint64_t &launches;
     bool frozen = false;             // later rounds look names up and add none
     PassColumns *yield = nullptr;    // the first round's pass columns: under the budget they give way to the dictionaries
@@ -2142,14 +2154,23 @@ struct TextKeys {
                         (uint8_t *)d.arena.p, (uint64_t *)d.off.p, (uint64_t *)d.hash.p, (unsigned long long *)d.state.p,
                         frozen ? 1u : 0u};
     }
-    // the dictionaries' names and bytes (exact again), and their decode error flags
+    // text slot t is read: a key slot, or a namespace slot of a job whose ignore list filters rows
+    bool read(int t) const { return job->text[t] && (t < 2 || ns); }
+    // the dictionaries' names and bytes (exact again), and the decode error flags of every slot
     void sync()
     {
         for (int t = 0; t < 2; t++)
             if (ctx->tdict[t].state.p)
                 CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWTextState + 8 * t, ctx->tdict[t].state.p, 8 * 8,
                                    cudaMemcpyDeviceToHost, ctx->copy_stream));
+        const bool nst = read(2) || read(3);
+        unsigned long long *w_ns = ctx->h_small + tad_ctx::kWTextState + 16;
+        if (nst) CU(cudaMemcpyAsync(w_ns, ctx->nsl.p, kNsStateWords * 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
         CU(cudaStreamSynchronize(ctx->copy_stream));
+        for (int t = 0; t < 2 && nst; t++)
+            if (w_ns[8 * t + 2])
+                fail(TAD_ERR_INVALID_ARG, "invalid request: the %s text column of a streamed block does not match its marks "
+                     "(a VarUInt length runs past a mark or the column's end)", t ? "dst_ns" : "src_ns");
         for (int t = 0; t < 2; t++) {
             auto &d = ctx->tdict[t];
             if (!d.state.p) continue;
@@ -2243,8 +2264,8 @@ struct TextKeys {
     // for a single segment larger than it
     uint64_t fit(const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n)
     {
-        for (int t = 0; t < 2; t++) {
-            if (!job->text[t]) continue;
+        for (int t = 0; t < 4; t++) {
+            if (!read(t)) continue;
             const uint64_t s0 = lo / 32;
             uint64_t s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
             const uint64_t room_b = ctx->tstage.cap - tmarks, a = mark_at(tx[t], rows, s0);
@@ -2269,23 +2290,32 @@ struct TextKeys {
         }
         return n;
     }
-    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids in the chunk's staged key columns `c`.  A
-    // filtered job then marks the rows its predicates drop (the first round also evaluates them on the names the chunk
-    // added) using the chunk's staged proto column.
+    // text slots of rows [lo, lo + n) of a block of `rows` rows -> their ids in the chunk's staged key columns `c`, and
+    // the ignore list's verdicts in its staged namespace columns.  A filtered job then marks the rows its predicates drop
+    // (the first round also evaluates them on the names the chunk added) using the chunk's staged proto column.
     void encode(const tad_text_column *tx, uint64_t rows, uint64_t lo, uint64_t n, const ColPtrs &c)
     {
-        uint32_t *dst[2] = {job->text[0] ? const_cast<uint32_t *>(c.src_ip) : nullptr,
-                            job->text[1] ? const_cast<uint32_t *>(c.dst_ip) : nullptr};
-        for (int t = 0; t < 2; t++) {
-            if (!job->text[t]) continue;
+        uint32_t *dst[4] = {job->text[0] ? const_cast<uint32_t *>(c.src_ip) : nullptr,
+                            job->text[1] ? const_cast<uint32_t *>(c.dst_ip) : nullptr,
+                            const_cast<uint32_t *>(c.src_ns), const_cast<uint32_t *>(c.dst_ns)};
+        for (int t = 0; t < 4; t++) {
+            if (!read(t)) continue;
             const uint64_t s0 = lo / 32, s1 = std::min((rows + 31) / 32, (lo + n + 31) / 32);
             const uint64_t a = mark_at(tx[t], rows, s0), span = mark_at(tx[t], rows, s1) - a;
             // the first round builds the dictionary; later rounds look names up in it and add none (a frozen table
             // needs no room: a missing name fails the round)
-            if (!frozen || !ctx->tdict[t].state.p) grow(t, n, span);
+            if (t < 2 && (!frozen || !ctx->tdict[t].state.p)) grow(t, n, span);
             char *m = static_cast<char *>(ctx->tstage.p);
             CU(cudaMemcpyAsync(m, tx[t].marks + s0, (s1 - s0) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
             if (span) CU(cudaMemcpyAsync(m + tmarks, tx[t].bytes + a, span, cudaMemcpyHostToDevice, ctx->copy_stream));
+            if (t >= 2) {                         // a namespace: no dictionary, the row's verdict only
+                CU(launch_ns_match(ctx->copy_stream, ctx->nsl.p, job->ns_names, job->ns_image.size(),
+                                   static_cast<unsigned long long *>(ctx->nsl.p) + 8 * (t - 2),
+                                   reinterpret_cast<const uint8_t *>(m + tmarks), span, reinterpret_cast<const uint64_t *>(m),
+                                   (uint32_t)(s1 - s0), s0 * 32, rows, lo, n, ctx->tscratch.p, ctx->tscratch.cap, dst[t]));
+                launches += kNsLaunches;
+                continue;
+            }
             CU(launch_text_encode(ctx->copy_stream, dict(t), reinterpret_cast<const uint8_t *>(m + tmarks), span,
                                   reinterpret_cast<const uint64_t *>(m), (uint32_t)(s1 - s0), s0 * 32, rows, lo, n,
                                   ctx->tscratch.p, ctx->tscratch.cap, dst[t]));
@@ -2350,7 +2380,7 @@ struct Sweep {
 
     // `text_row`: text staging and encode scratch bytes per staged row, planned into the staging's 1/16 of the budget
     Sweep(tad_ctx *c, const tad_job *j, PassOut &a, bool host_input, uint64_t budget, size_t text_row)
-        : ctx(c), job(j), acc(a), ns(!j->ns_ignore.empty() && (j->cols.src_ns || j->cols.dst_ns)),
+        : ctx(c), job(j), acc(a), ns(!j->ns_ignore.empty() && (has_col(j, 8) || has_col(j, 9))),
           mark(j->filtered() ? (j->text[0] ? 1 : 2) : 0)
     {
         size_t row_bytes = 0;
@@ -2365,7 +2395,7 @@ struct Sweep {
     size_t stage_bytes() const { return 2 * half_bytes; }
 
     // staging half h from row `at` as kernel input, with rows [lo, lo + n) of block `b` copied there on the copy stream
-    // (a null `b`: none); text slots are left to the encoder
+    // (a null `b`: none); text slots are left to the encoder (TextKeys)
     ColPtrs stage(const tad_columns *b, uint64_t lo, uint64_t n, int h, uint64_t at) const
     {
         ColPtrs c{};
@@ -2373,7 +2403,7 @@ struct Sweep {
         for (int i = 0; i < 10; i++) {
             if (!staged(i)) continue;
             char *d = dst + col_bytes(i, at);
-            if (b && !(i < 2 && job->text[i]))
+            if (b && !is_text(job, i))
                 CU(cudaMemcpyAsync(d, static_cast<const char *>(col_ptr(*b, i)) + col_bytes(i, lo), col_bytes(i, n),
                                    b->mem == TAD_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
                                    ctx->copy_stream));
@@ -2656,20 +2686,23 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     const bool stream = job->stream;
     // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
     tad_columns pend{};
-    tad_text_column pend_txt[2]{};
+    tad_text_column pend_txt[4]{};
     bool have_pend = stream && next_block(job, pend, pend_txt);
     const tad_columns &hc = job->cols;
     const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
     const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
-    // host input: double-buffered chunk staging, at most 1/16 of the budget; text key slots: per staged row,
-    // kTextRowBytes of text staging (any IPv6 text) and the encode scratch
+    // host input: double-buffered chunk staging, at most 1/16 of the budget; text slots: per staged row, kTextRowBytes
+    // of text staging (any IPv6 text) and the encode scratch.  `text`: key slots with dictionaries; `staged_text`: those
+    // or namespace text slots that an ignore list tests (no dictionary), which share the staging one slot at a time
     const bool text = job->text[0] || job->text[1];
+    const bool ns_text = !job->ns_ignore.empty() && (job->text[2] || job->text[3]);
+    const bool staged_text = text || ns_text;
     constexpr size_t kTextRowBytes = 48;
     Sweep sw(ctx, job, acc, host_input, budget,
-             text ? kTextRowBytes + text_scratch_bytes(1u << 20) / (1u << 20) + 1 : 0);
+             staged_text ? kTextRowBytes + text_scratch_bytes(1u << 20) / (1u << 20) + 1 : 0);
     const uint64_t chunk = sw.chunk;
     size_t tmarks = 0, text_bytes = 0;
-    if (text && chunk) {
+    if (staged_text && chunk) {
         tmarks = exact_bytes((chunk / 32 + 2) * 8);
         text_bytes = alloc_bytes(tmarks + chunk * kTextRowBytes) + alloc_bytes(text_scratch_bytes(chunk));
     }
@@ -2707,10 +2740,14 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);   // [0, 64): rows per residue, [64]: pass cursor
     const unsigned long long *h_cnt = ctx->h_small;
     sw.f = row_filter(ctx, job, sw.ns);
+    if (ns_text) {                   // the ignore list's names, with its decode error flags cleared
+        ensure(ctx, ctx->nsl, job->ns_image.size());
+        CU(cudaMemcpyAsync(ctx->nsl.p, job->ns_image.data(), job->ns_image.size(), cudaMemcpyHostToDevice, ctx->copy_stream));
+    }
     sw.cnt = d_cnt;
     sw.cursor = d_cnt + kMaxPasses;
-    TextKeys tk{ctx, job, budget, tmarks, sw.mark, acc.launches, false, &pc};
-    if (text) sw.text = &tk;
+    TextKeys tk{ctx, job, budget, tmarks, sw.mark, ns_text, acc.launches, false, &pc};
+    if (staged_text) sw.text = &tk;
     bool count_only = false;         // the first round's rows are only counted (the store fell back, or the pass columns
                                      // gave way to the text key dictionaries)
     uint32_t sweeps = 0;
@@ -2769,8 +2806,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             uint64_t rows = 0, k = 0;
             ub = 0;
             tad_columns b{};
-            tad_text_column tx[2]{};
-            bool got = have_pend ? (b = pend, tx[0] = pend_txt[0], tx[1] = pend_txt[1], true) : next_block(job, b, tx);
+            tad_text_column tx[4]{};
+            bool got = have_pend ? (b = pend, std::copy(pend_txt, pend_txt + 4, tx), true) : next_block(job, b, tx);
             have_pend = false;
             if (sweeps == 0 && host_budget && P > 1)         // the hint plans passes: the round goes to the store
                 rs.start(ostage_bytes);
@@ -2810,7 +2847,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             open = true;
         }
         sw.end(true);
-        if (text) tk.sync();
+        if (staged_text) tk.sync();
         if (sweeps > 0)
             for (int j = 0; j < kMaxPasses; j++)
                 if (h_cnt[j] != counts[j])
@@ -3440,17 +3477,19 @@ int stream_gate(tad_job *job, std::unique_lock<std::mutex> &lk)
 
 // A streamed block: host or device memory, fewer than 2^32 rows, flow_end and value, and the first block's column set,
 // text slots included.  A text slot: host memory, its u32 column NULL, one mark per 32 rows from 0, not decreasing, none
-// past the column's end.
+// past the column's end.  Namespace slots: all text or all u32, text only with the ignore list as names and names only
+// with text.
 int check_block(const tad_job *job, const tad_columns *b, const tad_text_column *const *txt, char *msg, size_t n)
 {
-    for (int t = 0; t < 2; t++) {
+    static const char *kSlot[4] = {"src_ip", "dst_ip", "src_ns", "dst_ns"};
+    for (int t = 0; t < 4; t++) {
         const tad_text_column *x = txt[t];
         if (!x) continue;
         if (b->mem != TAD_MEM_HOST) {
             snprintf(msg, n, "invalid request: text key columns are accepted in host blocks only");
             return TAD_ERR_INVALID_ARG;
         }
-        if (col_ptr(*b, t)) {
+        if (col_ptr(*b, t < 2 ? t : t + 6)) {
             snprintf(msg, n, "invalid request: a slot given as text must have its u32 column NULL");
             return TAD_ERR_INVALID_ARG;
         }
@@ -3465,11 +3504,24 @@ int check_block(const tad_job *job, const tad_columns *b, const tad_text_column 
                 return TAD_ERR_INVALID_ARG;
             }
     }
+    if ((txt[2] || txt[3]) && (b->src_ns || b->dst_ns)) {
+        snprintf(msg, n, "invalid request: a streamed block gives one namespace column as text and the other as u32 ids");
+        return TAD_ERR_INVALID_ARG;
+    }
+    if ((txt[2] || txt[3]) && job->spec.n_ns_ignore) {
+        snprintf(msg, n, "invalid request: namespace text needs the ignore list as names (tad_submit_stream_filtered_ns), "
+                 "not as ids");
+        return TAD_ERR_INVALID_ARG;
+    }
+    if (job->ns_names && (b->src_ns || b->dst_ns)) {
+        snprintf(msg, n, "invalid request: an ignore list of names needs the namespace columns as text, not as u32 ids");
+        return TAD_ERR_INVALID_ARG;
+    }
     if (job->in.pushed > 0)
-        for (int t = 0; t < 2; t++)
+        for (int t = 0; t < 4; t++)
             if (job->text[t] != (txt[t] != nullptr)) {
                 snprintf(msg, n, "invalid request: a streamed block gives %s as %s, the job's first block did not",
-                         t ? "dst_ip" : "src_ip", txt[t] ? "text" : "u32");
+                         kSlot[t], txt[t] ? "text" : "u32");
                 return TAD_ERR_INVALID_ARG;
             }
     if (b->mem != TAD_MEM_HOST && b->mem != TAD_MEM_DEVICE) {
@@ -3728,7 +3780,16 @@ int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t 
                                tad_job **out)
 {
     if (!filter) return tad_submit_stream(ctx, spec, rows_hint, out);
+    const tad_stream_filter_ns f{*filter, 0, nullptr, nullptr};
+    return tad_submit_stream_filtered_ns(ctx, spec, rows_hint, &f, out);
+}
+
+int tad_submit_stream_filtered_ns(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint,
+                                  const tad_stream_filter_ns *filter_ns, tad_job **out)
+{
+    if (!filter_ns) return tad_submit_stream(ctx, spec, rows_hint, out);
     if (!ctx || !spec || !out) return TAD_ERR_INVALID_ARG;
+    const tad_stream_filter *filter = &filter_ns->rows;
     const char *bad = nullptr;
     for (int t = 0; t < 2 && !bad; t++) {
         const int op = filter->op[t];
@@ -3740,6 +3801,15 @@ int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t 
                 if (filter->pattern[t][k] >= 0x80) bad = "an ICONTAINS pattern holds a byte >= 0x80 (ASCII only)";
     }
     if (!bad && (filter->proto_eq < -1 || filter->proto_eq > 255)) bad = "proto_eq is outside -1..255";
+    const uint32_t nn = filter_ns->n_ns_ignore;
+    const uint64_t *off = filter_ns->ns_ignore_offsets;
+    if (!bad && nn && (!off || !filter_ns->ns_ignore_bytes)) bad = "the ignore list's bytes or offsets are NULL";
+    if (!bad && nn && spec->n_ns_ignore) bad = "the ignore list is given both as names and as ids";
+    if (!bad && nn > kNsMaxNames) bad = "the ignore list holds more than 1024 names";
+    if (!bad && nn && off[0] != 0) bad = "the ignore list's offsets do not start at 0";
+    for (uint32_t k = 0; k < nn && !bad; k++)
+        if (off[k + 1] < off[k]) bad = "the ignore list's offsets decrease";
+    if (!bad && nn && off[nn] > kNsMaxBytes) bad = "the ignore list's names hold more than 32 KiB";
     tad_job *job = new tad_job();
     job->stream = true;
     job->rows_hint = rows_hint;
@@ -3760,26 +3830,40 @@ int tad_submit_stream_filtered(tad_ctx *ctx, const tad_job_spec *spec, uint64_t 
             job->name_pat[t].assign(filter->pattern[t], filter->pattern[t] + filter->pattern_len[t]);
     }
     job->proto_eq = filter->proto_eq;
+    if (nn) {                    // the namespace text slots stage kNsListed for a listed name: the row filter drops it
+        job->ns_image = ns_list_image(filter_ns->ns_ignore_bytes, off, nn);
+        job->ns_names = nn;
+        job->ns_ignore.assign(1, kNsListed);
+    }
     tad_columns none{};
     return submit_job(ctx, job, spec, &none, out);
 }
 
-int tad_stream_push(tad_job *job, const tad_columns *block) { return tad_stream_push_text(job, block, nullptr, nullptr); }
+int tad_stream_push(tad_job *job, const tad_columns *block)
+{
+    return tad_stream_push_text_ns(job, block, nullptr, nullptr, nullptr, nullptr);
+}
 
 int tad_stream_push_text(tad_job *job, const tad_columns *block, const tad_text_column *src_ip, const tad_text_column *dst_ip)
 {
+    return tad_stream_push_text_ns(job, block, src_ip, dst_ip, nullptr, nullptr);
+}
+
+int tad_stream_push_text_ns(tad_job *job, const tad_columns *block, const tad_text_column *src_ip,
+                            const tad_text_column *dst_ip, const tad_text_column *src_ns, const tad_text_column *dst_ns)
+{
     if (!job || !block) return TAD_ERR_INVALID_ARG;
-    if ((src_ip || dst_ip) && !job->stream) return TAD_ERR_UNSUPPORTED;
+    if ((src_ip || dst_ip || src_ns || dst_ns) && !job->stream) return TAD_ERR_UNSUPPORTED;
     std::unique_lock<std::mutex> lk(job->mu);
     int rc = stream_gate(job, lk);
     if (rc != TAD_OK) return rc;
     char msg[200];
-    const tad_text_column *txt[2] = {src_ip, dst_ip};
+    const tad_text_column *txt[4] = {src_ip, dst_ip, src_ns, dst_ns};
     rc = check_block(job, block, txt, msg, sizeof(msg));
     if (rc != TAD_OK) return stream_abort(job, lk, rc, msg);
     if (job->in.pushed == 0) {                         // the column set of the job
         job->cols = *block;
-        for (int t = 0; t < 2; t++) job->text[t] = txt[t] != nullptr;
+        for (int t = 0; t < 4; t++) job->text[t] = txt[t] != nullptr;
     }
 
     // one block of look-ahead: hand this one over once the worker has taken the previous one, then return once the
@@ -3787,7 +3871,7 @@ int tad_stream_push_text(tad_job *job, const tad_columns *block, const tad_text_
     while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
     if (finished(job)) return job->st.error;
     job->in.blk = *block;
-    for (int t = 0; t < 2; t++) job->in.txt[t] = txt[t] ? *txt[t] : tad_text_column{};
+    for (int t = 0; t < 4; t++) job->in.txt[t] = txt[t] ? *txt[t] : tad_text_column{};
     job->in.has_blk = true;
     const uint64_t k = job->in.pushed++;
     job->cv.notify_all();

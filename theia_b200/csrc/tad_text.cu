@@ -1,5 +1,9 @@
-// Text key slots on the device (tad_text.h): decode of Native String column bytes, and the job's dictionary of names.
+// Text key slots on the device (tad_text.h): decode of Native String column bytes, the job's dictionary of names, and
+// the namespace ignore list tested on namespace text.
 // A translation unit of its own, so that no existing kernel's unit gains a CUB instance or a constant.
+#include <algorithm>
+#include <cstring>
+
 #include <cub/device/device_scan.cuh>
 
 #include "tad_text.h"
@@ -13,7 +17,7 @@ constexpr uint32_t kNone = 0xffffffffu;
 constexpr uint64_t kByteBits = 40;           // scan word: new names << 40 | their bytes (a chunk has < 2^24 rows)
 constexpr int kThreads = 256;
 
-__device__ __forceinline__ uint64_t name_hash(const uint8_t *s, uint32_t len)
+__host__ __device__ __forceinline__ uint64_t name_hash(const uint8_t *s, uint32_t len)
 {
     uint64_t h = 1469598103934665603ull;     // FNV-1a, then a fold so that the low (slot) bits see the high bytes
     for (uint32_t k = 0; k < len; k++) h = (h ^ s[k]) * 1099511628211ull;
@@ -282,6 +286,54 @@ __global__ void text_mark_kernel(TextMark m, uint64_t n)
     if (!keep) m.mark[i] |= kTextDropped;
 }
 
+// Whether the name s (m bytes, hash h) is in an ignore list of `names` names sorted by hash: every entry whose hash
+// equals h is compared byte for byte, so a hash collision never lists a name.
+__host__ __device__ __forceinline__ bool ns_listed(uint32_t names, const uint64_t *hash, const uint32_t *off,
+                                                   const uint8_t *bytes, const uint8_t *s, uint32_t m, uint64_t h)
+{
+    uint32_t lo = 0, hi = names;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (hash[mid] < h) lo = mid + 1; else hi = mid;
+    }
+    for (; lo < names && hash[lo] == h; lo++)
+        if (same_bytes(s, m, bytes + off[lo], off[lo + 1] - off[lo])) return true;
+    return false;
+}
+
+// Where an ignore list image's parts start, past its state words.
+struct NsParts {
+    size_t hash, off, bytes, end;
+};
+__host__ __device__ __forceinline__ NsParts ns_parts(uint32_t names, size_t nbytes)
+{
+    NsParts p;
+    p.hash = 0;
+    p.off = p.hash + (size_t)names * 8;
+    p.bytes = p.off + ((size_t)names + 1) * 4;
+    p.end = (p.bytes + nbytes + 7) & ~size_t(7);
+    return p;
+}
+
+// One thread per row: the row's namespace (decoded into off / len) tested against the list, held in shared memory.
+__global__ void ns_match_kernel(const uint64_t *__restrict__ list, uint32_t words, uint32_t names,
+                                const uint8_t *__restrict__ text, const uint32_t *__restrict__ off,
+                                const uint32_t *__restrict__ len, uint64_t n, uint32_t *__restrict__ verdict)
+{
+    extern __shared__ uint64_t sh[];
+    for (uint32_t k = threadIdx.x; k < words; k += blockDim.x) sh[k] = list[k];
+    __syncthreads();
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const NsParts p = ns_parts(names, 0);
+    const char *b = reinterpret_cast<const char *>(sh);
+    const uint8_t *s = text + off[i];
+    const uint32_t m = len[i];
+    const bool hit = ns_listed(names, reinterpret_cast<const uint64_t *>(b + p.hash), reinterpret_cast<const uint32_t *>(b + p.off),
+                               reinterpret_cast<const uint8_t *>(b + p.bytes), s, m, name_hash(s, m));
+    verdict[i] = hit ? kNsListed : 0u;
+}
+
 unsigned grid(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 }  // namespace
@@ -339,6 +391,48 @@ cudaError_t launch_text_encode(cudaStream_t st, const TextDict &d, const uint8_t
     return cudaGetLastError();
 }
 
+std::vector<uint8_t> ns_list_image(const uint8_t *bytes, const uint64_t *off, uint32_t names, uint64_t hash_mask)
+{
+    std::vector<uint32_t> order(names);
+    std::vector<uint64_t> h(names);
+    for (uint32_t k = 0; k < names; k++) {
+        order[k] = k;
+        h[k] = name_hash(bytes + off[k], (uint32_t)(off[k + 1] - off[k])) & hash_mask;
+    }
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return h[a] < h[b]; });
+    const NsParts p = ns_parts(names, off[names] - off[0]);
+    std::vector<uint8_t> img(kNsStateWords * 8 + p.end, 0);
+    uint8_t *q = img.data() + kNsStateWords * 8;
+    uint32_t at = 0;
+    for (uint32_t j = 0; j < names; j++) {
+        const uint32_t k = order[j], m = (uint32_t)(off[k + 1] - off[k]);
+        memcpy(q + p.hash + 8 * j, &h[k], 8);
+        memcpy(q + p.off + 4 * j, &at, 4);
+        if (m) memcpy(q + p.bytes + at, bytes + off[k], m);
+        at += m;
+    }
+    memcpy(q + p.off + 4 * names, &at, 4);
+    return img;
+}
+
+cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, unsigned long long *state,
+                            const uint8_t *text, uint64_t span_bytes, const uint64_t *marks, uint32_t nseg, uint64_t seg0_row,
+                            uint64_t block_rows, uint64_t lo, uint64_t n, void *scratch, size_t scratch_bytes,
+                            uint32_t *verdict)
+{
+    if (n == 0) return cudaSuccess;
+    const size_t held = image_bytes - kNsStateWords * 8;      // the hashes, offsets and bytes: a multiple of 8
+    if (scratch_bytes < text_scratch_bytes(n) || n >= (1ull << 24) || names > kNsMaxNames ||
+        held > ns_parts(kNsMaxNames, kNsMaxBytes).end)
+        return cudaErrorInvalidValue;
+    ChunkScratch c = carve(scratch, n);
+    text_decode_kernel<<<(nseg + 127) / 128, 128, 0, st>>>(text, span_bytes, marks, nseg, seg0_row, block_rows, lo, n, c.off,
+                                                          c.len, state);
+    const uint64_t *list = reinterpret_cast<const uint64_t *>(static_cast<const char *>(image) + kNsStateWords * 8);
+    ns_match_kernel<<<grid(n), kThreads, held, st>>>(list, (uint32_t)(held / 8), names, text, c.off, c.len, n, verdict);
+    return cudaGetLastError();
+}
+
 }  // namespace tad
 
 // The device's name predicate run on the host, for the tests: 1 when `name` passes op / pattern, 0 when not, -1 for a bad op.
@@ -347,4 +441,17 @@ extern "C" int tad_debug_name_match(int op, const uint8_t *name, uint32_t name_l
 {
     if (op < tad::kNameAny || op > tad::kNameIContains) return -1;
     return tad::name_match(op, name, name_len, pattern, pattern_len) ? 1 : 0;
+}
+
+// The device's namespace ignore-list test run on the host, for the tests: 1 when `name` is one of the `names` names of
+// the list (name k = bytes[offsets[k] .. offsets[k + 1])), else 0.  `hash_mask` is ANDed into every hash (~0: as the
+// engine hashes; a narrow mask forces collisions).
+extern "C" int tad_debug_ns_match(const uint8_t *name, uint32_t name_len, const uint8_t *bytes, const uint64_t *offsets,
+                                  uint32_t names, uint64_t hash_mask)
+{
+    const std::vector<uint8_t> img = tad::ns_list_image(bytes, offsets, names, hash_mask);
+    const uint8_t *q = img.data() + tad::kNsStateWords * 8;
+    const tad::NsParts p = tad::ns_parts(names, 0);
+    return tad::ns_listed(names, reinterpret_cast<const uint64_t *>(q + p.hash), reinterpret_cast<const uint32_t *>(q + p.off),
+                          q + p.bytes, name, name_len, tad::name_hash(name, name_len) & hash_mask) ? 1 : 0;
 }

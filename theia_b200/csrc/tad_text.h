@@ -3,6 +3,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <vector>
 
 #include <cuda_runtime.h>
 
@@ -68,5 +69,26 @@ struct TextMark {
     uint32_t *mark;
 };
 cudaError_t launch_text_mark(cudaStream_t st, const TextMark &m, uint64_t n);
+
+// The namespace ignore list of a job whose namespace slots are text (tad_submit_stream_filtered_ns).  Its device image,
+// built once per job on the host: kNsStateWords state words (slot t's decode error flag at word 8t + 2, as a TextDict's
+// state[2]), then the names' 64-bit hashes in ascending order, the u32 offsets of their bytes (names + 1) and the bytes,
+// padded to 8 bytes.  The kernel holds everything after the state words in shared memory.
+constexpr uint32_t kNsMaxNames = 1024, kNsMaxBytes = 32768;
+constexpr int kNsStateWords = 16;
+// The verdict a namespace slot stages per row: the row filter's one-entry ignore list {kNsListed} drops listed rows.
+constexpr uint32_t kNsListed = 1;
+// `hash_mask` is ANDed into every hash (~0 in the engine; a narrow mask makes hashes collide, for the tests).
+std::vector<uint8_t> ns_list_image(const uint8_t *bytes, const uint64_t *off, uint32_t names, uint64_t hash_mask = ~0ull);
+
+// Rows [lo, lo + n) of a block's namespace text slot (staged as for launch_text_encode) -> verdict[i] = kNsListed when
+// the row's name is in the list `image` (device memory, `names` names, `image_bytes` long), else 0.  A segment that does
+// not decode sets state[2] (the slot's state words) and its rows read as the empty name.  Two launches; `scratch` as
+// for launch_text_encode.
+cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, unsigned long long *state,
+                            const uint8_t *text, uint64_t span_bytes, const uint64_t *marks, uint32_t nseg, uint64_t seg0_row,
+                            uint64_t block_rows, uint64_t lo, uint64_t n, void *scratch, size_t scratch_bytes,
+                            uint32_t *verdict);
+constexpr int kNsLaunches = 2;
 
 }  // namespace tad

@@ -206,6 +206,7 @@ def _block_columns(block):
 
 
 _EMPTY = C.c_uint64(0)     # a non-NULL address for the columns of an empty numpy block
+_TEXT_SLOTS = ("src_ip", "dst_ip", "src_ns", "dst_ns")
 
 
 class StreamJob(Job):
@@ -217,12 +218,14 @@ class StreamJob(Job):
         self._last = None
 
     def push(self, block, text=None):
-        """``text``: {"src_ip" / "dst_ip": (column bytes, marks)} -- those slots as Native String column bytes with the
-        byte offset of every 32nd row (tad_stream_push_text), encoded into job-wide ids on the GPU."""
+        """``text``: {"src_ip" / "dst_ip" / "src_ns" / "dst_ns": (column bytes, marks)} -- those slots as Native String
+        column bytes with the byte offset of every 32nd row (tad_stream_push_text_ns).  The address slots are encoded
+        into job-wide ids on the GPU; the namespace slots are tested there against the ignore list given as names
+        (submit_stream's ``ns_ignore_names``)."""
         c, keep = _block_columns(block)
         if text:
             tx = []
-            for slot in ("src_ip", "dst_ip"):
+            for slot in _TEXT_SLOTS:
                 if slot not in text:
                     tx.append(None)
                     continue
@@ -236,7 +239,7 @@ class StreamJob(Job):
                 keep = [keep, data, marks]
                 tx.append(t)
             keep = [keep, tx]
-            rc = self.eng.lib.tad_stream_push_text(self.h, C.byref(c), *(C.byref(t) if t is not None else None for t in tx))
+            rc = self.eng.lib.tad_stream_push_text_ns(self.h, C.byref(c), *(C.byref(t) if t is not None else None for t in tx))
         else:
             rc = self.eng.lib.tad_stream_push(self.h, C.byref(c))
         if rc != 0:
@@ -362,19 +365,22 @@ class TadEngine:
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
                       check: bool = True, text_filter=None, share: bool = False,
-                      fit_beside: bool = False) -> StreamJob:
+                      fit_beside: bool = False, ns_ignore_names=None) -> StreamJob:
         """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
         ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
         (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
         for every row.  ``share``: TAD_FLAG_SHARE, the job takes part in fit sharing (set_fit_sharing): an ARIMA job's
         fit yields, an EWMA or DBSCAN job may run while a fit is parked.  ``fit_beside``: TAD_FLAG_FIT_BESIDE, with
-        ``share`` an ARIMA job queued behind another ARIMA job's fit may fit beside it once its first block is pushed."""
+        ``share`` an ARIMA job queued behind another ARIMA job's fit may fit beside it once its first block is pushed.
+        ``ns_ignore_names``: the namespace ignore list as names (bytes), for a job that pushes its namespace columns as
+        text (tad_submit_stream_filtered_ns); ``ns_ignore`` (ids) is then empty."""
         keep = []
         spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share, fit_beside)
         h = C.c_void_p()
-        if text_filter is None:
+        if text_filter is None and ns_ignore_names is None:
             rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
         else:
+            text_filter = text_filter or {}
             flt = L.TadStreamFilter()
             for t, slot in enumerate(("src_ip", "dst_ip")):
                 op, pat = text_filter.get(slot, ("any", b""))
@@ -385,7 +391,17 @@ class TadEngine:
                 flt.pattern[t] = C.cast(buf, C.c_void_p).value
                 flt.pattern_len[t] = len(pat)
             flt.proto_eq = int(text_filter.get("proto_eq", -1))
-            rc = self.lib.tad_submit_stream_filtered(self.ctx, C.byref(spec), int(rows_hint), C.byref(flt), C.byref(h))
+            if ns_ignore_names is None:
+                rc = self.lib.tad_submit_stream_filtered(self.ctx, C.byref(spec), int(rows_hint), C.byref(flt), C.byref(h))
+            else:
+                names = [bytes(x) for x in ns_ignore_names]
+                data = np.frombuffer(b"".join(names) or b"\0", dtype=np.uint8)
+                off = np.zeros(len(names) + 1, dtype=np.uint64)
+                off[1:] = np.cumsum([len(x) for x in names], dtype=np.uint64)
+                keep += [data, off]
+                fns = L.TadStreamFilterNs(flt, len(names), data.ctypes.data, off.ctypes.data)
+                rc = self.lib.tad_submit_stream_filtered_ns(self.ctx, C.byref(spec), int(rows_hint), C.byref(fns),
+                                                            C.byref(h))
         return self._checked(StreamJob(self, h, keep), rc, check)
 
     def run(self, table: dict, on_job=None, memory_budget: int | None = None, **kw):
