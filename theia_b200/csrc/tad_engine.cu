@@ -394,8 +394,11 @@ void ensure(tad_ctx *ctx, DevBuf &b, size_t bytes)
 }
 
 // A pass whose oversized-bucket spill scratch or result buffer (sizes known only while it runs) would not fit the budget:
-// the job driver splits it by the next hash bit.
-struct PassSplit {};
+// the job driver splits it by the next hash bit.  `what` needed `bytes` beside the `held` bytes of workspace.
+struct PassSplit {
+    const char *what = "";
+    size_t bytes = 0, held = 0;
+};
 
 // Lifetimes of the workspace buffers (workspace_bufs).  kJobs and kPasses name the events a buffer is kept across (the
 // others free it); kParked, what a parked ARIMA pass takes out of the context.
@@ -1754,7 +1757,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
     mark(TAD_PHASE_GROUP);
     if (n_big) {
         const size_t need = spill_scratch_bytes(big_rows);
-        if (!fits(ctx, ctx->spill, need)) throw PassSplit{};
+        if (!fits(ctx, ctx->spill, need)) throw PassSplit{"oversized-bucket scratch", need, ctx->held};
         ensure(ctx, ctx->spill, need);
         int l = 0;
         CU(run_spill(st, seg, entries, offsets, big_list, big_base, n_big, big_rows, ctx->spill.p, ctx->spill.cap, csr_v, csr_t,
@@ -1788,7 +1791,7 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         shape.out_cap = out_cap;
         z = pipe_sizes(shape);
         L = out_layout(out_cap);
-        if (!fits(ctx, ctx->outb, z.outb)) throw PassSplit{};
+        if (!fits(ctx, ctx->outb, z.outb)) throw PassSplit{"result buffer", z.outb, ctx->held};
         ensure(ctx, ctx->outb, z.outb);
         oc = out_cols(ctx->outb.p, L);
         CU(cudaMemsetAsync(d_stats + ST_OUTCOUNT, 0, 4, st));
@@ -2926,9 +2929,13 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         if (!opt && pass_need(ctx, job, rows, cap, false, stage_bytes, false) > budget) free_pass_buffers(ctx);
         try {
             run_pipeline(ctx, job, pc.as_input(rows), false, !opt, o);
-        } catch (const PassSplit &) {
+        } catch (const PassSplit &e) {
             CU(cudaStreamSynchronize(st));
-            if (M >= (uint32_t)kMaxPasses) too_big(rows);
+            // the planned workspace fitted; what outgrew the budget is known only now (a result rerun, a spill)
+            if (M >= (uint32_t)kMaxPasses)
+                fail(TAD_ERR_NOMEM, "the %s of a 1/%d hash range of the table (%llu rows) needs %zu bytes beside the %zu bytes "
+                     "of workspace the pass holds: more than the memory budget of %llu bytes", e.what, kMaxPasses,
+                     (unsigned long long)rows, e.bytes, e.held, (unsigned long long)budget);
             return true;
         }
         return false;
