@@ -117,6 +117,8 @@ def load():
     L.tad_cancel.argtypes = [C.c_void_p]
     L.tad_release.argtypes = [C.c_void_p]
     L.tad_get_unique_id.argtypes = [C.c_void_p, C.c_size_t]
+    L.tad_debug_loopback_id.argtypes = [C.c_int, C.c_void_p, C.c_size_t]
+    L.tad_debug_loopback_release.argtypes = [C.c_void_p, C.c_size_t]
     L.tad_job_progress.argtypes = [C.c_void_p, C.POINTER(TadProgress)]
     L.tad_set_memory_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]

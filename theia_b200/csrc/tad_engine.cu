@@ -1277,7 +1277,7 @@ cudaError_t unmap_peers(tad_ctx *ctx)
 {
     cudaError_t err = cudaSuccess;
     for (void *&p : ctx->peer_x) {
-        const cudaError_t e = p ? cudaIpcCloseMemHandle(p) : cudaSuccess;
+        const cudaError_t e = p ? nccl_ipc_unmap(&ctx->nccl, p) : cudaSuccess;
         if (err == cudaSuccess) err = e;
         p = nullptr;
     }
@@ -1497,23 +1497,18 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         // the decision must be the same on every rank: it is taken on the size the ranks last agreed on, not on the local
         // capacity (which may differ when one rank's allocation fell back to the exact size under memory pressure)
         if (need <= ctx->x_agreed && ctx->peers_mapped) return;
-        static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
         CU(unmap_peers(ctx));
         memset(ctx->h_small, 0, G * 8);
         gather_small(ctx, G, false);
         ensure(ctx, ctx->xbuf, need);
-        cudaIpcMemHandle_t mine;
-        CU(cudaIpcGetMemHandle(&mine, ctx->xbuf.p));
         memset(ctx->h_small, 0, G * 8);
         ctx->h_small[0] = ctx->xbuf.cap;
-        memcpy(ctx->h_small + 2, &mine, sizeof(mine));
+        CU(nccl_ipc_export(&ctx->nccl, ctx->xbuf.p, ctx->h_small + 2));      // a 64-byte handle in words 2..9
         gather_small(ctx, G, false);
         for (int r = 0; r < world; r++) {
             if (r == me) continue;
-            cudaIpcMemHandle_t h;
-            memcpy(&h, ctx->h_small + G * (1 + r) + 2, sizeof(h));
             if (ctx->h_small[G * (1 + r)] < need) fail(TAD_ERR_INTERNAL, "rank %d exports a smaller partition buffer", r);
-            cudaError_t e = cudaIpcOpenMemHandle(&ctx->peer_x[r], h, cudaIpcMemLazyEnablePeerAccess);
+            cudaError_t e = nccl_ipc_map(&ctx->nccl, ctx->h_small + G * (1 + r) + 2, &ctx->peer_x[r]);
             if (e != cudaSuccess) {
                 cudaGetLastError();
                 ctx->peer_x[r] = nullptr;
@@ -3214,6 +3209,8 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
 void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
 {
     CU(cudaSetDevice(ctx->cfg.device));
+    // a loopback rank (ranks as contexts of one process) waits for its turn on the device; released by worker_main
+    if (nccl_job_begin(&ctx->nccl)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
     // several GPUs under a budget: every rank joins the plan all-gather, a job cancelled before it started too
     const uint64_t multi_budget = ctx->cfg.world_size > 1 ? ctx->budget.load() : 0;
     if (!multi_budget && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
@@ -3371,6 +3368,7 @@ void worker_main(tad_ctx *ctx)
             ctx->queue.pop_front();
         }
         run_one(ctx, job, 0);
+        nccl_job_end(&ctx->nccl);      // a loopback rank's streams are idle: its peers may take the device
     }
 }
 
@@ -3651,6 +3649,9 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
         return TAD_ERR_CUDA;
     }
     if (cfg->world_size > 1) {
+        ctx->nccl.streams[0] = ctx->stream;
+        ctx->nccl.streams[1] = ctx->copy_stream;
+        ctx->nccl.streams[2] = ctx->d2h_stream;
         int rc = nccl_comm_init(&ctx->nccl, cfg->world_size, cfg->rank, cfg->nccl_unique_id, cfg->nccl_unique_id_bytes);
         if (rc != 0) {
             tad_shutdown(ctx);

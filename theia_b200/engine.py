@@ -319,6 +319,26 @@ class TadEngine:
             raise TadError(rc, "tad_get_unique_id")
         return buf.raw
 
+    @staticmethod
+    def loopback_id(world_size: int) -> bytes:
+        """A 128-byte id for ``world_size`` rank engines on ONE device in this process (tad_debug_loopback_id): passed
+        as their ``nccl_unique_id``, they talk through an in-process loopback instead of NCCL and CUDA IPC, and take
+        turns on the device.  For tests of the multi-rank paths on a single GPU.  Once the ranks are created (or their
+        creation failed), release_loopback_id(id) drops it, so that no context joins it later and an id not every rank
+        joined is not kept for the life of the process."""
+        buf = C.create_string_buffer(128)
+        rc = L.load().tad_debug_loopback_id(int(world_size), buf, 128)
+        if rc != 0:
+            raise TadError(-1, "tad_debug_loopback_id(%d)" % world_size)
+        return buf.raw
+
+    @staticmethod
+    def release_loopback_id(uid: bytes):
+        """tad_debug_loopback_release: the ranks that joined keep their group; no further context may join it."""
+        buf = C.create_string_buffer(bytes(uid), 128)
+        if L.load().tad_debug_loopback_release(buf, 128) != 0:
+            raise TadError(-1, "tad_debug_loopback_release")
+
     def alloc_columns(self, capacity: int, mem: int = L.TAD_MEM_HOST) -> Columns:
         return Columns(self, capacity, mem)
 
