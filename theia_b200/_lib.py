@@ -106,6 +106,19 @@ def load():
                                                 C.POINTER(C.c_void_p)]
     L.tad_debug_name_match.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     L.tad_debug_ns_match.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64]
+    L.tad_debug_name_hash.restype = C.c_uint64
+    L.tad_debug_name_hash.argtypes = [C.c_void_p, C.c_uint32]
+    L.tad_debug_text_dict_new.argtypes = [C.c_int, C.c_uint32, C.c_uint64, C.POINTER(C.c_void_p)]
+    L.tad_debug_text_dict_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_uint64,
+                                             C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
+    L.tad_debug_text_dict_grow.argtypes = [C.c_void_p, C.c_uint32]
+    L.tad_debug_text_dict_freeze.argtypes = [C.c_void_p]
+    L.tad_debug_text_dict_names.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_void_p,
+                                            C.c_void_p, C.c_void_p]
+    L.tad_debug_text_dict_free.argtypes = [C.c_void_p]
+    L.tad_debug_ns_match_device.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p,
+                                            C.c_uint64, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64,
+                                            C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
     L.tad_stream_push.argtypes = [C.c_void_p, C.POINTER(TadColumns)]
     L.tad_stream_end.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
     L.tad_stream_push_text.argtypes = [C.c_void_p, C.POINTER(TadColumns), C.POINTER(TadTextColumn), C.POINTER(TadTextColumn)]

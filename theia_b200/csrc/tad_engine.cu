@@ -225,6 +225,8 @@ struct tad_ctx {
     bool stop = false;
     std::atomic<int> stopping{0};                   // tad_shutdown: a streamed job waiting for input is cancelled
     int debug_logb = -1;
+    uint64_t text_mask = ~0ull;  // TAD_DEBUG_TEXT_MASK (hex): ANDed into the name hashes of the text dictionaries and the
+                                 // ignore list, so that the tests can make names collide
     int debug_target = 0;      // TAD_GROUP_TARGET: mean rows per bucket (tuning)
     int num_sms = 132;
     // device workspace (grow-only, reused across jobs; jobs are serialized by the worker)
@@ -2150,7 +2152,7 @@ struct TextKeys {
         auto &d = ctx->tdict[t];
         return TextDict{(unsigned long long *)d.slots.p, (uint32_t *)d.minrow.p, (uint32_t *)d.slot_id.p, d.cap,
                         (uint8_t *)d.arena.p, (uint64_t *)d.off.p, (uint64_t *)d.hash.p, (unsigned long long *)d.state.p,
-                        frozen ? 1u : 0u};
+                        frozen ? 1u : 0u, ctx->text_mask};
     }
     // text slot t is read: a key slot, or a namespace slot of a job whose ignore list filters rows
     bool read(int t) const { return job->text[t] && (t < 2 || ns); }
@@ -2307,7 +2309,7 @@ struct TextKeys {
             CU(cudaMemcpyAsync(m, tx[t].marks + s0, (s1 - s0) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
             if (span) CU(cudaMemcpyAsync(m + tmarks, tx[t].bytes + a, span, cudaMemcpyHostToDevice, ctx->copy_stream));
             if (t >= 2) {                         // a namespace: no dictionary, the row's verdict only
-                CU(launch_ns_match(ctx->copy_stream, ctx->nsl.p, job->ns_names, job->ns_image.size(),
+                CU(launch_ns_match(ctx->copy_stream, ctx->nsl.p, job->ns_names, job->ns_image.size(), ctx->text_mask,
                                    static_cast<unsigned long long *>(ctx->nsl.p) + 8 * (t - 2),
                                    reinterpret_cast<const uint8_t *>(m + tmarks), span, reinterpret_cast<const uint64_t *>(m),
                                    (uint32_t)(s1 - s0), s0 * 32, rows, lo, n, ctx->tscratch.p, ctx->tscratch.cap, dst[t]));
@@ -3605,6 +3607,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     ctx->cfg = *cfg;
     ctx->cfg.nccl_unique_id = nullptr;
     if (const char *e = getenv("TAD_DEBUG_LOGB")) ctx->debug_logb = atoi(e);
+    if (const char *e = getenv("TAD_DEBUG_TEXT_MASK")) ctx->text_mask = strtoull(e, nullptr, 16);
     if (const char *e = getenv("TAD_GROUP_TARGET")) ctx->debug_target = atoi(e);
     cudaDeviceGetAttribute(&ctx->num_sms, cudaDevAttrMultiProcessorCount, cfg->device);
     ctx->numa = numa_of_device(cfg->device);
@@ -3839,7 +3842,7 @@ int tad_submit_stream_filtered_ns(tad_ctx *ctx, const tad_job_spec *spec, uint64
     }
     job->proto_eq = filter->proto_eq;
     if (nn) {                    // the namespace text slots stage kNsListed for a listed name: the row filter drops it
-        job->ns_image = ns_list_image(filter_ns->ns_ignore_bytes, off, nn);
+        job->ns_image = ns_list_image(filter_ns->ns_ignore_bytes, off, nn, ctx->text_mask);
         job->ns_names = nn;
         job->ns_ignore.assign(1, kNsListed);
     }

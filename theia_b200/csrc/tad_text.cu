@@ -6,6 +6,7 @@
 
 #include <cub/device/device_scan.cuh>
 
+#include "../../include/theia_tad.h"
 #include "tad_text.h"
 
 namespace tad {
@@ -113,7 +114,7 @@ __global__ void text_probe_kernel(TextDict d, const uint8_t *__restrict__ text, 
     if (i >= n) return;
     const uint8_t *s = text + off[i];
     const uint32_t m = len[i];
-    const uint64_t h = name_hash(s, m);
+    const uint64_t h = name_hash(s, m) & d.hash_mask;
     const uint32_t tag = (uint32_t)(h >> 32), mask = d.cap - 1;
     uint32_t p = (uint32_t)h & mask;
     for (;;) {
@@ -182,7 +183,7 @@ __global__ void text_assign_kernel(TextDict d, const uint8_t *__restrict__ text,
     const uint32_t m = len[i];
     for (uint32_t k = 0; k < m; k++) d.arena[at + k] = s[k];
     d.off[id] = at;
-    const uint64_t h = name_hash(s, m);
+    const uint64_t h = name_hash(s, m) & d.hash_mask;
     d.hash[id] = h;
     const uint32_t p = slot_of[i];
     d.slot_id[p] = id;
@@ -316,7 +317,7 @@ __host__ __device__ __forceinline__ NsParts ns_parts(uint32_t names, size_t nbyt
 }
 
 // One thread per row: the row's namespace (decoded into off / len) tested against the list, held in shared memory.
-__global__ void ns_match_kernel(const uint64_t *__restrict__ list, uint32_t words, uint32_t names,
+__global__ void ns_match_kernel(const uint64_t *__restrict__ list, uint32_t words, uint32_t names, uint64_t hash_mask,
                                 const uint8_t *__restrict__ text, const uint32_t *__restrict__ off,
                                 const uint32_t *__restrict__ len, uint64_t n, uint32_t *__restrict__ verdict)
 {
@@ -330,7 +331,7 @@ __global__ void ns_match_kernel(const uint64_t *__restrict__ list, uint32_t word
     const uint8_t *s = text + off[i];
     const uint32_t m = len[i];
     const bool hit = ns_listed(names, reinterpret_cast<const uint64_t *>(b + p.hash), reinterpret_cast<const uint32_t *>(b + p.off),
-                               reinterpret_cast<const uint8_t *>(b + p.bytes), s, m, name_hash(s, m));
+                               reinterpret_cast<const uint8_t *>(b + p.bytes), s, m, name_hash(s, m) & hash_mask);
     verdict[i] = hit ? kNsListed : 0u;
 }
 
@@ -415,7 +416,8 @@ std::vector<uint8_t> ns_list_image(const uint8_t *bytes, const uint64_t *off, ui
     return img;
 }
 
-cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, unsigned long long *state,
+cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, uint64_t hash_mask,
+                            unsigned long long *state,
                             const uint8_t *text, uint64_t span_bytes, const uint64_t *marks, uint32_t nseg, uint64_t seg0_row,
                             uint64_t block_rows, uint64_t lo, uint64_t n, void *scratch, size_t scratch_bytes,
                             uint32_t *verdict)
@@ -429,7 +431,8 @@ cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, 
     text_decode_kernel<<<(nseg + 127) / 128, 128, 0, st>>>(text, span_bytes, marks, nseg, seg0_row, block_rows, lo, n, c.off,
                                                           c.len, state);
     const uint64_t *list = reinterpret_cast<const uint64_t *>(static_cast<const char *>(image) + kNsStateWords * 8);
-    ns_match_kernel<<<grid(n), kThreads, held, st>>>(list, (uint32_t)(held / 8), names, text, c.off, c.len, n, verdict);
+    ns_match_kernel<<<grid(n), kThreads, held, st>>>(list, (uint32_t)(held / 8), names, hash_mask, text, c.off, c.len, n,
+                                                     verdict);
     return cudaGetLastError();
 }
 
@@ -454,4 +457,247 @@ extern "C" int tad_debug_ns_match(const uint8_t *name, uint32_t name_len, const 
     const tad::NsParts p = tad::ns_parts(names, 0);
     return tad::ns_listed(names, reinterpret_cast<const uint64_t *>(q + p.hash), reinterpret_cast<const uint32_t *>(q + p.off),
                           q + p.bytes, name, name_len, tad::name_hash(name, name_len) & hash_mask) ? 1 : 0;
+}
+
+// ---- the text kernels on one device, for the tests ---------------------------------------------------------------------
+// A dictionary driven through launch_text_* as TextKeys drives it, with its own buffers and a hash mask, and the ignore
+// list's device lookup with an explicit mask.  Every call synchronises before it returns.  Error codes as theia_tad.h:
+// 0, -1 (TAD_ERR_INVALID_ARG: an argument the kernels cannot take safely), -2 (a CUDA error).
+
+// The hash the dictionaries and the ignore list use.
+extern "C" uint64_t tad_debug_name_hash(const uint8_t *bytes, uint32_t len) { return tad::name_hash(bytes, len); }
+
+namespace {
+
+struct DebugDict {
+    int device;
+    tad::TextDict d;
+    uint64_t names = 0, bytes = 0;               // state[0], state[1] after the last encode
+    uint64_t arena_cap = 0, names_cap = 0;       // arena bytes; names the off / hash arrays hold
+};
+
+cudaError_t debug_alloc_slots(tad::TextDict &d, uint32_t cap)
+{
+    d.slots = nullptr;
+    d.minrow = d.slot_id = nullptr;
+    d.cap = cap;
+    cudaError_t e = cudaMalloc(&d.slots, (size_t)cap * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&d.minrow, (size_t)cap * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&d.slot_id, (size_t)cap * 4);
+    if (e == cudaSuccess) e = tad::launch_text_clear(0, d);
+    return e;
+}
+
+void debug_free_slots(tad::TextDict &d)
+{
+    cudaFree(d.slots);
+    cudaFree(d.minrow);
+    cudaFree(d.slot_id);
+}
+
+// *p (have bytes, of which `keep` are live) grown to at least `need` bytes
+template <typename T> cudaError_t debug_grow(T *&p, size_t have, size_t need, size_t keep)
+{
+    if (need <= have) return cudaSuccess;
+    T *q = nullptr;
+    cudaError_t e = cudaMalloc(&q, need);
+    if (e == cudaSuccess && keep) e = cudaMemcpy(q, p, keep, cudaMemcpyDeviceToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(q);
+        return e;
+    }
+    cudaFree(p);
+    p = q;
+    return cudaSuccess;
+}
+
+// The rows [lo, lo + n) lie inside the segments' rows and the block, and the offsets fit the kernels' u32.
+bool debug_rows_ok(uint64_t span, uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo, uint64_t n)
+{
+    return n < (1ull << 24) && span < (1ull << 32) && seg0_row % 32 == 0 && lo >= seg0_row &&
+           lo + n <= std::min<uint64_t>(seg0_row + 32ull * nseg, block_rows);
+}
+
+// The segments' marks and bytes copied to the device (marks first, text after, as the text staging holds them).
+cudaError_t debug_stage(const uint8_t *text, uint64_t span, const uint64_t *marks, uint32_t nseg, uint64_t n, char *&buf,
+                        void *&scratch, size_t &scratch_bytes)
+{
+    scratch_bytes = tad::text_scratch_bytes(n);
+    const size_t at = tad::align256((size_t)nseg * 8 + 8);
+    cudaError_t e = cudaMalloc(&buf, at + span + 1);
+    if (e == cudaSuccess) e = cudaMalloc(&scratch, scratch_bytes);
+    if (e == cudaSuccess && nseg) e = cudaMemcpy(buf, marks, (size_t)nseg * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && span) e = cudaMemcpy(buf + at, text, span, cudaMemcpyHostToDevice);
+    return e;
+}
+
+}  // namespace
+
+// A dictionary of `cap` slots (a power of two, >= 2) on `device`, every name's hash ANDed with hash_mask.
+extern "C" int tad_debug_text_dict_new(int device, uint32_t cap, uint64_t hash_mask, void **out)
+{
+    if (!out || cap < 2 || (cap & (cap - 1))) return TAD_ERR_INVALID_ARG;
+    *out = nullptr;
+    if (cudaSetDevice(device) != cudaSuccess) return TAD_ERR_CUDA;
+    DebugDict *h = new DebugDict();
+    h->device = device;
+    tad::TextDict &d = h->d;
+    d.arena = nullptr;
+    d.off = d.hash = nullptr;
+    d.state = nullptr;
+    d.frozen = 0;
+    d.hash_mask = hash_mask;
+    cudaError_t e = debug_alloc_slots(d, cap);
+    if (e == cudaSuccess) e = cudaMalloc(&d.state, 64);
+    if (e == cudaSuccess) e = cudaMemset(d.state, 0, 64);
+    if (e == cudaSuccess) e = cudaMalloc(&d.off, 8);
+    if (e == cudaSuccess) e = cudaMemset(d.off, 0, 8);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        debug_free_slots(d);
+        cudaFree(d.state);
+        cudaFree(d.off);
+        delete h;
+        return TAD_ERR_CUDA;
+    }
+    *out = h;
+    return TAD_OK;
+}
+
+// One chunk through launch_text_encode (arguments as there; text / marks in host memory): ids_out[0, n) and the state
+// words after it (state_out[8]).  An open dictionary refuses a chunk that could take it past half full,
+// 2 * (names + n) > cap, as the engine grows before that.
+extern "C" int tad_debug_text_dict_encode(void *handle, const uint8_t *text, uint64_t span, const uint64_t *marks,
+                                          uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo, uint64_t n,
+                                          uint32_t *ids_out, uint64_t *state_out)
+{
+    DebugDict *h = static_cast<DebugDict *>(handle);
+    if (!h || !state_out || (n && (!ids_out || !marks || !nseg)) || (span && !text)) return TAD_ERR_INVALID_ARG;
+    if (n && !debug_rows_ok(span, nseg, seg0_row, block_rows, lo, n)) return TAD_ERR_INVALID_ARG;
+    tad::TextDict &d = h->d;
+    if (!d.frozen && 2 * (h->names + n) > d.cap) return TAD_ERR_INVALID_ARG;
+    if (cudaSetDevice(h->device) != cudaSuccess) return TAD_ERR_CUDA;
+    const uint64_t nn = h->names + n;
+    cudaError_t e = debug_grow(d.arena, h->arena_cap, std::max<uint64_t>(h->bytes + span, 1), h->bytes);
+    if (e == cudaSuccess) h->arena_cap = std::max<uint64_t>(h->arena_cap, std::max<uint64_t>(h->bytes + span, 1));
+    if (e == cudaSuccess) e = debug_grow(d.off, (h->names_cap + 1) * 8, (nn + 1) * 8, (h->names + 1) * 8);
+    if (e == cudaSuccess) e = debug_grow(d.hash, h->names_cap * 8, std::max<uint64_t>(nn, 1) * 8, h->names * 8);
+    if (e == cudaSuccess) h->names_cap = std::max(h->names_cap, std::max<uint64_t>(nn, 1));
+    char *buf = nullptr;
+    void *scratch = nullptr;
+    uint32_t *ids = nullptr;
+    size_t scratch_bytes = 0;
+    if (e == cudaSuccess) e = debug_stage(text, span, marks, nseg, n, buf, scratch, scratch_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&ids, std::max<uint64_t>(n, 1) * 4);
+    if (e == cudaSuccess)
+        e = tad::launch_text_encode(0, d, reinterpret_cast<const uint8_t *>(buf + tad::align256((size_t)nseg * 8 + 8)), span,
+                                    reinterpret_cast<const uint64_t *>(buf), nseg, seg0_row, block_rows, lo, n, scratch,
+                                    scratch_bytes, ids);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess && n) e = cudaMemcpy(ids_out, ids, n * 4, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(state_out, d.state, 64, cudaMemcpyDeviceToHost);
+    cudaFree(buf);
+    cudaFree(scratch);
+    cudaFree(ids);
+    if (e != cudaSuccess) return TAD_ERR_CUDA;
+    h->names = state_out[0];
+    h->bytes = state_out[1];
+    return TAD_OK;
+}
+
+// A table of new_cap slots (a power of two holding the names at most half full): cleared and every name re-inserted
+// from its stored hash, as TextKeys::grow does.
+extern "C" int tad_debug_text_dict_grow(void *handle, uint32_t new_cap)
+{
+    DebugDict *h = static_cast<DebugDict *>(handle);
+    if (!h || new_cap < 2 || (new_cap & (new_cap - 1)) || 2 * h->names > new_cap) return TAD_ERR_INVALID_ARG;
+    if (cudaSetDevice(h->device) != cudaSuccess) return TAD_ERR_CUDA;
+    tad::TextDict nd = h->d;
+    cudaError_t e = debug_alloc_slots(nd, new_cap);
+    if (e == cudaSuccess) e = tad::launch_text_rehash(0, h->d, nd, h->names);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        debug_free_slots(nd);
+        return TAD_ERR_CUDA;
+    }
+    debug_free_slots(h->d);
+    h->d = nd;
+    return TAD_OK;
+}
+
+// Later chunks look names up and add none; a name the dictionary lacks sets state[5] and gets id 0.
+extern "C" int tad_debug_text_dict_freeze(void *handle)
+{
+    DebugDict *h = static_cast<DebugDict *>(handle);
+    if (!h) return TAD_ERR_INVALID_ARG;
+    h->d.frozen = 1;
+    return TAD_OK;
+}
+
+// The dictionary's name and byte counts; with non-null buffers also its arena (bytes), offsets (names + 1) and the
+// stored hash of every name (names).
+extern "C" int tad_debug_text_dict_names(void *handle, uint64_t *names, uint64_t *bytes, uint8_t *arena_out,
+                                         uint64_t *off_out, uint64_t *hash_out)
+{
+    DebugDict *h = static_cast<DebugDict *>(handle);
+    if (!h || !names || !bytes) return TAD_ERR_INVALID_ARG;
+    *names = h->names;
+    *bytes = h->bytes;
+    if (cudaSetDevice(h->device) != cudaSuccess) return TAD_ERR_CUDA;
+    cudaError_t e = cudaSuccess;
+    if (arena_out && h->bytes) e = cudaMemcpy(arena_out, h->d.arena, h->bytes, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && off_out) e = cudaMemcpy(off_out, h->d.off, (h->names + 1) * 8, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && hash_out && h->names) e = cudaMemcpy(hash_out, h->d.hash, h->names * 8, cudaMemcpyDeviceToHost);
+    return e == cudaSuccess ? TAD_OK : TAD_ERR_CUDA;
+}
+
+extern "C" int tad_debug_text_dict_free(void *handle)
+{
+    DebugDict *h = static_cast<DebugDict *>(handle);
+    if (!h) return TAD_ERR_INVALID_ARG;
+    cudaSetDevice(h->device);
+    debug_free_slots(h->d);
+    cudaFree(h->d.arena);
+    cudaFree(h->d.off);
+    cudaFree(h->d.hash);
+    cudaFree(h->d.state);
+    delete h;
+    return TAD_OK;
+}
+
+// The device twin of tad_debug_ns_match: rows [lo, lo + n) of a namespace text column (arguments as for
+// tad_debug_text_dict_encode) tested by launch_ns_match against the list, image and lookup both under hash_mask.
+// verdict_out[0, n): 1 = listed; *error = the decode error flag (state word 2).
+extern "C" int tad_debug_ns_match_device(int device, const uint8_t *list_bytes, const uint64_t *list_off, uint32_t names,
+                                         uint64_t hash_mask, const uint8_t *text, uint64_t span, const uint64_t *marks,
+                                         uint32_t nseg, uint64_t seg0_row, uint64_t block_rows, uint64_t lo, uint64_t n,
+                                         uint32_t *verdict_out, uint64_t *error)
+{
+    if (!list_off || (names && !list_bytes) || !error || (span && !text) || (n && (!verdict_out || !marks || !nseg)))
+        return TAD_ERR_INVALID_ARG;
+    if (names > tad::kNsMaxNames || list_off[names] - list_off[0] > tad::kNsMaxBytes) return TAD_ERR_INVALID_ARG;
+    if (n && !debug_rows_ok(span, nseg, seg0_row, block_rows, lo, n)) return TAD_ERR_INVALID_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) return TAD_ERR_CUDA;
+    const std::vector<uint8_t> img = tad::ns_list_image(list_bytes, list_off, names, hash_mask);
+    void *dimg = nullptr, *scratch = nullptr;
+    char *buf = nullptr;
+    uint32_t *verdict = nullptr;
+    size_t scratch_bytes = 0;
+    cudaError_t e = cudaMalloc(&dimg, img.size());
+    if (e == cudaSuccess) e = cudaMemcpy(dimg, img.data(), img.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = debug_stage(text, span, marks, nseg, n, buf, scratch, scratch_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&verdict, std::max<uint64_t>(n, 1) * 4);
+    if (e == cudaSuccess)
+        e = tad::launch_ns_match(0, dimg, names, img.size(), hash_mask, static_cast<unsigned long long *>(dimg),
+                                 reinterpret_cast<const uint8_t *>(buf + tad::align256((size_t)nseg * 8 + 8)), span,
+                                 reinterpret_cast<const uint64_t *>(buf), nseg, seg0_row, block_rows, lo, n, scratch,
+                                 scratch_bytes, verdict);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess && n) e = cudaMemcpy(verdict_out, verdict, n * 4, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(error, static_cast<uint64_t *>(dimg) + 2, 8, cudaMemcpyDeviceToHost);
+    cudaFree(dimg);
+    cudaFree(buf);
+    cudaFree(scratch);
+    cudaFree(verdict);
+    return e == cudaSuccess ? TAD_OK : TAD_ERR_CUDA;
 }

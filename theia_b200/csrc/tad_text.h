@@ -24,6 +24,7 @@ struct TextDict {
     uint64_t *hash;              // names: each name's hash, for the rehash
     unsigned long long *state;   // 8 words
     uint32_t frozen;             // the dictionary is complete: a name not in it sets state[5] and is not added
+    uint64_t hash_mask;          // ANDed into every name's hash: ~0, or narrower to make hashes collide (TAD_DEBUG_TEXT_MASK)
 };
 
 // Scratch of one chunk of `n` rows: per row (offset, length) into the staged text, the pending slot it reached, and the
@@ -79,13 +80,14 @@ constexpr int kNsStateWords = 16;
 // The verdict a namespace slot stages per row: the row filter's one-entry ignore list {kNsListed} drops listed rows.
 constexpr uint32_t kNsListed = 1;
 // `hash_mask` is ANDed into every hash (~0 in the engine; a narrow mask makes hashes collide, for the tests).
-std::vector<uint8_t> ns_list_image(const uint8_t *bytes, const uint64_t *off, uint32_t names, uint64_t hash_mask = ~0ull);
+std::vector<uint8_t> ns_list_image(const uint8_t *bytes, const uint64_t *off, uint32_t names, uint64_t hash_mask);
 
 // Rows [lo, lo + n) of a block's namespace text slot (staged as for launch_text_encode) -> verdict[i] = kNsListed when
 // the row's name is in the list `image` (device memory, `names` names, `image_bytes` long), else 0.  A segment that does
 // not decode sets state[2] (the slot's state words) and its rows read as the empty name.  Two launches; `scratch` as
-// for launch_text_encode.
-cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, unsigned long long *state,
+// for launch_text_encode; `hash_mask` as the image was built with.
+cudaError_t launch_ns_match(cudaStream_t st, const void *image, uint32_t names, size_t image_bytes, uint64_t hash_mask,
+                            unsigned long long *state,
                             const uint8_t *text, uint64_t span_bytes, const uint64_t *marks, uint32_t nseg, uint64_t seg0_row,
                             uint64_t block_rows, uint64_t lo, uint64_t n, void *scratch, size_t scratch_bytes,
                             uint32_t *verdict);
