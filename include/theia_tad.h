@@ -205,12 +205,20 @@ int tad_result(tad_job *job, tad_rows *rows);
 /* Replaces: DeleteSparkApplication (controller.go:385-424).  tad_cancel returns at once; the job then fails with
  * TAD_ERR_CANCELLED at its next check.  An ARIMA job on one GPU checks inside its fit kernel: every warp stops at its
  * next evaluation round and drops the fits in flight, so the job stops within one likelihood evaluation of the longest
- * prefix being fitted, whatever the series' length (within one phase of the pipeline otherwise, and at the end of the job
- * when world_size > 1, or of the current pass under a memory budget).  An ARIMA job whose fit is parked while other jobs
- * run (tad_set_fit_sharing) fails once the job running in its place has ended; its parked buffers are then freed.
- * tad_release of a job that has not finished cancels it and waits until it has failed (for a parked ARIMA job, at most
- * the run time of the job running in its place; when that is a streamed ARIMA job fitting beside it, until that job's
- * input has ended and its result is published); the context then runs the next queued job. */
+ * prefix being fitted, whatever the series' length (within one phase of the pipeline otherwise).  An ARIMA job whose fit
+ * is parked while other jobs run (tad_set_fit_sharing) fails once the job running in its place has ended; its parked
+ * buffers are then freed.
+ * Several GPUs (world_size > 1): call it on any one rank; the job then fails with TAD_ERR_CANCELLED on every rank, its
+ * err_msg naming the rank that cancelled, and no rank is ever left waiting in a collective.  The ranks decide at points
+ * they reach together -- the end of the job, or of the current pass under a memory budget -- on what every rank brings
+ * there.  An ARIMA fit stops within one evaluation round on every rank when the ranks map each other's memory (the
+ * default), otherwise on the cancelling rank only, and the others at the end of their fits.  A cancel that arrives after
+ * the rank has reached the job's last such point while no peer is still fitting changes nothing: the job completes on
+ * every rank.  A job cancelled in the queue still meets its peers once.
+ * tad_release of a job that has not finished cancels it (on several GPUs as above, failing the job on every rank) and
+ * waits until it has failed (for a parked ARIMA job, at most the run time of the job running in its place; when that is a
+ * streamed ARIMA job fitting beside it, until that job's input has ended and its result is published); the context then
+ * runs the next queued job. */
 int tad_cancel(tad_job *job);
 int tad_release(tad_job *job);
 
@@ -303,8 +311,8 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * above.  A cancel of it ends the joint launch, and its feeder's pending push or end call returns TAD_ERR_CANCELLED.  A
  * cancel of the yielded job takes effect once the streamed job's input has ended and its result is published; a
  * tad_release of the yielded job waits that long too.
- * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit left
- * early would strand its peers, as for the cancel). */
+ * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit
+ * yielded alone would leave its peers waiting for it; the ranks would have to agree on each yield). */
 int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);
 /* For a COMPLETED ARIMA job: how many times its fit phase yielded and the time it spent parked (ms).  TAD_ERR_STATE for
  * any other job or state. */

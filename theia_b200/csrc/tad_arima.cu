@@ -661,12 +661,49 @@ __global__ void __launch_bounds__(128) arima_boxcox_kernel(const SeriesEntry *__
 // are the warp's first resume[2i + 1] hand-outs; resume[2S + 1] counts those that have finished again, which lets the host
 // hold the next yield until all have (so no fit is dropped twice).  kMode: 0 a fit that cannot yield (resume is null),
 // 1 one that can, 2 its resume launch; mode 0 is the fit kernel as it is without fit sharing.
-// arima_fit_series is the work of the warp that fits series i (lane = its lane): the one body of both fit kernels.
-template <int kMode>
+// Stop: what lane 0 reads every round and whether it says leave -- CancelWord (one GPU: the job's cancel word) or StopBoard
+// (several GPUs: the ranks' stop board, mode 0 only).
+// arima_fit_series is the work of the warp that fits series i (lane = its lane): the one body of the fit kernels.
+struct CancelWord {
+    const volatile uint32_t *word;
+    typedef uint32_t Read;
+    __device__ __forceinline__ Read read() const { return *word; }
+    __device__ __forceinline__ uint32_t stops(Read r) const { return r; }
+};
+
+// The stop board of a multi-GPU job: 8 u32 (one per rank, at most 8 ranks) in this rank's memory, word r written only by rank r, through its
+// mapping, with the ordinal of a job rank r cancelled (0: none yet).  The warp leaves once any word equals this job's
+// ordinal.  Unused words stay 0 (ordinals start at 1), so lane 0 reads all of them, one 32-byte sector in two 16-byte
+// volatile loads, whatever the world size; the comparison waits for the next round, so the loads' latency overlaps the
+// evaluation as the cancel word's does.
+struct StopBoard {
+    const uint32_t *board;
+    uint32_t ordinal;
+    struct Read {
+        uint4 lo, hi;
+    };
+    __device__ __forceinline__ Read read() const
+    {
+        Read r;
+        asm volatile("ld.volatile.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.lo.x), "=r"(r.lo.y), "=r"(r.lo.z), "=r"(r.lo.w)
+                     : "l"(board));
+        asm volatile("ld.volatile.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.hi.x), "=r"(r.hi.y), "=r"(r.hi.z), "=r"(r.hi.w)
+                     : "l"(board + 4));
+        return r;
+    }
+    __device__ __forceinline__ uint32_t stops(const Read &r) const
+    {
+        const uint32_t k = ordinal;
+        return (r.lo.x == k) | (r.lo.y == k) | (r.lo.z == k) | (r.lo.w == k) | (r.hi.x == k) | (r.hi.y == k) |
+               (r.hi.z == k) | (r.hi.w == k);
+    }
+};
+
+template <int kMode, class Stop = CancelWord>
 __device__ __forceinline__ void arima_fit_series(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
                                                  const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
                                                  const double *__restrict__ yb, const double *__restrict__ lam,
-                                                 double *__restrict__ pred, const volatile uint32_t *cancel,
+                                                 double *__restrict__ pred, const Stop cancel,
                                                  uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume,
                                                  const uint32_t i, const uint32_t lane)
 {
@@ -693,9 +730,9 @@ __device__ __forceinline__ void arima_fit_series(const SeriesEntry *__restrict__
     Lbfgs st;
     // lane 0: the cancel word as read in the previous round; the first read is here, so that a warp which starts after
     // the cancel fits nothing
-    uint32_t stop = lane == 0 ? *cancel : 0u;
+    typename Stop::Read stop = lane == 0 ? cancel.read() : typename Stop::Read{};
     for (;;) {
-        if (__shfl_sync(0xffffffffu, stop, 0)) break;      // cancelled: the fits in flight are dropped
+        if (__shfl_sync(0xffffffffu, cancel.stops(stop), 0)) break;      // cancelled: the fits in flight are dropped
         // ---- hand the next jobs to the idle lanes --------------------------------------------
         uint32_t idle = __ballot_sync(0xffffffffu, !busy);
         if (kResume) {
@@ -727,7 +764,7 @@ __device__ __forceinline__ void arima_fit_series(const SeriesEntry *__restrict__
         }
         if (!__any_sync(0xffffffffu, busy)) break;
         // the next round's cancel word, read here so that its latency overlaps the evaluation
-        if (lane == 0) stop = *cancel;
+        if (lane == 0) stop = cancel.read();
         // ---- all busy lanes evaluate together -------------------------------------------------
         double f = 0.0, g[3] = {0.0, 0.0, 0.0};
         if (busy) arima_fg(o, u, f, g);
@@ -768,8 +805,19 @@ __global__ void __launch_bounds__(128) arima_fit_sync_kernel(const SeriesEntry *
                                                              double *__restrict__ pred, const volatile uint32_t *cancel,
                                                              uint32_t *__restrict__ fits_done, uint32_t *__restrict__ resume)
 {
-    arima_fit_series<kMode>(entries, offsets, sbase, B, S, yb, lam, pred, cancel, fits_done, resume,
+    arima_fit_series<kMode>(entries, offsets, sbase, B, S, yb, lam, pred, CancelWord{cancel}, fits_done, resume,
                             (blockIdx.x * blockDim.x + threadIdx.x) >> 5, threadIdx.x & 31);
+}
+
+// The fit kernel of a multi-GPU job (mode 0): it stops on the ranks' stop board instead of a cancel word.
+__global__ void __launch_bounds__(128) arima_fit_board_kernel(const SeriesEntry *__restrict__ entries, const uint32_t *__restrict__ offsets,
+                                                              const uint32_t *__restrict__ sbase, uint32_t B, uint32_t S,
+                                                              const double *__restrict__ yb, const double *__restrict__ lam,
+                                                              double *__restrict__ pred, StopBoard board,
+                                                              uint32_t *__restrict__ fits_done)
+{
+    arima_fit_series<0>(entries, offsets, sbase, B, S, yb, lam, pred, board, fits_done, nullptr,
+                        (blockIdx.x * blockDim.x + threadIdx.x) >> 5, threadIdx.x & 31);
 }
 
 // The lowest series of `a` a resume launch still has fits for (resume point >= 3), into *from (set to ~0 by the caller).
@@ -800,14 +848,14 @@ __global__ void __launch_bounds__(128) arima_fit_pair_kernel(FitPart a, uint32_t
     if (kModeB == 2) {              // both parts resume: one call site
         arima_fit_series<2>(on_b ? b.entries : a.entries, on_b ? b.offsets : a.offsets, on_b ? b.sbase : a.sbase,
                             on_b ? b.B : a.B, on_b ? b.S : a.S, on_b ? b.y : a.y, on_b ? b.lam : a.lam, on_b ? b.pred : a.pred,
-                            on_b ? b.cancel : a.cancel, on_b ? b.fits_done : a.fits_done, on_b ? b.resume : a.resume,
-                            on_b ? at : a_from + at, lane);
+                            CancelWord{on_b ? b.cancel : a.cancel}, on_b ? b.fits_done : a.fits_done,
+                            on_b ? b.resume : a.resume, on_b ? at : a_from + at, lane);
     } else if (on_b) {
-        arima_fit_series<kModeB>(b.entries, b.offsets, b.sbase, b.B, b.S, b.y, b.lam, b.pred, b.cancel, b.fits_done, b.resume,
-                                 at, lane);
+        arima_fit_series<kModeB>(b.entries, b.offsets, b.sbase, b.B, b.S, b.y, b.lam, b.pred, CancelWord{b.cancel}, b.fits_done,
+                                 b.resume, at, lane);
     } else {
-        arima_fit_series<2>(a.entries, a.offsets, a.sbase, a.B, a.S, a.y, a.lam, a.pred, a.cancel, a.fits_done, a.resume,
-                            a_from + at, lane);
+        arima_fit_series<2>(a.entries, a.offsets, a.sbase, a.B, a.S, a.y, a.lam, a.pred, CancelWord{a.cancel}, a.fits_done,
+                            a.resume, a_from + at, lane);
     }
 }
 
@@ -904,13 +952,18 @@ __global__ void __launch_bounds__(NT) detect_arima_kernel(const SeriesEntry *__r
 
 cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                              uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume)
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume,
+                             const uint32_t *board, uint32_t ordinal)
 {
     if (S == 0) return cudaSuccess;
     arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam, fits,
                                                          resume ? scratch_pred : nullptr);
     const uint64_t threads = (uint64_t)S * 32;
-    if (resume)
+    if (board)
+        arima_fit_board_kernel<<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
+                                                                                  scratch_lam, scratch_pred,
+                                                                                  StopBoard{board, ordinal}, fits + 1);
+    else if (resume)
         arima_fit_sync_kernel<1><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
                                                                                     scratch_lam, scratch_pred, cancel, fits + 1,
                                                                                     resume);

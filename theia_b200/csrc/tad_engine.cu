@@ -39,7 +39,8 @@ struct PinnedBlock {
 
 constexpr int kMaxEvents = 24;
 constexpr int kMaxChunks = 16;          // host-resident input is copied and histogrammed in chunks
-constexpr int kMaxRanks = 8;
+constexpr int kMaxRanks = 8;      // also the stop board's words, all of which the multi-GPU fit kernel reads (StopBoard)
+static_assert(kMaxRanks == 8, "the fit kernel reads the stop board as 8 words");
 constexpr int kMaxXChunks = kMaxSeg / kMaxRanks;   // exchange chunks: scatter of chunk c+1 overlaps the all-to-all of chunk c
 constexpr int kTotalStages = 6;   // ingest, partition, exchange, group, detect, egress
 
@@ -155,6 +156,8 @@ struct tad_job {
     std::condition_variable cv;
     tad_status st{};
     std::atomic<int> cancel{0};
+    uint32_t ordinal = 0;            // the job's place among the context's submissions, from 1: the same on every rank
+    bool started = false;            // the worker has taken the job (a multi-GPU cancel then writes the stop board), under `mu`
     PinnedBlock result_block;
     tad_rows rows{};
     double t_submit = 0;
@@ -274,6 +277,16 @@ struct tad_ctx {
     DevBuf xbuf;                                    // exported: [counters: B x u32, padded][slots: B x slot x Row32]
     void *peer_x[kMaxRanks]{};                      // peers' xbuf mapped into this process
     bool peers_mapped = false;
+    // stop board of a multi-GPU context (DESIGN.md section 6): kMaxRanks u32 in device memory, word r the ordinal of the
+    // last job rank r cancelled (0: none), read by the fit kernel every round.  Each rank writes its own word into every
+    // board it has mapped (post_stop); a word has one writer and only grows.
+    uint32_t job_seq = 0;                           // ordinals of the jobs queued so far, under `mu`
+    uint32_t *board = nullptr;
+    uint32_t *peer_board[kMaxRanks]{};              // rank r's board as mapped here ([rank] = board); null: not mapped
+    bool boards_shared = false;                     // the ranks have exchanged their boards' handles (the same on every rank)
+    std::mutex board_mu;                            // post_stop
+    cudaStream_t board_stream = nullptr;            // non-blocking: a board write waits for no job's work
+    uint32_t *h_board = nullptr;                    // pinned: [0] the ordinal this rank last wrote; [8, 16) its board read back
     size_t x_agreed = 0;                            // exported size all ranks agreed on at the last (re)mapping
     DevBuf xcnt, xtotal;                            // per-source counts / totals of the owned bucket range
     // memory budget and hash-range passes (DESIGN.md section 9)
@@ -605,8 +618,8 @@ void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progres
 
 // The ARIMA fit launch of a pass (launch_arima_fit with d_fits = its counters and cancel word, enqueued on ctx->stream behind
 // their reset and fit_ev[0]), waited for without blocking behind it: the worker polls an event recorded after the fit
-// kernel, copies tad_cancel into the kernel's cancel word (single GPU only: on several GPUs a rank that left early would
-// strand its peers at the end-of-job all-gather) and about every 50 ms copies the pass's fit counters back; both copies
+// kernel, copies tad_cancel into the kernel's cancel word (single GPU only: on several GPUs the fit reads the stop board,
+// which tad_cancel writes itself, post_stop) and about every 50 ms copies the pass's fit counters back; both copies
 // run on the copy stream, beside the kernel.  The counters are published added to the job's counts before the pass.
 // Fit sharing (tad_set_fit_sharing): when a fit that can yield (job->share) sees a job waiting that interleave() would run,
 // it copies 2 into the cancel word instead; once the kernel has left, the pass is parked, the waiting jobs run, and
@@ -1287,12 +1300,112 @@ cudaError_t unmap_peers(tad_ctx *ctx)
     return err;
 }
 
+// ---- cancel on several GPUs (DESIGN.md section 6) ------------------------------------------------------------------------
+// Maps every peer's stop board (the first job of a multi-GPU context: every rank runs it, so every rank meets here).
+// Without peer pull (TAD_PEER_PULL=0) a rank exports nothing, and a board that fails to map is left out: a cancel then
+// reaches only the boards that are mapped, and the ranks whose fits it does not stop fail at the verdict.
+void share_boards(tad_ctx *ctx)
+{
+    constexpr int G = tad_ctx::kGatherMax;
+    const int me = ctx->cfg.rank;
+    ensure(ctx, ctx->small, tad_ctx::kSmallDevWords * 8);
+    memset(ctx->h_small, 0, G * 8);
+    ctx->h_small[0] = ctx->peer_pull ? 1 : 0;
+    if (ctx->peer_pull) CU(nccl_ipc_export(&ctx->nccl, ctx->board, ctx->h_small + 2));      // a 64-byte handle in words 2..9
+    gather_small(ctx, G, false);
+    uint32_t *mapped[kMaxRanks] = {};
+    for (int r = 0; r < ctx->cfg.world_size; r++) {
+        if (r == me || !ctx->peer_pull || !ctx->h_small[G * (1 + r)]) continue;
+        void *p = nullptr;
+        if (nccl_ipc_map(&ctx->nccl, ctx->h_small + G * (1 + r) + 2, &p) == cudaSuccess) mapped[r] = static_cast<uint32_t *>(p);
+        else cudaGetLastError();
+    }
+    std::lock_guard<std::mutex> lk(ctx->board_mu);
+    for (int r = 0; r < ctx->cfg.world_size; r++)
+        if (r != me) ctx->peer_board[r] = mapped[r];
+    ctx->boards_shared = true;
+}
+
+// Writes `ordinal` into this rank's word of every board it has mapped, its own included, so that the fit of that job
+// stops on every rank within one evaluation round.  Called under the cancelled job's `mu`, from tad_cancel or tad_release
+// while the job runs, or by the worker as it takes a job cancelled in the queue.  The copies run on board_stream, so the
+// write waits for no job's work (the worker may be blocked in a collective or waiting for the loopback device turn), and
+// the calling thread's current device is left as it was.  A word only grows: the write of a job that precedes the last
+// one written is dropped, so a stop for job k never stops another job.
+void post_stop(tad_ctx *ctx, uint32_t ordinal)
+{
+    std::lock_guard<std::mutex> lk(ctx->board_mu);
+    if (!ctx->board || ordinal <= ctx->h_board[0]) return;
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) dev = -1;
+    if (cudaSetDevice(ctx->cfg.device) != cudaSuccess) return;
+    ctx->h_board[0] = ordinal;
+    cudaError_t e = cudaSuccess;
+    for (int r = 0; r < ctx->cfg.world_size; r++)
+        if (ctx->peer_board[r] && e == cudaSuccess)
+            e = cudaMemcpyAsync(ctx->peer_board[r] + ctx->cfg.rank, ctx->h_board, 4, cudaMemcpyDefault, ctx->board_stream);
+    if (cudaStreamSynchronize(ctx->board_stream) != cudaSuccess || e != cudaSuccess)
+        cudaGetLastError();      // a write that did not land: the verdict still fails the job on every rank
+    if (dev >= 0) cudaSetDevice(dev);
+}
+
+// A multi-GPU cancel of `job` by tad_cancel or tad_release (under job->mu): the stop board is written while the worker
+// runs the job; a queued job's is written as the worker takes it (run_job).
+void stop_running(tad_job *job)
+{
+    const int s = job->st.state;
+    if (job->ctx && job->ctx->cfg.world_size > 1 && job->started && s != TAD_STATE_COMPLETED && s != TAD_STATE_FAILED)
+        post_stop(job->ctx, job->ordinal);
+}
+
+// After a multi-GPU fit that left with fits undone: the rank whose board word holds this job's ordinal (kMaxRanks: none).
+int board_stopper(tad_ctx *ctx, const tad_job *job)
+{
+    CU(cudaMemcpyAsync(ctx->h_board + 8, ctx->board, 4 * kMaxRanks, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (int r = 0; r < ctx->cfg.world_size; r++)
+        if (ctx->h_board[8 + r] == job->ordinal) return r;
+    return kMaxRanks;
+}
+
+// The agreed points of a multi-GPU job -- the verdict all-gather that ends it and, in hash-range passes, the end of every
+// pass -- carry one 8-byte word per rank: 2 its job was cancelled there (its own flag, read once); 4 its fit stopped on
+// the board, with bits 8.. the rank whose word stopped it (kMaxRanks: none); bit 0 is the pass driver's split.  A rank
+// that cancelled after its flag was read can still stop a peer's fit that is running, so a stopped fit fails the job
+// even where no rank flags the cancel; and every rank decides on the same gathered words.
+uint64_t stop_word(const tad_job *job, int fit_stop)
+{
+    return (job->cancel.load() ? 2u : 0u) | (fit_stop >= 0 ? 4u | ((uint64_t)fit_stop << 8) : 0u);
+}
+
+bool any_stop(const unsigned long long *w, int world)
+{
+    for (int r = 0; r < world; r++)
+        if (w[r] & 6) return true;
+    return false;
+}
+
+// Fails the job alike on every rank when a word of `w` (one per rank) carries a cancel or a stopped fit: TAD_ERR_CANCELLED
+// naming the first rank that cancelled, TAD_ERR_INTERNAL for a fit stopped with no board word holding the job's ordinal.
+void agree_stop(const unsigned long long *w, int world)
+{
+    for (int r = 0; r < world; r++)
+        if (w[r] & 2) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", r);
+    for (int r = 0; r < world; r++) {
+        if (!(w[r] & 4)) continue;
+        const int by = (int)((w[r] >> 8) & 0xff);
+        if (by >= world) fail(TAD_ERR_INTERNAL, "rank %d: the ARIMA fit stopped with no cancel on any rank", r);
+        fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", by);
+    }
+}
+
 // Result of one pipeline run: a one-pass job or one hash-range pass.
 struct PassOut {
     uint64_t kept = 0, owned = 0, points = 0, series = 0, out_rows = 0, spill_rows = 0, launches = 0;
     double phase_ms[TAD_NPHASES] = {0};
     double device_ms = 0;
     PinnedBlock block;               // result rows, out_layout(out_rows) in pinned host memory
+    int fit_stop = -1;               // multi-GPU ARIMA: the fit stopped on the board, by this rank's word (board_stopper)
 };
 
 // The pipeline (ingest, partition, exchange, group, detect, egress) over `hc`.  `filters`: apply the job's time window
@@ -1301,8 +1414,9 @@ struct PassOut {
 // `pass`: one pass of a multi-GPU job in passes (run_passes_multi), null otherwise.  Its sizes come from the all-gathered
 // counts, so they are the same on every rank: the bucket count follows its global rows and the NCCL exchange's chunk count
 // its largest shard.  The pipeline then leaves every decision that changes which collectives a rank issues to the
-// driver's end-of-pass all-gather: a cancel does not throw here, and the peer-pull end barrier is that all-gather, so a
-// rank that throws PassSplit has issued every collective its peers have.
+// driver's end-of-pass all-gather: a cancel or a stopped fit does not throw here, and the peer-pull end barrier is that
+// all-gather, so a rank that throws PassSplit has issued every collective its peers have.  Outside passes a multi-GPU job
+// ends with the verdict all-gather, which takes those decisions the same way.
 struct AgreedPass {
     uint64_t global_rows;            // the pass's rows over all ranks
     uint64_t max_rows;               // the most rows one rank holds in the pass
@@ -1322,8 +1436,8 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             ev_phase[nev++] = phase;
         }
     };
-    auto check_cancel = [&]() {
-        if (!pass && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
+    auto check_cancel = [&]() {          // several GPUs: a cancel acts at the verdict, where every rank decides alike
+        if (ctx->cfg.world_size == 1 && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
     };
 
     CU(cudaSetDevice(ctx->cfg.device));
@@ -1539,7 +1653,6 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             seg.off[r] = off + r * off_stride;
         }
     };
-    bool sync_at_end = false;
     if (world > 1 && slots_allowed(ctx, R_total) && !force_exact) {
         ensure_exported(slot_xbuf_bytes(ctx, B));
         uint32_t *xcursor = static_cast<uint32_t *>(ctx->xbuf.p);
@@ -1567,7 +1680,6 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         check_cancel();
         uint64_t any_ovf = 0;
         for (int r = 0; r < world; r++) any_ovf += (uint32_t)ctx->h_small[tad_ctx::kWOvf + r];
-        sync_at_end = true;       // peers may still read this rank's slots: no rank starts its next job before all are done
         if (any_ovf == 0) {
             partitioned = true;
             kept = ctx->h_stats[ST_LOCALKEPT];
@@ -1676,7 +1788,6 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             if (peer_barrier(ctx)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
             mark(TAD_PHASE_SYNC);
             peer_segments(seg_off, Bl + 1, pull_skip);      // rows in front of my range skipped
-            sync_at_end = true;
         } else {
             ensure(ctx, ctx->exch, recv_total ? recv_total : 32);
             for (int cx = 0; cx < K; cx++) {
@@ -1827,17 +1938,20 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
                 } else {
                     CU(cudaEventRecord(ctx->fit_ev[0], st));
                     CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, y, pred, lam, d_stats + ST_FITS + 2,
-                                        d_stats + ST_FITS, res));
+                                        d_stats + ST_FITS, res, world > 1 ? ctx->board : nullptr, job->ordinal));
                     parked_ms = wait_arima_fit(ctx, job, d_stats + ST_FITS, res ? res + 2 * (size_t)S : nullptr, launches,
                                                res ? &yf : nullptr, [&] {
                         CU(launch_arima_resume(st, entries, offsets, sbase, Bl, S, y, pred, lam, d_stats + ST_FITS + 2,
                                                d_stats + ST_FITS, res));
                     });
                 }
-                if (ctx->cfg.world_size == 1) check_cancel();      // pred[] is incomplete: no detect
+                // pred[] is incomplete: no detect.  Several GPUs: the rank goes on to the verdict, which fails the job
+                check_cancel();
+                if (world > 1 && ctx->h_fits[3] < ctx->h_fits[2]) out.fit_stop = board_stopper(ctx, job);
             }
-            CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
-                                   (const double *)ctx->ar_lam.p, oc, (uint32_t)out_cap, d_stats, emit_all));
+            if (out.fit_stop < 0)
+                CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
+                                       (const double *)ctx->ar_lam.p, oc, (uint32_t)out_cap, d_stats, emit_all));
             launches += S ? (attempt == 0 ? 3 : 1) : 0;
         } else {
             fail(TAD_ERR_UNSUPPORTED, "algorithm %d is not implemented by this build", sp.algo);
@@ -1857,12 +1971,20 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
         set_progress(job, TAD_STATE_RUNNING, 4);
     }
     set_progress(job, TAD_STATE_RUNNING, 5);
-    if (sync_at_end && !pass) {
-        // end-of-job barrier of the peer-pull path: my slots and counters may be overwritten (next job) only after every
-        // peer's group kernel has read them; its wait is the ranks' arrival skew, accounted as TAD_PHASE_SYNC
+    if (world > 1 && !pass) {
+        // the verdict: an 8-byte all-gather of every rank's stop_word, on which every rank fails or goes on alike, so a
+        // cancel on one rank never leaves a peer waiting in a collective.  It is also the end-of-job barrier of the
+        // peer-pull paths: my slots and counters may be overwritten (next job) only after every peer's group kernel has
+        // read them.  Its wait is the ranks' arrival skew, accounted as TAD_PHASE_SYNC.
         mark(-1);
+        ctx->h_small[tad_ctx::kWBarrier] = stop_word(job, out.fit_stop);
+        CU(cudaMemcpyAsync(d_small + tad_ctx::kWBarrier, ctx->h_small + tad_ctx::kWBarrier, 8, cudaMemcpyHostToDevice, st));
         if (peer_barrier(ctx)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
         mark(TAD_PHASE_SYNC);
+        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWBarrierIn, d_small + tad_ctx::kWBarrierIn, 8 * world,
+                           cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        agree_stop(ctx->h_small + tad_ctx::kWBarrierIn, world);
     }
 
     // ---- egress: result rows -> pinned host memory -------------------------------------------
@@ -2989,8 +3111,9 @@ size_t mp_pipe_bytes(tad_ctx *ctx, const tad_job *job, uint64_t global, uint64_t
 //           input and owned rows of every pass for every P, so P is raised (pass 0 swept again, at most once) where some
 //           rank would not fit, and the job fails with TAD_ERR_NOMEM on every rank where a 1/64 range does not fit one;
 //   passes  run_pipeline at world_size > 1 over the pass columns, global_rows = the pass's total from the counts;
-//   end     every pass ends with an 8-byte all-gather of {split, cancelled}: a rank whose spill scratch or result buffer
-//           does not fit skips the rest of its pass but still gets there, and then every rank splits the pass or stops.
+//   end     every pass ends with an 8-byte all-gather of {split, cancelled, fit stopped} (stop_word): a rank whose spill
+//           scratch or result buffer does not fit, or whose fit stopped on the board, skips the rest of its pass but still
+//           gets there, and then every rank splits the pass or stops.
 uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
 {
     cudaStream_t st = ctx->stream;
@@ -3184,17 +3307,16 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
             CU(cudaStreamSynchronize(st));
             split_here = true;
         }
-        // ---- the agreed end of the pass: {split, cancelled} of every rank ----
-        ctx->h_small[0] = (split_here ? 1u : 0u) | (job->cancel.load() ? 2u : 0u);
+        // ---- the agreed end of the pass: {split, cancelled, fit stopped} of every rank ----
+        ctx->h_small[0] = (split_here ? 1u : 0u) | stop_word(job, o.fit_stop);
         gather_ms += gather_small(ctx, 1, true);
-        int split_r = -1, cancel_r = -1;
-        for (int r = W - 1; r >= 0; r--) {
+        int split_r = -1;
+        for (int r = W - 1; r >= 0; r--)
             if (ctx->h_small[1 + r] & 1) split_r = r;
-            if (ctx->h_small[1 + r] & 2) cancel_r = r;
-        }
-        if (cancel_r < 0 && split_r < 0) return false;
+        const bool stop = any_stop(ctx->h_small + 1, W);
+        if (!stop && split_r < 0) return false;
         give_pinned(ctx, o.block);
-        if (cancel_r >= 0) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", cancel_r);
+        agree_stop(ctx->h_small + 1, W);
         if (M >= (uint32_t)kMaxPasses)
             fail(TAD_ERR_NOMEM, "rank %d: the oversized-bucket scratch or result buffer of a 1/%d hash range of the "
                  "table (%llu rows owned) does not fit its memory budget of %llu bytes", split_r, kMaxPasses,
@@ -3213,9 +3335,17 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
     CU(cudaSetDevice(ctx->cfg.device));
     // a loopback rank (ranks as contexts of one process) waits for its turn on the device; released by worker_main
     if (nccl_job_begin(&ctx->nccl)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
-    // several GPUs under a budget: every rank joins the plan all-gather, a job cancelled before it started too
+    // several GPUs: a job cancelled in the queue runs to its first agreed point (the plan all-gather under a budget, else
+    // the verdict), and its stop is written now, so that the peers' fits stop at once
+    if (ctx->cfg.world_size > 1) {
+        if (!ctx->boards_shared) share_boards(ctx);
+        std::lock_guard<std::mutex> lk(job->mu);
+        job->started = true;
+        if (job->cancel.load()) post_stop(ctx, job->ordinal);
+    } else if (job->cancel.load()) {
+        fail(TAD_ERR_CANCELLED, "job cancelled");
+    }
     const uint64_t multi_budget = ctx->cfg.world_size > 1 ? ctx->budget.load() : 0;
-    if (!multi_budget && job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
     const tad_columns &hc = job->cols;     // a streamed job's first push writes it: not read here for streams
     const uint64_t R = job->stream ? 0 : hc.rows;
     ctx->limit = 0;
@@ -3449,6 +3579,7 @@ int submit_job(tad_ctx *ctx, tad_job *job, const tad_job_spec *spec, const tad_c
             snprintf(job->st.err_msg, sizeof(job->st.err_msg), "context is shutting down");
             return TAD_ERR_STATE;
         }
+        job->ordinal = ++ctx->job_seq;      // jobs are queued in the same order on every rank: so are the ordinals
         ctx->queue.push_back(job);
     }
     ctx->cv.notify_one();
@@ -3647,6 +3778,17 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     }
     for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->fit_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->fits_ev, cudaEventDisableTiming) == cudaSuccess;
+    if (ok && cfg->world_size > 1) {
+        // the stop board: allocated here, once, and mapped by the peers in the first job (share_boards)
+        ok = cudaMalloc((void **)&ctx->board, 4 * kMaxRanks) == cudaSuccess;
+        ok = ok && cudaMemset(ctx->board, 0, 4 * kMaxRanks) == cudaSuccess;
+        ok = ok && cudaStreamCreateWithFlags(&ctx->board_stream, cudaStreamNonBlocking) == cudaSuccess;
+        ok = ok && cudaHostAlloc((void **)&ctx->h_board, 16 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
+        if (ok) {
+            memset(ctx->h_board, 0, 16 * sizeof(uint32_t));
+            ctx->peer_board[cfg->rank] = ctx->board;
+        }
+    }
     if (!ok) {
         tad_shutdown(ctx);      // releases whatever was created
         return TAD_ERR_CUDA;
@@ -3677,9 +3819,13 @@ void tad_shutdown(tad_ctx *ctx)
     ctx->cv.notify_all();
     if (ctx->worker.joinable()) ctx->worker.join();
     cudaSetDevice(ctx->cfg.device);
-    if (ctx->peers_mapped && ctx->nccl.comm && ctx->small.p && ctx->stream) {
-        // an exported buffer must outlive every peer's mapping of it: unmap, meet the peers, only then free
+    if ((ctx->peers_mapped || ctx->boards_shared) && ctx->nccl.comm && ctx->small.p && ctx->stream) {
+        // an exported buffer or board must outlive every peer's mapping of it: unmap, meet the peers, only then free
         unmap_peers(ctx);
+        for (int r = 0; r < ctx->cfg.world_size; r++) {
+            if (r != ctx->cfg.rank && ctx->peer_board[r]) nccl_ipc_unmap(&ctx->nccl, ctx->peer_board[r]);
+            ctx->peer_board[r] = nullptr;
+        }
         if (peer_barrier(ctx) == 0) cudaStreamSynchronize(ctx->stream);
     }
     nccl_comm_destroy(&ctx->nccl);
@@ -3691,6 +3837,9 @@ void tad_shutdown(tad_ctx *ctx)
     if (ctx->h_stats) cudaFreeHost(ctx->h_stats);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
     if (ctx->h_fits) cudaFreeHost(ctx->h_fits);
+    if (ctx->h_board) cudaFreeHost(ctx->h_board);
+    if (ctx->board) cudaFree(ctx->board);
+    if (ctx->board_stream) cudaStreamDestroy(ctx->board_stream);
     for (int i = 0; i < 2; i++)
         if (ctx->fit_ev[i]) cudaEventDestroy(ctx->fit_ev[i]);
     if (ctx->fits_ev) cudaEventDestroy(ctx->fits_ev);
@@ -3945,6 +4094,7 @@ int tad_cancel(tad_job *job)
     if (!job) return TAD_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> lk(job->mu);
     job->cancel.store(1);
+    stop_running(job);
     job->cv.notify_all();        // a worker waiting for streamed input
     return TAD_OK;
 }
@@ -4032,6 +4182,7 @@ int tad_release(tad_job *job)
         const int s = job->st.state;
         if (s == TAD_STATE_SCHEDULED || s == TAD_STATE_RUNNING) {
             job->cancel.store(1);
+            stop_running(job);
             job->cv.notify_all();
             while (!(job->st.state == TAD_STATE_COMPLETED || job->st.state == TAD_STATE_FAILED))
                 job->cv.wait_for(lk, std::chrono::milliseconds(1));

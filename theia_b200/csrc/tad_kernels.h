@@ -83,9 +83,12 @@ cudaError_t launch_detect_dbscan(cudaStream_t st, const SeriesEntry *entries, co
 // the dropped fits a resume launch has finished again (both zeroed by the caller).  launch_arima_resume fits what is left
 // (the fits dropped in flight and those never started) into the same pred[] and counters, so the forecasts and counts are
 // those of one launch.
+// board (multi-GPU jobs, with resume null): the fit stops on the ranks' stop board instead of the cancel word -- 8 u32 in
+// this rank's device memory, one per rank (the rest 0); every warp leaves at its next round once a word equals `ordinal`.
 cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                              uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
+                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume,
+                             const uint32_t *board = nullptr, uint32_t ordinal = 0);
 cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
                                 uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
                                 const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
