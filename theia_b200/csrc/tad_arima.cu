@@ -950,39 +950,39 @@ __global__ void __launch_bounds__(NT) detect_arima_kernel(const SeriesEntry *__r
     }
 }
 
-cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                             uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume,
-                             const uint32_t *board, uint32_t ordinal)
+// blocks of 128 threads for one warp per series
+static uint32_t warp_blocks(uint64_t series) { return (uint32_t)((series * 32 + 127) / 128); }
+
+cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &p, const uint64_t *csr_v)
 {
-    if (S == 0) return cudaSuccess;
-    arima_boxcox_kernel<<<(S + 127) / 128, 128, 0, st>>>(entries, offsets, sbase, B, S, csr_v, scratch_y, scratch_lam, fits,
-                                                         resume ? scratch_pred : nullptr);
-    const uint64_t threads = (uint64_t)S * 32;
-    if (board)
-        arima_fit_board_kernel<<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                                  scratch_lam, scratch_pred,
-                                                                                  StopBoard{board, ordinal}, fits + 1);
-    else if (resume)
-        arima_fit_sync_kernel<1><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                                    scratch_lam, scratch_pred, cancel, fits + 1,
-                                                                                    resume);
-    else
-        arima_fit_sync_kernel<0><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                                    scratch_lam, scratch_pred, cancel, fits + 1,
-                                                                                    nullptr);
+    if (p.S == 0) return cudaSuccess;
+    arima_boxcox_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p.entries, p.offsets, p.sbase, p.B, p.S, csr_v, p.y, p.lam,
+                                                           p.fits_total, p.resume ? p.pred : nullptr);
     return cudaGetLastError();
 }
 
-cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                                uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
-                                const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume)
+cudaError_t launch_arima_fit(cudaStream_t st, const FitPart &p, const uint64_t *csr_v, const uint32_t *board, uint32_t ordinal)
 {
-    if (S == 0) return cudaSuccess;
-    const uint64_t threads = (uint64_t)S * 32;
-    arima_fit_sync_kernel<2><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(entries, offsets, sbase, B, S, scratch_y,
-                                                                                  scratch_lam, scratch_pred, cancel, fits + 1,
-                                                                                  resume);
+    const cudaError_t e = launch_arima_boxcox(st, p, csr_v);
+    if (e != cudaSuccess || p.S == 0) return e;
+    const uint32_t grid = warp_blocks(p.S);
+    if (board)
+        arima_fit_board_kernel<<<grid, 128, 0, st>>>(p.entries, p.offsets, p.sbase, p.B, p.S, p.y, p.lam, p.pred,
+                                                     StopBoard{board, ordinal}, p.fits_done);
+    else if (p.resume)
+        arima_fit_sync_kernel<1><<<grid, 128, 0, st>>>(p.entries, p.offsets, p.sbase, p.B, p.S, p.y, p.lam, p.pred, p.cancel,
+                                                       p.fits_done, p.resume);
+    else
+        arima_fit_sync_kernel<0><<<grid, 128, 0, st>>>(p.entries, p.offsets, p.sbase, p.B, p.S, p.y, p.lam, p.pred, p.cancel,
+                                                       p.fits_done, nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_arima_resume(cudaStream_t st, const FitPart &p)
+{
+    if (p.S == 0) return cudaSuccess;
+    arima_fit_sync_kernel<2><<<warp_blocks(p.S), 128, 0, st>>>(p.entries, p.offsets, p.sbase, p.B, p.S, p.y, p.lam, p.pred,
+                                                               p.cancel, p.fits_done, p.resume);
     return cudaGetLastError();
 }
 
@@ -994,20 +994,12 @@ cudaError_t launch_arima_unfinished(cudaStream_t st, const FitPart &a, uint32_t 
     return cudaGetLastError();
 }
 
-cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &b, const uint64_t *csr_v, uint32_t *fits_total)
-{
-    if (b.S == 0) return cudaSuccess;
-    arima_boxcox_kernel<<<(b.S + 127) / 128, 128, 0, st>>>(b.entries, b.offsets, b.sbase, b.B, b.S, csr_v, b.y, b.lam,
-                                                           fits_total, b.pred);
-    return cudaGetLastError();
-}
-
 cudaError_t launch_arima_pair(cudaStream_t st, const FitPart &a, uint32_t a_from, uint32_t n_a, const FitPart &b, bool b_first)
 {
-    const uint64_t threads = ((uint64_t)n_a + b.S) * 32;
-    if (threads == 0) return cudaSuccess;
-    if (b_first) arima_fit_pair_kernel<1><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(a, a_from, n_a, b);
-    else arima_fit_pair_kernel<2><<<(uint32_t)((threads + 127) / 128), 128, 0, st>>>(a, a_from, n_a, b);
+    const uint64_t series = (uint64_t)n_a + b.S;
+    if (series == 0) return cudaSuccess;
+    if (b_first) arima_fit_pair_kernel<1><<<warp_blocks(series), 128, 0, st>>>(a, a_from, n_a, b);
+    else arima_fit_pair_kernel<2><<<warp_blocks(series), 128, 0, st>>>(a, a_from, n_a, b);
     return cudaGetLastError();
 }
 

@@ -128,8 +128,9 @@ enum {
     ST_GPOINTS,         // then count the spilled buckets only); adjacent: zeroed together before every scoring attempt
     ST_COUNT
 };
-// ARIMA fit launch, outside the ST_COUNT readback: [ST_FITS, +2) the fit counters (launch_arima_fit's fits[0..1]), which
-// the worker copies back while the fit kernel runs, and [ST_FITS + 2] the kernel's cancel word
+// ARIMA fit launch, outside the ST_COUNT readback: [ST_FITS, +2) the fit counters (FitPart's fits_total, fits_done), which
+// the worker copies back while the fit kernel runs, [ST_FITS + 2] the kernel's cancel word, and [ST_FITS + 3] scratch of
+// a fit beside a yielded one
 constexpr int ST_FITS = 32;
 
 constexpr int kGroupCap = group_class(kGroupClasses - 1).cap;   // rows a bucket may hold to take the shared-memory path

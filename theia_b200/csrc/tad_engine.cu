@@ -135,15 +135,13 @@ double now_ms()
 
 }  // namespace
 
-// A fit that has yielded (fit sharing), as a flagged ARIMA job run in its yield fits beside it (wait_pair_fit): its
-// buffers stay parked in device memory, so its part of the joint launch needs only its launch arguments.
+// The fit of an ARIMA pass, as its wait (wait_fit) and its yields see it.  While the pass is parked its buffers stay in
+// device memory, so a flagged ARIMA job run in its yield fits beside it (ctx->beside) from its part alone.
 struct YieldedFit {
     tad_job *job;
-    FitPart part;                    // its series, buffers, cancel word, fits finished and resume points
-    uint32_t *d_fits;                // its fit counters [0, 2) and cancel word [2]
+    FitPart part;                    // its series, buffers, words and resume points
     uint64_t done0 = 0, total0 = 0;  // its fit counts before the pass (tad_job_progress adds the pass's counters to them)
     uint32_t dropped = 0;            // fits its last leave dropped: the next launch it takes part in redoes them
-    bool joint = false;              // a joint launch ran since the yield: `dropped` is that launch's
     double fit_ms = 0;               // time its part spent in joint launches since the yield: fit time, not parked time
 };
 
@@ -254,14 +252,17 @@ struct tad_ctx {
                   "pass scratch regions overlap");
     uint32_t scan_epoch = 0;
     uint32_t *h_stats = nullptr;   // pinned readback of the device scalars
-    // ARIMA fit launch (wait_arima_fit): pinned [0, 2): the fit counters while the kernel runs, [2, 4): once it has ended,
-    // [4]: 1, the value a cancel copies into the kernel's cancel word; [5]: 2, the value a yield copies there; [6], [7]:
-    // the fits the last yield dropped, and those of them finished again
-    // [8, 16): the same words for the yielded part of a joint fit (wait_pair_fit)
-    uint32_t *h_fits = nullptr;
+    // Pinned words of the fit launch in flight (wait_fit).  Per part ([0] the job's own fit, [1] the yielded fit beside
+    // it): its counters (fits_total, fits_done) as last copied back while the kernel runs and once it has ended, and its
+    // redo words (the fits its leave dropped; of those, finished again).  Then the values a cancel (1) and a leave (2)
+    // copy into a cancel word, and the yielded fit's lowest unfinished series (launch_arima_unfinished).
+    struct FitCounts { uint32_t total, done; };
+    struct FitWords { FitCounts run, end; uint32_t dropped, redone; };
+    struct FitPinned { FitWords part[2]; uint32_t cancel = 1, leave = 2, from = 0; };
+    FitPinned *h_fit = nullptr;
     std::atomic<uint64_t> fit_share{0};             // tad_set_fit_sharing: the reserve of the jobs run beside a fit (0: off)
     cudaEvent_t fit_ev[2]{};        // [0]: the fit counters are reset; [1]: the fit kernel has ended
-    cudaEvent_t fits_ev = nullptr;  // a copy of the fit counters has reached h_fits
+    cudaEvent_t fits_ev = nullptr;  // a copy of the fit counters has reached h_fit
     std::mutex pool_mu;
     std::vector<PinnedBlock> pinned_pool;
     NcclComm nccl;
@@ -452,7 +453,7 @@ constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad
 //     that pipeline allocates and zeroes it again for the scan's epochs);
 //   d_col[8..10): a one-pass job's host namespace columns, read before the fit only;
 //   h_stats and h_small: read back again after the fit (read_stats) and after every sweep (the counts);
-//   h_fits: the fit counters are published before the park;
+//   h_fit: the fit counters are published before the park;
 //   ev: the interleaved jobs record ev_alt, so the pass's phase events survive; the other events of a sweep are
 //     recorded in that sweep before they are waited for;
 //   limit, peak and store_peak: restored.
@@ -616,131 +617,13 @@ void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progres
     }
 }
 
-// The ARIMA fit launch of a pass (launch_arima_fit with d_fits = its counters and cancel word, enqueued on ctx->stream behind
-// their reset and fit_ev[0]), waited for without blocking behind it: the worker polls an event recorded after the fit
-// kernel, copies tad_cancel into the kernel's cancel word (single GPU only: on several GPUs the fit reads the stop board,
-// which tad_cancel writes itself, post_stop) and about every 50 ms copies the pass's fit counters back; both copies
-// run on the copy stream, beside the kernel.  The counters are published added to the job's counts before the pass.
-// Fit sharing (tad_set_fit_sharing): when a fit that can yield (job->share) sees a job waiting that interleave() would run,
-// it copies 2 into the cancel word instead; once the kernel has left, the pass is parked, the waiting jobs run, and
-// `resume` launches the rest of the fit (launch_arima_resume), waited for the same way.  d_redo (the resume array's words
-// [2S, 2S + 2), zeroed before the fit launch): the fits a yield dropped, and those of them the resume has finished again.
-// Fairness: after a resume the fit does not yield again until every fit the last yield dropped has finished again and it
-// has run at least as long as that interleave took (job->quiet_until).  So no fit is dropped twice: the work yields throw
-// away is at most one fitting of each prefix, and under a steady stream of short jobs the fit phase (parked time left
-// out) takes at most about twice as long.  Each resume launch is added to `launches`.
-// yf (a fit that can yield, null otherwise): its launch arguments, which a flagged ARIMA job run in the yield fits beside
-// (wait_pair_fit); the time its part of such joint launches took is fit time, not parked time.
-// Returns once the kernel has ended, its final counts published: the time the pass was parked (ms).
-bool interleave_waiting(tad_ctx *ctx, const tad_job *job);
-void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf);
 bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve);
-template <class Resume>
-double wait_arima_fit(tad_ctx *ctx, tad_job *job, uint32_t *d_fits, uint32_t *d_redo, uint64_t &launches, YieldedFit *yf,
-                      Resume resume)
-{
-    uint64_t done0, total0;
-    {
-        std::lock_guard<std::mutex> lk(job->mu);
-        done0 = job->prog.fits_done;
-        total0 = job->prog.fits_total;
-    }
-    auto publish = [&](const uint32_t *h) {
-        std::lock_guard<std::mutex> lk(job->mu);
-        job->prog.fits_total = total0 + h[0];
-        job->prog.fits_done = done0 + h[1];
-    };
-    const bool cancellable = ctx->cfg.world_size == 1;
-    double parked = 0;
-    uint32_t dropped = 0, redone = 0;    // the fits the last yield dropped; of those, finished again (as last copied back)
-    double t_word = 0;
-    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));     // no copy touches the words before their reset
-    for (;;) {
-        CU(cudaEventRecord(ctx->fit_ev[1], ctx->stream));
-        bool copying = false, cancelled = false, yielded = false;
-        double next_copy = now_ms();
-        for (;;) {
-            if (cancellable && !cancelled && job->cancel.load()) {
-                CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 4, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-                cancelled = true;
-            }
-            if (job->share && !cancelled && !yielded && redone >= dropped && now_ms() >= job->quiet_until &&
-                interleave_waiting(ctx, job)) {
-                CU(cudaMemcpyAsync(d_fits + 2, ctx->h_fits + 5, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-                yielded = true;
-                t_word = now_ms();
-            }
-            const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
-            if (e != cudaErrorNotReady) {
-                CU(e);
-                break;
-            }
-            if (copying) {
-                const cudaError_t c = cudaEventQuery(ctx->fits_ev);
-                if (c != cudaErrorNotReady) {
-                    CU(c);
-                    publish(ctx->h_fits);
-                    if (redone < dropped) redone = ctx->h_fits[7];
-                    copying = false;
-                }
-            }
-            // every 50 ms; every poll while the next yield waits for the dropped fits only
-            if (!copying && (now_ms() >= next_copy || redone < dropped)) {
-                CU(cudaMemcpyAsync(ctx->h_fits, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                if (redone < dropped) CU(cudaMemcpyAsync(ctx->h_fits + 7, d_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
-                copying = true;
-                next_copy = now_ms() + 50.0;
-            }
-            std::this_thread::sleep_for(std::chrono::milliseconds(1));
-        }
-        CU(cudaMemcpyAsync(ctx->h_fits + 2, d_fits, 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        publish(ctx->h_fits + 2);
-        // not yielded, cancelled (the caller fails the job), or every fit finished before the kernel saw the word
-        if (!yielded || cancelled || ctx->h_fits[3] == ctx->h_fits[2]) return parked;
-        const double t0 = now_ms();
-        CU(cudaStreamSynchronize(ctx->copy_stream));           // the yield has reached the word before it is reset
-        CU(cudaMemcpyAsync(ctx->h_fits + 6, d_redo, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        dropped = ctx->h_fits[6];
-        redone = 0;
-        if (getenv("TAD_DEBUG_YIELD")) fprintf(stderr, "yield: kernel left %.2f ms after the word, %u fits dropped\n", t0 - t_word, dropped);
-        if (yf) {
-            yf->done0 = done0;
-            yf->total0 = total0;
-            yf->dropped = dropped;
-            yf->joint = false;
-            yf->fit_ms = 0;
-        }
-        interleave(ctx, job, yf);
-        double away = now_ms() - t0;
-        if (yf && yf->joint) {           // its part fitted beside another job: those fits are the ones to finish again
-            dropped = yf->dropped;
-            away = std::max(0.0, away - yf->fit_ms);
-        }
-        CU(cudaMemsetAsync(d_fits + 2, 0, 4, ctx->stream));
-        CU(cudaMemsetAsync(d_redo, 0, 8, ctx->stream));
-        CU(cudaEventRecord(ctx->fit_ev[0], ctx->stream));
-        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
-        const double t1 = now_ms();
-        parked += away;
-        job->quiet_until = t1 + away;
-        {
-            std::lock_guard<std::mutex> lk(job->mu);
-            job->yields++;
-            job->parked_ms += away;
-        }
-        resume();
-        launches++;
-    }
-}
 
-// Whether a wait_arima_fit may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
+// Whether a fit's yield may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
 // large for the reserve.  A streamed one only with TAD_FLAG_SHARE and once its feeder has handed over its first block or
 // closed its round: a job whose caller has not started delivering would hold the fit parked while it waits.
 // `beside`: the yield is that of a fit parked at the outer level whose reserve halves to the 64 MiB floor or more; then an
-// ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (wait_pair_fit): a tad_submit one, or a streamed one
+// ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (fit_beside): a tad_submit one, or a streamed one
 // with TAD_FLAG_SHARE as well, fed as above.
 bool interleavable(tad_job *j, bool beside)
 {
@@ -864,138 +747,192 @@ void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
     if (cancelled) fail(TAD_ERR_CANCELLED, "job cancelled");
 }
 
-// The fit of `job`, an ARIMA job run in the yield of the fit `a` (TAD_FLAG_FIT_BESIDE): Box-Cox, then joint launches of
-// its series beside the ones `a` has left (launch_arima_pair), waited for as wait_arima_fit waits for one fit.  `b`: its
-// part, with its counters d_fits[0, 2) and cancel word d_fits[2] (zeroed by the caller, as are b's resume words [2S, 2S + 2));
-// d_fits[3] is scratch.  The worker watches both jobs, polling every millisecond:
-//   end: once every fit of `job` is done and `a` has finished again all fits its last leave dropped (so none of them is
-//     dropped twice), 2 goes into a's word: its part leaves within one evaluation round, its resume points written;
-//   a cancel of `job` ends the launch (1 in its word, 2 in a's); one of `a` puts 1 in a's word only: its part leaves and
-//     job's goes on (`a` fails once `job` has ended, like any parked job);
-//   yield: an EWMA or DBSCAN job waiting makes both parts leave (2 in both words), once both have finished again the fits
-//     their last leave dropped and the quiet time of job's last yield has passed; job's pass is parked in turn
-//     (interleave, one level deeper, which runs EWMA and DBSCAN jobs only, in job's reserve), and both parts then resume
-//     in one joint launch;
-//   both jobs' fit counts (tad_job_progress) are published as they are copied back.
-// a->dropped, a->joint and a->fit_ms tell a's wait_arima_fit what its part did.  Returns the time job's pass was parked (ms).
-double wait_pair_fit(tad_ctx *ctx, tad_job *job, YieldedFit *a, const FitPart &b, const uint64_t *csr_v, uint32_t *d_fits,
-                     uint64_t &launches)
+// ---- the fit launches of an ARIMA pass ----------------------------------------------------------------------------------
+// A pass's fit (fit_solo, or fit_beside for a job run in another fit's yield) is enqueued on ctx->stream behind the reset
+// of its words and fit_ev[0], and waited for without blocking behind it (wait_fit): the worker polls, every millisecond,
+// an event recorded after the kernel, and watches each part of the launch in flight -- one for a job's own fit or resume,
+// two for a joint launch: b, the job fitting beside a yielded fit, and a, that fit.  Its copies and word writes run on the
+// copy stream, beside the kernel:
+//   cancel: a cancel of a part's job writes 1 into the part's cancel word (one GPU only: on several GPUs the fit reads the
+//     stop board, which tad_cancel writes itself, post_stop).  A cancel of b makes a leave too (2), so b fails at once; a
+//     cancelled a fails once b has ended, like any parked job;
+//   end: once every fit of b is counted done and a is clear, 2 goes into a's word: its part leaves within one evaluation
+//     round, its resume points written.  A part is clear when it is cancelled or has finished again every fit its last
+//     leave dropped (so none is dropped twice);
+//   yield (fit sharing, tad_set_fit_sharing): once the job whose wait this is (the solo job, or b) can yield (share), is
+//     neither cancelled nor yielded in this launch, a has not been told to leave, every part is clear, the job's quiet
+//     time has passed and a job is waiting that interleave() would run, 2 goes into every part's word that holds neither
+//     1 nor 2.  Once the kernel has left, the pass is parked, the waiting jobs run (park_pass), and the rest of the fit is
+//     launched: the solo fit's resume (launch_arima_resume) or the next joint launch.  Fairness: after a resume the fit
+//     does not yield again until every fit the last yield dropped has finished again and it has run at least as long as
+//     that interleave took (job->quiet_until).  So the work yields throw away is at most one fitting of each prefix, and
+//     under a steady stream of short jobs the fit phase (parked time left out) takes at most about twice as long;
+//   counts: the parts' counters come back every 50 ms for a solo fit, every poll during a joint launch or while a part
+//     has a redo pending, and are published added to each job's counts before the pass (tad_job_progress).
+// Once the kernel has ended the final counts are published and each part's fits dropped read; a's part in joint launches
+// is fit time for a, not parked time.  Returns whether the launch yielded: the fit has fits left, and the pass is parked
+// before its next launch.
+bool wait_fit(tad_ctx *ctx, YieldedFit &own, YieldedFit *a)
+{
+    struct Watch {
+        YieldedFit *f;
+        tad_ctx::FitWords *h;
+        uint32_t redone = 0;             // of the fits f's last leave dropped, those finished again (as last copied back)
+        bool cancelled = false, left = false;   // 1 / 2 written into its cancel word in this launch
+        bool redoing() const { return redone < f->dropped; }
+        bool clear() const { return cancelled || !redoing(); }
+        uint32_t *redo() const { return f->part.resume + 2 * (size_t)f->part.S; }
+    };
+    tad_ctx::FitPinned *H = ctx->h_fit;
+    const int n = a ? 2 : 1;
+    Watch w[2] = {{&own, &H->part[0]}, {a, &H->part[1]}};
+    auto word = [&](Watch &p, const uint32_t *value) {
+        CU(cudaMemcpyAsync(p.f->part.cancel, value, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+    };
+    auto leave = [&](Watch &p) {
+        if (!p.cancelled && !p.left) word(p, &H->leave);
+        p.left = true;
+    };
+    auto publish = [](const YieldedFit *f, const tad_ctx::FitCounts &c) {
+        std::lock_guard<std::mutex> lk(f->job->mu);
+        f->job->prog.fits_total = f->total0 + c.total;
+        f->job->prog.fits_done = f->done0 + c.done;
+    };
+    const bool cancellable = ctx->cfg.world_size == 1;
+    const double t_launch = now_ms();
+    double next_copy = t_launch, t_word = 0;
+    bool copying = false, counted = false;
+    CU(cudaEventRecord(ctx->fit_ev[1], ctx->stream));
+    for (;;) {
+        for (int i = n - 1; i >= 0; i--)
+            if (cancellable && !w[i].cancelled && w[i].f->job->cancel.load()) {
+                word(w[i], &H->cancel);
+                w[i].cancelled = true;
+                if (i == 0 && a) leave(w[1]);
+            }
+        if (a && counted && !w[1].left && !w[1].cancelled && w[1].clear() && w[0].h->run.done == w[0].h->run.total)
+            leave(w[1]);
+        if (own.job->share && !w[0].cancelled && !w[0].left && !w[1].left && w[0].clear() && (!a || w[1].clear()) &&
+            now_ms() >= own.job->quiet_until && interleave_waiting(ctx, own.job)) {
+            for (int i = 0; i < n; i++) leave(w[i]);
+            t_word = now_ms();
+        }
+        const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
+        if (e != cudaErrorNotReady) {
+            CU(e);
+            break;
+        }
+        if (copying) {
+            const cudaError_t c = cudaEventQuery(ctx->fits_ev);
+            if (c != cudaErrorNotReady) {
+                CU(c);
+                for (int i = 0; i < n; i++) {
+                    publish(w[i].f, w[i].h->run);
+                    if (w[i].redoing()) w[i].redone = w[i].h->redone;
+                }
+                counted = true;
+                copying = false;
+            }
+        }
+        if (!copying && (a || w[0].redoing() || now_ms() >= next_copy)) {
+            for (int i = 0; i < n; i++) {
+                CU(cudaMemcpyAsync(&w[i].h->run, w[i].f->part.fits_total, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
+                if (w[i].redoing())
+                    CU(cudaMemcpyAsync(&w[i].h->redone, w[i].redo() + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
+            }
+            CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
+            copying = true;
+            next_copy = now_ms() + 50.0;
+        }
+        std::this_thread::sleep_for(std::chrono::milliseconds(1));
+    }
+    CU(cudaStreamSynchronize(ctx->copy_stream));            // no copy or word write is left behind the kernel
+    for (int i = 0; i < n; i++) {
+        CU(cudaMemcpyAsync(&w[i].h->end, w[i].f->part.fits_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        if (w[i].f->part.resume) CU(cudaMemcpyAsync(&w[i].h->dropped, w[i].redo(), 4, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    const double t_end = now_ms();
+    for (int i = 0; i < n; i++) {
+        publish(w[i].f, w[i].h->end);
+        if (w[i].f->part.resume) w[i].f->dropped = w[i].h->dropped;
+    }
+    if (a) a->fit_ms += t_end - t_launch;
+    // not yielded, cancelled (the caller fails the job), or every fit finished before the kernel saw the word
+    const bool yielded = w[0].left && !w[0].cancelled && w[0].h->end.done != w[0].h->end.total;
+    if (yielded && getenv("TAD_DEBUG_YIELD"))
+        fprintf(stderr, "yield: kernel left %.2f ms after the word, %u + %u fits dropped\n", t_end - t_word, own.dropped,
+                a ? a->dropped : 0u);
+    return yielded;
+}
+
+// Before a fit launch: the cancel and redo words the last launch of p and q left are zeroed (null: none to zero), and the
+// copy stream's reads and writes of the fit's words wait for that (fit_ev[0]).
+void arm_fit(tad_ctx *ctx, const FitPart *p, const FitPart *q = nullptr)
+{
+    for (const FitPart *r : {p, q})
+        if (r) {
+            CU(cudaMemsetAsync(r->cancel, 0, 4, ctx->stream));
+            CU(cudaMemsetAsync(r->resume + 2 * (size_t)r->S, 0, 8, ctx->stream));
+        }
+    CU(cudaEventRecord(ctx->fit_ev[0], ctx->stream));
+    CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
+}
+
+// After a launch has yielded: the pass of `job` is parked while the waiting jobs run (interleave); yf: its fit, which an
+// ARIMA job run there may fit beside.  Returns the time parked, yf's part of joint launches left out; the fit does not
+// yield again before it has run as long.
+double park_pass(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
+{
+    if (yf) yf->fit_ms = 0;
+    const double t0 = now_ms();
+    interleave(ctx, job, yf);
+    const double t1 = now_ms();
+    const double away = std::max(0.0, t1 - t0 - (yf ? yf->fit_ms : 0.0));
+    job->quiet_until = t1 + away;
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->yields++;
+    job->parked_ms += away;
+    return away;
+}
+
+// A pass's own fit: launch_arima_fit, then after each yield the resume of what is left.  Returns the time parked (ms).
+double fit_solo(tad_ctx *ctx, YieldedFit &fit, const uint64_t *csr_v, uint64_t &launches)
+{
+    arm_fit(ctx, nullptr);
+    CU(launch_arima_fit(ctx->stream, fit.part, csr_v, ctx->cfg.world_size > 1 ? ctx->board : nullptr, fit.job->ordinal));
+    launches += 2;
+    double parked = 0;
+    while (wait_fit(ctx, fit, nullptr)) {
+        parked += park_pass(ctx, fit.job, &fit);
+        arm_fit(ctx, &fit.part);
+        CU(launch_arima_resume(ctx->stream, fit.part));
+        launches++;
+    }
+    return parked;
+}
+
+// The fit of b, an ARIMA job run in the yield of the fit a (TAD_FLAG_FIT_BESIDE): Box-Cox, then joint launches of b's
+// series beside those a has left, from a's lowest unfinished series, until b's fit has ended.  After a yield of b only
+// b's pass is parked (one level deeper, EWMA and DBSCAN jobs only).  d_from: a device word of scratch.  Returns the time
+// b's pass was parked (ms).
+double fit_beside(tad_ctx *ctx, YieldedFit &b, YieldedFit &a, const uint64_t *csr_v, uint32_t *d_from, uint64_t &launches)
 {
     cudaStream_t st = ctx->stream;
-    uint32_t *hb = ctx->h_fits, *ha = ctx->h_fits + 8;      // [0, 2) counters while running, [2, 4) at the end, [6] [7] redo
-    uint32_t *b_redo = b.resume + 2 * (size_t)b.S, *a_redo = a->part.resume + 2 * (size_t)a->part.S;
-    uint64_t done0, total0;
-    {
-        std::lock_guard<std::mutex> lk(job->mu);
-        done0 = job->prog.fits_done;
-        total0 = job->prog.fits_total;
-    }
-    auto publish = [&](const uint32_t *h_b, const uint32_t *h_a) {
-        {
-            std::lock_guard<std::mutex> lk(job->mu);
-            job->prog.fits_total = total0 + h_b[0];
-            job->prog.fits_done = done0 + h_b[1];
-        }
-        std::lock_guard<std::mutex> lk(a->job->mu);
-        a->job->prog.fits_total = a->total0 + h_a[0];
-        a->job->prog.fits_done = a->done0 + h_a[1];
-    };
-    auto word = [&](uint32_t *d_word, int value) {          // value 1 (cancel) or 2 (leave), beside the kernel
-        CU(cudaMemcpyAsync(d_word, ctx->h_fits + 3 + value, 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-    };
-    CU(launch_arima_boxcox(st, b, csr_v, d_fits));          // job's fit count is final before the joint launch
+    CU(launch_arima_boxcox(st, b.part, csr_v));             // b's fit count is final before the joint launch
+    launches++;
     double parked = 0;
-    uint32_t b_dropped = 0;
     for (bool first = true;; first = false) {
-        // a's part: its series from the lowest one with fits left on
-        CU(cudaMemsetAsync(a->d_fits + 2, 0, 4, st));
-        CU(cudaMemsetAsync(a_redo, 0, 8, st));
-        CU(launch_arima_unfinished(st, a->part, d_fits + 3));
-        CU(cudaMemcpyAsync(ha + 6, d_fits + 3, 4, cudaMemcpyDeviceToHost, st));
+        CU(launch_arima_unfinished(st, a.part, d_from));
+        launches++;
+        CU(cudaMemcpyAsync(&ctx->h_fit->from, d_from, 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        const uint32_t from = ha[6] == ~0u ? 0 : ha[6], n_a = ha[6] == ~0u ? 0 : a->part.S - ha[6];
-        if (!first) {
-            CU(cudaMemsetAsync(d_fits + 2, 0, 4, st));
-            CU(cudaMemsetAsync(b_redo, 0, 8, st));
-        }
-        CU(cudaEventRecord(ctx->fit_ev[0], st));
-        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
-        const double t_launch = now_ms();
-        CU(launch_arima_pair(st, a->part, from, n_a, b, first));
-        launches += first ? 1 : 2;          // the caller counts the Box-Cox and the first joint launch
-        CU(cudaEventRecord(ctx->fit_ev[1], st));
-        bool copying = false, counted = false, a_cancelled = false, a_left = false, b_cancelled = false, yielded = false;
-        uint32_t a_redone = 0, b_redone = 0;
-        for (;;) {
-            if (!a_cancelled && !a_left && a->job->cancel.load()) {
-                word(a->d_fits + 2, 1);
-                a_cancelled = true;
-            }
-            if (!b_cancelled && job->cancel.load()) {
-                word(d_fits + 2, 1);
-                if (!a_cancelled && !a_left) word(a->d_fits + 2, 2);
-                b_cancelled = a_left = true;
-            }
-            const bool a_clear = a_cancelled || a_redone >= a->dropped;
-            if (counted && !a_left && !a_cancelled && hb[1] == hb[0] && a_clear) {      // every fit of job is done
-                word(a->d_fits + 2, 2);
-                a_left = true;
-            }
-            if (job->share && !b_cancelled && !a_left && !yielded && a_clear && b_redone >= b_dropped &&
-                now_ms() >= job->quiet_until && interleave_waiting(ctx, job)) {
-                word(d_fits + 2, 2);
-                if (!a_cancelled) word(a->d_fits + 2, 2);
-                yielded = true;
-            }
-            const cudaError_t e = cudaEventQuery(ctx->fit_ev[1]);
-            if (e != cudaErrorNotReady) {
-                CU(e);
-                break;
-            }
-            if (copying) {
-                const cudaError_t c = cudaEventQuery(ctx->fits_ev);
-                if (c != cudaErrorNotReady) {
-                    CU(c);
-                    publish(hb, ha);
-                    b_redone = hb[7];
-                    a_redone = ha[7];
-                    counted = true;
-                    copying = false;
-                }
-            }
-            if (!copying) {
-                CU(cudaMemcpyAsync(hb, d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                CU(cudaMemcpyAsync(ha, a->d_fits, 8, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                CU(cudaMemcpyAsync(hb + 7, b_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                CU(cudaMemcpyAsync(ha + 7, a_redo + 1, 4, cudaMemcpyDeviceToHost, ctx->copy_stream));
-                CU(cudaEventRecord(ctx->fits_ev, ctx->copy_stream));
-                copying = true;
-            }
-            std::this_thread::sleep_for(std::chrono::milliseconds(1));
-        }
-        CU(cudaStreamSynchronize(ctx->copy_stream));            // no copy or word write is left behind the kernel
-        CU(cudaMemcpyAsync(hb + 2, d_fits, 8, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(ha + 2, a->d_fits, 8, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(hb + 6, b_redo, 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(ha + 6, a_redo, 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        publish(hb + 2, ha + 2);
-        a->dropped = ha[6];
-        a->joint = true;
-        const double t0 = now_ms();
-        a->fit_ms += t0 - t_launch;
-        b_dropped = hb[6];
-        // done, cancelled (the caller fails the job), or every fit finished before the kernel saw the yield
-        if (!yielded || b_cancelled || hb[3] == hb[2]) return parked;
-        if (getenv("TAD_DEBUG_YIELD")) fprintf(stderr, "joint yield: %u + %u fits dropped\n", b_dropped, a->dropped);
-        interleave(ctx, job, nullptr);
-        CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->fit_ev[0], 0));
-        const double t1 = now_ms();
-        parked += t1 - t0;
-        job->quiet_until = t1 + (t1 - t0);
-        std::lock_guard<std::mutex> lk(job->mu);
-        job->yields++;
-        job->parked_ms += t1 - t0;
+        const uint32_t lo = ctx->h_fit->from;               // ~0u: a has no fits left
+        arm_fit(ctx, &a.part, first ? nullptr : &b.part);
+        CU(launch_arima_pair(st, a.part, lo == ~0u ? 0 : lo, lo == ~0u ? 0 : a.part.S - lo, b.part, first));
+        launches++;
+        if (!wait_fit(ctx, b, &a)) return parked;
+        parked += park_pass(ctx, b.job, nullptr);
     }
 }
 
@@ -1926,33 +1863,30 @@ void run_pipeline(tad_ctx *ctx, tad_job *job, const tad_columns &hc, bool filter
             ensure(ctx, ctx->ar_lam, z.ar_lam);
             ensure(ctx, ctx->ar_res, z.ar_res);
             if (attempt == 0 && S) {
-                double *y = (double *)ctx->ar_y.p, *pred = (double *)ctx->ar_pred.p, *lam = (double *)ctx->ar_lam.p;
                 uint32_t *res = job->share ? (uint32_t *)ctx->ar_res.p : nullptr;
                 CU(cudaMemsetAsync(d_stats + ST_FITS, 0, 12, st));      // fit counters and cancel word
                 if (res) CU(cudaMemsetAsync(res + 2 * (size_t)S, 0, 8, st));
-                // this pass's fit as the part a job run in its yield may fit beside (its buffers stay parked meanwhile)
-                YieldedFit yf{job, FitPart{entries, offsets, sbase, Bl, S, y, lam, pred, d_stats + ST_FITS + 2,
-                                           d_stats + ST_FITS + 1, res}, d_stats + ST_FITS};
-                if (ctx->beside && ctx->beside->job != job) {      // this job runs in that yield: it fits beside it
-                    parked_ms = wait_pair_fit(ctx, job, ctx->beside, yf.part, csr_v, d_stats + ST_FITS, launches);
-                } else {
-                    CU(cudaEventRecord(ctx->fit_ev[0], st));
-                    CU(launch_arima_fit(st, entries, offsets, sbase, Bl, S, csr_v, y, pred, lam, d_stats + ST_FITS + 2,
-                                        d_stats + ST_FITS, res, world > 1 ? ctx->board : nullptr, job->ordinal));
-                    parked_ms = wait_arima_fit(ctx, job, d_stats + ST_FITS, res ? res + 2 * (size_t)S : nullptr, launches,
-                                               res ? &yf : nullptr, [&] {
-                        CU(launch_arima_resume(st, entries, offsets, sbase, Bl, S, y, pred, lam, d_stats + ST_FITS + 2,
-                                               d_stats + ST_FITS, res));
-                    });
-                }
+                // this pass's fit, also the part a job run in its yield may fit beside (its buffers stay parked meanwhile)
+                const tad_progress before = progress_of(job);
+                YieldedFit fit{job,
+                               FitPart{entries, offsets, sbase, Bl, S, (double *)ctx->ar_y.p, (double *)ctx->ar_lam.p,
+                                       (double *)ctx->ar_pred.p, d_stats + ST_FITS + 2, d_stats + ST_FITS + 1, res,
+                                       d_stats + ST_FITS},
+                               before.fits_done, before.fits_total};
+                if (ctx->beside && ctx->beside->job != job)        // this job runs in that yield: it fits beside it
+                    parked_ms = fit_beside(ctx, fit, *ctx->beside, csr_v, d_stats + ST_FITS + 3, launches);
+                else
+                    parked_ms = fit_solo(ctx, fit, csr_v, launches);
                 // pred[] is incomplete: no detect.  Several GPUs: the rank goes on to the verdict, which fails the job
                 check_cancel();
-                if (world > 1 && ctx->h_fits[3] < ctx->h_fits[2]) out.fit_stop = board_stopper(ctx, job);
+                const tad_ctx::FitCounts &end = ctx->h_fit->part[0].end;
+                if (world > 1 && end.done < end.total) out.fit_stop = board_stopper(ctx, job);
             }
-            if (out.fit_stop < 0)
+            if (out.fit_stop < 0) {
                 CU(launch_detect_arima(st, entries, offsets, sbase, Bl, S, csr_v, csr_t, (const double *)ctx->ar_pred.p,
                                        (const double *)ctx->ar_lam.p, oc, (uint32_t)out_cap, d_stats, emit_all));
-            launches += S ? (attempt == 0 ? 3 : 1) : 0;
+                launches += S ? 1 : 0;
+            }
         } else {
             fail(TAD_ERR_UNSUPPORTED, "algorithm %d is not implemented by this build", sp.algo);
         }
@@ -3771,11 +3705,8 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     ok = ok && cudaHostAlloc((void **)&ctx->h_stats, 64 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_small, tad_ctx::kSmallWords * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
     ok = ok && cudaHostAlloc((void **)&ctx->h_chunk, 2 * kMaxPasses * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void **)&ctx->h_fits, 16 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-    if (ok) {
-        ctx->h_fits[4] = 1;
-        ctx->h_fits[5] = 2;
-    }
+    ok = ok && cudaHostAlloc((void **)&ctx->h_fit, sizeof(tad_ctx::FitPinned), cudaHostAllocDefault) == cudaSuccess;
+    if (ok) *ctx->h_fit = tad_ctx::FitPinned{};
     for (int i = 0; ok && i < 2; i++) ok = cudaEventCreateWithFlags(&ctx->fit_ev[i], cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ctx->fits_ev, cudaEventDisableTiming) == cudaSuccess;
     if (ok && cfg->world_size > 1) {
@@ -3836,7 +3767,7 @@ void tad_shutdown(tad_ctx *ctx)
     if (ctx->h_chunk) cudaFreeHost(ctx->h_chunk);
     if (ctx->h_stats) cudaFreeHost(ctx->h_stats);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
-    if (ctx->h_fits) cudaFreeHost(ctx->h_fits);
+    if (ctx->h_fit) cudaFreeHost(ctx->h_fit);
     if (ctx->h_board) cudaFreeHost(ctx->h_board);
     if (ctx->board) cudaFree(ctx->board);
     if (ctx->board_stream) cudaStreamDestroy(ctx->board_stream);

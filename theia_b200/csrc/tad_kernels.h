@@ -72,42 +72,40 @@ cudaError_t launch_detect_dbscan(cudaStream_t st, const SeriesEntry *entries, co
                                  uint32_t *scratch_pc, uint8_t *scratch_flag, const OutCols &out, uint32_t out_cap,
                                  uint32_t *stats, int emit_all);
 
-// ARIMA (tad_arima.cu): launch_arima_fit runs Box-Cox + the per-prefix ARIMA(1,1,1) MLE fits into scratch_pred (two
-// launches), launch_detect_arima then scores / flags / compacts (one launch, rerun alone when the result grows).
-// scratch_y / scratch_pred: one double per point slot; scratch_lam: one double per series.
-// cancel: a device word the fit kernel reads in every round; nonzero = every warp leaves at its next round and drops the
-// fits in flight, so pred[] is then incomplete.  fits[0] gains the prefix fits of the series, fits[1] the fits finished
-// (u32: one fit per point, fewer than 2^32 points per pass).
-// resume (2 S + 2 u32, or null): the fit can yield.  A cancel word of 2 makes every warp leave like a cancel, after it has
-// written its series' resume point and the fits it dropped there ([2i], [2i + 1]); [2S] gains the fits dropped, [2S + 1]
-// the dropped fits a resume launch has finished again (both zeroed by the caller).  launch_arima_resume fits what is left
-// (the fits dropped in flight and those never started) into the same pred[] and counters, so the forecasts and counts are
-// those of one launch.
-// board (multi-GPU jobs, with resume null): the fit stops on the ranks' stop board instead of the cancel word -- 8 u32 in
-// this rank's device memory, one per rank (the rest 0); every warp leaves at its next round once a word equals `ordinal`.
-cudaError_t launch_arima_fit(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                             uint32_t B, uint32_t S, const uint64_t *csr_v, double *scratch_y, double *scratch_pred,
-                             double *scratch_lam, const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume,
-                             const uint32_t *board = nullptr, uint32_t ordinal = 0);
-cudaError_t launch_arima_resume(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
-                                uint32_t B, uint32_t S, const double *scratch_y, double *scratch_pred, const double *scratch_lam,
-                                const volatile uint32_t *cancel, uint32_t *fits, uint32_t *resume);
-// Fitting beside a yielded fit (TAD_FLAG_FIT_BESIDE): one job's fit as a part of a joint launch -- its series, the
-// buffers launch_arima_fit takes, its cancel word, fits finished (fits[1]) and resume array (2 S + 2 words, not null).
+// ARIMA (tad_arima.cu): the per-prefix ARIMA(1,1,1) MLE fits of a pass's series into pred[], then launch_detect_arima
+// scores / flags / compacts (one launch, rerun alone when the result grows).
+// FitPart: one job's fit as a launcher takes it.  y / pred: one double per point slot; lam: one double per series.
+// fits_total, fits_done, cancel: the words of the fit (u32: one fit per point, fewer than 2^32 points per pass).
+//   fits_total gains the prefix fits of the series (Box-Cox) and fits_done, the word after it (the worker copies both
+//   back at once), the fits finished.  The fit kernel reads the cancel word in every round; nonzero = every warp leaves
+//   at its next round and drops the fits in flight, so pred[] is then incomplete.
+// resume (2 S + 2 u32): the fit can yield (null: it cannot).  A cancel word of 2 makes every warp leave like a cancel,
+//   after it has written its series' resume point and the fits it dropped there ([2i], [2i + 1]); [2S] gains the fits
+//   dropped, [2S + 1] the dropped fits a resume launch has finished again (both zeroed by the caller).
 struct FitPart {
     const SeriesEntry *entries;
     const uint32_t *offsets, *sbase;
     uint32_t B, S;
     double *y, *lam, *pred;
-    const volatile uint32_t *cancel;
+    uint32_t *cancel;
     uint32_t *fits_done, *resume;
+    uint32_t *fits_total;
 };
-// launch_arima_boxcox: launch_arima_fit's Box-Cox kernel for part b (its pred[] marked for a fit that can yield).
-// launch_arima_unfinished: *from = the lowest series of the yielded part a that has fits left (~0u: none).
-// launch_arima_pair: one launch fits part b beside the fits a has left, a's series a_from ..< a_from + n_a, each part as
-// its own launch would (a as its resume launch, b as launch_arima_fit's fit kernel when b_first, else as its resume
-// launch), about half the warps each.
-cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &b, const uint64_t *csr_v, uint32_t *fits_total);
+// launch_arima_boxcox: y = the Box-Cox transformed series, lam, and fits_total; with resume, pred[] marked as not fitted.
+// launch_arima_fit: launch_arima_boxcox, then the fit kernel (two launches).  board (multi-GPU jobs, with resume null):
+//   the fit stops on the ranks' stop board instead of the cancel word -- 8 u32 in this rank's device memory, one per rank
+//   (the rest 0); every warp leaves at its next round once a word equals `ordinal`.
+// launch_arima_resume: fits what a yield left (the fits dropped in flight and those never started) into the same pred[]
+//   and counters, so the forecasts and counts are those of one launch.
+// Fitting beside a yielded fit (TAD_FLAG_FIT_BESIDE), part b beside the yielded part a:
+// launch_arima_unfinished: *from = the lowest series of a that has fits left (~0u: none).
+// launch_arima_pair: one launch fits b beside the fits a has left, a's series a_from ..< a_from + n_a, each part as its
+//   own launch would (a as its resume launch, b as launch_arima_fit's fit kernel when b_first, else as its resume launch),
+//   about half the warps each.  b's Box-Cox is launch_arima_boxcox.
+cudaError_t launch_arima_boxcox(cudaStream_t st, const FitPart &p, const uint64_t *csr_v);
+cudaError_t launch_arima_fit(cudaStream_t st, const FitPart &p, const uint64_t *csr_v, const uint32_t *board = nullptr,
+                             uint32_t ordinal = 0);
+cudaError_t launch_arima_resume(cudaStream_t st, const FitPart &p);
 cudaError_t launch_arima_unfinished(cudaStream_t st, const FitPart &a, uint32_t *from);
 cudaError_t launch_arima_pair(cudaStream_t st, const FitPart &a, uint32_t a_from, uint32_t n_a, const FitPart &b, bool b_first);
 cudaError_t launch_detect_arima(cudaStream_t st, const SeriesEntry *entries, const uint32_t *offsets, const uint32_t *sbase,
