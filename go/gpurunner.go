@@ -71,6 +71,7 @@ type gpuJobRunner struct {
 	jobs   sync.Map    // id -> *gpuJob
 	share  atomic.Bool // SetFitSharing turned fit sharing on: StartStream flags its jobs
 	beside atomic.Bool // SetFitBeside: Start (StartStream while share is on) flags its ARIMA jobs to fit beside a running fit
+	lend   atomic.Bool // SetStreamLend: StartStream flags its jobs to lend the GPU while their SELECT is read
 }
 
 func newGPUJobRunner(device int) (*gpuJobRunner, error) {
@@ -125,6 +126,15 @@ func (r *gpuJobRunner) SetFitSharing(reserve uint64) error {
 // call.
 func (r *gpuJobRunner) SetFitBeside(on bool) {
 	r.beside.Store(on)
+}
+
+// SetStreamLend makes StartStream flag its jobs with TAD_FLAG_LEND (off by default).  While fit sharing is on
+// (SetFitSharing), a streamed job then plans in the memory budget less the reserve and, while its worker waits for the
+// SELECT's next block, runs the queued EWMA and DBSCAN jobs from Start in the reserve, so they no longer wait until the
+// whole SELECT has been read; a block that arrives meanwhile waits for at most one such job.  It takes effect for jobs
+// that start after the call.
+func (r *gpuJobRunner) SetStreamLend(on bool) {
+	r.lend.Store(on)
 }
 
 func algoCode(a string) C.int32_t {
@@ -268,6 +278,10 @@ func (r *gpuJobRunner) StartStream(spec JobSpec, rowsHint uint64, blockRows int,
 		if r.beside.Load() && js.algo == C.TAD_ALGO_ARIMA {
 			js.flags |= C.TAD_FLAG_FIT_BESIDE
 		}
+	}
+	if r.lend.Load() {
+		// the engine ignores the flag while fit sharing is off
+		js.flags |= C.TAD_FLAG_LEND
 	}
 	// The ignore list goes as ids, and every block carries the SrcNS / DstNS ids the BlockReader's dictionary gave the
 	// namespaces.  A reader that hands over the two namespace String columns as clickhouse-go received them (their

@@ -65,6 +65,10 @@ typedef enum { TAD_MEM_HOST = 0, TAD_MEM_DEVICE = 1 } tad_mem;
                                /* on (tad_set_fit_sharing): a tad_submit job, or a streamed one that  */
                                /* has TAD_FLAG_SHARE too; ignored on EWMA and DBSCAN jobs, on         */
                                /* streamed jobs without TAD_FLAG_SHARE and while sharing is off       */
+#define TAD_FLAG_LEND    16u   /* a streamed job lends the GPU to queued EWMA and DBSCAN tad_submit   */
+                               /* jobs while it waits for its caller's next block, while fit sharing  */
+                               /* is on (tad_set_fit_sharing); ignored on tad_submit jobs and while   */
+                               /* sharing is off                                                      */
 
 typedef struct tad_ctx tad_ctx;
 typedef struct tad_job tad_job;
@@ -311,12 +315,34 @@ int tad_job_memory(tad_job *job, uint32_t *passes, uint64_t *peak_workspace_byte
  * above.  A cancel of it ends the joint launch, and its feeder's pending push or end call returns TAD_ERR_CANCELLED.  A
  * cancel of the yielded job takes effect once the streamed job's input has ended and its result is published; a
  * tad_release of the yielded job waits that long too.
+ *
+ * Lending (TAD_FLAG_LEND).  A streamed job holds the context while its worker waits for the caller's next block, and
+ * the caller's source (a ClickHouse SELECT) is usually far slower than the GPU.  A streamed job (tad_submit_stream,
+ * _filtered, _filtered_ns) with TAD_FLAG_LEND, started while sharing is on, plans in the budget less the reserve (its
+ * text key dictionaries grow inside that amount) and lends the GPU while it waits: when no block is pending and its
+ * round has not ended (before the first block, between blocks, before tad_stream_end, between rounds), the wait has
+ * lasted a few milliseconds and an EWMA or DBSCAN tad_submit job is queued.  Its workspace is then parked as a yielded
+ * fit's is, the blocks it has taken are released, and the EWMA and DBSCAN tad_submit jobs queued at that moment run in
+ * submit order with the reserve as their budget; one whose 1/64 hash range does not fit it is put back, as in a yield.
+ * ARIMA and streamed jobs never run in a lend.  Before each job the lend ends if a block is pending, the round has
+ * ended or the job is cancelled, so a pushed block waits for at most one lent job.  After a lend the job does not lend
+ * again until as much time has passed as the lend took, so under a steady stream of short jobs its own time from the
+ * first block to the result at most about doubles.  A job running in a fit's yield or beside a fit does not lend.  A
+ * streamed ARIMA job with TAD_FLAG_SHARE | TAD_FLAG_LEND lends while it reads its input and yields while it fits.
+ * Every job's rows, text ids, fit counts and pass counts are those of a run without lending.  A cancel of the lending
+ * job takes effect once the lent job in progress has ended: its parked buffers are freed and its feeder's pending push
+ * or end call returns TAD_ERR_CANCELLED (tad_release waits that long).  The lending job's device_ms and h2d phase leave
+ * out the time it was lent (tad_job_lent), its tad_job_memory peak leaves out the lent jobs' workspace, theirs stays
+ * within the reserve, and its host row store pages are untouched.
  * TAD_ERR_INVALID_ARG for a nonzero value below 64 MiB; TAD_ERR_UNSUPPORTED when world_size > 1 (a rank whose fit
  * yielded alone would leave its peers waiting for it; the ranks would have to agree on each yield). */
 int tad_set_fit_sharing(tad_ctx *ctx, uint64_t reserve_bytes);
 /* For a COMPLETED ARIMA job: how many times its fit phase yielded and the time it spent parked (ms).  TAD_ERR_STATE for
  * any other job or state. */
 int tad_job_yields(tad_job *job, uint32_t *yields, double *parked_ms);
+/* For a COMPLETED streamed job: the number of jobs that ran in its lends (TAD_FLAG_LEND) and the time it was lent (ms),
+ * both 0 if it never lent.  TAD_ERR_STATE for any other job or state; TAD_ERR_INVALID_ARG for a NULL argument. */
+int tad_job_lent(tad_job *job, uint32_t *jobs_run, double *lent_ms);
 
 /* Pinned host memory this context may hold for its host row store (bytes).  0 (default) = no store.  With a store, a
  * streamed job (tad_submit_stream) that needs more than one hash-range pass keeps its first round's filtered rows in
@@ -349,7 +375,8 @@ int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host
  * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.  The
  * one exception is fit sharing (tad_set_fit_sharing): with TAD_FLAG_SHARE in its spec, a streamed EWMA or DBSCAN job
  * whose caller has pushed its first block may run while an ARIMA fit is parked, and a streamed ARIMA job's fit yields;
- * with TAD_FLAG_FIT_BESIDE as well, a streamed ARIMA job so fed may fit beside a parked fit.
+ * with TAD_FLAG_FIT_BESIDE as well, a streamed ARIMA job so fed may fit beside a parked fit; with TAD_FLAG_LEND, a
+ * streamed job lends the GPU to queued EWMA and DBSCAN tad_submit jobs while it waits for its caller.
  *
  * Blocks: mem is TAD_MEM_HOST (any host memory; pinned buffers from tad_alloc_columns copy at the full PCIe rate) or
  * TAD_MEM_DEVICE (read in place); fewer than 2^32 rows; flow_end and value are required; every block carries the same

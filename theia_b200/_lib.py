@@ -14,7 +14,7 @@ PHASE_NAMES = ("h2d", "hist", "scan", "scatter", "exchange", "group", "spill", "
 ALGOS = {"EWMA": 0, "ARIMA": 1, "DBSCAN": 2}
 STATE_NAMES = ("NEW", "SCHEDULED", "RUNNING", "COMPLETED", "FAILED")
 TAD_MEM_HOST, TAD_MEM_DEVICE = 0, 1
-TAD_FLAG_EMIT_ALL, TAD_FLAG_PROFILE, TAD_FLAG_SHARE, TAD_FLAG_FIT_BESIDE = 1, 2, 4, 8
+TAD_FLAG_EMIT_ALL, TAD_FLAG_PROFILE, TAD_FLAG_SHARE, TAD_FLAG_FIT_BESIDE, TAD_FLAG_LEND = 1, 2, 4, 8, 16
 TAD_REDUCE_MAX, TAD_REDUCE_SUM = 0, 1
 
 EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_alloc_columns",
@@ -23,7 +23,8 @@ EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_a
            "tad_ch_format_ipv4", "tad_ch_dictionary", "tad_set_memory_budget", "tad_job_memory", "tad_submit_stream",
            "tad_stream_push", "tad_stream_end", "tad_set_host_budget", "tad_job_host_memory",
            "tad_stream_push_text", "tad_job_names", "tad_ch_format_names", "tad_submit_stream_filtered", "tad_job_progress",
-           "tad_set_fit_sharing", "tad_job_yields", "tad_submit_stream_filtered_ns", "tad_stream_push_text_ns")
+           "tad_set_fit_sharing", "tad_job_yields", "tad_submit_stream_filtered_ns", "tad_stream_push_text_ns",
+           "tad_job_lent")
 TAD_NAME_OPS = {"any": 0, "eq": 1, "nonempty": 2, "icontains": 3}
 
 
@@ -137,6 +138,7 @@ def load():
     L.tad_job_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     L.tad_set_fit_sharing.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_yields.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
+    L.tad_job_lent.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
     L.tad_set_host_budget.argtypes = [C.c_void_p, C.c_uint64]
     L.tad_job_host_memory.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.tad_ch_string_index.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]

@@ -168,6 +168,11 @@ struct tad_job {
     uint32_t yields = 0;             // times the fit phase yielded (tad_job_yields), under `mu`
     double parked_ms = 0;            // time the job was parked, under `mu`
     double quiet_until = 0;          // now_ms() before which the fit does not yield again
+    // lending (TAD_FLAG_LEND): a streamed job runs queued jobs while it waits for its caller (lend)
+    uint64_t lend = 0;               // the reserve read when it started (0: it does not lend)
+    uint32_t lent_jobs = 0;          // jobs run in its lends (tad_job_lent), under `mu`
+    double lent_ms = 0;              // time it was lent, under `mu`
+    double lend_until = 0;           // now_ms() before which it does not lend again
     // streamed input (tad_submit_stream): the caller hands the worker one column block at a time, under `mu`.  `cols`
     // then holds the first block: its non-NULL columns are the set every block must carry.
     bool stream = false;
@@ -417,10 +422,10 @@ struct PassSplit {
 };
 
 // Lifetimes of the workspace buffers (workspace_bufs).  kJobs and kPasses name the events a buffer is kept across (the
-// others free it); kParked, what a parked ARIMA pass takes out of the context.
+// others free it); kParked, what a parked ARIMA pass, or a streamed job lending the GPU, takes out of the context.
 constexpr int kJobs = 1;     // kept when a job ends: all but the text key dictionaries, which live for one job
 constexpr int kPasses = 2;   // kept across the passes of a job: what every pass reads (free_pass_buffers frees the rest)
-constexpr int kParked = 4;   // moved out of the context while an ARIMA pass is parked (Parked), the rest left for reuse
+constexpr int kParked = 4;   // moved out of the context while a pass is parked (Parked), the rest left for reuse
 constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad_set_memory_budget accepts
 
 // Every workspace buffer with its lifetime, the exported multi-GPU buffer `xbuf` apart (ranks agree on its size).
@@ -443,10 +448,20 @@ constexpr uint64_t kBudgetFloor = 64ull << 20;     // smallest memory budget tad
 //     with their sizes), which its later rounds look names up in and its end copies out, so its ids stay the same, and
 //     the text staging and encode scratch its sweeps take as sized, and the ignore list its namespace text slots are
 //     tested against in every later round.  They were planned in the budget less the reserve.
+// A streamed job lending the GPU (lend) parks between two blocks of a round, or before its first block, with these same
+// buffers.  Besides them its sweep reads, between two blocks, the pass counters and cursor (pcnt), the pass columns, the
+// double-buffered staging (a host row store round may have a partly filled half), the open dictionaries with their
+// sizes, the namespace list image and the out-stage of a round going to the host row store (ostage, two halves of
+// packed rows whose copies to the pages are issued with the next chunk): all parked.  Its planning state and sweep
+// cursors are host variables of run_passes, and the events it waits for between blocks (stage_ev, blk_ev, ost_ev,
+// cnt_ev) have completed before the lend (its streams are synchronised) and are either left alone by the lent jobs or
+// recorded by them on work that has ended before the restore.  A fit's pass never holds the out-stage: a round frees it
+// at its end (RowStore::end).
 // What else a parked streamed pass needs is not in the workspace and no interleaved job touches it: the job's stream
 // input state (tad_job::in: its feeder, blocked in a push or end call, goes on with the same round) and the host row
-// store pages of its passes (its RowStore's lists).  An interleaved job takes store pages only from the free list and
-// new slabs within the host budget less the slabs held (store_share), and frees no slab.
+// store pages of its passes (its RowStore's lists and pinned chunk counts h_chunk, which only a streamed round uses; a
+// lend runs no streamed job).  An interleaved job takes store pages only from the free list and new slabs within the
+// host budget less the slabs held (store_share), and frees no slab.
 // What the interleaved jobs may overwrite is rebuilt before the ARIMA job reads it again:
 //   hist, cursor, big_list, big_base, cls_list, nsb, npb, csr_p, ovf, spill, sortb, dbx, dbi, small: the partition and
 //     group scratch, which the next pass's pipeline ensures and writes before reading (scan_sync: freed at the restore, so
@@ -466,10 +481,10 @@ std::vector<std::pair<DevBuf *, int>> workspace_bufs(tad_ctx *ctx)
     };
     add(kJobs, {&c.hist, &c.cursor, &c.big_list, &c.big_base, &c.cls_list, &c.csr_p, &c.nsb, &c.npb, &c.ovf, &c.spill,
                 &c.sortb, &c.dbx, &c.dbi, &c.scan_sync, &c.exch, &c.hist_all, &c.seg_off, &c.seg_total, &c.xcnt,
-                &c.xtotal, &c.ostage, &c.d_col[8], &c.d_col[9]});
+                &c.xtotal, &c.d_col[8], &c.d_col[9]});
     add(kJobs | kPasses, {&c.small});
     add(kJobs | kParked, {&c.part, &c.entries, &c.offsets, &c.sbase, &c.csr_v, &c.csr_t, &c.ar_y, &c.ar_pred, &c.ar_lam,
-                          &c.ar_res, &c.outb});
+                          &c.ar_res, &c.outb, &c.ostage});
     add(kJobs | kPasses | kParked, {&c.stats, &c.stage, &c.pcnt, &c.ns_ignore, &c.tstage, &c.tscratch, &c.nsl});
     for (int i = 0; i < 8; i++) add(kJobs | kPasses | kParked, {&c.d_col[i]});
     for (auto &t : c.tdict) add(kPasses | kParked, t.bufs());
@@ -618,6 +633,7 @@ void set_passes(tad_job *job, uint32_t done, uint32_t planned, const tad_progres
 }
 
 bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve);
+void release_blocks(tad_job *job, uint64_t n);
 
 // Whether a fit's yield may hand its place to `j`, a queued job: an EWMA or DBSCAN job that has not been found too
 // large for the reserve.  A streamed one only with TAD_FLAG_SHARE and once its feeder has handed over its first block or
@@ -625,9 +641,12 @@ bool run_one(tad_ctx *ctx, tad_job *job, uint64_t reserve);
 // `beside`: the yield is that of a fit parked at the outer level whose reserve halves to the 64 MiB floor or more; then an
 // ARIMA job with TAD_FLAG_FIT_BESIDE may run too, and fits beside it (fit_beside): a tad_submit one, or a streamed one
 // with TAD_FLAG_SHARE as well, fed as above.
-bool interleavable(tad_job *j, bool beside)
+// `lend`: the hand-over is a streamed job's lend, which runs tad_submit EWMA and DBSCAN jobs only: an ARIMA fit would keep
+// its caller waiting for minutes, and a streamed job's own caller could leave the GPU idle in turn.
+bool interleavable(tad_job *j, bool beside, bool lend = false)
 {
     if (j->no_interleave) return false;
+    if (lend) return !j->stream && (j->spec.algo == TAD_ALGO_EWMA || j->spec.algo == TAD_ALGO_DBSCAN);
     if (j->spec.algo == TAD_ALGO_ARIMA) {
         if (!beside || !(j->spec.flags & TAD_FLAG_FIT_BESIDE)) return false;
     } else if (j->spec.algo != TAD_ALGO_EWMA && j->spec.algo != TAD_ALGO_DBSCAN) {
@@ -646,14 +665,21 @@ bool beside_ok(const tad_ctx *ctx, const tad_job *job)
     return ctx->park_depth == 0 && job->share / 2 >= kBudgetFloor;
 }
 
-// Whether a yield would run a job now: a cancelled one is not worth a yield (it fails at once in its turn).
-bool interleave_waiting(tad_ctx *ctx, const tad_job *job)
+// Whether a yield (a lend) would run a job now: a cancelled one is not worth it (it fails at once in its turn).
+bool interleave_waiting(tad_ctx *ctx, const tad_job *job, bool lend = false)
 {
-    const bool beside = beside_ok(ctx, job);
+    const bool beside = !lend && beside_ok(ctx, job);
     std::lock_guard<std::mutex> lk(ctx->mu);
     for (tad_job *j : ctx->queue)
-        if (interleavable(j, beside) && !j->cancel.load()) return true;
+        if (interleavable(j, beside, lend) && !j->cancel.load()) return true;
     return false;
+}
+
+// A lending job's caller has handed over a block or closed its round: the lend ends before the next queued job.
+bool input_ready(tad_job *job)
+{
+    std::lock_guard<std::mutex> lk(job->mu);
+    return job->in.has_blk || job->in.end_req;
 }
 
 // A parked ARIMA pass: the buffers workspace_bufs() marks kParked, with the dictionaries' sizes, are moved out of the
@@ -707,14 +733,17 @@ struct Parked {
 // `job` takes effect once the job in progress has ended: the parked buffers are freed and the job fails.
 // At most one ARIMA job (TAD_FLAG_FIT_BESIDE) runs per yield, the first queued: its fit runs beside the rest of `job`'s,
 // described by `yf` (ctx->beside while the batch runs).
-void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
+// `lend`: `job` is a streamed job lending the GPU while it waits for its caller (lend): the jobs run in its lend reserve,
+// and the batch also stops once its caller hands over a block or closes its round, so a pushed block waits for at most
+// one job.  Returns the number of jobs run (those put back left out).
+uint32_t interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf, bool lend = false)
 {
     std::vector<tad_job *> batch;
     bool beside = yf && beside_ok(ctx, job);
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         for (tad_job *j : ctx->queue)
-            if (interleavable(j, beside)) {
+            if (interleavable(j, beside, lend)) {
                 batch.push_back(j);
                 if (j->spec.algo == TAD_ALGO_ARIMA) beside = false;
             }
@@ -723,8 +752,9 @@ void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
     Parked park(ctx);
     if (yf && ctx->park_depth == 1) ctx->beside = yf;
     const double t1 = now_ms();
+    uint32_t ran = 0;
     for (tad_job *j : batch) {
-        if (job->cancel.load()) break;
+        if (job->cancel.load() || (lend && input_ready(job))) break;
         size_t at;
         {
             std::lock_guard<std::mutex> lk(ctx->mu);       // only this thread takes jobs out of the queue
@@ -732,7 +762,9 @@ void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
             if (at == ctx->queue.size()) continue;
             ctx->queue.erase(ctx->queue.begin() + at);
         }
-        if (!run_one(ctx, j, job->share)) {
+        if (run_one(ctx, j, lend ? job->lend : job->share)) {
+            ran++;
+        } else {
             std::lock_guard<std::mutex> lk(ctx->mu);       // jobs submitted meanwhile went behind it
             ctx->queue.insert(ctx->queue.begin() + at, j);
         }
@@ -743,8 +775,50 @@ void interleave(tad_ctx *ctx, tad_job *job, YieldedFit *yf)
     const bool cancelled = job->cancel.load() != 0;
     park.restore(cancelled);
     if (getenv("TAD_DEBUG_YIELD"))
-        fprintf(stderr, "yield: park %.2f ms, %zu jobs %.2f ms, restore %.2f ms\n", t1 - t0, batch.size(), t2 - t1, now_ms() - t2);
+        fprintf(stderr, "%s: park %.2f ms, %u of %zu jobs %.2f ms, restore %.2f ms\n", lend ? "lend" : "yield", t1 - t0,
+                ran, batch.size(), t2 - t1, now_ms() - t2);
     if (cancelled) fail(TAD_ERR_CANCELLED, "job cancelled");
+    return ran;
+}
+
+// ---- lending the GPU while a streamed job waits for its caller (TAD_FLAG_LEND) --------------------------------------------
+// A streamed job's worker waits in next_block until its caller hands over the next block or closes the round; the
+// caller's source (a ClickHouse SELECT) is usually far slower than the GPU.  A job with TAD_FLAG_LEND started while fit
+// sharing was on (job->lend: the reserve) runs the queued tad_submit EWMA and DBSCAN jobs meanwhile (interleave), its
+// workspace parked as a yielded fit's is (workspace_bufs), and resumes once a block is pending or the round has ended.
+//
+// kLendWaitMs: how long the worker must have waited in one next_block call before it lends.  A caller that pushes
+// back to back hands the next block over within the first poll of the wait loop (5 ms), so a lend there would only make
+// that block wait for a job; a caller whose source has stalled for longer is slower than any lent job's parking
+// overhead.  DESIGN.md section 10 ("Lending the GPU while a streamed job waits") has the measurement.
+constexpr double kLendWaitMs = 5.0;
+
+// Called by next_block, without the job's lock, once the worker has waited `waited` ms in it: lends when every rule
+// holds.  Before lending the context's streams are synchronised, so that every block taken has been read, and those
+// blocks are released: no push waits for a lend it does not need to.  Fairness as for a fit's yields: after a lend the
+// job does not lend again until as much time has passed as the lend took.
+void lend(tad_job *job, double waited)
+{
+    tad_ctx *ctx = job->ctx;
+    if (!job->lend || ctx->park_depth > 0 || waited < kLendWaitMs || now_ms() < job->lend_until ||
+        !interleave_waiting(ctx, job, true))
+        return;
+    CU(cudaStreamSynchronize(ctx->stream));
+    CU(cudaStreamSynchronize(ctx->copy_stream));
+    CU(cudaStreamSynchronize(ctx->d2h_stream));
+    uint64_t taken;
+    {
+        std::lock_guard<std::mutex> lk(job->mu);
+        taken = job->in.taken;
+    }
+    release_blocks(job, taken);
+    const double t0 = now_ms();
+    const uint32_t ran = interleave(ctx, job, nullptr, true);
+    const double t1 = now_ms();
+    job->lend_until = t1 + (t1 - t0);
+    std::lock_guard<std::mutex> lk(job->mu);
+    job->lent_jobs += ran;
+    job->lent_ms += t1 - t0;
 }
 
 // ---- the fit launches of an ARIMA pass ----------------------------------------------------------------------------------
@@ -2047,9 +2121,11 @@ void join_passes(tad_ctx *ctx, std::vector<PassOut> &outs, PassOut &acc)
 }
 
 // ---- streamed input: the worker's side of the hand-over (the caller's side is tad_stream_push / tad_stream_end) ----------
-// The next block of the current round; false once the caller has closed the round.
+// The next block of the current round; false once the caller has closed the round.  While it waits, a job with
+// TAD_FLAG_LEND may lend the GPU to queued jobs (lend).
 bool next_block(tad_job *job, tad_columns &b, tad_text_column *txt)
 {
+    const double t_wait = now_ms();
     std::unique_lock<std::mutex> lk(job->mu);
     for (;;) {
         if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
@@ -2064,6 +2140,12 @@ bool next_block(tad_job *job, tad_columns &b, tad_text_column *txt)
             return true;
         }
         if (job->in.end_req) return false;
+        if (job->lend) {
+            lk.unlock();
+            lend(job, now_ms() - t_wait);
+            lk.lock();
+            if (job->in.has_blk || job->in.end_req || job->cancel.load()) continue;
+        }
         job->cv.wait_for(lk, std::chrono::milliseconds(5));
     }
 }
@@ -2433,6 +2515,7 @@ struct Sweep {
     TextKeys *text = nullptr;        // the job's text key slots, encoded into the staged key columns
     uint64_t nchunk = 0;             // host chunks staged in this sweep
     bool any_host = false;
+    double lent0 = 0;                // the job's lent time when the sweep began (lend)
 
     // `text_row`: text staging and encode scratch bytes per staged row, planned into the staging's 1/16 of the budget
     Sweep(tad_ctx *c, const tad_job *j, PassOut &a, bool host_input, uint64_t budget, size_t text_row)
@@ -2475,6 +2558,7 @@ struct Sweep {
         CU(cudaEventRecord(ctx->ev[0], ctx->stream));
         nchunk = 0;
         any_host = false;
+        lent0 = job->lent_ms;
         if (host_input) {
             CU(cudaEventRecord(ctx->start_ev, ctx->stream));
             CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
@@ -2510,8 +2594,8 @@ struct Sweep {
             CU(cudaEventRecord(ctx->stage_ev[h], st));
         }
     }
-    // the sweep's end: its time goes to the h2d phase where it staged host rows (the split runs behind the copies);
-    // `counts`: the counters and the cursor are copied to h_small
+    // the sweep's end: its time goes to the h2d phase where it staged host rows (the split runs behind the copies), the
+    // time the job lent the GPU meanwhile left out; `counts`: the counters and the cursor are copied to h_small
     void end(bool counts)
     {
         CU(cudaEventRecord(ctx->ev[1], ctx->stream));
@@ -2519,6 +2603,7 @@ struct Sweep {
         CU(cudaStreamSynchronize(ctx->stream));
         float ms = 0;
         CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
+        ms = (float)std::max(0.0, ms - (job->lent_ms - lent0));
         acc.phase_ms[any_host ? TAD_PHASE_H2D : TAD_PHASE_SCATTER] += ms;
         acc.device_ms += ms;
     }
@@ -3291,6 +3376,10 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
     // an ARIMA job run in a yield fits beside the parked fit (TAD_FLAG_FIT_BESIDE): it is a sharing job whose budget is
     // the reserve and whose own reserve, where the jobs run in its yields go, is half of it
     if (reserve && job->spec.algo == TAD_ALGO_ARIMA) job->share = reserve / 2;
+    // lending (TAD_FLAG_LEND): a single-GPU streamed job run in its own turn, not in a yield, while sharing is on; it plans
+    // in the budget less the reserve, where the jobs run in its lends go
+    job->lend = !reserve && job->stream && (job->spec.flags & TAD_FLAG_LEND) && ctx->cfg.world_size == 1
+                    ? ctx->fit_share.load() : 0;
     // ---- plan (single GPU): one pass as today when it fits the budget, else hash-range passes ----------------------
     uint64_t budget = 0;
     bool force_exact = false, split = false;
@@ -3301,12 +3390,13 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
         CU(cudaMemGetInfo(&free_b, &total_b));
         return free_b + ctx->held > kBudgetHeadroom ? free_b + ctx->held - kBudgetHeadroom : 0;
     };
+    const uint64_t held_back = std::max(job->share, job->lend);      // the reserve of a job that yields, lends or both
     auto less_reserve = [&](uint64_t b) {
-        if (!job->share) return b;
-        if (b < job->share + kBudgetFloor)
+        if (!held_back) return b;
+        if (b < held_back + kBudgetFloor)
             fail(TAD_ERR_NOMEM, "a memory budget of %llu bytes less the fit-sharing reserve of %llu bytes is below the "
-                 "64 MiB floor", (unsigned long long)b, (unsigned long long)job->share);
-        return b - job->share;
+                 "64 MiB floor", (unsigned long long)b, (unsigned long long)held_back);
+        return b - held_back;
     };
     if (job->stream) {
         // streamed input always runs through the pass columns (one pass when it fits), under the budget
@@ -4062,6 +4152,16 @@ int tad_job_yields(tad_job *job, uint32_t *yields, double *parked_ms)
     if (job->st.state != TAD_STATE_COMPLETED || job->spec.algo != TAD_ALGO_ARIMA) return TAD_ERR_STATE;
     if (yields) *yields = job->yields;
     if (parked_ms) *parked_ms = job->parked_ms;
+    return TAD_OK;
+}
+
+int tad_job_lent(tad_job *job, uint32_t *jobs_run, double *lent_ms)
+{
+    if (!job || !jobs_run || !lent_ms) return TAD_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->st.state != TAD_STATE_COMPLETED || !job->stream) return TAD_ERR_STATE;
+    *jobs_run = job->lent_jobs;
+    *lent_ms = job->lent_ms;
     return TAD_OK;
 }
 

@@ -173,6 +173,15 @@ class Job:
             raise TadError(rc, "tad_job_yields")
         return {"yields": n.value, "parked_ms": ms.value}
 
+    def lent(self) -> dict:
+        """Of a COMPLETED streamed job (tad_job_lent): the number of queued jobs that ran while it lent the GPU waiting
+        for its caller, and the time it was lent (see TadEngine.submit_stream's ``lend``)."""
+        n, ms = C.c_uint32(), C.c_double()
+        rc = self.eng.lib.tad_job_lent(self.h, C.byref(n), C.byref(ms))
+        if rc != 0:
+            raise TadError(rc, "tad_job_lent")
+        return {"jobs_run": n.value, "lent_ms": ms.value}
+
     def cancel(self):
         """tad_cancel: returns at once; an ARIMA job on one GPU stops within one evaluation round of its fit kernel."""
         self.eng.lib.tad_cancel(self.h)
@@ -347,13 +356,13 @@ class TadEngine:
 
     @staticmethod
     def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep, share=False,
-              fit_beside=False):
+              fit_beside=False, lend=False):
         spec = L.TadJobSpec()
         spec.algo = L.ALGOS[algo] if isinstance(algo, str) else int(algo)
         spec.reducer = reducer
         spec.start_time, spec.end_time = int(start_time), int(end_time)
         spec.flags = (L.TAD_FLAG_EMIT_ALL if emit_all else 0) | (L.TAD_FLAG_SHARE if share else 0) | \
-            (L.TAD_FLAG_FIT_BESIDE if fit_beside else 0)
+            (L.TAD_FLAG_FIT_BESIDE if fit_beside else 0) | (L.TAD_FLAG_LEND if lend else 0)
         spec.id = tad_id.encode()[:39]
         spec.global_rows = int(global_rows)
         if len(ns_ignore):
@@ -385,7 +394,7 @@ class TadEngine:
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
                       check: bool = True, text_filter=None, share: bool = False,
-                      fit_beside: bool = False, ns_ignore_names=None) -> StreamJob:
+                      fit_beside: bool = False, ns_ignore_names=None, lend: bool = False) -> StreamJob:
         """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
         ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
         (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
@@ -393,9 +402,12 @@ class TadEngine:
         fit yields, an EWMA or DBSCAN job may run while a fit is parked.  ``fit_beside``: TAD_FLAG_FIT_BESIDE, with
         ``share`` an ARIMA job queued behind another ARIMA job's fit may fit beside it once its first block is pushed.
         ``ns_ignore_names``: the namespace ignore list as names (bytes), for a job that pushes its namespace columns as
-        text (tad_submit_stream_filtered_ns); ``ns_ignore`` (ids) is then empty."""
+        text (tad_submit_stream_filtered_ns); ``ns_ignore`` (ids) is then empty.  ``lend``: TAD_FLAG_LEND, while fit
+        sharing is on the job plans in the budget less the reserve and, while it waits for the next block, runs queued
+        EWMA and DBSCAN submit() jobs in the reserve (StreamJob.lent())."""
         keep = []
-        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share, fit_beside)
+        spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share, fit_beside,
+                          lend)
         h = C.c_void_p()
         if text_filter is None and ns_ignore_names is None:
             rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
