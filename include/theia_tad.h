@@ -69,6 +69,9 @@ typedef enum { TAD_MEM_HOST = 0, TAD_MEM_DEVICE = 1 } tad_mem;
                                /* jobs while it waits for its caller's next block, while fit sharing  */
                                /* is on (tad_set_fit_sharing); ignored on tad_submit jobs and while   */
                                /* sharing is off                                                      */
+#define TAD_FLAG_RANK_STREAM 32u /* world_size > 1: a tad_submit_stream job that is this rank's part of a  */
+                                 /* job streamed to every rank (see "Several GPUs" under Streamed input); */
+                                 /* ignored on one GPU                                                    */
 
 typedef struct tad_ctx tad_ctx;
 typedef struct tad_job tad_job;
@@ -257,7 +260,7 @@ int tad_job_progress(tad_job *job, tad_progress *p);
  * every rank, naming the rank and the bytes, when a 1/64 hash range does not fit one rank, and a tad_cancel on any rank
  * fails the job with TAD_ERR_CANCELLED on every rank, at the end of the current pass (a job cancelled before it started
  * still meets its peers once).  The contexts stay usable in both cases.  The exported partition buffer of earlier jobs is
- * freed at the start of such a job.  Host or device columns as for tad_submit; streamed input is single GPU only. */
+ * freed at the start of such a job.  Host or device columns as for tad_submit; streamed input as under "Several GPUs" below. */
 int tad_set_memory_budget(tad_ctx *ctx, uint64_t bytes);
 /* For a COMPLETED job: the passes it ran in (the same count on every rank of a multi-GPU job) and the largest device
  * workspace the context held while it ran (TAD_ERR_STATE otherwise). */
@@ -371,7 +374,7 @@ int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host
  *
  * Submit: rows_hint is the caller's estimate of one round's rows (its SELECT count()), 0 = unknown.  It only chooses the
  * pass count and sizes the pass columns before the first round: a wrong hint may cost one round more, never a different
- * result.  TAD_ERR_UNSUPPORTED when world_size > 1.  A context still runs one job at a time: a streamed job holds the
+ * result.  TAD_ERR_UNSUPPORTED when world_size > 1 without TAD_FLAG_RANK_STREAM.  A context still runs one job at a time: a streamed job holds the
  * worker from when it starts until its input ends, and pushes made before the worker reaches the job wait for it.  The
  * one exception is fit sharing (tad_set_fit_sharing): with TAD_FLAG_SHARE in its spec, a streamed EWMA or DBSCAN job
  * whose caller has pushed its first block may run while an ARIMA fit is parked, and a streamed ARIMA job's fit yields;
@@ -398,7 +401,35 @@ int tad_job_host_memory(tad_job *job, uint64_t *stored_rows, uint64_t *peak_host
  * tad_shutdown cancels a streamed job that waits for input; as for every job, release it before tad_shutdown.
  *
  * Threads: while the feeding thread is inside tad_stream_push or tad_stream_end, other threads may call tad_poll and
- * tad_cancel on the job, but not tad_release: release it after the feeding thread has returned. */
+ * tad_cancel on the job, but not tad_release: release it after the feeding thread has returned.
+ *
+ * Several GPUs (world_size > 1): tad_submit_stream with TAD_FLAG_RANK_STREAM in the spec's flags submits this rank's part
+ * of a job whose rows are streamed to every rank; without the flag a rank engine refuses it (TAD_ERR_UNSUPPORTED), and
+ * tad_submit_stream_filtered / _filtered_ns with a filter refuse rank engines with or without it (with a NULL filter
+ * they are tad_submit_stream).  Every rank submits its part, in the
+ * same order relative to its other jobs, as for tad_submit on several GPUs.
+ *   Rows: each rank's caller pushes any disjoint share of the table, in any split: rows of one connection may arrive on
+ *     any rank, since the owner rank still comes from the key hash.  Every rank's blocks carry the same non-NULL columns
+ *     (a rank whose first round is empty carries none and agrees with any); key ids (host dictionary ids) must mean the
+ *     same on every rank.  A mismatched column set fails every rank with TAD_ERR_INVALID_ARG.
+ *   rows_hint: this rank's own share of one round, 0 = unknown; spec.global_rows is ignored.  As on one GPU, it only
+ *     seeds the plan: a wrong hint may cost one round more, never a different result.
+ *   Threads: each rank is fed from its own thread or process.  tad_stream_end returns once every rank has ended the
+ *     round, and its *again is the same on every rank: the ranks decide it from all-gathered counts.  A rank whose caller
+ *     stops delivering without ending its round holds its peers at the round's end until someone cancels the job.
+ *   Rounds: every later round must deliver, on every rank, the per-residue counts that rank's first round delivered;
+ *     otherwise every rank fails with TAD_ERR_INVALID_ARG, its err_msg naming the rank.
+ *   Budget: a rank stream job always plans, as a single-GPU streamed job does, in tad_set_memory_budget or, when that is
+ *     0, the free device memory less a 512 MiB headroom, each rank in its own.  (The "0 = no planning" rule of rank
+ *     tad_submit jobs is unchanged.)  A 1/64 hash range that does not fit one rank fails every rank with TAD_ERR_NOMEM.
+ *   Cancel: tad_cancel on any rank makes that rank's pending and later push or end calls return TAD_ERR_CANCELLED at
+ *     once; its engine treats the rest of the round as empty and still meets its peers.  The job fails with
+ *     TAD_ERR_CANCELLED on every rank: within one block on the peers where the ranks map each other's stop board (the
+ *     default), and their pending push or end calls return TAD_ERR_CANCELLED too; otherwise at the end of the round.
+ *     tad_release of a rank job whose input has not ended cancels it the same way.
+ *   Refused or ignored: tad_stream_push_text and _text_ns return TAD_ERR_UNSUPPORTED, and the job fails with it on every
+ *     rank at the round's end.  TAD_FLAG_SHARE, TAD_FLAG_FIT_BESIDE and TAD_FLAG_LEND are ignored (fit sharing is single
+ *     GPU), and there is no host row store (tad_set_host_budget is single GPU). */
 int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint, tad_job **out);
 /* Hands one block of the current round to the job; returns once the engine has finished reading the previous block. */
 int tad_stream_push(tad_job *job, const tad_columns *block);

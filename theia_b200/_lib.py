@@ -15,6 +15,7 @@ ALGOS = {"EWMA": 0, "ARIMA": 1, "DBSCAN": 2}
 STATE_NAMES = ("NEW", "SCHEDULED", "RUNNING", "COMPLETED", "FAILED")
 TAD_MEM_HOST, TAD_MEM_DEVICE = 0, 1
 TAD_FLAG_EMIT_ALL, TAD_FLAG_PROFILE, TAD_FLAG_SHARE, TAD_FLAG_FIT_BESIDE, TAD_FLAG_LEND = 1, 2, 4, 8, 16
+TAD_FLAG_RANK_STREAM = 32
 TAD_REDUCE_MAX, TAD_REDUCE_SUM = 0, 1
 
 EXPORTS = ("tad_abi_version", "tad_strerror", "tad_init", "tad_shutdown", "tad_alloc_columns",

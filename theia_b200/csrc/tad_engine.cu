@@ -176,6 +176,8 @@ struct tad_job {
     // streamed input (tad_submit_stream): the caller hands the worker one column block at a time, under `mu`.  `cols`
     // then holds the first block: its non-NULL columns are the set every block must carry.
     bool stream = false;
+    bool rank_stream = false;        // this rank's part of a job streamed to every rank (TAD_FLAG_RANK_STREAM)
+    std::atomic<int> peer_stop{0};   // a rank stream job: a peer's stop for it was read off this rank's board
     uint64_t rows_hint = 0;          // the caller's estimate of one round's rows (0 = unknown)
     uint64_t round_rows = 0;         // rows of the first round (tad_status.rows_in)
     uint64_t stored_rows = 0;        // rows the host row store held for the passes (tad_job_host_memory)
@@ -231,6 +233,8 @@ struct tad_ctx {
     bool stop = false;
     std::atomic<int> stopping{0};                   // tad_shutdown: a streamed job waiting for input is cancelled
     int debug_logb = -1;
+    bool debug_no_grow = false;  // TAD_DEBUG_NO_GROW=1: a first streamed round's guarded pass columns never grow (RoundGrowth),
+                                 // so that the tests reach its count-only fallback
     uint64_t text_mask = ~0ull;  // TAD_DEBUG_TEXT_MASK (hex): ANDed into the name hashes of the text dictionaries and the
                                  // ignore list, so that the tests can make names collide
     int debug_target = 0;      // TAD_GROUP_TARGET: mean rows per bucket (tuning)
@@ -1061,6 +1065,20 @@ void set_col(ColPtrs &c, int i, const void *p)
     }
 }
 
+// A rank stream job whose first round was empty takes its peers' column set `mask` (run_passes_multi), so that it holds
+// the pass columns they hold; the pointers stand for columns of no rows and are never read.
+void adopt_columns(tad_job *job, uint64_t mask)
+{
+    static uint64_t none = 0;
+    std::lock_guard<std::mutex> lk(job->mu);
+    if (job->in.pushed) return;
+    tad_columns &c = job->cols;
+    void **slot[10] = {(void **)&c.src_ip, (void **)&c.dst_ip, (void **)&c.src_port, (void **)&c.dst_port, (void **)&c.proto,
+                       (void **)&c.flow_start, (void **)&c.flow_end, (void **)&c.value, (void **)&c.src_ns, (void **)&c.dst_ns};
+    for (int i = 0; i < 10; i++)
+        if (mask >> i & 1) *slot[i] = &none;
+}
+
 // Whether column i of a job's blocks arrives as text: a key slot (src_ip, dst_ip) or a namespace slot (src_ns, dst_ns).
 bool is_text(const tad_job *job, int i) { return i < 2 ? job->text[i] : i >= 8 && job->text[i - 6]; }
 
@@ -1389,6 +1407,18 @@ uint64_t stop_word(const tad_job *job, int fit_stop)
     return (job->cancel.load() ? 2u : 0u) | (fit_stop >= 0 ? 4u | ((uint64_t)fit_stop << 8) : 0u);
 }
 
+// A rank stream job between two blocks: the rank whose stop for `job` is on this rank's board (-1: none).  Read on
+// board_stream, so the job's work in flight is not waited for.
+int board_stop(tad_ctx *ctx, const tad_job *job)
+{
+    std::lock_guard<std::mutex> lk(ctx->board_mu);
+    CU(cudaMemcpyAsync(ctx->h_board + 8, ctx->board, 4 * kMaxRanks, cudaMemcpyDeviceToHost, ctx->board_stream));
+    CU(cudaStreamSynchronize(ctx->board_stream));
+    for (int r = 0; r < ctx->cfg.world_size; r++)
+        if (ctx->h_board[8 + r] == job->ordinal) return r;
+    return -1;
+}
+
 bool any_stop(const unsigned long long *w, int world)
 {
     for (int r = 0; r < world; r++)
@@ -1408,6 +1438,23 @@ void agree_stop(const unsigned long long *w, int world)
         if (by >= world) fail(TAD_ERR_INTERNAL, "rank %d: the ARIMA fit stopped with no cancel on any rank", r);
         fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", by);
     }
+}
+
+// Fails a rank stream job alike on every rank when a word of `w` (one per rank) carries an input verdict (run_passes_multi):
+// bits 40.., a block that rank refused (its error code, negated); bit 32, a later round whose per-residue counts differ
+// from that rank's first round's.
+void agree_input(const tad_job *job, const unsigned long long *w, int world, int me)
+{
+    for (int r = 0; r < world; r++) {
+        const int code = -(int)((w[r] >> 40) & 0xff);
+        if (code == TAD_ERR_UNSUPPORTED)
+            fail(code, "rank %d: text key columns are not supported on a job streamed to several GPUs", r);
+        if (code) fail(code, "rank %d: %s", r, r == me ? job->in.msg : "a block of its stream was refused");
+    }
+    for (int r = 0; r < world; r++)
+        if (w[r] >> 32 & 1)
+            fail(TAD_ERR_INVALID_ARG, "rank %d: a round delivered other per-residue row counts than its first round: the "
+                 "source changed between reads", r);
 }
 
 // Result of one pipeline run: a one-pass job or one hash-range pass.
@@ -2122,12 +2169,15 @@ void join_passes(tad_ctx *ctx, std::vector<PassOut> &outs, PassOut &acc)
 
 // ---- streamed input: the worker's side of the hand-over (the caller's side is tad_stream_push / tad_stream_end) ----------
 // The next block of the current round; false once the caller has closed the round.  While it waits, a job with
-// TAD_FLAG_LEND may lend the GPU to queued jobs (lend).
+// TAD_FLAG_LEND may lend the GPU to queued jobs (lend).  A rank stream job fails only where its peers fail with it: once
+// it is cancelled, its context shuts down or a block was refused, the rest of its round is empty (StreamRound).
 bool next_block(tad_job *job, tad_columns &b, tad_text_column *txt)
 {
     const double t_wait = now_ms();
     std::unique_lock<std::mutex> lk(job->mu);
     for (;;) {
+        if (job->rank_stream && job->ctx->stopping.load()) job->cancel.store(1);
+        if (job->rank_stream && (job->cancel.load() || job->peer_stop.load() || job->in.err)) return false;
         if (job->cancel.load()) fail(TAD_ERR_CANCELLED, "job cancelled");
         if (job->ctx->stopping.load()) fail(TAD_ERR_CANCELLED, "context is shutting down");
         if (job->in.err) fail(job->in.err, "%s", job->in.msg);
@@ -2249,6 +2299,98 @@ struct PassColumns {
         const PassCols o = out();
         return tad_columns{rows, rows, TAD_MEM_DEVICE, 0, o.src_ip, o.dst_ip, o.src_port, o.dst_port, o.proto,
                            o.flow_start, o.flow_end, o.value, nullptr, nullptr};
+    }
+};
+
+// ---- one streamed round (run_passes, run_passes_multi) -------------------------------------------------------------------
+// first() waits for the round's first block, or for its end, before the job is planned: the job's column set is that
+// block's.  run() takes every block of the round: block(b, tx) enqueues the block's reads and returns the stream they end
+// on; block k is released (its push returns) once block k+1 is enqueued and k's reads are done.  A rank stream job reads
+// its board between blocks and ends its round early on a peer's stop (`stopper`: that rank), as next_block does on its
+// own cancel; it releases every block it took before it meets its peers, so its caller's calls return at once.
+struct StreamRound {
+    tad_ctx *ctx;
+    tad_job *job;
+    tad_columns pend{};
+    tad_text_column pend_txt[4]{};
+    bool have_pend = false;
+    int stopper = -1;
+
+    bool first() { return have_pend = next_block(job, pend, pend_txt); }
+
+    template <class Block>
+    uint64_t run(Block block)
+    {
+        uint64_t rows = 0, k = 0;
+        tad_columns b{};
+        tad_text_column tx[4]{};
+        bool got = have_pend ? (b = pend, std::copy(pend_txt, pend_txt + 4, tx), true) : next_block(job, b, tx);
+        have_pend = false;
+        while (got) {
+            CU(cudaEventRecord(ctx->blk_ev[k & 1], block(b, (const tad_text_column *)tx)));
+            if (k > 0) {
+                CU(cudaEventSynchronize(ctx->blk_ev[(k - 1) & 1]));
+                release_blocks(job, taken() - 1);
+            }
+            rows += b.rows;
+            k++;
+            if (job->rank_stream && stopper < 0 && (stopper = board_stop(ctx, job)) >= 0) {
+                std::lock_guard<std::mutex> lk(job->mu);
+                job->peer_stop.store(1);
+                job->cv.notify_all();
+            }
+            got = next_block(job, b, tx);
+        }
+        if (job->rank_stream && k) {
+            CU(cudaEventSynchronize(ctx->blk_ev[(k - 1) & 1]));
+            release_blocks(job, taken());
+        }
+        return rows;
+    }
+    uint64_t taken()
+    {
+        std::lock_guard<std::mutex> lk(job->mu);
+        return job->in.taken;
+    }
+};
+
+// The first streamed round's pass columns: sized from the hint before it, grown geometrically up to `cap` rows while it
+// arrives, the rows held carried over.  `ub` bounds the rows written so far; a block that could pass the columns has the
+// cursor read back first.  `guarded` (beside the text key dictionaries; on a rank, which may not fail alone): where the
+// growth does not fit the budget, the columns are dropped and the rest of the round is only counted.
+struct RoundGrowth {
+    tad_ctx *ctx;
+    PassColumns &pc;
+    const unsigned long long *d_cursor;
+    uint64_t cap;
+    bool to_store;                   // with a host row store: rows past `cap` go there
+    bool guarded;
+    bool &count_only;
+    uint64_t ub = 0, have = 0;       // bound of the rows in the pass columns; the rows they hold (read back)
+
+    // room for every row the next `n` input rows can add; false (to_store) when they would pass `cap`
+    bool room(uint64_t n)
+    {
+        if ((pc.cap >= cap && !to_store) || ub + n <= pc.cap) { ub += n; return true; }
+        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWPassCursor, d_cursor, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        have = std::min<uint64_t>(ctx->h_small[tad_ctx::kWPassCursor], pc.cap);
+        if (to_store && have + n > cap) return false;
+        if (have + n > pc.cap) {
+            const uint64_t want = std::min(cap, std::max(2 * pc.cap, have + n));
+            if (guarded) {
+                size_t grow = 0;
+                for (int i = 0; i < 8; i++) grow += has_col(pc.job, i) ? exact_bytes(col_bytes(i, want)) : 0;
+                if (!can_grow(ctx, grow) || ctx->debug_no_grow) {
+                    pc.drop();
+                    count_only = true;
+                    return true;
+                }
+            }
+            pc.size(want, true, have);
+        }
+        ub = have + n;
+        return true;
     }
 };
 
@@ -2826,9 +2968,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     cudaStream_t st = ctx->stream;
     const bool stream = job->stream;
     // a streamed job's column set is that of its first block: wait for it (or for an empty round) before planning
-    tad_columns pend{};
-    tad_text_column pend_txt[4]{};
-    bool have_pend = stream && next_block(job, pend, pend_txt);
+    StreamRound round{ctx, job};
+    if (stream) round.first();
     const tad_columns &hc = job->cols;
     const uint64_t R = stream ? job->rows_hint : hc.rows;        // rows to plan for (0: unknown)
     const bool host_input = stream || hc.mem != TAD_MEM_DEVICE;  // a streamed round may bring host blocks
@@ -2892,33 +3033,9 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
     bool count_only = false;         // the first round's rows are only counted (the store fell back, or the pass columns
                                      // gave way to the text key dictionaries)
     uint32_t sweeps = 0;
-    uint64_t ub = 0, have = 0;       // first streamed round: bound of the rows in the pass columns; rows they hold
-    // first streamed round: make room in the pass columns for every row the next `n` input rows can add (`ub` bounds the
-    // rows written so far; when it would pass the columns, the cursor is read back and the columns grow, rows carried over)
-    // With a host budget, rows that would pass `cap` go to the host row store instead: false, `have` = the rows the
-    // pass columns hold.
-    auto room = [&](uint64_t n) {
-        if ((pc.cap >= cap && !host_budget) || ub + n <= pc.cap) { ub += n; return true; }
-        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWPassCursor, d_cnt + kMaxPasses, 8, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        have = std::min<uint64_t>(ctx->h_small[tad_ctx::kWPassCursor], pc.cap);
-        if (host_budget && have + n > cap) return false;
-        if (have + n > pc.cap) {
-            const uint64_t want = std::min(cap, std::max(2 * pc.cap, have + n));
-            if (text) {                      // beside the dictionaries the columns may not grow: the round only counts
-                size_t grow = 0;
-                for (int i = 0; i < 8; i++) grow += has_col(job, i) ? exact_bytes(col_bytes(i, want)) : 0;
-                if (!can_grow(ctx, grow)) {
-                    pc.drop();
-                    count_only = true;
-                    return true;
-                }
-            }
-            pc.size(want, true, have);
-        }
-        ub = have + n;
-        return true;
-    };
+    // first streamed round: the pass columns grow as it arrives; beside the dictionaries they may not grow past the
+    // budget, and the round then only counts.  With a host budget, rows that would pass `cap` go to the host row store.
+    RoundGrowth grow{ctx, pc, d_cnt + kMaxPasses, cap, host_budget != 0, text, count_only};
     RowStore rs(ctx, sw, host_budget, pack_scratch);
     bool stored = false;             // the store holds the whole first round: the passes load from it
     bool dropped = false;            // the store fell back in the first round: it only counted
@@ -2930,6 +3047,7 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
             return;
         }
         rs.start(ostage_bytes);
+        const uint64_t have = grow.have;
         const ColPtrs held = col_ptrs(pc.as_input(have));
         for (uint64_t lo = 0; lo < have && rs.active; lo += chunk) rs.pack(offset_cols(held, lo), std::min(chunk, have - lo), false);
         if (!rs.active) count_only = true;   // the store fell back: the rest of the round is only counted
@@ -2943,20 +3061,14 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
         if (!stream) {
             sw.feed(hc, 0, v, M, pc, count_only, nullptr);
         } else {
-            // the round's blocks; block k is released (its push returns) once block k+1 is enqueued and k's copy is done
-            uint64_t rows = 0, k = 0;
-            ub = 0;
-            tad_columns b{};
-            tad_text_column tx[4]{};
-            bool got = have_pend ? (b = pend, std::copy(pend_txt, pend_txt + 4, tx), true) : next_block(job, b, tx);
-            have_pend = false;
+            grow.ub = 0;
             if (sweeps == 0 && host_budget && P > 1)         // the hint plans passes: the round goes to the store
                 rs.start(ostage_bytes);
-            while (got) {
+            const uint64_t rows = round.run([&](const tad_columns &b, const tad_text_column *tx) {
                 // TextKeys::room drops the first round's pass columns (cap 0) for the dictionaries: the rest is only counted
                 if (sweeps == 0 && pc.cap == 0 && !rs.active) count_only = true;
-                if (sweeps == 0 && host_budget && !rs.active && !count_only && !room(b.rows)) switch_to_store();
-                else if (sweeps == 0 && !host_budget && !count_only) room(b.rows);
+                if (sweeps == 0 && host_budget && !rs.active && !count_only && !grow.room(b.rows)) switch_to_store();
+                else if (sweeps == 0 && !host_budget && !count_only) grow.room(b.rows);
                 const bool to_store = rs.active;
                 const uint64_t took = to_store ? rs.put(b, tx) : 0;
                 count_only = count_only || (to_store && !rs.active);   // the store fell back: the rest is only counted
@@ -2965,20 +3077,8 @@ uint32_t run_passes(tad_ctx *ctx, tad_job *job, uint64_t budget, uint64_t host_b
                     CU(cudaEventRecord(ctx->start_ev, st));
                     CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->start_ev, 0));
                 }
-                CU(cudaEventRecord(ctx->blk_ev[k & 1], b.mem == TAD_MEM_DEVICE && !to_store ? st : ctx->copy_stream));
-                if (k > 0) {
-                    CU(cudaEventSynchronize(ctx->blk_ev[(k - 1) & 1]));
-                    uint64_t taken;
-                    {
-                        std::lock_guard<std::mutex> lk(job->mu);
-                        taken = job->in.taken;
-                    }
-                    release_blocks(job, taken - 1);
-                }
-                rows += b.rows;
-                k++;
-                got = next_block(job, b, tx);
-            }
+                return b.mem == TAD_MEM_DEVICE && !to_store ? st : ctx->copy_stream;
+            });
             if (sweeps == 0) job->round_rows = rows;
             if (sweeps == 0 && ctx->ostage.p) {
                 stored = rs.end();
@@ -3133,18 +3233,31 @@ size_t mp_pipe_bytes(tad_ctx *ctx, const tad_job *job, uint64_t global, uint64_t
 //   end     every pass ends with an 8-byte all-gather of {split, cancelled, fit stopped} (stop_word): a rank whose spill
 //           scratch or result buffer does not fit, or whose fit stopped on the board, skips the rest of its pass but still
 //           gets there, and then every rank splits the pass or stops.
+// A rank stream job (TAD_FLAG_RANK_STREAM, DESIGN.md section 10, "Several GPUs") sweeps one round of its caller's blocks
+// instead of its columns.  Its plan waits for its first block and carries its hint as its rows and its column set; the
+// hint only seeds P0.  Its counts carry whether its first round's pass columns held all of pass (0, P0), its stop word,
+// its input verdict, the rows its pass columns hold and the rows it delivered: P then comes from the delivered rows and
+// the counts, and the pass columns are planned from the counts.  Every later round ends with an 8-byte all-gather of its
+// stop word and verdict (its counts differ from its first round's), before the pipeline reads the pass.  Its rounds close
+// on the same decisions on every rank, so every caller's tad_stream_end returns the same *again.
 uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &acc)
 {
     cudaStream_t st = ctx->stream;
     const int W = ctx->cfg.world_size, me = ctx->cfg.rank, logW = log_world(ctx);
+    const bool stream = job->rank_stream;
+    set_progress(job, TAD_STATE_RUNNING, 0);
+    StreamRound round{ctx, job};
+    if (stream) round.first();
     const tad_columns &hc = job->cols;
-    const uint64_t R = hc.rows;
-    const bool host = hc.mem != TAD_MEM_DEVICE && R > 0;
+    const uint64_t R = stream ? job->rows_hint : hc.rows;      // rows to plan for (a stream: its hint, 0 = unknown)
+    const bool host = stream || (hc.mem != TAD_MEM_DEVICE && R > 0);
     Sweep sw(ctx, job, acc, host, budget, 0);
     const size_t stage_bytes = sw.stage_bytes();
     const size_t NC = (size_t)W * kMaxPasses;               // one rank's (owner, residue) counters
-    const size_t pcnt_bytes = (NC * (W + 1) + 1) * 8;        // mine, every rank's (all-gathered), the pass cursor
-    set_progress(job, TAD_STATE_RUNNING, 0);
+    // behind them, a stream's first round: pass 0 loaded, stop word, input verdict, pass-column rows held, rows delivered
+    constexpr size_t kRoundWords = 5;
+    const size_t NM = NC + kRoundWords;                      // one rank's counts message
+    const size_t pcnt_bytes = (NM * (W + 1) + 1) * 8;        // mine, every rank's (all-gathered), the pass cursor
 
     // ---- plan ----------------------------------------------------------------------------------------------------------
     // what every pass keeps: pass columns of `n` rows, staging, counters, the ns_ignore list (and kFixedBytes)
@@ -3158,9 +3271,13 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     // are all n fits the budget (exact partition)
     const uint64_t cap = largest_fit(kMaxPassRows, budget, [&](uint64_t n) {
         const uint64_t g = n * (uint64_t)W;
-        return kept_bytes(std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) + alloc_bytes(xbuf_bytes(ctx, g, n, false));
+        return kept_bytes(stream ? n : std::min(n, R)) + mp_pipe_bytes(ctx, job, g, n, n, false) +
+               alloc_bytes(xbuf_bytes(ctx, g, n, false));
     });
-    const uint64_t colcap = std::min(cap, R);
+    // rows the pass columns may hold: a table's shard; a stream's any count up to `cap` (its hint only seeds the plan)
+    const uint64_t colcap = stream ? cap : std::min(cap, R);
+    uint64_t mask = 0;               // the column set (a stream's agreed one: a rank whose first round is empty has none)
+    for (int i = 0; i < 10; i++) mask |= has_col(job, i) ? 1ull << i : 0;
 
     // The budget applies from the plan on: until then the context may still hold the exported buffer of an earlier job,
     // larger than this budget, which only the plan all-gather lets it free.  No rank may fail on its own before it.
@@ -3174,76 +3291,169 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     struct RankPlan {
         uint64_t rows, cap, budget, kept;
         bool cancel;
+        uint64_t colcap, mask;
     } rk[kMaxRanks];
     memset(ctx->h_small, 0, tad_ctx::kGatherMax * 8);
     ctx->h_small[0] = R;
     ctx->h_small[1] = cap;
     ctx->h_small[2] = budget;
-    ctx->h_small[3] = kept_bytes(colcap);
+    ctx->h_small[3] = kept_bytes(stream ? 0 : colcap);   // a stream's pass columns are planned from its counts (need)
     ctx->h_small[4] = job->cancel.load() ? 1 : 0;
+    ctx->h_small[5] = colcap;
+    ctx->h_small[6] = mask;
     gather_ms += gather_small(ctx, tad_ctx::kGatherMax, true);
-    uint64_t total = 0;
     for (int r = 0; r < W; r++) {
         const unsigned long long *w = ctx->h_small + tad_ctx::kGatherMax * (1 + r);
-        rk[r] = RankPlan{w[0], w[1], w[2], w[3], w[4] != 0};
-        total += w[0];
+        rk[r] = RankPlan{w[0], w[1], w[2], w[3], w[4] != 0, w[5], w[6]};
     }
     free_buf(ctx, ctx->xbuf);
     ctx->limit = budget;
     ctx->peak = ctx->held;
     for (int r = 0; r < W; r++)
         if (rk[r].cancel) fail(TAD_ERR_CANCELLED, "job cancelled (rank %d)", r);
+    if (stream) {
+        int from = -1;
+        for (int r = 0; r < W; r++) {
+            if (!rk[r].mask) continue;
+            if (from >= 0 && rk[r].mask != rk[from].mask)
+                fail(TAD_ERR_INVALID_ARG, "invalid request: rank %d's blocks carry another set of columns than rank %d's",
+                     r, from);
+            if (from < 0) from = r;
+        }
+        if (!mask && from >= 0) adopt_columns(job, rk[from].mask);
+        if (from >= 0) mask = rk[from].mask;
+    }
     for (int r = 0; r < W; r++)
         if (rk[r].cap == 0)
             fail(TAD_ERR_NOMEM, "rank %d: a memory budget of %llu bytes does not hold one row of a pass", r,
                  (unsigned long long)rk[r].budget);
-    // P from the rows: every rank's input and its share of the table within its capacity, with 1/8 head-room
-    auto guess_ok = [&](uint32_t p) {
-        for (int r = 0; r < W; r++)
-            if (std::max(rk[r].rows, (total + W - 1) / W) / p > rk[r].cap / 8 * 7) return false;
-        return true;
+    // P from the rows rows_of(r): every rank's input and its share of the table within its capacity, with 1/8 head-room
+    auto guess = [&](auto rows_of) {
+        uint64_t total = 0;
+        for (int r = 0; r < W; r++) total += rows_of(r);
+        auto ok = [&](uint32_t p) {
+            for (int r = 0; r < W; r++)
+                if (std::max<uint64_t>(rows_of(r), (total + W - 1) / W) / p > rk[r].cap / 8 * 7) return false;
+            return true;
+        };
+        uint32_t p = 1;
+        while (p < (uint32_t)kMaxPasses && !ok(p)) p *= 2;
+        return p;
     };
-    uint32_t P = 1;
-    while (P < (uint32_t)kMaxPasses && !guess_ok(P)) P *= 2;
+    uint32_t P = guess([&](int r) { return rk[r].rows; });
+    const uint32_t P0 = P;
+    // a stream's pass columns of n rows (at least kMinCols, so that a pass of no rows on a rank still has columns)
+    constexpr uint64_t kMinCols = 2048;
+    auto col_need = [&](uint64_t n) {
+        size_t b = 0;
+        for (int i = 0; i < 8; i++) b += mask >> i & 1 ? alloc_bytes(col_bytes(i, std::max(n, kMinCols))) : 0;
+        return b;
+    };
 
     // ---- pass columns and the sweep --------------------------------------------------------------------------------------
+    // a stream's pass columns: from its hint (1M rows without one, kMinCols for an empty first round), grown while its
+    // first round arrives (RoundGrowth)
     PassColumns pc(ctx, job);
-    pc.size(colcap);
+    pc.size(!stream ? colcap : std::min(colcap, !round.have_pend ? kMinCols : R ? R / P + R / P / 8 + kMinCols : uint64_t(1) << 20));
     if (stage_bytes) ensure(ctx, ctx->stage, stage_bytes);
     ensure(ctx, ctx->pcnt, pcnt_bytes);
     ensure(ctx, ctx->stats, 64 * sizeof(uint32_t));
     unsigned long long *d_cnt = static_cast<unsigned long long *>(ctx->pcnt.p);
-    unsigned long long *d_cursor = d_cnt + NC * (W + 1);
+    unsigned long long *d_cursor = d_cnt + NM * (W + 1);
     sw.f = row_filter(ctx, job, sw.ns);
     sw.cnt = d_cnt;
     sw.cursor = d_cursor;
     sw.log_world = logW;
+    bool count_only = false;         // the first round's pass columns could not grow inside the budget: it only counts
+    RoundGrowth grow{ctx, pc, d_cursor, colcap, false, true, count_only};
+    uint32_t sweeps = 0;
+    bool unplanned = false;          // a later round brought host rows to a rank whose first round was empty (no staging)
+    bool open = false;               // a streamed round is swept and its caller waits in tad_stream_end
     // the rows of pass (v, M) -> the pass columns, counted under (owner, residue)
     auto sweep = [&](uint32_t v, uint32_t M) {
         CU(cudaMemsetAsync(d_cnt, 0, NC * 8, st));
         CU(cudaMemsetAsync(d_cursor, 0, 8, st));
         sw.begin(host);
-        sw.feed(hc, 0, v, M, pc, false, nullptr);
+        if (!stream) {
+            sw.feed(hc, 0, v, M, pc, false, nullptr);
+        } else {
+            grow.ub = 0;
+            const uint64_t rows = round.run([&](const tad_columns &b, const tad_text_column *) {
+                if (b.rows && b.mem != TAD_MEM_DEVICE && !sw.chunk) {
+                    unplanned = true;
+                    return st;
+                }
+                if (sweeps == 0 && !count_only) grow.room(b.rows);
+                sw.feed(b, 0, v, M, pc, count_only, nullptr);
+                return b.mem == TAD_MEM_DEVICE ? st : ctx->copy_stream;
+            });
+            if (sweeps == 0) job->round_rows = rows;
+            open = true;
+        }
         sw.end(false);
+        sweeps++;
+    };
+    // a stream's input verdict in the agreed words: bit 32, a later round's counts differ from its first round's `mine`;
+    // bits 40.., a block this rank refused (its error code, negated)
+    auto input_word = [&](const uint64_t *mine) -> uint64_t {
+        uint64_t w = 0;
+        if (mine) {
+            PinnedBlock hb = take_pinned(ctx, NC * 8);
+            const cudaError_t e1 = cudaMemcpyAsync(hb.p, d_cnt, NC * 8, cudaMemcpyDeviceToHost, st);
+            const cudaError_t e2 = cudaStreamSynchronize(st);
+            const bool same = e1 == cudaSuccess && e2 == cudaSuccess && memcmp(hb.p, mine, NC * 8) == 0;
+            give_pinned(ctx, hb);
+            CU(e1);
+            CU(e2);
+            if (!same || unplanned) w |= 1ull << 32;
+        }
+        std::lock_guard<std::mutex> lk(job->mu);
+        return w | (uint64_t)(uint32_t)(-job->in.err) << 40;
     };
 
     // ---- counts ----------------------------------------------------------------------------------------------------------
     sweep(0, P);
     std::vector<uint64_t> cnt(NC * W);       // [source rank][owner rank][residue]
+    unsigned long long loaded_w[kMaxRanks], stop_w[kMaxRanks], input_w[kMaxRanks], pcap_w[kMaxRanks], rows_w[kMaxRanks];
     {
+        CU(cudaMemcpyAsync(ctx->h_small + tad_ctx::kWPassCursor, d_cursor, 8, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        ctx->h_small[0] = !count_only && ctx->h_small[tad_ctx::kWPassCursor] <= pc.cap;
+        ctx->h_small[1] = stop_word(job, round.stopper);
+        ctx->h_small[2] = stream ? input_word(nullptr) : 0;
+        ctx->h_small[3] = pc.cap;
+        ctx->h_small[4] = job->round_rows;
+        CU(cudaMemcpyAsync(d_cnt + NC, ctx->h_small, kRoundWords * 8, cudaMemcpyHostToDevice, st));
         CU(cudaEventRecord(ctx->ev[0], st));
-        if (nccl_allgather(&ctx->nccl, d_cnt, d_cnt + NC, NC * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
+        if (nccl_allgather(&ctx->nccl, d_cnt, d_cnt + NM, NM * 8, st)) fail(TAD_ERR_NCCL, "%s", nccl_last_error());
         CU(cudaEventRecord(ctx->ev[1], st));
-        PinnedBlock hb = take_pinned(ctx, NC * W * 8);
-        const cudaError_t e1 = cudaMemcpyAsync(hb.p, d_cnt + NC, NC * W * 8, cudaMemcpyDeviceToHost, st);
+        PinnedBlock hb = take_pinned(ctx, NM * W * 8);
+        const cudaError_t e1 = cudaMemcpyAsync(hb.p, d_cnt + NM, NM * W * 8, cudaMemcpyDeviceToHost, st);
         const cudaError_t e2 = cudaStreamSynchronize(st);
-        if (e1 == cudaSuccess && e2 == cudaSuccess) memcpy(cnt.data(), hb.p, NC * W * 8);
+        if (e1 == cudaSuccess && e2 == cudaSuccess)
+            for (int s = 0; s < W; s++) {
+                const uint64_t *m = static_cast<const uint64_t *>(hb.p) + s * NM;
+                memcpy(&cnt[s * NC], m, NC * 8);
+                loaded_w[s] = m[NC];
+                stop_w[s] = m[NC + 1];
+                input_w[s] = m[NC + 2];
+                pcap_w[s] = m[NC + 3];
+                rows_w[s] = m[NC + 4];
+            }
         give_pinned(ctx, hb);
         CU(e1);
         CU(e2);
         float ms = 0;
         CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
         gather_ms += ms;
+    }
+    if (stream) {
+        agree_stop(stop_w, W);
+        agree_input(job, input_w, W, me);
+        count_only = false;          // later rounds split their pass into the pass columns
+        // a wrong hint must not cost a round per surplus pass: plan from the rows the first round delivered, as exact hints
+        // would have, at the price of that one round (loaded is then false unless P comes back to P0)
+        P = std::min(P, guess([&](int r) { return rows_w[r]; }));
     }
     struct PassDims {
         uint64_t global = 0, max_rows = 0, rows[kMaxRanks] = {}, owned[kMaxRanks] = {};
@@ -3270,8 +3480,10 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
         }
         return x;
     };
-    auto need = [&](int r, const PassDims &d, bool slots, size_t x) {
-        return rk[r].kept + mp_pipe_bytes(ctx, job, d.global, d.rows[r], d.owned[r], slots) + alloc_bytes(x);
+    // a rank's workspace in pass d; a stream's pass columns hold `cols` rows (the pass's rows when they are sized for it)
+    auto need = [&](int r, const PassDims &d, bool slots, size_t x, uint64_t cols = 0) {
+        return rk[r].kept + (stream ? col_need(std::max(cols, d.rows[r])) : 0) +
+               mp_pipe_bytes(ctx, job, d.global, d.rows[r], d.owned[r], slots) + alloc_bytes(x);
     };
     int bad_r = 0;
     uint32_t bad_v = 0;
@@ -3282,7 +3494,7 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
             const PassDims d = dims(v, M);
             if (!d.global) continue;
             for (int r = 0; r < W; r++)
-                if (d.rows[r] > std::min(rk[r].cap, rk[r].rows) || d.owned[r] > kMaxPassRows ||
+                if (d.rows[r] > rk[r].colcap || d.owned[r] > kMaxPassRows ||
                     need(r, d, slots, x) > rk[r].budget) {
                     bad_r = r;
                     bad_v = v;
@@ -3291,7 +3503,6 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
         }
         return true;
     };
-    const uint32_t P0 = P;
     while (P < (uint32_t)kMaxPasses && !fits_all(P, false)) P *= 2;
     auto too_big = [&](int r, uint32_t v, uint32_t M) {
         const PassDims d = dims(v, M);
@@ -3303,16 +3514,51 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
     // the slot path where its exported buffer fits next to the workspace of every pass on every rank
     const bool slots = ctx->peer_pull && ctx->optimistic && fits_all(P, true);
     const size_t xplan = xbuf_of(P, slots);
-    bool loaded = P == P0;           // pass (0, P) is in the pass columns already
+    bool loaded = P == P0;           // pass (0, P) is in the pass columns already (a stream's: on every rank, in columns
+                                     // that fit its plan)
+    for (int r = 0; r < W && stream && loaded; r++)
+        loaded = loaded_w[r] && need(r, dims(0, P), slots, xplan, pcap_w[r]) <= rk[r].budget;
+    // a stream's round stays open until the ranks know whether another round follows: one does while a queued pass has
+    // rows (a loaded pass 0 may still split)
+    auto finish_round = [&](bool more) {
+        if (!open) return;
+        close_round(job, more);
+        open = false;
+    };
+    uint64_t counted = 0;
+    for (uint64_t n : cnt) counted += n;
+    if (!loaded) finish_round(counted > 0);
 
     // ---- passes ----------------------------------------------------------------------------------------------------------
-    auto run_one = [&](uint32_t v, uint32_t M, const PassList &, PassOut &o) {
+    auto run_one = [&](uint32_t v, uint32_t M, const PassList &rest, PassOut &o) {
         const PassDims d = dims(v, M);
+        if (!loaded) {                // the round the previous pass was swept in closes once that pass has run
+            bool more = d.global > 0;
+            for (const auto &e : rest) more = more || dims(e.first, e.second).global > 0;
+            finish_round(more);
+        }
         if (!d.global) {              // the same on every rank: no collective
             loaded = false;
             return false;
         }
-        if (!loaded) sweep(v, M);
+        if (!loaded && stream) {
+            // columns too small, or too large for the plan: sized for the pass, the earlier passes' buffers freed first
+            if (d.rows[me] > pc.cap || pc.cap < kMinCols || need(me, d, slots, xplan, pc.cap) > budget) {
+                free_pass_buffers(ctx);
+                pc.drop();
+                pc.size(std::max(d.rows[me], kMinCols));
+            }
+            sweep(v, M);
+            // the round's verdict, agreed before the pipeline reads the pass: a cancel, a stop read off the board, a
+            // refused block, or counts that differ from the first round's (the pass columns then disagree with the
+            // agreed sizes the pipeline's exchange is planned from)
+            ctx->h_small[0] = stop_word(job, round.stopper) | input_word(&cnt[me * NC]);
+            gather_ms += gather_small(ctx, 1, true);
+            agree_stop(ctx->h_small + 1, W);
+            agree_input(job, ctx->h_small + 1, W, me);
+        } else if (!loaded) {
+            sweep(v, M);
+        }
         loaded = false;
         // the buffers of earlier passes go where this pass's growth would pass the budget
         const size_t xgrow = alloc_bytes(xplan) > ctx->xbuf.cap ? alloc_bytes(xplan) - ctx->xbuf.cap : 0;
@@ -3327,7 +3573,7 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
             split_here = true;
         }
         // ---- the agreed end of the pass: {split, cancelled, fit stopped} of every rank ----
-        ctx->h_small[0] = (split_here ? 1u : 0u) | stop_word(job, o.fit_stop);
+        ctx->h_small[0] = (split_here ? 1u : 0u) | stop_word(job, o.fit_stop >= 0 ? o.fit_stop : round.stopper);
         gather_ms += gather_small(ctx, 1, true);
         int split_r = -1;
         for (int r = W - 1; r >= 0; r--)
@@ -3343,6 +3589,7 @@ uint32_t run_passes_multi(tad_ctx *ctx, tad_job *job, uint64_t budget, PassOut &
         return true;
     };
     const uint32_t passes = run_pass_queue(ctx, job, P, acc, run_one);
+    finish_round(false);
     acc.phase_ms[TAD_PHASE_SYNC] += gather_ms;
     acc.device_ms += gather_ms;
     return passes;
@@ -3399,7 +3646,8 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
         return b - held_back;
     };
     if (job->stream) {
-        // streamed input always runs through the pass columns (one pass when it fits), under the budget
+        // streamed input always runs through the pass columns (one pass when it fits), under the budget (a rank stream
+        // job's: run_passes_multi applies it once the plan has freed the exported buffer)
         set_progress(job, TAD_STATE_RUNNING, 0);
         budget = less_reserve(context_budget());
         ctx->limit = budget;
@@ -3427,7 +3675,8 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
     ctx->peak = ctx->held;
     PassOut acc;
     uint32_t passes = 1;
-    if (multi_budget) {
+    const bool multi = multi_budget || job->rank_stream;
+    if (multi) {
         passes = run_passes_multi(ctx, job, budget, acc);
     } else if (!split) {
         set_passes(job, 0, 1);
@@ -3442,7 +3691,7 @@ void run_job(tad_ctx *ctx, tad_job *job, uint64_t reserve)
             split = true;
         }
     }
-    if (split) passes = run_passes(ctx, job, budget, host_budget, reserve != 0, acc);
+    if (split && !multi) passes = run_passes(ctx, job, budget, host_budget, reserve != 0, acc);
     publish_rows(job, acc.block, acc.out_rows);
     ctx->limit = 0;
     {
@@ -3582,8 +3831,8 @@ int submit_job(tad_ctx *ctx, tad_job *job, const tad_job_spec *spec, const tad_c
     *out = job;
     char msg[200];
     int rc = validate(spec, cols, msg, sizeof(msg));
-    if (rc == TAD_OK && job->stream && ctx->cfg.world_size > 1) {
-        snprintf(msg, sizeof(msg), "streamed input runs on a single GPU only");
+    if (rc == TAD_OK && job->stream && ctx->cfg.world_size > 1 && !job->rank_stream) {
+        snprintf(msg, sizeof(msg), "streamed input runs on a single GPU only, or on every rank with TAD_FLAG_RANK_STREAM");
         rc = TAD_ERR_UNSUPPORTED;
     }
     if (rc != TAD_OK) {
@@ -3624,11 +3873,24 @@ int stream_abort(tad_job *job, std::unique_lock<std::mutex> &lk, int code, const
     return code;
 }
 
+// A rank stream job cancelled on this rank, or whose engine read a peer's stop off its board: its caller's push and end
+// calls return TAD_ERR_CANCELLED without waiting for its peers, once the engine reads none of its blocks (a block handed
+// over but not taken is withdrawn).
+bool rank_halted(const tad_job *job) { return job->rank_stream && (job->cancel.load() || job->peer_stop.load()); }
+
+int rank_cancelled(tad_job *job, std::unique_lock<std::mutex> &lk)
+{
+    job->in.has_blk = false;
+    while (!finished(job) && job->in.released < job->in.taken) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    return TAD_ERR_CANCELLED;
+}
+
 // Whether a push or end call is legal now: TAD_ERR_STATE on a job without streamed input or after its input is complete;
 // TAD_ERR_CANCELLED (once the job is FAILED) after tad_cancel; the job's error once it has failed.
 int stream_gate(tad_job *job, std::unique_lock<std::mutex> &lk)
 {
     if (!job->stream || job->in.input_done) return TAD_ERR_STATE;
+    if (rank_halted(job)) return rank_cancelled(job, lk);
     if (job->cancel.load()) {
         while (!finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
         return TAD_ERR_CANCELLED;
@@ -3763,6 +4025,7 @@ int tad_init(const tad_config *cfg, tad_ctx **out)
     ctx->cfg.nccl_unique_id = nullptr;
     if (const char *e = getenv("TAD_DEBUG_LOGB")) ctx->debug_logb = atoi(e);
     if (const char *e = getenv("TAD_DEBUG_TEXT_MASK")) ctx->text_mask = strtoull(e, nullptr, 16);
+    if (const char *e = getenv("TAD_DEBUG_NO_GROW")) ctx->debug_no_grow = atoi(e) != 0;
     if (const char *e = getenv("TAD_GROUP_TARGET")) ctx->debug_target = atoi(e);
     cudaDeviceGetAttribute(&ctx->num_sms, cudaDevAttrMultiProcessorCount, cfg->device);
     ctx->numa = numa_of_device(cfg->device);
@@ -3952,6 +4215,7 @@ int tad_submit_stream(tad_ctx *ctx, const tad_job_spec *spec, uint64_t rows_hint
     if (!ctx || !spec || !out) return TAD_ERR_INVALID_ARG;
     tad_job *job = new tad_job();
     job->stream = true;
+    job->rank_stream = (spec->flags & TAD_FLAG_RANK_STREAM) && ctx->cfg.world_size > 1;
     job->rows_hint = rows_hint;
     tad_columns none{};
     return submit_job(ctx, job, spec, &none, out);
@@ -4038,6 +4302,14 @@ int tad_stream_push_text_ns(tad_job *job, const tad_columns *block, const tad_te
     std::unique_lock<std::mutex> lk(job->mu);
     int rc = stream_gate(job, lk);
     if (rc != TAD_OK) return rc;
+    if ((src_ip || dst_ip || src_ns || dst_ns) && job->rank_stream) {   // the ranks would need a dictionary they agree on
+        if (!job->in.err) {
+            job->in.err = TAD_ERR_UNSUPPORTED;
+            snprintf(job->in.msg, sizeof(job->in.msg), "text key columns are not supported on a job streamed to several GPUs");
+            job->cv.notify_all();
+        }
+        return TAD_ERR_UNSUPPORTED;
+    }
     char msg[200];
     const tad_text_column *txt[4] = {src_ip, dst_ip, src_ns, dst_ns};
     rc = check_block(job, block, txt, msg, sizeof(msg));
@@ -4049,14 +4321,16 @@ int tad_stream_push_text_ns(tad_job *job, const tad_columns *block, const tad_te
 
     // one block of look-ahead: hand this one over once the worker has taken the previous one, then return once the
     // engine no longer reads the previous one
-    while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    while (job->in.has_blk && !finished(job) && !rank_halted(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (rank_halted(job)) return rank_cancelled(job, lk);
     if (finished(job)) return job->st.error;
     job->in.blk = *block;
     for (int t = 0; t < 4; t++) job->in.txt[t] = txt[t] ? *txt[t] : tad_text_column{};
     job->in.has_blk = true;
     const uint64_t k = job->in.pushed++;
     job->cv.notify_all();
-    while (job->in.released < k && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    while (job->in.released < k && !finished(job) && !rank_halted(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (rank_halted(job)) return rank_cancelled(job, lk);
     return finished(job) ? job->st.error : TAD_OK;
 }
 
@@ -4066,11 +4340,13 @@ int tad_stream_end(tad_job *job, int32_t *again)
     std::unique_lock<std::mutex> lk(job->mu);
     int rc = stream_gate(job, lk);
     if (rc != TAD_OK) return rc;
-    while (job->in.has_blk && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    while (job->in.has_blk && !finished(job) && !rank_halted(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (rank_halted(job)) return rank_cancelled(job, lk);
     if (finished(job)) return job->st.error;
     job->in.end_req = true;
     job->cv.notify_all();
-    while (!job->in.round_done && !finished(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    while (!job->in.round_done && !finished(job) && !rank_halted(job)) job->cv.wait_for(lk, std::chrono::milliseconds(5));
+    if (rank_halted(job)) return rank_cancelled(job, lk);
     if (!job->in.round_done) return job->st.error;
     job->in.round_done = false;
     job->in.input_done = !job->in.again;

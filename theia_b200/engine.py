@@ -356,13 +356,14 @@ class TadEngine:
 
     @staticmethod
     def _spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, global_rows, keep, share=False,
-              fit_beside=False, lend=False):
+              fit_beside=False, lend=False, ranks=False):
         spec = L.TadJobSpec()
         spec.algo = L.ALGOS[algo] if isinstance(algo, str) else int(algo)
         spec.reducer = reducer
         spec.start_time, spec.end_time = int(start_time), int(end_time)
         spec.flags = (L.TAD_FLAG_EMIT_ALL if emit_all else 0) | (L.TAD_FLAG_SHARE if share else 0) | \
-            (L.TAD_FLAG_FIT_BESIDE if fit_beside else 0) | (L.TAD_FLAG_LEND if lend else 0)
+            (L.TAD_FLAG_FIT_BESIDE if fit_beside else 0) | (L.TAD_FLAG_LEND if lend else 0) | \
+            (L.TAD_FLAG_RANK_STREAM if ranks else 0)
         spec.id = tad_id.encode()[:39]
         spec.global_rows = int(global_rows)
         if len(ns_ignore):
@@ -394,7 +395,8 @@ class TadEngine:
     def submit_stream(self, algo="EWMA", reducer: int = L.TAD_REDUCE_MAX, start_time: int = 0, end_time: int = 0,
                       ns_ignore=(), rows_hint: int = 0, emit_all: bool = False, tad_id: str = "",
                       check: bool = True, text_filter=None, share: bool = False,
-                      fit_beside: bool = False, ns_ignore_names=None, lend: bool = False) -> StreamJob:
+                      fit_beside: bool = False, ns_ignore_names=None, lend: bool = False,
+                      ranks: bool = False) -> StreamJob:
         """A job whose rows arrive as blocks (tad_submit_stream); ``rows_hint``: one round's rows, 0 = unknown.
         ``text_filter``: row predicates evaluated on the GPU (tad_submit_stream_filtered): {"src_ip" / "dst_ip":
         (op, pattern bytes) with op one of "any", "eq", "nonempty", "icontains", "proto_eq": 0..255}; absent keys hold
@@ -404,10 +406,12 @@ class TadEngine:
         ``ns_ignore_names``: the namespace ignore list as names (bytes), for a job that pushes its namespace columns as
         text (tad_submit_stream_filtered_ns); ``ns_ignore`` (ids) is then empty.  ``lend``: TAD_FLAG_LEND, while fit
         sharing is on the job plans in the budget less the reserve and, while it waits for the next block, runs queued
-        EWMA and DBSCAN submit() jobs in the reserve (StreamJob.lent())."""
+        EWMA and DBSCAN submit() jobs in the reserve (StreamJob.lent()).  ``ranks``: TAD_FLAG_RANK_STREAM, on a rank
+        engine (world_size > 1) the job is this rank's part of a job streamed to every rank: each rank's caller pushes
+        any disjoint share of the rows, ``rows_hint`` is this rank's share; ignored on one GPU."""
         keep = []
         spec = self._spec(algo, reducer, start_time, end_time, tad_id, emit_all, ns_ignore, 0, keep, share, fit_beside,
-                          lend)
+                          lend, ranks)
         h = C.c_void_p()
         if text_filter is None and ns_ignore_names is None:
             rc = self.lib.tad_submit_stream(self.ctx, C.byref(spec), int(rows_hint), C.byref(h))
